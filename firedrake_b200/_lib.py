@@ -16,6 +16,7 @@ MAX_1D = 8
 
 FORM_HELMHOLTZ = 1
 FORM_DG_ADVECTION = 2
+FORM_HELMHOLTZ_COEF = 3
 CELL_HEX_EXTRUDED = 1
 CELL_HEX = 2
 CELL_TRIANGLE = 3

@@ -473,12 +473,26 @@ class DirichletBC:
 
 @dataclass
 class Form:
-    """alpha*inner(grad(u), grad(v))*dx + beta*inner(u, v)*dx on ``V``."""
+    """alpha*inner(grad(u), grad(v))*dx + beta*inner(u, v)*dx on ``V``.
+
+    With ``kappa`` (a scalar Dat on ``V``): alpha*inner(kappa*grad(u), grad(v))*dx +
+    beta*inner(u, v)*dx -- a heterogeneous material, or the Jacobian of a nonlinear diffusion
+    problem at the current iterate.  Runs on the hand-written coefficient kernel (scalar spaces)."""
     V: FunctionSpace
     alpha: float = 1.0
     beta: float = 0.0
+    kappa: op2.Dat | None = None
 
-    def kernel(self, rank):
+    def coefficient_args(self):
+        """The parloop arguments that follow the coordinates: kappa, read through the argument map."""
+        return [] if self.kappa is None else [self.kappa(op2.READ, self.V.cell_node_map)]
+
+    def kernel(self, rank, diagonal=False):
+        if self.kappa is not None:
+            if self.V.cdim != 1:
+                raise NotImplementedError("coefficient forms take scalar spaces only")
+            return op2.Kernel("helmholtz_coef", degree=self.V.degree, alpha=self.alpha, beta=self.beta,
+                              rank=rank, diagonal=diagonal)
         import os
         # per-cell metric on meshes whose cells are all parallelepipeds (checked on the device;
         # GPU-validated in round 2, FDB_AFFINE=0 opts out)
@@ -519,7 +533,8 @@ class OneFormAssembler:
             self._loop = op2.Parloop(self._gk, V.cell_set,
                                      [tensor(op2.INC, V.cell_node_map),
                                       V.coordinates(op2.READ, V.coord_map),
-                                      self.u(op2.READ, V.cell_node_map)], location="device")
+                                      self.u(op2.READ, V.cell_node_map)] + self.form.coefficient_args(),
+                                     location="device")
         tensor.zero()
         self._loop()
         for bc in self.bcs:
@@ -556,7 +571,7 @@ def assemble(form: Form, u=None, tensor=None, bcs=(), mat_type="aij"):
         lg = (lgm, lgm)
     op2.par_loop(form.kernel(2), V.cell_set,
                  tensor(op2.INC, (V.cell_node_map, V.cell_node_map), lgmaps=lg),
-                 V.coordinates(op2.READ, V.coord_map))
+                 V.coordinates(op2.READ, V.coord_map), *form.coefficient_args())
     owned = V.node_set.size
     for bc in bcs:
         # on a partitioned space a constrained node gets its unit diagonal from its OWNER only:
@@ -610,10 +625,14 @@ class ImplicitMatrixContext:
         """``assemble(a, diagonal=True)`` then 1 on the constrained rows
         (matrix_free/operators.py:199-205; firedrake/assemble.py:1226-1241)."""
         V = self.form.V
-        k = op2.Kernel("helmholtz", degree=V.degree, alpha=self.form.alpha, beta=self.form.beta,
-                       diagonal=True)
+        if self.form.kappa is not None:
+            k = self.form.kernel(1, diagonal=True)
+        else:
+            k = op2.Kernel("helmholtz", degree=V.degree, alpha=self.form.alpha, beta=self.form.beta,
+                           diagonal=True)
         D.zero()
-        op2.par_loop(k, V.cell_set, D(op2.INC, V.cell_node_map), V.coordinates(op2.READ, V.coord_map))
+        op2.par_loop(k, V.cell_set, D(op2.INC, V.cell_node_map), V.coordinates(op2.READ, V.coord_map),
+                     *self.form.coefficient_args())
         for bc in self.bcs:
             bc.set(D, 1.0)
         return D
@@ -789,8 +808,12 @@ def solve(form: Form, L: op2.Dat, u: op2.Dat, bcs=(), solver_parameters=None, hi
         elif pc == "mg":
             if hierarchy is None:
                 raise ValueError("pc_type mg needs the mesh hierarchy")
-            vc = _mg.VCycle(hierarchy, V.degree, lambda W: Form(W, form.alpha, form.beta),
-                            bc_domains=tuple(s for bc in bcs for s in bc.sub_domains), allreduce=allreduce)
+            # with a coefficient field, every coarser level gets the injection of the next finer
+            # level's kappa (VCycle's ``kappa``), as Firedrake coarsens coefficients for rediscretised
+            # multigrid
+            vc = _mg.VCycle(hierarchy, V.degree, lambda W, k=None: Form(W, form.alpha, form.beta, k),
+                            bc_domains=tuple(s for bc in bcs for s in bc.sub_domains), allreduce=allreduce,
+                            kappa=form.kappa)
             top = len(hierarchy) - 1
             M = lambda r, z: vc.apply(top, r, z)
         else:

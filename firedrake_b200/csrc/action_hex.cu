@@ -25,6 +25,8 @@
 // (rank 2: columns of the element tensor as actions on unit vectors, also the
 // diagonal), SLIM (p = 5: one staged map row per column, indices recomputed).
 // DESIGN.md section 4.1 has the measurements behind each of these choices.
+// helmholtz_coef_kernel is the same body (action_hex_body.cuh) with COEF set: a coefficient field
+// kappa scales the stiffness term (FDB_FORM_HELMHOLTZ_COEF, DESIGN.md section 4.5).
 //
 // Arithmetic: the basis is first interpolated to the N Gauss points per axis
 // (B (x) B (x) B), gradients are then taken with the collocated derivative
@@ -77,6 +79,21 @@ struct HelmParams {
     double wq[N];
     double xq[N];
 };
+
+// FDB_FORM_HELMHOLTZ_COEF: the coefficient field kappa, gathered through map0 like x.  A derived
+// struct, so that the parameter layout of the constant-coefficient kernels stays as it is.
+template <int N>
+struct HelmCoefParams : HelmParams<N> {
+    const double *kappa;
+};
+
+// the quadrature weight of the stiffness flux, times kappa at the point (COEF: s_kap[q])
+template <bool COEF>
+__device__ __forceinline__ double coef_weight(double w, const double *s_kap, int q)
+{
+    if constexpr (COEF) return w * s_kap[q];
+    else return w;
+}
 
 __device__ __forceinline__ double fast_rcp(double x)
 {
@@ -197,11 +214,12 @@ constexpr bool OPT_STASH = true;
 #endif
 // warps per CTA: 4 everywhere except degree 5 (N = 6), whose per-warp staging is 38 KB:
 // one CTA of 5 warps fills the 227 KB of shared memory better than one of 4
-template <int N, bool SLIM = false>
+template <int N, bool SLIM = false, bool COEF = false>
 struct WPC {
     // degree 5 (N = 6): 38 KB of staging per warp -> 5 warps; 27.5 KB when SLIM -> 8 warps
-    // (255 registers x 256 threads = the whole register file)
-    static constexpr int value = (N == 6) ? (SLIM ? 8 : 5) : FDB_WARPS;
+    // (255 registers x 256 threads = the whole register file).  The coefficient kernel stages
+    // 10.4 KB more per warp at degree 5: 4 warps (5 when SLIM) fit the 227 KB.
+    static constexpr int value = (N == 6) ? (COEF ? (SLIM ? 5 : 4) : (SLIM ? 8 : 5)) : FDB_WARPS;
 };
 
 __device__ __forceinline__ void cp_async8(void *smem, const void *gmem)
@@ -234,7 +252,9 @@ __device__ __forceinline__ void cp_async4(void *smem, const void *gmem)
 // row -- and one staged row per distinct COLUMN of the warp (at most two when a
 // column has at least 32/N layers) instead of one per cell, triple-buffered over
 // the three items in flight (compute / value prefetch / row prefetch).
-template <int N, bool SLIM = false>
+// COEF: one more cell-strided buffer for kappa, first its gathered dof values (layout Z), then,
+// overwritten in place, its values at the quadrature points (layout Y: [qx][qy][qz] at qy = lane)
+template <int N, bool SLIM = false, bool COEF = false>
 struct WarpSmem {
     static constexpr int CW = 32 / N;
     static constexpr int CWS = (32 % N == 0) ? CW : CW + 1;   // idle lanes get a scratch slot
@@ -249,11 +269,13 @@ struct WarpSmem {
 #endif
     static constexpr int GS = FDB_STASH_STRIDE;                // stash stride: c2 c4 c5 c7 (12) + A1 of 4 lanes (4 apart)
     static constexpr int STASH = (OPT_STASH && N == 4 && !SLIM) ? CWS * GS : 0;   // doubles
+    static constexpr int KAPPA = COEF ? CWS * US : 0;          // doubles: kappa (single buffer)
     static constexpr int IDX = SLIM ? 0 : 2 * CWS * US;        // ints: global dof index per local dof
     static constexpr int MAPRAW = SLIM ? 3 * 2 * US : CWS * US;   // ints: bottom-cell map row(s)
     static constexpr int VIDX = SLIM ? 3 * 2 * 8 : 2 * CWS * 8;   // ints: bottom-cell vertex row(s)
-    static constexpr int BYTES = (((TILE + UBUF + COORD + STASH) * 8 + (IDX + MAPRAW + VIDX) * 4) + 15) / 16 * 16;
-    static constexpr int CTA_BYTES = WPC<N, SLIM>::value * BYTES + ND * 4 + 32;
+    static constexpr int BYTES =
+        (((TILE + UBUF + COORD + STASH + KAPPA) * 8 + (IDX + MAPRAW + VIDX) * 4) + 15) / 16 * 16;
+    static constexpr int CTA_BYTES = WPC<N, SLIM, COEF>::value * BYTES + ND * 4 + 32;
 };
 
 // One pipeline unit = (item, component): the cells a warp works on next.
@@ -272,521 +294,41 @@ struct Unit {
 // the trilinear terms of the coordinate field vanish, the Jacobian is constant per cell and the
 // metric G = (alpha / |det|) K K^T (K = cofactor rows) is formed once per cell instead of at
 // each of the N^3 quadrature points (DESIGN.md section 8b).
+// COEF: alpha*inner(kappa*grad u, grad v)*dx + beta*inner(u, v)*dx with kappa in the argument space
+// (FDB_FORM_HELMHOLTZ_COEF): kappa's dof values are gathered with x's indices, interpolated to the
+// quadrature points once per cell and scale the stiffness flux (DESIGN.md section 4.5).
 template <int N, bool MASS, bool ATOMIC, int MINB, bool MATRIX = false, bool SLIM = false, bool AFFINE = false>
 __global__ void __launch_bounds__(WPC<N, SLIM>::value * 32, MINB)
 helmholtz_action_kernel(const __grid_constant__ HelmParams<N> P)
 {
-    static_assert(!(SLIM && MATRIX), "matrix mode keeps the per-cell index buffer");
-    static_assert(!(AFFINE && MATRIX), "the affine variant exists for 1-forms only");
-    using WS = WarpSmem<N, SLIM>;
-    constexpr int CW = WS::CW;
-    constexpr int CWS = WS::CWS;
-    constexpr int ND = N * N * N;
-    constexpr int US = WS::US;
-    constexpr int CS = WS::CS;
-    extern __shared__ __align__(16) unsigned char smem_raw[];
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    double *wbase = reinterpret_cast<double *>(smem_raw + (size_t)warp * WS::BYTES);
-    double *s_tile = wbase;
-    double *s_u = s_tile + WS::TILE;                 // [CWS][US]   (single buffer)
-    double *s_coord = s_u + WS::UBUF;                // [CWS][CS]   (single buffer)
-    double *s_stash = s_coord + WS::COORD;           // [CWS][GS]   (geometry coefficients, if STASH)
-    constexpr bool STASH = WS::STASH > 0 && !MATRIX && !AFFINE;
-    int *s_idx = reinterpret_cast<int *>(s_stash + WS::STASH);   // [2][CWS][US]  (empty if SLIM)
-    int *s_mapraw = s_idx + WS::IDX;                 // [CWS][US], or [3][2][US] if SLIM
-    int *s_vidx = s_mapraw + WS::MAPRAW;             // [2][CWS][8], or [3][2][8] if SLIM
-    int *s_off0 = reinterpret_cast<int *>(smem_raw + (size_t)WPC<N, SLIM>::value * WS::BYTES);
-    int *s_off1 = s_off0 + ND;
+    constexpr bool COEF = false;
+    [[maybe_unused]] const double *kappa = nullptr;
+#include "action_hex_body.cuh"
+}
 
-    for (int i = threadIdx.x; i < ND; i += blockDim.x) s_off0[i] = P.off0[i];
-    if (threadIdx.x < 8) s_off1[threadIdx.x] = P.off1[threadIdx.x];
-    __syncthreads();
-
-    const int cw = lane / N, t = lane - cw * N;
-    const bool lane_active = cw < CW;
-    Tile<N> tile(s_tile, cw, t);
-
-    const int ncells = P.ncols * P.nlay_items;      // < 2^31, checked by the launcher
-    const int nitems = (ncells + CW - 1) / CW;
-    const double eta = P.xq[lane_active ? t : 0];
-    const double wy_alpha = P.wq[lane_active ? t : 0] * P.alpha;
-    const double wy_beta = P.wq[lane_active ? t : 0] * P.beta;
-
-    // warp-uniform work iterator: chunks of consecutive items (one column's
-    // worth) handed out by an atomic counter -> locality inside a chunk,
-    // dynamic balance across SMs
-    auto advance = [&](Unit u) -> Unit {
-        if (u.item >= 0 && u.comp + 1 < P.cdim) {
-            u.comp++;
-            return u;
-        }
-        u.comp = 0;
-        u.ib = SLIM ? (u.ib == 2 ? 0 : u.ib + 1) : (u.ib ^ 1);
-        if (u.item >= 0 && u.cur + 1 < u.end) {
-            u.cur++;
-            u.item = u.cur;
-            return u;
-        }
-        if (u.item == -2) return u;                  // queue already drained
-        int base = 0;
-        if (lane == 0) base = atomicAdd(P.counter, P.chunk);
-        base = __shfl_sync(0xffffffffu, base, 0);
-        if (base >= nitems) {
-            u.item = -2;
-            return u;
-        }
-        u.cur = base;
-        u.end = min(base + P.chunk, nitems);
-        u.item = base;
-        return u;
-    };
-
-    // per-lane decode of a unit (cell -> column, layer); division by the
-    // launch-constant layer count through a precomputed reciprocal
-    auto decode = [&](Unit &u) {
-        const int lin = u.item * CW + cw;
-        u.valid = lane_active && u.item >= 0 && lin < ncells;
-        unsigned ci = __umulhi((unsigned)lin, P.nlay_rcp);
-        int kk = lin - (int)ci * P.nlay_items;
-        if (kk >= P.nlay_items) { kk -= P.nlay_items; ci++; }
-        if (!u.valid) { ci = 0; kk = 0; }
-        u.layer = P.lay_first + P.lay_step * kk;
-        u.col = P.collist ? __ldg(P.collist + ci) : (P.col0 + (int)ci);
-        // cells of the warp that sit in the same column share one staged copy of
-        // the map / vertex rows: the lowest such cell (leader) copies, the
-        // others read its slot
-        if (SLIM) {
-            // at most two distinct columns per warp (launcher guarantees nlay_items >= CW)
-            const int col0 = __shfl_sync(0xffffffffu, u.col, 0);
-            u.src = (u.col != col0) ? 1 : 0;
-            const unsigned peers = __match_any_sync(0xffffffffu, u.valid ? u.src : -1 - cw);
-            u.lead = (__ffs(peers) - 1) / N == cw;
-        } else {
-            const unsigned peers = __match_any_sync(0xffffffffu, u.valid ? u.col : -1 - cw);
-            u.src = (__ffs(peers) - 1) / N;
-            u.lead = u.src == cw;
-        }
-    };
-    auto row_of = [&](const Unit &u) -> int * {
-        return SLIM ? s_mapraw + (u.ib * 2 + u.src) * US : s_mapraw + u.src * US;
-    };
-    auto vrow_of = [&](const Unit &u) -> int * {
-        return SLIM ? s_vidx + (u.ib * 2 + u.src) * 8 : s_vidx + (u.ib * CWS + u.src) * 8;
-    };
-
-    // Three-stage gather pipeline, all through cp.async (no registers held, no
-    // load the warp has to wait for):
-    //   stage A (unit i+2): copy the bottom-cell map row / vertex row to smem
-    //   stage B (unit i+1): indices = row + offset*layer; copy x values and
-    //                       vertex coordinates to smem
-    //   stage C (unit i)  : compute + scatter
-    // Stage B is issued in N slices from inside the quadrature loop so that its
-    // integer/LSU instructions fill issue slots the fp64 pipe leaves free.
-    // Every lane touches only its own slots of s_u / s_idx / s_mapraw; s_vidx and
-    // s_coord are shared by the N lanes of a cell and are read after the
-    // wait + __syncwarp at the top of the loop.
-    auto stageA = [&](const Unit &u) {
-        if (u.valid && u.comp == 0 && u.lead) {
-            const int *mrow = P.map0 + (long long)u.col * ND;
-            int *sm = row_of(u);
-            if ((ND % 4) == 0 && (US % 4) == 0) {
-                // rows are 16-byte aligned: 128-bit copies
-                for (int j = t; j < ND / 4; j += N) cp_async16(sm + 4 * j, mrow + 4 * j);
-            } else {
-#pragma unroll
-                for (int j = 0; j < N * N; j++) cp_async4(sm + j * N + t, mrow + j * N + t);
-            }
-            int *sv = vrow_of(u);
-            for (int v = t; v < 8; v += N) cp_async4(sv + v, P.map1 + (long long)u.col * 8 + v);
-        }
-    };
-    auto stageB_coords = [&](const Unit &u) {
-        if (u.valid && u.comp == 0) {
-            const int *sv = vrow_of(u);
-            double *scd = s_coord + cw * CS;
-            for (int i = t; i < 24; i += N) {
-                int v = i / 3, a = i - v * 3;
-                int g = sv[v] + s_off1[v] * u.layer;
-                cp_async8(scd + i, P.coords + (long long)g * 3 + a);
-            }
-        }
-    };
-    auto stageB_part = [&](const Unit &u, int ubuf, int part) {
-        if (u.valid) {
-            double *su = s_u + cw * US;
-            int *si = s_idx + (u.ib * CWS + cw) * US;
-            const int *sm = row_of(u);
-            int g[N];
-            if (SLIM || u.comp == 0) {
-#pragma unroll
-                for (int j = 0; j < N; j++) {
-                    const int loc = (part * N + j) * N + t;
-                    g[j] = sm[loc] + s_off0[loc] * u.layer;
-                }
-                if (!SLIM) {
-#pragma unroll
-                    for (int j = 0; j < N; j++) si[(part * N + j) * N + t] = g[j];
-                }
-            } else {
-#pragma unroll
-                for (int j = 0; j < N; j++) g[j] = si[(part * N + j) * N + t];
-            }
-            if (!MATRIX) {
-#pragma unroll
-                for (int j = 0; j < N; j++)
-                    cp_async8(su + (part * N + j) * N + t, P.x + (long long)g[j] * P.cdim + u.comp);
-            }
-        }
-    };
-
-    Unit cur{-1, 0, 0, 0, 0, false, 0, 0, 0, false};
-    cur = advance(cur);
-    decode(cur);
-    Unit nxt = advance(cur);
-    decode(nxt);
-    stageA(cur);
-    cp_async_commit();
-    cp_async_wait<0>();
-    __syncwarp();
-    int ubuf = 0;
-    stageB_coords(cur);
-#pragma unroll
-    for (int part = 0; part < N; part++) stageB_part(cur, ubuf, part);
-    stageA(nxt);
-    cp_async_commit();
-    double A1[3], A3[3], A6[3], c2[3], c4[3], c5[3], c7[3];
-    double Gm[6], adet_c = 1.0;       // AFFINE: metric (xx, xy, xz, yy, yz, zz) and |det J| of the cell
-#pragma unroll
-    for (int i = 0; i < 6; i++) Gm[i] = 0.0;
-
-    while (cur.item >= 0) {
-        cp_async_wait<0>();      // values of `cur`, rows of `nxt` have landed
-        __syncwarp();
-        Unit nn = advance(nxt);
-        decode(nn);
-
-        const bool valid = cur.valid;
-        const int cbuf = cur.ib;
-        const double *sc = s_coord + cw * CS;
-        if (cur.comp == 0) {
-            // trilinear coefficients reduced at this lane's eta (see header comment)
-#pragma unroll
-            for (int a = 0; a < 3; a++) {
-                double X000 = sc[0 * 3 + a], X001 = sc[1 * 3 + a], X010 = sc[2 * 3 + a],
-                       X011 = sc[3 * 3 + a], X100 = sc[4 * 3 + a], X101 = sc[5 * 3 + a],
-                       X110 = sc[6 * 3 + a], X111 = sc[7 * 3 + a];
-                if (!valid) {   // keep idle lanes finite: unit cube
-                    X000 = 0; X001 = (a == 2); X010 = (a == 1); X011 = (a >= 1);
-                    X100 = (a == 0); X101 = (a != 1); X110 = (a != 2); X111 = 1;
-                }
-                double c1 = X100 - X000;
-                c2[a] = X010 - X000;
-                double c3 = X001 - X000;
-                c4[a] = X110 - X100 - X010 + X000;
-                c5[a] = X011 - X010 - X001 + X000;
-                double c6 = X101 - X100 - X001 + X000;
-                c7[a] = X111 - X110 - X101 - X011 + X100 + X010 + X001 - X000;
-                A1[a] = fma(c4[a], eta, c1);
-                A3[a] = fma(c5[a], eta, c3);
-                A6[a] = fma(c7[a], eta, c6);
-            }
-            if (AFFINE) {
-                // constant Jacobian: columns a = A1 (dx/dxi), b = c2 (dx/deta), c = A3 (dx/dzeta)
-                double r0[3], r1[3], r2[3];
-                r0[0] = c2[1] * A3[2] - c2[2] * A3[1];
-                r0[1] = c2[2] * A3[0] - c2[0] * A3[2];
-                r0[2] = c2[0] * A3[1] - c2[1] * A3[0];
-                r1[0] = A3[1] * A1[2] - A3[2] * A1[1];
-                r1[1] = A3[2] * A1[0] - A3[0] * A1[2];
-                r1[2] = A3[0] * A1[1] - A3[1] * A1[0];
-                r2[0] = A1[1] * c2[2] - A1[2] * c2[1];
-                r2[1] = A1[2] * c2[0] - A1[0] * c2[2];
-                r2[2] = A1[0] * c2[1] - A1[1] * c2[0];
-                const double det = A1[0] * r0[0] + A1[1] * r0[1] + A1[2] * r0[2];
-                adet_c = fabs(det);
-                const double rd = fast_rcp(adet_c);
-                Gm[0] = rd * (r0[0] * r0[0] + r0[1] * r0[1] + r0[2] * r0[2]);
-                Gm[1] = rd * (r0[0] * r1[0] + r0[1] * r1[1] + r0[2] * r1[2]);
-                Gm[2] = rd * (r0[0] * r2[0] + r0[1] * r2[1] + r0[2] * r2[2]);
-                Gm[3] = rd * (r1[0] * r1[0] + r1[1] * r1[1] + r1[2] * r1[2]);
-                Gm[4] = rd * (r1[0] * r2[0] + r1[1] * r2[1] + r1[2] * r2[2]);
-                Gm[5] = rd * (r2[0] * r2[0] + r2[1] * r2[1] + r2[2] * r2[2]);
-            }
-        }
-        if (STASH && cur.comp == 0) {
-            // c2, c4, c5, c7 (cell) and A1 (lane) are needed once per zeta plane only: park them in
-            // shared memory and free 30 registers for the quadrature loop
-            double *sg = s_stash + cw * WS::GS;
-            if (t == 0) {
-                double2 *d = reinterpret_cast<double2 *>(sg);
-                d[0] = make_double2(c2[0], c2[1]);
-                d[1] = make_double2(c2[2], c4[0]);
-                d[2] = make_double2(c4[1], c4[2]);
-                d[3] = make_double2(c5[0], c5[1]);
-                d[4] = make_double2(c5[2], c7[0]);
-                d[5] = make_double2(c7[1], c7[2]);
-            }
-            double2 *d = reinterpret_cast<double2 *>(sg + 12 + 4 * t);
-            d[0] = make_double2(A1[0], A1[1]);
-            sg[12 + 4 * t + 2] = A1[2];
-            __syncwarp();
-        }
-        const int comp = cur.comp;
-        const int *si = s_idx + (cbuf * CWS + cw) * US;
-        {
-            // ---- gathered values, layout Z (lane t == a_z)
-            const double *su = s_u + cw * US;
-            double u[N][N];
-#pragma unroll
-            for (int x = 0; x < N; x++)
-#pragma unroll
-                for (int yy = 0; yy < N; yy++) {
-                    if (MATRIX) u[x][yy] = ((x * N + yy) * N + t == comp) ? 1.0 : 0.0;
-                    else u[x][yy] = valid ? su[(x * N + yy) * N + t] : 0.0;
-                }
-            double tmp[N][N], U[N][N];
-            double Vp[N][N];
-            // ---- forward: interpolate to the quadrature points
-            apply_first<N, false>(P.B, u, tmp);          // a_x -> q_x
-            apply_second<N, false>(P.B, tmp, u);         // a_y -> q_y     u = w[qx][qy] @ a_z
-            __syncwarp();
-            tile.store_Z(u);
-            __syncwarp();
-            tile.load_Y(tmp);                            // tmp = w[qx][az] @ q_y
-            apply_second<N, false>(P.B, tmp, U);         // a_z -> q_z     U[qx][qz] @ q_y
-            __syncwarp();
-            tile.store_Y(U);
-            __syncwarp();
-            tile.load_Z(tmp);                            // U[qx][qy] @ q_z
-            apply_second<N, false>(P.Dt, tmp, u);        // d/d eta, still layout Z
-            __syncwarp();
-            tile.store_Z(u);
-            __syncwarp();
-            // d/d eta now sits in the tile in layout-Y order; each lane reads its
-            // own slot (qx, qz) inside the quadrature loop and overwrites it
-            // with the eta-flux, which the transpose path picks up from there
-
-            // ---- quadrature points (layout Y), fused with the x/z derivative
-            //      and its transpose so only U, Gy and Vp stay live
-#pragma unroll
-            for (int i = 0; i < N; i++)
-#pragma unroll
-                for (int j = 0; j < N; j++) Vp[i][j] = 0.0;
-            // single-buffered staging: the values / coordinates of `cur` were
-            // consumed (and a __syncwarp passed) before this point
-            stageB_coords(nxt);
-            // The zeta loop is ROLLED (the fully unrolled body did not fit the
-            // 32 KB instruction cache: ~15-20 % no-instruction stalls).  Register
-            // arrays cannot be indexed by a run-time qz, so U and Vp are kept
-            // rotated: column 0 is always the current zeta plane, and both are
-            // rotated by one column at the end of each trip (N trips = identity).
-            // DtR[qz][j] = Dt[qz][(j + qz) % N] is the matching rotation of the
-            // derivative row.
-#pragma unroll 1
-            for (int qz = 0; qz < N; qz++) {
-                stageB_part(nxt, ubuf ^ 1, qz);
-                const double zeta = P.xq[qz];
-                double dz[N];
-#pragma unroll
-                for (int j = 0; j < N; j++) dz[j] = P.DtR[qz * N + j];
-                double ca[3], pb[3], qb[3];
-                if (STASH) {
-                    const double *sg = s_stash + cw * WS::GS;
-                    const double2 *d = reinterpret_cast<const double2 *>(sg);
-                    const double2 g0 = d[0], g1 = d[1], g2 = d[2], g3 = d[3], g4 = d[4], g5 = d[5];
-                    const double2 a01 = *reinterpret_cast<const double2 *>(sg + 12 + 4 * t);
-                    const double a2 = sg[12 + 4 * t + 2];
-                    pb[0] = fma(g3.x, zeta, g0.x);     // c5 zeta + c2
-                    pb[1] = fma(g3.y, zeta, g0.y);
-                    pb[2] = fma(g4.x, zeta, g1.x);
-                    qb[0] = fma(g4.y, zeta, g1.y);     // c7 zeta + c4
-                    qb[1] = fma(g5.x, zeta, g2.x);
-                    qb[2] = fma(g5.y, zeta, g2.y);
-                    ca[0] = fma(A6[0], zeta, a01.x);   // dx/dxi
-                    ca[1] = fma(A6[1], zeta, a01.y);
-                    ca[2] = fma(A6[2], zeta, a2);
-                } else if (!AFFINE) {
-#pragma unroll
-                    for (int a = 0; a < 3; a++) {
-                        ca[a] = fma(A6[a], zeta, A1[a]);       // dx/dxi
-                        pb[a] = fma(c5[a], zeta, c2[a]);
-                        qb[a] = fma(c7[a], zeta, c4[a]);
-                    }
-                }
-                const double wyz_a = wy_alpha * P.wq[qz];
-                const double wyz_b = wy_beta * P.wq[qz];
-                double *trow = tile.row_Y(qz);
-#pragma unroll
-                for (int qx = 0; qx < N; qx++) {
-                    const double xi = P.xq[qx];
-                    double cb[3], cc[3];
-                    if (!AFFINE) {
-#pragma unroll
-                        for (int a = 0; a < 3; a++) {
-                            cb[a] = fma(qb[a], xi, pb[a]);     // dx/deta
-                            cc[a] = fma(A6[a], xi, A3[a]);     // dx/dzeta
-                        }
-                    }
-                    double gx = 0.0, gz = 0.0;
-#pragma unroll
-                    for (int q = 0; q < N; q++) {
-                        gx = fma(P.Dt[qx * N + q], U[q][0], gx);
-                        gz = fma(dz[q], U[qx][q], gz);
-                    }
-                    const double gy = trow[qx * N * N];
-                    if (AFFINE) {
-                        const double wq3 = wyz_a * P.wq[qx];
-                        const double fx = wq3 * (Gm[0] * gx + Gm[1] * gy + Gm[2] * gz);
-                        const double fy = wq3 * (Gm[1] * gx + Gm[3] * gy + Gm[4] * gz);
-                        const double fz = wq3 * (Gm[2] * gx + Gm[4] * gy + Gm[5] * gz);
-                        trow[qx * N * N] = fy;
-#pragma unroll
-                        for (int q = 0; q < N; q++) {
-                            Vp[q][0] = fma(P.Dt[qx * N + q], fx, Vp[q][0]);
-                            Vp[qx][q] = fma(dz[q], fz, Vp[qx][q]);
-                        }
-                        if (MASS) Vp[qx][0] = fma(wyz_b * P.wq[qx] * adet_c, U[qx][0], Vp[qx][0]);
-                        continue;
-                    }
-                    // cofactor rows: r0 = b x c, r1 = c x a, r2 = a x b
-                    double r0[3], r1[3], r2[3];
-                    r0[0] = cb[1] * cc[2] - cb[2] * cc[1];
-                    r0[1] = cb[2] * cc[0] - cb[0] * cc[2];
-                    r0[2] = cb[0] * cc[1] - cb[1] * cc[0];
-                    r1[0] = cc[1] * ca[2] - cc[2] * ca[1];
-                    r1[1] = cc[2] * ca[0] - cc[0] * ca[2];
-                    r1[2] = cc[0] * ca[1] - cc[1] * ca[0];
-                    r2[0] = ca[1] * cb[2] - ca[2] * cb[1];
-                    r2[1] = ca[2] * cb[0] - ca[0] * cb[2];
-                    r2[2] = ca[0] * cb[1] - ca[1] * cb[0];
-                    const double det = ca[0] * r0[0] + ca[1] * r0[1] + ca[2] * r0[2];
-                    const double adet = fabs(det);
-                    const double s = wyz_a * P.wq[qx] * fast_rcp(adet);
-                    double h[3];
-#pragma unroll
-                    for (int a = 0; a < 3; a++) h[a] = r0[a] * gx + r1[a] * gy + r2[a] * gz;
-                    const double fx = s * (r0[0] * h[0] + r0[1] * h[1] + r0[2] * h[2]);
-                    const double fy = s * (r1[0] * h[0] + r1[1] * h[1] + r1[2] * h[2]);
-                    const double fz = s * (r2[0] * h[0] + r2[1] * h[1] + r2[2] * h[2]);
-                    trow[qx * N * N] = fy;
-#pragma unroll
-                    for (int q = 0; q < N; q++) {
-                        Vp[q][0] = fma(P.Dt[qx * N + q], fx, Vp[q][0]);
-                        Vp[qx][q] = fma(dz[q], fz, Vp[qx][q]);
-                    }
-                    if (MASS) Vp[qx][0] = fma(wyz_b * P.wq[qx] * adet, U[qx][0], Vp[qx][0]);
-                }
-                // rotate: column j <- column j+1
-#pragma unroll
-                for (int x = 0; x < N; x++) {
-                    const double u0 = U[x][0], v0 = Vp[x][0];
-#pragma unroll
-                    for (int j = 0; j < N - 1; j++) {
-                        U[x][j] = U[x][j + 1];
-                        Vp[x][j] = Vp[x][j + 1];
-                    }
-                    U[x][N - 1] = u0;
-                    Vp[x][N - 1] = v0;
-                }
-            }
-
-            __syncwarp();            // all lanes are done reading the staged rows of `nxt`
-            stageA(nn);
-            cp_async_commit();
-
-            // ---- backward (the tile holds Fy[qx][qz] @ q_y)
-            __syncwarp();
-            tile.load_Z(tmp);                            // Fy[qx][qy] @ q_z
-            apply_second<N, true>(P.Dt, tmp, u);         // Dt^T along eta
-            __syncwarp();
-            tile.store_Z(u);
-            __syncwarp();
-            tile.load_Y(tmp);
-#pragma unroll
-            for (int i = 0; i < N; i++)
-#pragma unroll
-                for (int j = 0; j < N; j++) Vp[i][j] += tmp[i][j];
-            apply_second<N, true>(P.B, Vp, tmp);         // q_z -> a_z     W[qx][az] @ q_y
-            __syncwarp();
-            tile.store_Y(tmp);
-            __syncwarp();
-            tile.load_Z(u);                              // W[qx][qy] @ a_z
-            apply_first<N, true>(P.B, u, tmp);           // q_x -> a_x
-            apply_second<N, true>(P.B, tmp, u);          // q_y -> a_y     R[ax][ay] @ a_z
-
-            // ---- scatter-add, layout Z
-            if (MATRIX && P.vals == nullptr) {
-                // diagonal of the bilinear form: only the entry i == j of column j
-                if (valid) {
-#pragma unroll
-                    for (int x = 0; x < N; x++)
-#pragma unroll
-                        for (int yy = 0; yy < N; yy++)
-                            if ((x * N + yy) * N + t == comp) atomicAdd(P.y + si[comp], u[x][yy]);
-                }
-            } else if (MATRIX) {
-                // MatSetValuesLocal(ADD_VALUES): column = trial dof `comp`, rows = this
-                // lane's test dofs; negative (BC-masked) indices are dropped
-                int gcol = valid ? si[comp] : -1;
-                if (gcol >= 0 && P.col_lg) gcol = __ldg(P.col_lg + gcol);
-                const unsigned short *rk = nullptr;
-                if (P.rank_tab && valid) {
-                    const int lay = cur.layer;
-                    const int v = P.nlay_total < 3 ? lay : (lay == 0 ? 0 : (lay == P.nlay_total - 1 ? 2 : 1));
-                    rk = P.rank_tab + (((long long)cur.col * P.nvar + v) * ND + comp) * ND;
-                }
-                if (gcol >= 0) {
-#pragma unroll
-                    for (int x = 0; x < N; x++)
-#pragma unroll
-                        for (int yy = 0; yy < N; yy++) {
-                            int grow = si[(x * N + yy) * N + t];
-                            if (P.row_lg) grow = __ldg(P.row_lg + grow);
-                            if (grow < 0) continue;
-                            long long lo = __ldg(P.rowptr + grow);
-                            if (rk) {
-                                lo += __ldg(rk + (x * N + yy) * N + t);
-                            } else {
-                                long long hi = __ldg(P.rowptr + grow + 1);
-                                while (hi - lo > 1) {
-                                    long long mid = (lo + hi) >> 1;
-                                    if (__ldg(P.colidx + mid) <= gcol) lo = mid; else hi = mid;
-                                }
-                            }
-                            if (ATOMIC) atomicAdd(P.vals + lo, u[x][yy]);
-                            else P.vals[lo] += u[x][yy];
-                        }
-                }
-            } else if (valid) {
-                const int *smc = row_of(cur);
-#pragma unroll
-                for (int x = 0; x < N; x++)
-#pragma unroll
-                    for (int yy = 0; yy < N; yy++) {
-                        const int loc = (x * N + yy) * N + t;
-                        const int g = SLIM ? smc[loc] + s_off0[loc] * cur.layer : si[loc];
-                        double *dst = P.y + (long long)g * P.cdim + comp;
-                        if (ATOMIC) atomicAdd(dst, u[x][yy]);
-                        else *dst += u[x][yy];
-                    }
-            }
-        }
-        cur = nxt;
-        nxt = nn;
-        ubuf ^= 1;
-    }
-    cp_async_wait<0>();
+// FDB_FORM_HELMHOLTZ_COEF (action, element matrix, diagonal): the same body with COEF set
+template <int N, bool MASS, bool ATOMIC, int MINB, bool MATRIX = false, bool SLIM = false>
+__global__ void __launch_bounds__(WPC<N, SLIM, true>::value * 32, MINB)
+helmholtz_coef_kernel(const __grid_constant__ HelmCoefParams<N> P)
+{
+    constexpr bool COEF = true, AFFINE = false;
+    const double *kappa = P.kappa;
+#include "action_hex_body.cuh"
 }
 
 #include "action_hex_ws.cuh"
 
-template <int N, bool MASS, bool ATOMIC, int MINB, bool MATRIX = false, bool SLIM = false, bool AFFINE = false>
-int launch_one(int grid_cap_per_sm, cudaStream_t st, HelmParams<N> &P, int sm_count)
+template <int N, bool MASS, bool ATOMIC, int MINB, bool MATRIX = false, bool SLIM = false, bool AFFINE = false,
+          bool COEF = false>
+int launch_one(int grid_cap_per_sm, cudaStream_t st, HelmCoefParams<N> &P, int sm_count)
 {
-    using WS = WarpSmem<N, SLIM>;
-    constexpr int WARPS_PER_CTA = WPC<N, SLIM>::value;
+    using WS = WarpSmem<N, SLIM, COEF>;
+    constexpr int WARPS_PER_CTA = WPC<N, SLIM, COEF>::value;
     constexpr int T = WARPS_PER_CTA * 32;
-    auto kern = helmholtz_action_kernel<N, MASS, ATOMIC, MINB, MATRIX, SLIM, AFFINE>;
+    auto kern = [] {
+        if constexpr (COEF) return helmholtz_coef_kernel<N, MASS, ATOMIC, MINB, MATRIX, SLIM>;
+        else return helmholtz_action_kernel<N, MASS, ATOMIC, MINB, MATRIX, SLIM, AFFINE>;
+    }();
     static bool configured = false;
     static int occ = 1;
     if (!configured) {
@@ -819,13 +361,35 @@ int launch_one(int grid_cap_per_sm, cudaStream_t st, HelmParams<N> &P, int sm_co
     P.nlay_rcp = (unsigned)(0x100000000ull / (unsigned long long)P.nlay_items);
     if (P.nlay_items == 1) P.nlay_rcp = 0xffffffffu;
     FDB_CUDA(cudaMemsetAsync(P.counter, 0, sizeof(int), st));
-    kern<<<(int)grid, T, WS::CTA_BYTES, st>>>(P);
+    if constexpr (COEF) kern<<<(int)grid, T, WS::CTA_BYTES, st>>>(P);
+    else kern<<<(int)grid, T, WS::CTA_BYTES, st>>>(static_cast<const HelmParams<N> &>(P));
     FDB_LAUNCH_CHECK();
     return 0;
 }
 
+// register bound of the coefficient kernel (-Xptxas -v, DESIGN.md section 4.5): shared memory holds
+// two CTAs of 4 warps at degree 3 either way, so it gets the whole 255 registers there
+template <int N>
+struct CoefMinB {
+    static constexpr int value = (N >= 5) ? 1 : 2;
+};
+
+// coefficient form (action): the slab-thread kernel for every degree -- no thread-per-cell,
+// warp-specialised or affine variant
 template <int N, bool ATOMIC>
-int launch_variant(bool mass, int minb, int cap, cudaStream_t st, HelmParams<N> &P, int sm_count,
+int launch_coef(bool mass, int cap, cudaStream_t st, HelmCoefParams<N> &P, int sm_count)
+{
+    constexpr int MB = CoefMinB<N>::value;
+    if (N == 6 && P.nlay_items >= 32 / N) {
+        if (mass) return launch_one<N, true, ATOMIC, MB, false, (N == 6), false, true>(cap, st, P, sm_count);
+        return launch_one<N, false, ATOMIC, MB, false, (N == 6), false, true>(cap, st, P, sm_count);
+    }
+    if (mass) return launch_one<N, true, ATOMIC, MB, false, false, false, true>(cap, st, P, sm_count);
+    return launch_one<N, false, ATOMIC, MB, false, false, false, true>(cap, st, P, sm_count);
+}
+
+template <int N, bool ATOMIC>
+int launch_variant(bool mass, int minb, int cap, cudaStream_t st, HelmCoefParams<N> &P, int sm_count,
                    bool affine = false)
 {
     if (affine && ATOMIC) {
@@ -866,10 +430,11 @@ int launch_variant(bool mass, int minb, int cap, cudaStream_t st, HelmParams<N> 
 template <int N>
 int launch_n(fdb_kernel_s *k, fdb_int start, fdb_int end, int nlay, const fdb_int *subset,
              double *y, const double *coords, const double *x, const fdb_int *map0,
-             const fdb_int *map1)
+             const fdb_int *map1, const double *kappa)
 {
     fdb::Context &c = fdb::ctx();
-    HelmParams<N> P;
+    HelmCoefParams<N> P;
+    P.kappa = kappa;             // NULL: constant-coefficient form
     P.y = y;
     P.x = x;
     P.coords = coords;
@@ -907,6 +472,7 @@ int launch_n(fdb_kernel_s *k, fdb_int start, fdb_int end, int nlay, const fdb_in
         P.lay_first = 0;
         P.lay_step = 1;
         if (P.ncols <= 0 || nlay <= 0) return 0;
+        if (kappa) return launch_coef<N, true>(mass, cap, c.stream, P, c.sm_count);
         if constexpr (N == 4) {
             // degree 3, scalar: warp-specialised kernel (action_hex_ws.cuh)
             static const int ws = getenv("FDB_WS") ? atoi(getenv("FDB_WS")) : 0;
@@ -941,7 +507,9 @@ int launch_n(fdb_kernel_s *k, fdb_int start, fdb_int end, int nlay, const fdb_in
             P.lay_step = 2;
             P.nlay_items = (nlay - par + 1) / 2;
             if (P.ncols <= 0 || P.nlay_items <= 0) continue;
-            if (launch_variant<N, false>(mass, minb, cap, c.stream, P, c.sm_count)) return 1;
+            if (kappa ? launch_coef<N, false>(mass, cap, c.stream, P, c.sm_count)
+                      : launch_variant<N, false>(mass, minb, cap, c.stream, P, c.sm_count))
+                return 1;
         }
     }
     return 0;
@@ -950,11 +518,12 @@ int launch_n(fdb_kernel_s *k, fdb_int start, fdb_int end, int nlay, const fdb_in
 template <int N>
 int launch_matrix_n(fdb_kernel_s *k, fdb_int start, fdb_int end, int nlay, const fdb_int *subset,
                     fdb_mat_t mat, const double *coords, const fdb_int *map0, const fdb_int *map1,
-                    double *diag_out)
+                    double *diag_out, const double *kappa)
 {
     fdb::Context &c = fdb::ctx();
-    HelmParams<N> P;
+    HelmCoefParams<N> P;
     memset(&P, 0, sizeof(P));
+    P.kappa = kappa;             // NULL: constant-coefficient form
     P.coords = coords;
     P.map0 = map0;
     P.map1 = map1;
@@ -994,6 +563,12 @@ int launch_matrix_n(fdb_kernel_s *k, fdb_int start, fdb_int end, int nlay, const
     P.lay_first = 0;
     P.lay_step = 1;
     if (P.ncols <= 0 || nlay <= 0) return 0;
+    if (kappa) {
+        constexpr int MB = CoefMinB<N>::value;
+        if (k->desc.beta != 0.0)
+            return launch_one<N, true, true, MB, true, false, false, true>(0, c.stream, P, c.sm_count);
+        return launch_one<N, false, true, MB, true, false, false, true>(0, c.stream, P, c.sm_count);
+    }
     constexpr int DEF = (N >= 5) ? 1 : 2;
     if (k->desc.beta != 0.0) return launch_one<N, true, true, DEF, true>(0, c.stream, P, c.sm_count);
     return launch_one<N, false, true, DEF, true>(0, c.stream, P, c.sm_count);
@@ -1014,10 +589,10 @@ int fdb_launch_helmholtz_matrix(fdb_kernel_s *k, fdb_int start, fdb_int end, int
     if (mat && dmma != 0 && k->n1d <= 5 && k->n1d >= (dmma == 1 ? 3 : 4))
         return fdb_launch_helmholtz_matrix_dmma(k, start, end, nlay, subset, mat, coords, map0, map1);
     switch (k->n1d) {
-    case 2: return launch_matrix_n<2>(k, start, end, nlay, subset, mat, coords, map0, map1, diag_out);
-    case 3: return launch_matrix_n<3>(k, start, end, nlay, subset, mat, coords, map0, map1, diag_out);
-    case 4: return launch_matrix_n<4>(k, start, end, nlay, subset, mat, coords, map0, map1, diag_out);
-    case 5: return launch_matrix_n<5>(k, start, end, nlay, subset, mat, coords, map0, map1, diag_out);
+    case 2: return launch_matrix_n<2>(k, start, end, nlay, subset, mat, coords, map0, map1, diag_out, nullptr);
+    case 3: return launch_matrix_n<3>(k, start, end, nlay, subset, mat, coords, map0, map1, diag_out, nullptr);
+    case 4: return launch_matrix_n<4>(k, start, end, nlay, subset, mat, coords, map0, map1, diag_out, nullptr);
+    case 5: return launch_matrix_n<5>(k, start, end, nlay, subset, mat, coords, map0, map1, diag_out, nullptr);
     }
     fdb::set_error("helmholtz matrix: degree %d not instantiated (1..4)", k->n1d - 1);
     return 1;
@@ -1038,12 +613,45 @@ int fdb_launch_helmholtz_action(fdb_kernel_s *k, fdb_int start, fdb_int end, int
         k->desc.cell == FDB_CELL_HEX_EXTRUDED && nlay >= 16)
         return fdb_launch_q2_action(k, start, end, nlay, subset, y, coords, x, map0, map1);
     switch (k->n1d) {
-    case 2: return launch_n<2>(k, start, end, nlay, subset, y, coords, x, map0, map1);
-    case 3: return launch_n<3>(k, start, end, nlay, subset, y, coords, x, map0, map1);
-    case 4: return launch_n<4>(k, start, end, nlay, subset, y, coords, x, map0, map1);
-    case 5: return launch_n<5>(k, start, end, nlay, subset, y, coords, x, map0, map1);
-    case 6: return launch_n<6>(k, start, end, nlay, subset, y, coords, x, map0, map1);
+    case 2: return launch_n<2>(k, start, end, nlay, subset, y, coords, x, map0, map1, nullptr);
+    case 3: return launch_n<3>(k, start, end, nlay, subset, y, coords, x, map0, map1, nullptr);
+    case 4: return launch_n<4>(k, start, end, nlay, subset, y, coords, x, map0, map1, nullptr);
+    case 5: return launch_n<5>(k, start, end, nlay, subset, y, coords, x, map0, map1, nullptr);
+    case 6: return launch_n<6>(k, start, end, nlay, subset, y, coords, x, map0, map1, nullptr);
     }
     fdb::set_error("helmholtz action: degree %d not instantiated (1..5)", k->n1d - 1);
+    return 1;
+}
+
+// FDB_FORM_HELMHOLTZ_COEF: the slab-thread kernel for every degree (1..5 action, 1..4 matrix and
+// diagonal); never the thread-per-cell, warp-specialised, affine or DMMA kernels
+int fdb_launch_helmholtz_coef_action(fdb_kernel_s *k, fdb_int start, fdb_int end, int nlay,
+                                     const fdb_int *subset, double *y, const double *coords,
+                                     const double *x, const double *kappa, const fdb_int *map0,
+                                     const fdb_int *map1)
+{
+    switch (k->n1d) {
+    case 2: return launch_n<2>(k, start, end, nlay, subset, y, coords, x, map0, map1, kappa);
+    case 3: return launch_n<3>(k, start, end, nlay, subset, y, coords, x, map0, map1, kappa);
+    case 4: return launch_n<4>(k, start, end, nlay, subset, y, coords, x, map0, map1, kappa);
+    case 5: return launch_n<5>(k, start, end, nlay, subset, y, coords, x, map0, map1, kappa);
+    case 6: return launch_n<6>(k, start, end, nlay, subset, y, coords, x, map0, map1, kappa);
+    }
+    fdb::set_error("helmholtz_coef action: degree %d not instantiated (1..5)", k->n1d - 1);
+    return 1;
+}
+
+int fdb_launch_helmholtz_coef_matrix(fdb_kernel_s *k, fdb_int start, fdb_int end, int nlay,
+                                     const fdb_int *subset, fdb_mat_t mat, const double *coords,
+                                     const double *kappa, const fdb_int *map0, const fdb_int *map1,
+                                     double *diag_out)
+{
+    switch (k->n1d) {
+    case 2: return launch_matrix_n<2>(k, start, end, nlay, subset, mat, coords, map0, map1, diag_out, kappa);
+    case 3: return launch_matrix_n<3>(k, start, end, nlay, subset, mat, coords, map0, map1, diag_out, kappa);
+    case 4: return launch_matrix_n<4>(k, start, end, nlay, subset, mat, coords, map0, map1, diag_out, kappa);
+    case 5: return launch_matrix_n<5>(k, start, end, nlay, subset, mat, coords, map0, map1, diag_out, kappa);
+    }
+    fdb::set_error("helmholtz_coef matrix: degree %d not instantiated (1..4)", k->n1d - 1);
     return 1;
 }

@@ -119,3 +119,12 @@ int fdb_launch_q2_action(fdb_kernel_s *k, fdb_int start, fdb_int end, int nlay, 
 int fdb_launch_helmholtz_action(fdb_kernel_s *k, fdb_int start, fdb_int end, int nlay,
                                 const fdb_int *subset, double *y, const double *coords,
                                 const double *x, const fdb_int *map0, const fdb_int *map1);
+// FDB_FORM_HELMHOLTZ_COEF (action_hex.cu): kappa is a device pointer gathered through map0
+int fdb_launch_helmholtz_coef_action(fdb_kernel_s *k, fdb_int start, fdb_int end, int nlay,
+                                     const fdb_int *subset, double *y, const double *coords,
+                                     const double *x, const double *kappa, const fdb_int *map0,
+                                     const fdb_int *map1);
+int fdb_launch_helmholtz_coef_matrix(fdb_kernel_s *k, fdb_int start, fdb_int end, int nlay,
+                                     const fdb_int *subset, fdb_mat_t mat, const double *coords,
+                                     const double *kappa, const fdb_int *map0, const fdb_int *map1,
+                                     double *diag_out);

@@ -273,7 +273,27 @@ int fdb_kernel_create(const fdb_kernel_desc *d, fdb_kernel_t *out)
         *out = k;
         return 0;
     }
-    if (d->form != FDB_FORM_HELMHOLTZ) {
+    if (d->form == FDB_FORM_HELMHOLTZ_COEF) {
+        // kappa in the scalar argument space: the slab-thread kernel with its coefficient stage
+        if (d->cell != FDB_CELL_HEX_EXTRUDED && d->cell != FDB_CELL_HEX) {
+            set_error("fdb_kernel_create: helmholtz_coef needs hex cells (extruded or native), got cell %d", d->cell);
+            return 1;
+        }
+        if (d->cdim != 1) {
+            set_error("fdb_kernel_create: helmholtz_coef takes scalar spaces only (cdim %d)", d->cdim);
+            return 1;
+        }
+        if (d->affine_cells) {
+            set_error("fdb_kernel_create: helmholtz_coef has no affine-cell variant (affine_cells must be 0)");
+            return 1;
+        }
+        const int maxdeg = d->rank == 2 ? 4 : (d->diagonal ? 3 : 5);
+        if (d->degree < 1 || d->degree > maxdeg) {
+            set_error("fdb_kernel_create: helmholtz_coef %s: degree %d outside 1..%d",
+                      d->rank == 2 ? "matrix" : (d->diagonal ? "diagonal" : "action"), d->degree, maxdeg);
+            return 1;
+        }
+    } else if (d->form != FDB_FORM_HELMHOLTZ) {
         set_error("fdb_kernel_create: form %d is not in the supported set", d->form);
         return 1;
     }
@@ -410,6 +430,56 @@ int fdb_kernel_call(fdb_kernel_t k, const fdb_call_args *a)
         set_error("fdb_kernel_call: iteration set too large for IntType");
         return 1;
     }
+    const bool coef = k->desc.form == FDB_FORM_HELMHOLTZ_COEF;
+    if (coef && k->desc.rank == 2) {
+        // args = [Mat handle (INC), coords (READ), kappa (READ)], maps = [V map, coord map]
+        if (a->nargs != 3 || a->nmaps != 2) {
+            set_error("fdb_kernel_call: helmholtz_coef 2-form expects 3 args (mat, coords, kappa) and 2 maps");
+            return 1;
+        }
+        fdb_mat_t target = (fdb_mat_t)a->args[0];
+        int mat_bs = 1;
+        fdb_mat_block_size(target, &mat_bs);
+        if (mat_bs != 1) {
+            set_error("fdb_kernel_call: helmholtz_coef assembles scalar matrices only (block size %d)", mat_bs);
+            return 1;
+        }
+        if (k->desc.scatter != FDB_SCATTER_ATOMIC) {
+            set_error("fdb_kernel_call: coloured scatter is not implemented for matrices");
+            return 1;
+        }
+        const void *din[2];
+        const fdb_int *dm[2];
+        const fdb_int *dsub = a->subset;
+        if (a->location == FDB_LOC_HOST) {
+            if (!a->arg_bytes || !a->map_bytes) {
+                set_error("fdb_kernel_call: host mode needs arg_bytes and map_bytes");
+                return 1;
+            }
+            void *p;
+            for (int i = 0; i < 2; i++) {
+                uint64_t ver = a->arg_versions ? a->arg_versions[i + 1] : 0;
+                if (!a->arg_versions) fdb_mirror_drop(a->args[i + 1]);
+                if (fdb_mirror_acquire(a->args[i + 1], a->arg_bytes[i + 1], ver, 1, &p)) return 1;
+                din[i] = p;
+            }
+            for (int i = 0; i < 2; i++) {
+                if (fdb_mirror_acquire(a->maps[i], a->map_bytes[i], map_ver(a, i), 1, &p)) return 1;
+                dm[i] = (const fdb_int *)p;
+            }
+            if (a->subset) {
+                if (fdb_mirror_acquire(a->subset, sizeof(fdb_int) * (size_t)a->end, a->subset_version, 1, &p)) return 1;
+                dsub = (const fdb_int *)p;
+            }
+        } else {
+            din[0] = a->args[1];
+            din[1] = a->args[2];
+            dm[0] = a->maps[0];
+            dm[1] = a->maps[1];
+        }
+        return fdb_launch_helmholtz_coef_matrix(k, a->start, a->end, nlay, dsub, target, (const double *)din[0],
+                                                (const double *)din[1], dm[0], dm[1], nullptr);
+    }
     if (k->desc.rank == 2) {
         // 2-form: args = [Mat handle (INC), coords (READ)], maps = [V map, coord map]
         // (the reference passes the PETSc Mat handle in the same slot:
@@ -464,6 +534,16 @@ int fdb_kernel_call(fdb_kernel_t k, const fdb_call_args *a)
         int rc2 = fdb_mat_scalar_view_end(target, view);
         return rc ? rc : rc2;
     }
+    if (coef && k->desc.diagonal) {
+        // args = [d (INC), coords, kappa]; device-resident only
+        if (a->nargs != 3 || a->nmaps != 2 || a->location != FDB_LOC_DEVICE) {
+            set_error("fdb_kernel_call: helmholtz_coef diagonal expects 3 device args (d, coords, kappa) and 2 maps");
+            return 1;
+        }
+        return fdb_launch_helmholtz_coef_matrix(k, a->start, a->end, nlay, a->subset, nullptr,
+                                                (const double *)a->args[1], (const double *)a->args[2],
+                                                a->maps[0], a->maps[1], (double *)a->args[0]);
+    }
     if (k->desc.diagonal) {
         // args = [d (INC), coords]; device-resident only
         if (a->nargs != 2 || a->nmaps != 2 || a->location != FDB_LOC_DEVICE || k->desc.cdim != 1 ||
@@ -476,18 +556,26 @@ int fdb_kernel_call(fdb_kernel_t k, const fdb_call_args *a)
                                            (double *)a->args[0]);
     }
     // 1-form: args = [y (INC), coords (READ), x (READ)], maps = [V map, coord map]
-    if (a->nargs != 3 || a->nmaps != 2) {
+    // (helmholtz_coef: [y, coords, x, kappa (READ)])
+    if (coef && (a->nargs != 4 || a->nmaps != 2)) {
+        set_error("fdb_kernel_call: helmholtz_coef 1-form expects 4 args (y, coords, x, kappa) and 2 maps, got %d/%d",
+                  a->nargs, a->nmaps);
+        return 1;
+    }
+    if (!coef && (a->nargs != 3 || a->nmaps != 2)) {
         set_error("fdb_kernel_call: 1-form expects 3 args (y, coords, x) and 2 maps, got %d/%d",
                   a->nargs, a->nmaps);
         return 1;
     }
-    if (a->location == FDB_LOC_HOST && a->arg_versions && a->arg_bytes && a->map_bytes &&
+    // the pipelined host action moves x and y only: the coefficient form takes the monolithic path
+    if (!coef && a->location == FDB_LOC_HOST && a->arg_versions && a->arg_bytes && a->map_bytes &&
         a->writeback && a->output_is_zero && !a->subset && extruded &&
         k->desc.scatter == FDB_SCATTER_ATOMIC) {
         int rc = pipelined_host_action(k, a, nlay);
         if (rc >= 0) return rc;      // -1: not applicable, fall through to the monolithic path
     }
-    void *dargs[3];
+    const int nin = a->nargs;
+    void *dargs[4];
     const fdb_int *dmaps[2];
     const fdb_int *dsubset = a->subset;
     if (a->location == FDB_LOC_HOST) {
@@ -495,7 +583,7 @@ int fdb_kernel_call(fdb_kernel_t k, const fdb_call_args *a)
             set_error("fdb_kernel_call: host mode needs arg_bytes and map_bytes");
             return 1;
         }
-        for (int i = 0; i < 3; i++) {
+        for (int i = 0; i < nin; i++) {
             uint64_t ver = a->arg_versions ? a->arg_versions[i] : 0;
             // without versions every call re-uploads (drop-in default: the
             // reference hands over live NumPy buffers)
@@ -517,7 +605,7 @@ int fdb_kernel_call(fdb_kernel_t k, const fdb_call_args *a)
             dsubset = (const fdb_int *)p;
         }
     } else {
-        for (int i = 0; i < 3; i++) dargs[i] = a->args[i];
+        for (int i = 0; i < nin; i++) dargs[i] = a->args[i];
         for (int i = 0; i < 2; i++) dmaps[i] = a->maps[i];
     }
     if (k->desc.scatter == FDB_SCATTER_COLOURED &&
@@ -541,9 +629,12 @@ int fdb_kernel_call(fdb_kernel_t k, const fdb_call_args *a)
         set_error("fdb_kernel_call: coloured scatter needs start == 0");
         return 1;
     }
-    int rc = fdb_launch_helmholtz_action(k, a->start, a->end, nlay, dsubset, (double *)dargs[0],
-                                         (const double *)dargs[1], (const double *)dargs[2],
-                                         dmaps[0], dmaps[1]);
+    int rc = coef ? fdb_launch_helmholtz_coef_action(k, a->start, a->end, nlay, dsubset, (double *)dargs[0],
+                                                     (const double *)dargs[1], (const double *)dargs[2],
+                                                     (const double *)dargs[3], dmaps[0], dmaps[1])
+                  : fdb_launch_helmholtz_action(k, a->start, a->end, nlay, dsubset, (double *)dargs[0],
+                                                (const double *)dargs[1], (const double *)dargs[2],
+                                                dmaps[0], dmaps[1]);
     if (rc) return rc;
     if (a->location == FDB_LOC_HOST && a->writeback) {
         // the output mirror now differs from the host copy: write it back

@@ -25,6 +25,7 @@
 #include <stdlib.h>
 
 #include <algorithm>
+#include <mutex>
 #include <sstream>
 #include <string>
 #include <vector>
@@ -1043,10 +1044,27 @@ int fdb_wrapper_compile(const fdb_wrapper_desc *d, void *cubin, size_t cap, size
     Plan pl;
     if (validate(d, pl)) return 1;
     const std::string s = generate(d, pl);
-    std::vector<char> img;
-    if (compile_cubin(s, pl.name, img)) return 1;
-    if (needed) *needed = img.size();
-    if (cubin && cap >= img.size()) memcpy(cubin, img.data(), img.size());
+    // NVRTC's cubin for the same source differs in size from one compilation to the next, so the
+    // size query and the copy of the two-call protocol (cubin = NULL, then a buffer of *needed
+    // bytes) must see the same image: the last image is kept, keyed by its generated source
+    static std::mutex mu;
+    static std::string last_src;
+    static std::vector<char> last_img;
+    std::lock_guard<std::mutex> lock(mu);
+    if (s != last_src || last_img.empty()) {
+        std::vector<char> img;
+        if (compile_cubin(s, pl.name, img)) return 1;
+        last_src = s;
+        last_img.swap(img);
+    }
+    if (needed) *needed = last_img.size();
+    if (cubin) {
+        if (cap < last_img.size()) {
+            set_error("fdb_wrapper_compile: buffer of %zu bytes, the image needs %zu", cap, last_img.size());
+            return 1;
+        }
+        memcpy(cubin, last_img.data(), last_img.size());
+    }
     return 0;
 }
 

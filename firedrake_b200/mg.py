@@ -293,8 +293,11 @@ class VCycle:
     coarsest level solved by CG.  Everything stays on the device."""
 
     def __init__(self, hierarchy, degree, make_form, bc_domains=(), nu=2, omega=0.8,
-                 coarse_rtol=1e-2, coarse_maxit=200, allreduce=None):
-        """``allreduce``: callable summing a float over the ranks (partitioned hierarchies)."""
+                 coarse_rtol=1e-2, coarse_maxit=200, allreduce=None, kappa=None):
+        """``allreduce``: callable summing a float over the ranks (partitioned hierarchies).
+        ``kappa``: coefficient field on the finest level (a scalar Dat laid out like this V-cycle's
+        finest space); it is copied there, each coarser level gets the injection of the next finer
+        level's field, and the operators are ``make_form(V, kappa_l)``."""
         from .assemble import DirichletBC, FunctionSpace, assemble
         self.allreduce = allreduce
         if hierarchy.partitions is None:
@@ -303,8 +306,13 @@ class VCycle:
             parts = [hierarchy.partition(l, degree) for l in range(len(hierarchy))]
             self.spaces = [FunctionSpace(pt.mesh, degree, partition=pt) for pt in parts]
         self.bcs = [[DirichletBC(V, 0.0, s) for s in bc_domains] for V in self.spaces]
-        self.ops = [assemble(make_form(V), bcs=b, mat_type="matfree") for V, b in zip(self.spaces, self.bcs)]
         self.transfers = [TransferManager(self.spaces[l], self.spaces[l + 1]) for l in range(len(self.spaces) - 1)]
+        if kappa is None:
+            forms = [make_form(V) for V in self.spaces]
+        else:
+            self.kappas = self._coarsen_coefficient(kappa)
+            forms = [make_form(V, k) for V, k in zip(self.spaces, self.kappas)]
+        self.ops = [assemble(f, bcs=b, mat_type="matfree") for f, b in zip(forms, self.bcs)]
         self.nu, self.omega = nu, omega
         self.coarse_rtol, self.coarse_maxit = coarse_rtol, coarse_maxit
         self.invdiag = []
@@ -317,6 +325,21 @@ class VCycle:
         # b (restricted residual = its right-hand side) and x (its solution) -- x and e must be
         # distinct Dats: level l-1's solution is the input of the prolongation into level l's e
         self._work = [dict(r=V.dat(), e=V.dat(), t=V.dat(), b=V.dat(), x=V.dat()) for V in self.spaces]
+
+    def _coarsen_coefficient(self, kappa):
+        """kappa on every level, finest last: the finest is a device copy of ``kappa`` on this
+        V-cycle's own space, each coarser one the injection of the next finer."""
+        from . import _lib
+        top = self.spaces[-1]
+        fine = top.dat()
+        if kappa.nbytes != fine.nbytes:
+            raise ValueError("kappa does not match the finest level of the hierarchy")
+        _lib.check(_lib.lib().fdb_memcpy_d2d(fine.device_ptr, kappa.device_ptr, kappa.nbytes))
+        _touched(fine)
+        out = [fine]
+        for l in range(len(self.spaces) - 2, -1, -1):
+            out.insert(0, self.transfers[l].inject(out[0], self.spaces[l].dat()))
+        return out
 
     def _smooth(self, l, b, x):
         """x += omega D^-1 (b - A x), nu times."""

@@ -1356,7 +1356,10 @@ class Kernel:
     ``form``: "helmholtz" family = ``alpha*inner(grad u, grad v)*dx +
     beta*inner(u, v)*dx``.  ``rank`` 1 means the 1-form ``action(a, w)``
     (arguments: output Dat INC, coordinates READ, coefficient READ), the kernel
-    TSFC names ``form0_cell_integral``.
+    TSFC names ``form0_cell_integral``.  "helmholtz_coef" = ``alpha*inner(kappa*grad u, grad v)*dx
+    + beta*inner(u, v)*dx`` with a scalar coefficient field kappa in the argument space, passed as
+    the LAST argument (READ, through the argument map): action (INC, READ, READ, READ), diagonal and
+    rank 2 (INC, READ, READ).
     """
     form: str = "helmholtz"
     degree: int = 1
@@ -1384,6 +1387,12 @@ class Kernel:
         return super().__new__(cls)
 
     def __post_init__(self):
+        if self.form == "helmholtz_coef":
+            acc = (INC, READ, READ) if (self.diagonal or self.rank == 2) else (INC, READ, READ, READ)
+            object.__setattr__(self, "accesses", acc)
+            if self.rank == 2 and self.name == "form0_cell_integral":
+                object.__setattr__(self, "name", "form00_cell_integral")
+            return
         if self.form == "dg_advection":
             # args: out, coordinates, q, u, constants (dtc, q_in) [, local facet numbers]
             extra = {"cell": 0, "exterior_facet": 1, "interior_facet": 1, "fused": 2}[self.integral]
@@ -1403,7 +1412,8 @@ class Kernel:
         return 2 * 6 * n ** 4 * 2 + 130 * n ** 3
 
 
-_FORMS = {"helmholtz": _lib.FORM_HELMHOLTZ, "dg_advection": _lib.FORM_DG_ADVECTION}
+_FORMS = {"helmholtz": _lib.FORM_HELMHOLTZ, "dg_advection": _lib.FORM_DG_ADVECTION,
+          "helmholtz_coef": _lib.FORM_HELMHOLTZ_COEF}
 _INTEGRALS = {"cell": _lib.INTEGRAL_CELL, "exterior_facet": _lib.INTEGRAL_EXTERIOR_FACET,
               "interior_facet": _lib.INTEGRAL_INTERIOR_FACET, "fused": _lib.INTEGRAL_FUSED}
 
@@ -1643,9 +1653,10 @@ class Parloop:
                 if not hasattr(it, "_dev_idx"):
                     it._dev_idx = DeviceArray.from_host(it.indices)
                 subset = it._dev_idx.ptr
-            coords = self.args[1].data
+            # coordinates, then the coefficient field of a helmholtz_coef form
+            ins = [a.data.device_ptr for a in self.args[1:]]
             try:
-                gk(start, end, layers, subset, [out.handle.value, coords.device_ptr], None, None,
+                gk(start, end, layers, subset, [out.handle.value] + ins, None, None,
                    [m.device_ptr for m in maps], None, _lib.LOC_DEVICE, False, False)
             finally:
                 if lg is not None:

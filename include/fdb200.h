@@ -106,7 +106,20 @@ enum fdb_form {
                                    Poisson: (1,0)  mass: (0,1)  Helmholtz: (1,1)
                                    demos/helmholtz/helmholtz.py.rst:52-77,
                                    demos/matrix_free/poisson.py.rst:13-27        */
-    FDB_FORM_DG_ADVECTION = 2   /* demos/DG_advection/DG_advection.py.rst:182-217 */
+    FDB_FORM_DG_ADVECTION = 2,  /* demos/DG_advection/DG_advection.py.rst:182-217 */
+    FDB_FORM_HELMHOLTZ_COEF = 3 /* alpha*inner(kappa*grad u, grad v)*dx + beta*inner(u, v)*dx with a
+                                   scalar coefficient FIELD kappa in the argument space, gathered
+                                   through the same cell->node map (maps[0]); beta stays a constant.
+                                   Heterogeneous materials, Newton Jacobians of nonlinear diffusion.
+                                   Hex cells (extruded or native), cdim == 1, nq == degree+1,
+                                   affine_cells == 0; degrees 1..5 (action), 1..4 (rank 2), 1..3
+                                   (diagonal).  kappa is always the LAST argument:
+                                     action    [y INC, coords, u, kappa]  (atomic or coloured;
+                                               device or host mode, host mode monolithic)
+                                     diagonal  [d INC, coords, kappa]     (device mode)
+                                     rank 2    [Mat, coords, kappa]
+                                   Always the sum-factorised slab-thread kernel: the option
+                                   "matrix_kernel" (DMMA element matrices) does not apply.       */
 };
 
 enum fdb_cell {
@@ -315,7 +328,11 @@ typedef struct fdb_wrapper_desc {
 int fdb_wrapper_source(const fdb_wrapper_desc *d, char *buf, size_t cap, size_t *needed);
 /* Generate + NVRTC-compile for sm_90a into a cubin image (no GPU needed: this
  * is the ahead-of-time / disk-cache path, pyop2/compilation.py:424-455).  The
- * NVRTC log is available from fdb_last_error() on failure. */
+ * NVRTC log is available from fdb_last_error() on failure.  *needed is the
+ * image size; cubin = NULL only queries it, and a following call with the same
+ * descriptor copies that same image (the last one is kept: NVRTC's images of one
+ * source differ from compilation to compilation).  A non-NULL cubin smaller than
+ * the image is an error. */
 int fdb_wrapper_compile(const fdb_wrapper_desc *d, void *cubin, size_t cap, size_t *needed);
 /* Generate, compile and load; the handle is called with fdb_kernel_call using
  * the same arglist convention: args[] = one pointer per local-kernel argument
