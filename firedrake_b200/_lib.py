@@ -17,6 +17,8 @@ MAX_1D = 8
 FORM_HELMHOLTZ = 1
 FORM_DG_ADVECTION = 2
 FORM_HELMHOLTZ_COEF = 3
+FORM_NONLINEAR_DIFFUSION = 4
+FORM_NONLINEAR_DIFFUSION_JACOBIAN = 5
 CELL_HEX_EXTRUDED = 1
 CELL_HEX = 2
 CELL_TRIANGLE = 3
@@ -45,6 +47,7 @@ class KernelDesc(C.Structure):
         ("wq", C.c_double * MAX_1D), ("xq", C.c_double * MAX_1D),
         ("offset0", C.POINTER(C.c_int32)), ("offset1", C.POINTER(C.c_int32)),
         ("diagonal", C.c_int32), ("affine_cells", C.c_int32),
+        ("dcoef", C.c_double * 3),
     ]
 
 

@@ -501,6 +501,70 @@ class Form:
                           rank=rank, cdim=self.V.cdim, affine=affine)
 
 
+@dataclass
+class NonlinearDiffusion:
+    """The residual of nonlinear diffusion on ``V`` (scalar), without its source term:
+
+        F(u; v) = alpha*inner(D(u)*grad(u), grad(v))*dx + beta*inner(u, v)*dx,  D(s) = d0 + d1*s + d2*s**2
+
+    ``assemble(F, u=u)`` is the vector R(u); the problem F(u; v) = inner(f, v)*dx is solved by
+    :func:`solve_nonlinear` with ``L = assemble(mass(V), u=f)``.  D(u) is evaluated at each Gauss point
+    from the interpolated u, as TSFC evaluates a coefficient expression."""
+    V: FunctionSpace
+    alpha: float = 1.0
+    beta: float = 0.0
+    d: tuple = (1.0, 0.0, 0.0)
+    symmetric = False
+
+    def coefficient_args(self):
+        return []
+
+    def kernel(self, rank, diagonal=False):
+        if rank != 1 or diagonal:
+            raise ValueError("the residual is a 1-form: its matrix and diagonal are those of F.jacobian(u)")
+        if self.V.cdim != 1:
+            raise NotImplementedError("nonlinear diffusion takes scalar spaces only")
+        return op2.Kernel("nonlinear_diffusion", degree=self.V.degree, alpha=self.alpha, beta=self.beta,
+                          d=tuple(self.d))
+
+    def jacobian(self, u0: op2.Dat):
+        """The Gateaux derivative at ``u0`` (the exact Newton Jacobian, a bilinear form)."""
+        return NonlinearDiffusionJacobian(self.V, self.alpha, self.beta, tuple(self.d), u0)
+
+    def diffusivity(self, u: op2.Dat, target: op2.Dat = None):
+        """D(u) at the nodes of ``V`` (a pointwise node loop): the coefficient of the SPD operator
+        ``Form(V, alpha, beta, kappa=D(u))`` that the multigrid preconditioner of the Newton steps uses."""
+        if target is None:
+            target = self.V.dat()
+        d0, d1, d2 = (repr(float(c)) for c in self.d)
+        k = op2.Kernel(f"static void nodal_diffusivity(double *k, const double *u) "
+                       f"{{ *k = {d0} + u[0] * ({d1} + {d2} * u[0]); }}", "nodal_diffusivity")
+        op2.par_loop(k, self.V.node_set, target(op2.WRITE), u(op2.READ))
+        return target
+
+
+@dataclass
+class NonlinearDiffusionJacobian:
+    """J(u0)[w; v] = alpha*inner(D(u0)*grad(w) + D'(u0)*w*grad(u0), grad(v))*dx + beta*inner(w, v)*dx:
+    a bilinear form (``assemble(J, u=w)``, ``assemble(J)``, ``assemble(J, mat_type="matfree")``) whose
+    matrix is NOT symmetric when d1 or d2 is nonzero.  ``u0`` is read through the argument map."""
+    V: FunctionSpace
+    alpha: float
+    beta: float
+    d: tuple
+    u0: op2.Dat
+    symmetric = False
+
+    def coefficient_args(self):
+        return [self.u0(op2.READ, self.V.cell_node_map)]
+
+    def kernel(self, rank, diagonal=False):
+        if self.V.cdim != 1:
+            raise NotImplementedError("nonlinear diffusion takes scalar spaces only")
+        return op2.Kernel("nonlinear_diffusion_jacobian", degree=self.V.degree, alpha=self.alpha, beta=self.beta,
+                          rank=rank, diagonal=diagonal, d=tuple(self.d))
+
+
 def poisson(V):
     return Form(V, 1.0, 0.0)
 
@@ -625,7 +689,8 @@ class ImplicitMatrixContext:
         """``assemble(a, diagonal=True)`` then 1 on the constrained rows
         (matrix_free/operators.py:199-205; firedrake/assemble.py:1226-1241)."""
         V = self.form.V
-        if self.form.kappa is not None:
+        if self.form.coefficient_args():
+            # coefficient forms (kappa, a Jacobian's linearisation point) have their own diagonal kernel
             k = self.form.kernel(1, diagonal=True)
         else:
             k = op2.Kernel("helmholtz", degree=V.degree, alpha=self.form.alpha, beta=self.form.beta,
@@ -660,7 +725,10 @@ class ImplicitMatrixContext:
     def multTranspose(self, X: op2.Dat, Y: op2.Dat):
         """``Y = A^T X`` (matrix_free/operators.py:245-330: the action of ``adjoint(a)`` with the
         row and column conditions exchanged).  Every form of the supported family is
-        symmetric and row/column DirichletBCs coincide here (no EquationBC), so A^T = A."""
+        symmetric and row/column DirichletBCs coincide here (no EquationBC), so A^T = A.  The
+        Jacobian of nonlinear diffusion is not symmetric, and its transpose is not implemented."""
+        if not getattr(self.form, "symmetric", True):
+            raise NotImplementedError("multTranspose of a nonsymmetric form (the nonlinear diffusion Jacobian)")
         return self.mult(X, Y)
 
     def mult(self, X: op2.Dat, Y: op2.Dat):
@@ -753,6 +821,188 @@ def cg(A, b: op2.Dat, x: op2.Dat, rtol=1e-8, atol=0.0, maxit=1000, allreduce=Non
         it += 1
     x._device_written()
     return it, hist
+
+
+def gmres(A, b: op2.Dat, x: op2.Dat, M=None, rtol=1e-5, atol=0.0, restart=30, maxit=10000, allreduce=None):
+    """Restarted, right-preconditioned GMRES in its flexible form (``ksp_type fgmres``; with a fixed
+    preconditioner it is ``ksp_type gmres`` with right preconditioning) on device-resident Dats.
+    The preconditioned vectors z_j = M(v_j) are kept, so ``M`` may change from one application to
+    the next, as a V-cycle with an inner Krylov coarse solve does.  ``A`` needs ``mult(X, Y)``; ``M(r,
+    z)`` writes z from z = 0 (None: no preconditioner).  Inner products run over the owned dofs,
+    summed over the ranks by ``allreduce``; the (restart + 1) x restart Hessenberg least-squares
+    problem is solved on the host with Givens rotations.  Converged when the residual norm is at most
+    max(rtol * ||b - A x0||, atol).  Returns (iterations, residual norms)."""
+    import ctypes as C
+    from . import _lib
+    from .mg import _touched
+    L = _lib.lib()
+    Vd = b.dataset
+    n = b._data.size
+    n_owned = b.dataset.set.size * b.cdim
+    m = max(1, int(restart))
+    Vs = [op2.Dat(Vd) for _ in range(m + 1)]
+    Zs = [op2.Dat(Vd) for _ in range(m)] if M is not None else Vs
+    w = op2.Dat(Vd)
+
+    def dot(u, v):
+        out = C.c_double()
+        _lib.check(L.fdb_vec_dot(n_owned, u.device_ptr, v.device_ptr, C.byref(out)))
+        return allreduce(out.value) if allreduce else out.value
+
+    def residual(r):
+        """r = b - A x, returns ||r||"""
+        A.mult(x, w)
+        _lib.check(L.fdb_memcpy_d2d(r.device_ptr, b.device_ptr, b.nbytes))
+        _lib.check(L.fdb_vec_axpy(n, -1.0, w.device_ptr, r.device_ptr))
+        _touched(r)
+        return float(np.sqrt(dot(r, r)))
+
+    beta = residual(Vs[0])
+    hist = [beta]
+    tol = max(rtol * beta, atol)
+    it = 0
+    while beta > tol and it < maxit:
+        _lib.check(L.fdb_vec_scale(n, 1.0 / beta, Vs[0].device_ptr))
+        _touched(Vs[0])
+        H = np.zeros((m + 1, m))
+        cs, sn = np.zeros(m), np.zeros(m)
+        g = np.zeros(m + 1)
+        g[0] = beta
+        k = 0
+        for j in range(m):
+            if M is not None:
+                Zs[j].zero()
+                Zs[j].device_ptr
+                M(Vs[j], Zs[j])
+            A.mult(Zs[j], w)
+            for i in range(j + 1):                      # modified Gram-Schmidt
+                H[i, j] = dot(w, Vs[i])
+                _lib.check(L.fdb_vec_axpy(n, -H[i, j], Vs[i].device_ptr, w.device_ptr))
+            _touched(w)
+            H[j + 1, j] = np.sqrt(max(dot(w, w), 0.0))
+            if H[j + 1, j] > 0.0:
+                _lib.check(L.fdb_memcpy_d2d(Vs[j + 1].device_ptr, w.device_ptr, w.nbytes))
+                _lib.check(L.fdb_vec_scale(n, 1.0 / H[j + 1, j], Vs[j + 1].device_ptr))
+                _touched(Vs[j + 1])
+            for i in range(j):                          # previous rotations on the new column
+                t = cs[i] * H[i, j] + sn[i] * H[i + 1, j]
+                H[i + 1, j] = -sn[i] * H[i, j] + cs[i] * H[i + 1, j]
+                H[i, j] = t
+            r = np.hypot(H[j, j], H[j + 1, j])
+            cs[j], sn[j] = (H[j, j] / r, H[j + 1, j] / r) if r > 0.0 else (1.0, 0.0)
+            H[j, j] = r
+            H[j + 1, j] = 0.0
+            g[j + 1] = -sn[j] * g[j]
+            g[j] = cs[j] * g[j]
+            k = j + 1
+            it += 1
+            hist.append(abs(g[j + 1]))
+            if abs(g[j + 1]) <= tol or it >= maxit or r == 0.0:
+                break
+        # x += Z y, R y = g (upper triangular k x k)
+        y = np.zeros(k)
+        for i in range(k - 1, -1, -1):
+            y[i] = (g[i] - H[i, i + 1:k] @ y[i + 1:k]) / H[i, i] if H[i, i] != 0.0 else 0.0
+        for i in range(k):
+            _lib.check(L.fdb_vec_axpy(n, y[i], Zs[i].device_ptr, x.device_ptr))
+        _touched(x)
+        beta = residual(Vs[0])                          # the true residual at every restart
+        hist[-1] = beta
+    return it, hist
+
+
+def solve_nonlinear(F: NonlinearDiffusion, L: op2.Dat, u: op2.Dat, bcs=(), solver_parameters=None,
+                    hierarchy=None, allreduce=None):
+    """``solve(F == 0, u, bcs=bcs, solver_parameters=...)`` for nonlinear diffusion with the source
+    ``L`` (the assembled right-hand side, e.g. ``assemble(mass(V), u=f)``): Newton's method with the
+    full step (``snes_type newtonls``, ``snes_linesearch_type basic``) on the residual R(u) = F(u) - L,
+    each step solved by GMRES with the exact Jacobian ``F.jacobian(u)``.  ``u`` is the initial guess
+    and is overwritten with the solution.
+
+    The Dirichlet values are applied to u first; the residual's rows on constrained nodes are zeroed
+    and the Newton update vanishes there.  ``solver_parameters``: ``snes_rtol`` (1e-8), ``snes_atol``
+    (1e-50), ``snes_max_it`` (50); ``ksp_type`` "gmres", ``ksp_gmres_restart`` (30), ``ksp_rtol``
+    (1e-5), ``ksp_max_it`` (10000); ``mat_type`` "matfree" (default) | "aij"; ``pc_type`` "none"
+    (default) | "jacobi" (the Jacobian's exact diagonal) | "mg" (a V-cycle of the SPD operator
+    ``Form(V, alpha, beta, kappa=D(u))``, rebuilt at every Newton step; needs ``hierarchy``).
+    Converged when ||R(u)|| <= max(snes_rtol * ||R(u_0)||, snes_atol).  Returns (Newton residual
+    norms, Krylov iterations per Newton step)."""
+    from . import _lib
+    from . import mg as _mg
+    sp = {"snes_rtol": 1e-8, "snes_atol": 1e-50, "snes_max_it": 50, "ksp_type": "gmres",
+          "ksp_gmres_restart": 30, "ksp_rtol": 1e-5, "ksp_max_it": 10000, "mat_type": "matfree",
+          "pc_type": "none"}
+    sp.update(solver_parameters or {})
+    if sp["ksp_type"] != "gmres":
+        raise NotImplementedError("ksp_type gmres only (the Newton Jacobian is not symmetric)")
+    if sp["mat_type"] not in ("matfree", "aij"):
+        raise NotImplementedError(f"mat_type {sp['mat_type']!r}")
+    V = F.V
+    bcs = tuple(bcs)
+    lib = _lib.lib()
+    n = L._data.size
+    n_owned = L.dataset.set.size * L.cdim
+    u.device_ptr
+    for bc in bcs:
+        bc.apply(u)
+    R, du = V.dat(), V.dat()
+    res = OneFormAssembler(F, u)
+
+    def residual():
+        import ctypes as C
+        res.assemble(tensor=R)
+        R.axpy(-1.0, L)
+        for bc in bcs:
+            bc.zero(R)
+        out = C.c_double()
+        _lib.check(lib.fdb_vec_dot(n_owned, R.device_ptr, R.device_ptr, C.byref(out)))
+        return float(np.sqrt(allreduce(out.value) if allreduce else out.value))
+
+    hist = [residual()]
+    kits = []
+    tol = max(sp["snes_rtol"] * hist[0], sp["snes_atol"])
+    # J reads u in place: the matrix-free operator and the diagonal's context follow every update,
+    # an assembled matrix is assembled again at every step
+    J = F.jacobian(u)
+    pc = sp["pc_type"]
+    A = ctx = None
+    d = V.dat() if pc == "jacobi" else None
+    while hist[-1] > tol and len(kits) < sp["snes_max_it"]:
+        if A is None or sp["mat_type"] != "matfree":
+            A = assemble(J, bcs=bcs, mat_type=sp["mat_type"])
+        if pc == "none":
+            M = None
+        elif pc == "jacobi":
+            if ctx is None:
+                ctx = A if isinstance(A, ImplicitMatrixContext) else ImplicitMatrixContext(J, bcs)
+            ctx.getDiagonal(d)
+            op2.par_loop(op2.Kernel("static void recip(double *w) { *w = 1.0 / *w; }", "recip"), V.node_set,
+                         d(op2.RW))
+
+            def M(r, z, d=d):
+                _lib.check(lib.fdb_vec_pointwise_mult(n, r.device_ptr, d.device_ptr, z.device_ptr))
+                z._device_written()
+        elif pc == "mg":
+            if hierarchy is None:
+                raise ValueError("pc_type mg needs the mesh hierarchy")
+            kap = F.diffusivity(u)
+            vc = _mg.VCycle(hierarchy, V.degree, lambda W, k=None: Form(W, F.alpha, F.beta, k),
+                            bc_domains=tuple(s for bc in bcs for s in bc.sub_domains), allreduce=allreduce,
+                            kappa=kap)
+            top = len(hierarchy) - 1
+            M = lambda r, z, vc=vc: vc.apply(top, r, z)
+        else:
+            raise NotImplementedError(f"pc_type {pc!r}")
+        du.zero()
+        du.device_ptr
+        its, _ = gmres(A, R, du, M, rtol=sp["ksp_rtol"], restart=sp["ksp_gmres_restart"],
+                       maxit=sp["ksp_max_it"], allreduce=allreduce)
+        for bc in bcs:
+            bc.zero(du)
+        u.axpy(-1.0, du)
+        kits.append(its)
+        hist.append(residual())
+    return hist, kits
 
 
 def solve(form: Form, L: op2.Dat, u: op2.Dat, bcs=(), solver_parameters=None, hierarchy=None, allreduce=None):

@@ -27,6 +27,9 @@
 // DESIGN.md section 4.1 has the measurements behind each of these choices.
 // helmholtz_coef_kernel is the same body (action_hex_body.cuh) with COEF set: a coefficient field
 // kappa scales the stiffness term (FDB_FORM_HELMHOLTZ_COEF, DESIGN.md section 4.5).
+// nonlinear_residual_kernel and nonlinear_jacobian_kernel are the same body with NL = 1 / 2: the
+// residual and the exact Newton Jacobian of alpha*inner(D(u) grad u, grad v)*dx + beta*inner(u, v)*dx
+// (FDB_FORM_NONLINEAR_DIFFUSION[_JACOBIAN], DESIGN.md section 4.6).
 //
 // Arithmetic: the basis is first interpolated to the N Gauss points per axis
 // (B (x) B (x) B), gradients are then taken with the collocated derivative
@@ -87,12 +90,29 @@ struct HelmCoefParams : HelmParams<N> {
     const double *kappa;
 };
 
+// FDB_FORM_NONLINEAR_DIFFUSION[_JACOBIAN]: D(s) = dcoef[0] + dcoef[1] s + dcoef[2] s^2; the Jacobian
+// passes the linearisation point u as kappa
+template <int N>
+struct HelmNlParams : HelmCoefParams<N> {
+    double dcoef[3];
+};
+
 // the quadrature weight of the stiffness flux, times kappa at the point (COEF: s_kap[q])
 template <bool COEF>
 __device__ __forceinline__ double coef_weight(double w, const double *s_kap, int q)
 {
     if constexpr (COEF) return w * s_kap[q];
     else return w;
+}
+
+// the same for every mode of the slab-thread body: NL == 1 (residual) scales by D(u_q), u_q = x at the
+// point; NL == 2 (Jacobian) applies D and D' to the gradient instead and keeps w
+template <bool COEF, int NL>
+__device__ __forceinline__ double stiff_weight(double w, const double *s_kap, int q, double uq, const double *dcoef)
+{
+    if constexpr (NL == 1) return w * fma(fma(dcoef[2], uq, dcoef[1]), uq, dcoef[0]);
+    else if constexpr (NL == 2) return w;
+    else return coef_weight<COEF>(w, s_kap, q);
 }
 
 __device__ __forceinline__ double fast_rcp(double x)
@@ -302,7 +322,9 @@ __global__ void __launch_bounds__(WPC<N, SLIM>::value * 32, MINB)
 helmholtz_action_kernel(const __grid_constant__ HelmParams<N> P)
 {
     constexpr bool COEF = false;
+    constexpr int NL = 0;
     [[maybe_unused]] const double *kappa = nullptr;
+    [[maybe_unused]] const double *dcoef = nullptr;
 #include "action_hex_body.cuh"
 }
 
@@ -312,21 +334,52 @@ __global__ void __launch_bounds__(WPC<N, SLIM, true>::value * 32, MINB)
 helmholtz_coef_kernel(const __grid_constant__ HelmCoefParams<N> P)
 {
     constexpr bool COEF = true, AFFINE = false;
+    constexpr int NL = 0;
     const double *kappa = P.kappa;
+    [[maybe_unused]] const double *dcoef = nullptr;
+#include "action_hex_body.cuh"
+}
+
+// FDB_FORM_NONLINEAR_DIFFUSION (action only): the constant-coefficient layout, D(u_q) from the
+// gathered values themselves
+template <int N, bool MASS, bool ATOMIC, int MINB, bool SLIM = false>
+__global__ void __launch_bounds__(WPC<N, SLIM>::value * 32, MINB)
+nonlinear_residual_kernel(const __grid_constant__ HelmNlParams<N> P)
+{
+    constexpr bool COEF = false, MATRIX = false, AFFINE = false;
+    constexpr int NL = 1;
+    [[maybe_unused]] const double *kappa = nullptr;
+    const double *dcoef = P.dcoef;
+#include "action_hex_body.cuh"
+}
+
+// FDB_FORM_NONLINEAR_DIFFUSION_JACOBIAN (action, element matrix, diagonal): the coefficient layout,
+// u in the kappa buffer
+template <int N, bool MASS, bool ATOMIC, int MINB, bool MATRIX = false, bool SLIM = false>
+__global__ void __launch_bounds__(WPC<N, SLIM, true>::value * 32, MINB)
+nonlinear_jacobian_kernel(const __grid_constant__ HelmNlParams<N> P)
+{
+    constexpr bool COEF = true, AFFINE = false;
+    constexpr int NL = 2;
+    const double *kappa = P.kappa;
+    const double *dcoef = P.dcoef;
 #include "action_hex_body.cuh"
 }
 
 #include "action_hex_ws.cuh"
 
 template <int N, bool MASS, bool ATOMIC, int MINB, bool MATRIX = false, bool SLIM = false, bool AFFINE = false,
-          bool COEF = false>
-int launch_one(int grid_cap_per_sm, cudaStream_t st, HelmCoefParams<N> &P, int sm_count)
+          bool COEF = false, int NL = 0>
+int launch_one(int grid_cap_per_sm, cudaStream_t st, HelmNlParams<N> &P, int sm_count)
 {
+    static_assert(NL == 0 || COEF == (NL == 2), "the Jacobian takes the coefficient layout, the residual not");
     using WS = WarpSmem<N, SLIM, COEF>;
     constexpr int WARPS_PER_CTA = WPC<N, SLIM, COEF>::value;
     constexpr int T = WARPS_PER_CTA * 32;
     auto kern = [] {
-        if constexpr (COEF) return helmholtz_coef_kernel<N, MASS, ATOMIC, MINB, MATRIX, SLIM>;
+        if constexpr (NL == 1) return nonlinear_residual_kernel<N, MASS, ATOMIC, MINB, SLIM>;
+        else if constexpr (NL == 2) return nonlinear_jacobian_kernel<N, MASS, ATOMIC, MINB, MATRIX, SLIM>;
+        else if constexpr (COEF) return helmholtz_coef_kernel<N, MASS, ATOMIC, MINB, MATRIX, SLIM>;
         else return helmholtz_action_kernel<N, MASS, ATOMIC, MINB, MATRIX, SLIM, AFFINE>;
     }();
     static bool configured = false;
@@ -361,7 +414,8 @@ int launch_one(int grid_cap_per_sm, cudaStream_t st, HelmCoefParams<N> &P, int s
     P.nlay_rcp = (unsigned)(0x100000000ull / (unsigned long long)P.nlay_items);
     if (P.nlay_items == 1) P.nlay_rcp = 0xffffffffu;
     FDB_CUDA(cudaMemsetAsync(P.counter, 0, sizeof(int), st));
-    if constexpr (COEF) kern<<<(int)grid, T, WS::CTA_BYTES, st>>>(P);
+    if constexpr (NL != 0) kern<<<(int)grid, T, WS::CTA_BYTES, st>>>(P);
+    else if constexpr (COEF) kern<<<(int)grid, T, WS::CTA_BYTES, st>>>(static_cast<const HelmCoefParams<N> &>(P));
     else kern<<<(int)grid, T, WS::CTA_BYTES, st>>>(static_cast<const HelmParams<N> &>(P));
     FDB_LAUNCH_CHECK();
     return 0;
@@ -377,7 +431,7 @@ struct CoefMinB {
 // coefficient form (action): the slab-thread kernel for every degree -- no thread-per-cell,
 // warp-specialised or affine variant
 template <int N, bool ATOMIC>
-int launch_coef(bool mass, int cap, cudaStream_t st, HelmCoefParams<N> &P, int sm_count)
+int launch_coef(bool mass, int cap, cudaStream_t st, HelmNlParams<N> &P, int sm_count)
 {
     constexpr int MB = CoefMinB<N>::value;
     if (N == 6 && P.nlay_items >= 32 / N) {
@@ -388,8 +442,55 @@ int launch_coef(bool mass, int cap, cudaStream_t st, HelmCoefParams<N> &P, int s
     return launch_one<N, false, ATOMIC, MB, false, false, false, true>(cap, st, P, sm_count);
 }
 
+// register bound of the residual kernel (-Xptxas -v, DESIGN.md section 4.6): as the constant-coefficient
+// kernel, 3 CTAs x 4 warps x 168 registers at degree 3
+template <int N>
+struct NlResMinB {
+    static constexpr int value = (N == 4) ? 3 : ((N >= 5) ? 1 : 2);
+};
+
+// nonlinear diffusion (nl = 1 residual, 2 Jacobian action): the slab-thread kernel for every degree,
+// slim staging at degree 5 as for the other forms -- no thread-per-cell, warp-specialised or affine
+// variant
 template <int N, bool ATOMIC>
-int launch_variant(bool mass, int minb, int cap, cudaStream_t st, HelmCoefParams<N> &P, int sm_count,
+int launch_nl(int nl, bool mass, int cap, cudaStream_t st, HelmNlParams<N> &P, int sm_count)
+{
+    constexpr bool SL = (N == 6);
+    const bool slim = SL && P.nlay_items >= 32 / N;
+    if (nl == 1) {
+        constexpr int MB = NlResMinB<N>::value;
+        if (slim) {
+            if (mass) return launch_one<N, true, ATOMIC, MB, false, SL, false, false, 1>(cap, st, P, sm_count);
+            return launch_one<N, false, ATOMIC, MB, false, SL, false, false, 1>(cap, st, P, sm_count);
+        }
+        if (mass) return launch_one<N, true, ATOMIC, MB, false, false, false, false, 1>(cap, st, P, sm_count);
+        return launch_one<N, false, ATOMIC, MB, false, false, false, false, 1>(cap, st, P, sm_count);
+    }
+    constexpr int MB = CoefMinB<N>::value;
+    if (slim) {
+        if (mass) return launch_one<N, true, ATOMIC, MB, false, SL, false, true, 2>(cap, st, P, sm_count);
+        return launch_one<N, false, ATOMIC, MB, false, SL, false, true, 2>(cap, st, P, sm_count);
+    }
+    if (mass) return launch_one<N, true, ATOMIC, MB, false, false, false, true, 2>(cap, st, P, sm_count);
+    return launch_one<N, false, ATOMIC, MB, false, false, false, true, 2>(cap, st, P, sm_count);
+}
+
+// nonlinear mode of a kernel: 1 residual, 2 Jacobian, 0 any other form
+inline int nl_mode(const fdb_kernel_s *k)
+{
+    if (k->desc.form == FDB_FORM_NONLINEAR_DIFFUSION) return 1;
+    if (k->desc.form == FDB_FORM_NONLINEAR_DIFFUSION_JACOBIAN) return 2;
+    return 0;
+}
+
+template <int N>
+void set_dcoef(const fdb_kernel_s *k, HelmNlParams<N> &P)
+{
+    for (int i = 0; i < 3; i++) P.dcoef[i] = nl_mode(k) ? k->desc.dcoef[i] : 0.0;
+}
+
+template <int N, bool ATOMIC>
+int launch_variant(bool mass, int minb, int cap, cudaStream_t st, HelmNlParams<N> &P, int sm_count,
                    bool affine = false)
 {
     if (affine && ATOMIC) {
@@ -433,8 +534,10 @@ int launch_n(fdb_kernel_s *k, fdb_int start, fdb_int end, int nlay, const fdb_in
              const fdb_int *map1, const double *kappa)
 {
     fdb::Context &c = fdb::ctx();
-    HelmCoefParams<N> P;
-    P.kappa = kappa;             // NULL: constant-coefficient form
+    HelmNlParams<N> P;
+    P.kappa = kappa;             // NULL: constant-coefficient form and residual
+    set_dcoef(k, P);
+    const int nl = nl_mode(k);
     P.y = y;
     P.x = x;
     P.coords = coords;
@@ -472,7 +575,8 @@ int launch_n(fdb_kernel_s *k, fdb_int start, fdb_int end, int nlay, const fdb_in
         P.lay_first = 0;
         P.lay_step = 1;
         if (P.ncols <= 0 || nlay <= 0) return 0;
-        if (kappa) return launch_coef<N, true>(mass, cap, c.stream, P, c.sm_count);
+        if (kappa && !nl) return launch_coef<N, true>(mass, cap, c.stream, P, c.sm_count);
+        if (nl) return launch_nl<N, true>(nl, mass, cap, c.stream, P, c.sm_count);
         if constexpr (N == 4) {
             // degree 3, scalar: warp-specialised kernel (action_hex_ws.cuh)
             static const int ws = getenv("FDB_WS") ? atoi(getenv("FDB_WS")) : 0;
@@ -507,8 +611,9 @@ int launch_n(fdb_kernel_s *k, fdb_int start, fdb_int end, int nlay, const fdb_in
             P.lay_step = 2;
             P.nlay_items = (nlay - par + 1) / 2;
             if (P.ncols <= 0 || P.nlay_items <= 0) continue;
-            if (kappa ? launch_coef<N, false>(mass, cap, c.stream, P, c.sm_count)
-                      : launch_variant<N, false>(mass, minb, cap, c.stream, P, c.sm_count))
+            if (kappa && !nl ? launch_coef<N, false>(mass, cap, c.stream, P, c.sm_count)
+                : nl         ? launch_nl<N, false>(nl, mass, cap, c.stream, P, c.sm_count)
+                             : launch_variant<N, false>(mass, minb, cap, c.stream, P, c.sm_count))
                 return 1;
         }
     }
@@ -521,9 +626,10 @@ int launch_matrix_n(fdb_kernel_s *k, fdb_int start, fdb_int end, int nlay, const
                     double *diag_out, const double *kappa)
 {
     fdb::Context &c = fdb::ctx();
-    HelmCoefParams<N> P;
+    HelmNlParams<N> P;
     memset(&P, 0, sizeof(P));
     P.kappa = kappa;             // NULL: constant-coefficient form
+    set_dcoef(k, P);
     P.coords = coords;
     P.map0 = map0;
     P.map1 = map1;
@@ -563,11 +669,18 @@ int launch_matrix_n(fdb_kernel_s *k, fdb_int start, fdb_int end, int nlay, const
     P.lay_first = 0;
     P.lay_step = 1;
     if (P.ncols <= 0 || nlay <= 0) return 0;
-    if (kappa) {
+    if (kappa && nl_mode(k) == 0) {
         constexpr int MB = CoefMinB<N>::value;
         if (k->desc.beta != 0.0)
             return launch_one<N, true, true, MB, true, false, false, true>(0, c.stream, P, c.sm_count);
         return launch_one<N, false, true, MB, true, false, false, true>(0, c.stream, P, c.sm_count);
+    }
+    if (nl_mode(k) == 2) {
+        // the Jacobian's element matrix / diagonal: u in the kappa buffer, reused across the N^3 units
+        constexpr int MB = CoefMinB<N>::value;
+        if (k->desc.beta != 0.0)
+            return launch_one<N, true, true, MB, true, false, false, true, 2>(0, c.stream, P, c.sm_count);
+        return launch_one<N, false, true, MB, true, false, false, true, 2>(0, c.stream, P, c.sm_count);
     }
     constexpr int DEF = (N >= 5) ? 1 : 2;
     if (k->desc.beta != 0.0) return launch_one<N, true, true, DEF, true>(0, c.stream, P, c.sm_count);
@@ -624,7 +737,9 @@ int fdb_launch_helmholtz_action(fdb_kernel_s *k, fdb_int start, fdb_int end, int
 }
 
 // FDB_FORM_HELMHOLTZ_COEF: the slab-thread kernel for every degree (1..5 action, 1..4 matrix and
-// diagonal); never the thread-per-cell, warp-specialised, affine or DMMA kernels
+// diagonal); never the thread-per-cell, warp-specialised, affine or DMMA kernels.  The nonlinear
+// diffusion forms take the same entry points (launch_n / launch_matrix_n pick the mode from the
+// form): the residual with kappa = NULL, the Jacobian with kappa = the linearisation point u.
 int fdb_launch_helmholtz_coef_action(fdb_kernel_s *k, fdb_int start, fdb_int end, int nlay,
                                      const fdb_int *subset, double *y, const double *coords,
                                      const double *x, const double *kappa, const fdb_int *map0,

@@ -1,12 +1,21 @@
-// Body of the slab-thread kernels of action_hex.cu (helmholtz_action_kernel, helmholtz_coef_kernel),
-// included inside each __global__ function: the template parameters N, MASS, ATOMIC, MATRIX, SLIM,
-// AFFINE, the parameter block P and, from the including kernel, `constexpr bool COEF` and
-// `const double *kappa` are in scope.  A textual include rather than a __forceinline__ function taking
+// Body of the slab-thread kernels of action_hex.cu (helmholtz_action_kernel, helmholtz_coef_kernel,
+// nonlinear_residual_kernel, nonlinear_jacobian_kernel), included inside each __global__ function: the
+// template parameters N, MASS, ATOMIC, MATRIX, SLIM, AFFINE, the parameter block P and, from the
+// including kernel, `constexpr bool COEF`, `constexpr int NL`, `const double *kappa` and
+// `const double *dcoef` are in scope.  A textual include rather than a __forceinline__ function taking
 // P by reference: the reference changes the register allocation of the existing matrix-mode kernels,
 // whose machine code this layout keeps exactly as it was before the coefficient form existed.
+//
+// NL (nonlinear diffusion, D(s) = dcoef[0] + dcoef[1] s + dcoef[2] s^2):
+//   1  residual: x is u; the stiffness weight at a point is w D(u_q), u_q = U[qx][0] (no kappa buffer)
+//   2  Jacobian: x is w, u is gathered into the kappa buffer (COEF layout) and interpolated to the
+//      points there; the reference gradient g of w becomes D(u_q) g + D'(u_q) w_q ghat(u)_q, with
+//      ghat(u)_q taken by collocated differentiation (Dt) of the buffer's quadrature values
     static_assert(!(SLIM && MATRIX), "matrix mode keeps the per-cell index buffer");
     static_assert(!(AFFINE && MATRIX), "the affine variant exists for 1-forms only");
     static_assert(!(AFFINE && COEF), "the coefficient form has no affine variant");
+    static_assert(NL != 1 || (!COEF && !MATRIX && !AFFINE), "the residual is a 1-form without a kappa buffer");
+    static_assert(NL != 2 || (COEF && !AFFINE), "the Jacobian keeps u in the kappa buffer");
     using WS = WarpSmem<N, SLIM, COEF>;
     constexpr int CW = WS::CW;
     constexpr int CWS = WS::CWS;
@@ -41,6 +50,12 @@
     const double eta = P.xq[lane_active ? t : 0];
     const double wy_alpha = P.wq[lane_active ? t : 0] * P.alpha;
     const double wy_beta = P.wq[lane_active ? t : 0] * P.beta;
+    // NL == 2: this lane's row of Dt (d/d eta at qy = t), for the gradient of u along y
+    [[maybe_unused]] double dyr[N];
+    if constexpr (NL == 2) {
+#pragma unroll
+        for (int q = 0; q < N; q++) dyr[q] = P.Dt[(lane_active ? t : 0) * N + q];
+    }
 
     // warp-uniform work iterator: chunks of consecutive items (one column's
     // worth) handed out by an atomic counter -> locality inside a chunk,
@@ -439,11 +454,34 @@
                     r2[2] = ca[0] * cb[1] - ca[1] * cb[0];
                     const double det = ca[0] * r0[0] + ca[1] * r0[1] + ca[2] * r0[2];
                     const double adet = fabs(det);
-                    const double s = coef_weight<COEF>(wyz_a * P.wq[qx], s_kap + cw * US, (qx * N + t) * N + qz) *
-                                     fast_rcp(adet);
+                    const double s = stiff_weight<COEF, NL>(wyz_a * P.wq[qx], s_kap + cw * US, (qx * N + t) * N + qz,
+                                                            U[qx][0], dcoef) * fast_rcp(adet);
                     double h[3];
+                    if constexpr (NL == 2) {
+                        // u and its reference gradient at (qx, qy = t, qz) from the buffer's quadrature
+                        // values; the z row is dz (rotated), the buffer is not
+                        const double *sk = s_kap + cw * US;
+                        const int row = (qx * N + t) * N;
+                        const double uq = sk[row + qz];
+                        double ux = 0.0, uy = 0.0, uz = 0.0;
 #pragma unroll
-                    for (int a = 0; a < 3; a++) h[a] = r0[a] * gx + r1[a] * gy + r2[a] * gz;
+                        for (int q = 0; q < N; q++) {
+                            const int zq = (q + qz < N) ? q + qz : q + qz - N;
+                            ux = fma(P.Dt[qx * N + q], sk[(q * N + t) * N + qz], ux);
+                            uy = fma(dyr[q], sk[(qx * N + q) * N + qz], uy);
+                            uz = fma(dz[q], sk[row + zq], uz);
+                        }
+                        const double Dq = fma(fma(dcoef[2], uq, dcoef[1]), uq, dcoef[0]);
+                        const double dpw = fma(2.0 * dcoef[2], uq, dcoef[1]) * U[qx][0];   // D'(u_q) w_q
+                        const double g0 = fma(dpw, ux, Dq * gx);
+                        const double g1 = fma(dpw, uy, Dq * gy);
+                        const double g2 = fma(dpw, uz, Dq * gz);
+#pragma unroll
+                        for (int a = 0; a < 3; a++) h[a] = r0[a] * g0 + r1[a] * g1 + r2[a] * g2;
+                    } else {
+#pragma unroll
+                        for (int a = 0; a < 3; a++) h[a] = r0[a] * gx + r1[a] * gy + r2[a] * gz;
+                    }
                     const double fx = s * (r0[0] * h[0] + r0[1] * h[1] + r0[2] * h[2]);
                     const double fy = s * (r1[0] * h[0] + r1[1] * h[1] + r1[2] * h[2]);
                     const double fz = s * (r2[0] * h[0] + r2[1] * h[1] + r2[2] * h[2]);

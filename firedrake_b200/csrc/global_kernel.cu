@@ -273,23 +273,32 @@ int fdb_kernel_create(const fdb_kernel_desc *d, fdb_kernel_t *out)
         *out = k;
         return 0;
     }
-    if (d->form == FDB_FORM_HELMHOLTZ_COEF) {
-        // kappa in the scalar argument space: the slab-thread kernel with its coefficient stage
+    const bool nl_res = d->form == FDB_FORM_NONLINEAR_DIFFUSION;
+    const bool nl_jac = d->form == FDB_FORM_NONLINEAR_DIFFUSION_JACOBIAN;
+    if (d->form == FDB_FORM_HELMHOLTZ_COEF || nl_res || nl_jac) {
+        // kappa (or the nonlinear diffusion's u) in the scalar argument space: the slab-thread kernel
+        // with its coefficient stage, or the residual's D(u) weight
+        const char *name = nl_res ? "nonlinear_diffusion" : (nl_jac ? "nonlinear_diffusion_jacobian" : "helmholtz_coef");
         if (d->cell != FDB_CELL_HEX_EXTRUDED && d->cell != FDB_CELL_HEX) {
-            set_error("fdb_kernel_create: helmholtz_coef needs hex cells (extruded or native), got cell %d", d->cell);
+            set_error("fdb_kernel_create: %s needs hex cells (extruded or native), got cell %d", name, d->cell);
             return 1;
         }
         if (d->cdim != 1) {
-            set_error("fdb_kernel_create: helmholtz_coef takes scalar spaces only (cdim %d)", d->cdim);
+            set_error("fdb_kernel_create: %s takes scalar spaces only (cdim %d)", name, d->cdim);
             return 1;
         }
         if (d->affine_cells) {
-            set_error("fdb_kernel_create: helmholtz_coef has no affine-cell variant (affine_cells must be 0)");
+            set_error("fdb_kernel_create: %s has no affine-cell variant (affine_cells must be 0)", name);
+            return 1;
+        }
+        if (nl_res && (d->rank != 1 || d->diagonal)) {
+            set_error("fdb_kernel_create: nonlinear_diffusion is the residual, a 1-form action only: its matrix "
+                      "and diagonal are those of nonlinear_diffusion_jacobian");
             return 1;
         }
         const int maxdeg = d->rank == 2 ? 4 : (d->diagonal ? 3 : 5);
         if (d->degree < 1 || d->degree > maxdeg) {
-            set_error("fdb_kernel_create: helmholtz_coef %s: degree %d outside 1..%d",
+            set_error("fdb_kernel_create: %s %s: degree %d outside 1..%d", name,
                       d->rank == 2 ? "matrix" : (d->diagonal ? "diagonal" : "action"), d->degree, maxdeg);
             return 1;
         }
@@ -430,18 +439,24 @@ int fdb_kernel_call(fdb_kernel_t k, const fdb_call_args *a)
         set_error("fdb_kernel_call: iteration set too large for IntType");
         return 1;
     }
-    const bool coef = k->desc.form == FDB_FORM_HELMHOLTZ_COEF;
+    // forms with a trailing coefficient argument (kappa; the nonlinear diffusion Jacobian's u), and the
+    // nonlinear diffusion residual, whose args are those of the constant-coefficient action
+    const bool nl_jac = k->desc.form == FDB_FORM_NONLINEAR_DIFFUSION_JACOBIAN;
+    const bool coef = k->desc.form == FDB_FORM_HELMHOLTZ_COEF || nl_jac;
+    const bool nl_res = k->desc.form == FDB_FORM_NONLINEAR_DIFFUSION;
+    const char *cname = nl_jac ? "nonlinear_diffusion_jacobian" : "helmholtz_coef";
+    const char *cvar = nl_jac ? "u" : "kappa";
     if (coef && k->desc.rank == 2) {
         // args = [Mat handle (INC), coords (READ), kappa (READ)], maps = [V map, coord map]
         if (a->nargs != 3 || a->nmaps != 2) {
-            set_error("fdb_kernel_call: helmholtz_coef 2-form expects 3 args (mat, coords, kappa) and 2 maps");
+            set_error("fdb_kernel_call: %s 2-form expects 3 args (mat, coords, %s) and 2 maps", cname, cvar);
             return 1;
         }
         fdb_mat_t target = (fdb_mat_t)a->args[0];
         int mat_bs = 1;
         fdb_mat_block_size(target, &mat_bs);
         if (mat_bs != 1) {
-            set_error("fdb_kernel_call: helmholtz_coef assembles scalar matrices only (block size %d)", mat_bs);
+            set_error("fdb_kernel_call: %s assembles scalar matrices only (block size %d)", cname, mat_bs);
             return 1;
         }
         if (k->desc.scatter != FDB_SCATTER_ATOMIC) {
@@ -537,7 +552,7 @@ int fdb_kernel_call(fdb_kernel_t k, const fdb_call_args *a)
     if (coef && k->desc.diagonal) {
         // args = [d (INC), coords, kappa]; device-resident only
         if (a->nargs != 3 || a->nmaps != 2 || a->location != FDB_LOC_DEVICE) {
-            set_error("fdb_kernel_call: helmholtz_coef diagonal expects 3 device args (d, coords, kappa) and 2 maps");
+            set_error("fdb_kernel_call: %s diagonal expects 3 device args (d, coords, %s) and 2 maps", cname, cvar);
             return 1;
         }
         return fdb_launch_helmholtz_coef_matrix(k, a->start, a->end, nlay, a->subset, nullptr,
@@ -558,8 +573,8 @@ int fdb_kernel_call(fdb_kernel_t k, const fdb_call_args *a)
     // 1-form: args = [y (INC), coords (READ), x (READ)], maps = [V map, coord map]
     // (helmholtz_coef: [y, coords, x, kappa (READ)])
     if (coef && (a->nargs != 4 || a->nmaps != 2)) {
-        set_error("fdb_kernel_call: helmholtz_coef 1-form expects 4 args (y, coords, x, kappa) and 2 maps, got %d/%d",
-                  a->nargs, a->nmaps);
+        set_error("fdb_kernel_call: %s 1-form expects 4 args (y, coords, x, %s) and 2 maps, got %d/%d",
+                  cname, cvar, a->nargs, a->nmaps);
         return 1;
     }
     if (!coef && (a->nargs != 3 || a->nmaps != 2)) {
@@ -567,8 +582,9 @@ int fdb_kernel_call(fdb_kernel_t k, const fdb_call_args *a)
                   a->nargs, a->nmaps);
         return 1;
     }
-    // the pipelined host action moves x and y only: the coefficient form takes the monolithic path
-    if (!coef && a->location == FDB_LOC_HOST && a->arg_versions && a->arg_bytes && a->map_bytes &&
+    // the pipelined host action moves x and y only and runs the constant-coefficient kernels: the
+    // coefficient and nonlinear forms take the monolithic path
+    if (!coef && !nl_res && a->location == FDB_LOC_HOST && a->arg_versions && a->arg_bytes && a->map_bytes &&
         a->writeback && a->output_is_zero && !a->subset && extruded &&
         k->desc.scatter == FDB_SCATTER_ATOMIC) {
         int rc = pipelined_host_action(k, a, nlay);
@@ -629,9 +645,11 @@ int fdb_kernel_call(fdb_kernel_t k, const fdb_call_args *a)
         set_error("fdb_kernel_call: coloured scatter needs start == 0");
         return 1;
     }
-    int rc = coef ? fdb_launch_helmholtz_coef_action(k, a->start, a->end, nlay, dsubset, (double *)dargs[0],
-                                                     (const double *)dargs[1], (const double *)dargs[2],
-                                                     (const double *)dargs[3], dmaps[0], dmaps[1])
+    // (the residual: the coefficient entry point without a coefficient, see action_hex.cu)
+    int rc = (coef || nl_res)
+                 ? fdb_launch_helmholtz_coef_action(k, a->start, a->end, nlay, dsubset, (double *)dargs[0],
+                                                    (const double *)dargs[1], (const double *)dargs[2],
+                                                    coef ? (const double *)dargs[3] : nullptr, dmaps[0], dmaps[1])
                   : fdb_launch_helmholtz_action(k, a->start, a->end, nlay, dsubset, (double *)dargs[0],
                                                 (const double *)dargs[1], (const double *)dargs[2],
                                                 dmaps[0], dmaps[1]);

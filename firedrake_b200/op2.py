@@ -1360,6 +1360,13 @@ class Kernel:
     + beta*inner(u, v)*dx`` with a scalar coefficient field kappa in the argument space, passed as
     the LAST argument (READ, through the argument map): action (INC, READ, READ, READ), diagonal and
     rank 2 (INC, READ, READ).
+
+    Nonlinear diffusion with ``D(s) = d[0] + d[1]*s + d[2]*s**2`` (``d``): "nonlinear_diffusion" is
+    the residual ``alpha*inner(D(u)*grad u, grad v)*dx + beta*inner(u, v)*dx``, a rank-1 action
+    only (INC, READ, READ: output, coordinates, u); "nonlinear_diffusion_jacobian" is its Gateaux
+    derivative at u, ``alpha*inner(D(u)*grad w + D'(u)*w*grad u, grad v)*dx + beta*inner(w, v)*dx``,
+    with u as the LAST argument like kappa: action (output, coordinates, w, u), diagonal and rank 2
+    (output, coordinates, u).  Its matrix is not symmetric.
     """
     form: str = "helmholtz"
     degree: int = 1
@@ -1376,6 +1383,7 @@ class Kernel:
     accesses: tuple = (INC, READ, READ)
     # tabulation: a fiat_lite.Interval1D, or None for the default GLL/Gauss pair
     element: object = field(default=None, compare=False, hash=False)
+    d: tuple = (1.0, 0.0, 0.0)      # nonlinear diffusion: D(s) = d[0] + d[1] s + d[2] s^2
 
     def __new__(cls, *args, **kwargs):
         # ``op2.Kernel(code, name)`` with C source (pyop2/local_kernel.py:33-43) builds the
@@ -1387,7 +1395,13 @@ class Kernel:
         return super().__new__(cls)
 
     def __post_init__(self):
-        if self.form == "helmholtz_coef":
+        if self.form in ("nonlinear_diffusion", "nonlinear_diffusion_jacobian"):
+            object.__setattr__(self, "d", tuple(float(c) for c in self.d))
+            if len(self.d) != 3:
+                raise ValueError("d holds the three coefficients of D(s) = d0 + d1 s + d2 s^2")
+        if self.form == "nonlinear_diffusion":
+            return                       # residual: (INC, READ, READ), like the constant-coefficient action
+        if self.form in ("helmholtz_coef", "nonlinear_diffusion_jacobian"):
             acc = (INC, READ, READ) if (self.diagonal or self.rank == 2) else (INC, READ, READ, READ)
             object.__setattr__(self, "accesses", acc)
             if self.rank == 2 and self.name == "form0_cell_integral":
@@ -1413,7 +1427,8 @@ class Kernel:
 
 
 _FORMS = {"helmholtz": _lib.FORM_HELMHOLTZ, "dg_advection": _lib.FORM_DG_ADVECTION,
-          "helmholtz_coef": _lib.FORM_HELMHOLTZ_COEF}
+          "helmholtz_coef": _lib.FORM_HELMHOLTZ_COEF, "nonlinear_diffusion": _lib.FORM_NONLINEAR_DIFFUSION,
+          "nonlinear_diffusion_jacobian": _lib.FORM_NONLINEAR_DIFFUSION_JACOBIAN}
 _INTEGRALS = {"cell": _lib.INTEGRAL_CELL, "exterior_facet": _lib.INTEGRAL_EXTERIOR_FACET,
               "interior_facet": _lib.INTEGRAL_INTERIOR_FACET, "fused": _lib.INTEGRAL_FUSED}
 
@@ -1497,6 +1512,8 @@ class GlobalKernel:
         d.alpha, d.beta = lk.alpha, lk.beta
         d.diagonal = int(lk.diagonal)
         d.affine_cells = int(lk.affine and lk.rank == 1 and not lk.diagonal)
+        for i in range(3):
+            d.dcoef[i] = lk.d[i]
         for q in range(el.nq):
             d.wq[q] = el.wq[q]
             d.xq[q] = el.xq[q]
@@ -1653,7 +1670,8 @@ class Parloop:
                 if not hasattr(it, "_dev_idx"):
                     it._dev_idx = DeviceArray.from_host(it.indices)
                 subset = it._dev_idx.ptr
-            # coordinates, then the coefficient field of a helmholtz_coef form
+            # coordinates, then the coefficient field of a helmholtz_coef form (the linearisation
+            # point of a nonlinear_diffusion_jacobian)
             ins = [a.data.device_ptr for a in self.args[1:]]
             try:
                 gk(start, end, layers, subset, [out.handle.value] + ins, None, None,

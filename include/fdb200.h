@@ -107,7 +107,7 @@ enum fdb_form {
                                    demos/helmholtz/helmholtz.py.rst:52-77,
                                    demos/matrix_free/poisson.py.rst:13-27        */
     FDB_FORM_DG_ADVECTION = 2,  /* demos/DG_advection/DG_advection.py.rst:182-217 */
-    FDB_FORM_HELMHOLTZ_COEF = 3 /* alpha*inner(kappa*grad u, grad v)*dx + beta*inner(u, v)*dx with a
+    FDB_FORM_HELMHOLTZ_COEF = 3, /* alpha*inner(kappa*grad u, grad v)*dx + beta*inner(u, v)*dx with a
                                    scalar coefficient FIELD kappa in the argument space, gathered
                                    through the same cell->node map (maps[0]); beta stays a constant.
                                    Heterogeneous materials, Newton Jacobians of nonlinear diffusion.
@@ -120,6 +120,25 @@ enum fdb_form {
                                      rank 2    [Mat, coords, kappa]
                                    Always the sum-factorised slab-thread kernel: the option
                                    "matrix_kernel" (DMMA element matrices) does not apply.       */
+    FDB_FORM_NONLINEAR_DIFFUSION = 4,
+                                /* residual of nonlinear diffusion, no source term:
+                                     F(u; v) = alpha*inner(D(u) grad u, grad v)*dx + beta*inner(u, v)*dx
+                                   D(s) = dcoef[0] + dcoef[1] s + dcoef[2] s^2, evaluated at each
+                                   Gauss point from the interpolated u.  Rank 1 action only (not rank
+                                   2, not diagonal):  [y INC, coords, u].  Hex cells, cdim == 1,
+                                   nq == degree+1, affine_cells == 0, degrees 1..5; atomic or
+                                   coloured scatter, device or host mode (host mode monolithic).   */
+    FDB_FORM_NONLINEAR_DIFFUSION_JACOBIAN = 5
+                                /* its Gateaux derivative at u (exact Newton Jacobian, NOT symmetric):
+                                     J(u)[w; v] = alpha*inner(D(u) grad w + D'(u) w grad u, grad v)*dx
+                                                  + beta*inner(w, v)*dx
+                                   Same restrictions as FDB_FORM_HELMHOLTZ_COEF, degrees 1..5
+                                   (action), 1..4 (rank 2), 1..3 (diagonal).  u is always the LAST
+                                   argument, gathered through maps[0]:
+                                     action    [y INC, coords, w, u]
+                                     diagonal  [d INC, coords, u]      (device mode)
+                                     rank 2    [Mat, coords, u]  (row = test dof, column = trial dof)
+                                   Never the DMMA element-matrix kernels (they assume symmetry).  */
 };
 
 enum fdb_cell {
@@ -179,6 +198,9 @@ typedef struct fdb_kernel_desc {
      * TSFC has no such path for tensor-product cells (their coordinate element is not affine,
      * tsfc/fem.py:793-797 unrolls only simplices); fdb_cells_are_affine() checks the promise. */
     int32_t affine_cells;
+    /* FDB_FORM_NONLINEAR_DIFFUSION[_JACOBIAN]: D(s) = dcoef[0] + dcoef[1] s + dcoef[2] s^2.
+     * Ignored by every other form (a zeroed descriptor stays valid for them). */
+    double dcoef[3];
 } fdb_kernel_desc;
 
 typedef struct fdb_kernel_s *fdb_kernel_t;
