@@ -19,6 +19,7 @@ FORM_DG_ADVECTION = 2
 FORM_HELMHOLTZ_COEF = 3
 FORM_NONLINEAR_DIFFUSION = 4
 FORM_NONLINEAR_DIFFUSION_JACOBIAN = 5
+FORM_ELASTICITY = 6
 CELL_HEX_EXTRUDED = 1
 CELL_HEX = 2
 CELL_TRIANGLE = 3
@@ -48,6 +49,7 @@ class KernelDesc(C.Structure):
         ("offset0", C.POINTER(C.c_int32)), ("offset1", C.POINTER(C.c_int32)),
         ("diagonal", C.c_int32), ("affine_cells", C.c_int32),
         ("dcoef", C.c_double * 3),
+        ("lmbda", C.c_double),
     ]
 
 

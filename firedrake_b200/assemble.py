@@ -11,7 +11,8 @@ Mirrors (same names / call protocol, thin Python over the engine):
 * ``firedrake.matrix_free.operators.ImplicitMatrixContext`` (operators.py:74-242)
 
 Forms are described by :class:`Form` (the Helmholtz family on a
-:class:`FunctionSpace`) instead of UFL: UFL/TSFC are not available here, and the
+:class:`FunctionSpace`), :class:`NonlinearDiffusion` and :class:`Elasticity` (linear elasticity on a
+vector space) instead of UFL: UFL/TSFC are not available here, and the
 engine keys its kernels on a form descriptor (DESIGN.md section 1).
 """
 from __future__ import annotations
@@ -365,6 +366,123 @@ def assemble_variable_coefficient(V: "FunctionSpace", kappa: op2.Dat, u: op2.Dat
     return tensor
 
 
+def elasticity_kernel(degree, mu, lmbda, beta=0.0, name="elasticity_action"):
+    """C source of the 1-form ``action(inner(sigma(u), grad(v))*dx + beta*inner(u, v)*dx, u)`` of linear
+    elasticity, ``sigma(u) = 2*mu*sym(grad(u)) + lmbda*tr(sym(grad(u)))*Identity(3)``, on the vector
+    Q_p (x) P_p space (3 components, AoS), written the way TSFC's spectral mode would and run through the
+    generic wrapper builder: the independent statement of the hand-written FDB_FORM_ELASTICITY kernel.
+    Arguments: y (INC), coords, u."""
+    from .fiat_lite import interval_element
+    from .codegen import CStringKernel
+    el = interval_element(degree)
+    n = degree + 1
+    tab = lambda a: "{" + ", ".join("{" + ", ".join(repr(float(v)) for v in r) + "}" for r in a) + "}"
+    vec = lambda a: "{" + ", ".join(repr(float(v)) for v in a) + "}"
+    code = f"""
+#define EN {n}
+#define END (EN * EN * EN)
+static const double EB[EN][EN] = {tab(el.B)};      /* EB[q][a] */
+static const double ED[EN][EN] = {tab(el.D)};      /* ED[q][a] */
+static const double EX[EN] = {vec(el.xq)};
+static const double EW[EN] = {vec(el.wq)};
+/* out = (T applied along direction dir) in;  tr = 0: out[q] = sum_a T[q][a] in[a];  tr = 1: transpose */
+static inline void el_apply(const double T[EN][EN], int dir, int tr, const double *in, double *out)
+{{
+    const int st = dir == 0 ? EN * EN : (dir == 1 ? EN : 1);
+    for (int i = 0; i < END; ++i) {{
+        const int k = (i / st) % EN, base = i - k * st;
+        double s = 0.0;
+        for (int a = 0; a < EN; ++a) s += (tr ? T[a][k] : T[k][a]) * in[base + a * st];
+        out[i] = s;
+    }}
+}}
+static inline void el_tensor(const double (*T0)[EN], const double (*T1)[EN], const double (*T2)[EN], int tr,
+                             const double *in, double *out)
+{{
+    double t1[END], t2[END];
+    el_apply(T0, 0, tr, in, t1);
+    el_apply(T1, 1, tr, t1, t2);
+    el_apply(T2, 2, tr, t2, out);
+}}
+static void {name}(double *y, const double *X, const double *u)
+{{
+    double U[3][END], G[3][3][END], c[END], t[END];
+    for (int d = 0; d < 3; ++d) {{
+        for (int i = 0; i < END; ++i) c[i] = u[i * 3 + d];
+        el_tensor(EB, EB, EB, 0, c, U[d]);
+        el_tensor(ED, EB, EB, 0, c, G[d][0]);
+        el_tensor(EB, ED, EB, 0, c, G[d][1]);
+        el_tensor(EB, EB, ED, 0, c, G[d][2]);
+    }}
+    for (int qx = 0; qx < EN; ++qx) for (int qy = 0; qy < EN; ++qy) for (int qz = 0; qz < EN; ++qz) {{
+        const int q = (qx * EN + qy) * EN + qz;
+        const double xi[3] = {{EX[qx], EX[qy], EX[qz]}};
+        double J[3][3] = {{{{0}}}};
+        for (int v = 0; v < 8; ++v) {{
+            const int b[3] = {{(v >> 2) & 1, (v >> 1) & 1, v & 1}};
+            for (int r = 0; r < 3; ++r) {{
+                double g = b[r] ? 1.0 : -1.0;
+                for (int e = 0; e < 3; ++e) if (e != r) g *= b[e] ? xi[e] : 1.0 - xi[e];
+                for (int k = 0; k < 3; ++k) J[k][r] += X[v * 3 + k] * g;
+            }}
+        }}
+        /* Jinv[m][k] = dxi_m/dx_k */
+        const double det = J[0][0] * (J[1][1] * J[2][2] - J[1][2] * J[2][1])
+                         - J[0][1] * (J[1][0] * J[2][2] - J[1][2] * J[2][0])
+                         + J[0][2] * (J[1][0] * J[2][1] - J[1][1] * J[2][0]);
+        double Jinv[3][3];
+        Jinv[0][0] = (J[1][1] * J[2][2] - J[1][2] * J[2][1]) / det;
+        Jinv[0][1] = (J[0][2] * J[2][1] - J[0][1] * J[2][2]) / det;
+        Jinv[0][2] = (J[0][1] * J[1][2] - J[0][2] * J[1][1]) / det;
+        Jinv[1][0] = (J[1][2] * J[2][0] - J[1][0] * J[2][2]) / det;
+        Jinv[1][1] = (J[0][0] * J[2][2] - J[0][2] * J[2][0]) / det;
+        Jinv[1][2] = (J[0][2] * J[1][0] - J[0][0] * J[1][2]) / det;
+        Jinv[2][0] = (J[1][0] * J[2][1] - J[1][1] * J[2][0]) / det;
+        Jinv[2][1] = (J[0][1] * J[2][0] - J[0][0] * J[2][1]) / det;
+        Jinv[2][2] = (J[0][0] * J[1][1] - J[0][1] * J[1][0]) / det;
+        const double wd = EW[qx] * EW[qy] * EW[qz] * fabs(det);
+        double Gp[3][3], S[3][3];
+        for (int d = 0; d < 3; ++d)
+            for (int k = 0; k < 3; ++k)
+                Gp[d][k] = G[d][0][q] * Jinv[0][k] + G[d][1][q] * Jinv[1][k] + G[d][2][q] * Jinv[2][k];
+        const double tr = Gp[0][0] + Gp[1][1] + Gp[2][2];
+        for (int d = 0; d < 3; ++d)
+            for (int k = 0; k < 3; ++k)
+                S[d][k] = {float(mu)!r} * (Gp[d][k] + Gp[k][d]) + (d == k ? {float(lmbda)!r} * tr : 0.0);
+        for (int d = 0; d < 3; ++d) {{
+            for (int m = 0; m < 3; ++m)
+                G[d][m][q] = wd * (Jinv[m][0] * S[d][0] + Jinv[m][1] * S[d][1] + Jinv[m][2] * S[d][2]);
+            U[d][q] *= {float(beta)!r} * wd;
+        }}
+    }}
+    for (int d = 0; d < 3; ++d) {{
+        el_tensor(EB, EB, EB, 1, U[d], c);
+        el_tensor(ED, EB, EB, 1, G[d][0], t);  for (int i = 0; i < END; ++i) c[i] += t[i];
+        el_tensor(EB, ED, EB, 1, G[d][1], t);  for (int i = 0; i < END; ++i) c[i] += t[i];
+        el_tensor(EB, EB, ED, 1, G[d][2], t);  for (int i = 0; i < END; ++i) c[i] += t[i];
+        for (int i = 0; i < END; ++i) y[i * 3 + d] += c[i];
+    }}
+}}
+#undef END
+#undef EN
+"""
+    return CStringKernel(code, name)
+
+
+def assemble_elasticity_generic(V: "FunctionSpace", u: op2.Dat, mu, lmbda, beta=0.0, tensor=None):
+    """``assemble(action(a, u))`` of linear elasticity through the generic wrapper path
+    (:func:`elasticity_kernel`): the cross-check and the baseline of :class:`Elasticity`."""
+    if V.cdim != 3:
+        raise ValueError("elasticity needs a vector space with 3 components")
+    if tensor is None:
+        tensor = V.dat()
+    tensor.zero()
+    tensor.device_ptr
+    op2.par_loop(elasticity_kernel(V.degree, mu, lmbda, beta), V.cell_set, tensor(op2.INC, V.cell_node_map),
+                 V.coordinates(op2.READ, V.coord_map), u(op2.READ, V.cell_node_map))
+    return tensor
+
+
 def assemble_functional(V: "FunctionSpace", f: op2.Dat, measure="dx", integrand="avg"):
     """``assemble(f*dx)`` / ``assemble(f*ds_b)`` / ``ds_t`` / ``ds_v`` / ``ds`` for a scalar
     ``f`` in V: rank-0 parloops with a Global INC argument (firedrake/assemble.py
@@ -565,6 +683,34 @@ class NonlinearDiffusionJacobian:
                           rank=rank, diagonal=diagonal, d=tuple(self.d))
 
 
+@dataclass
+class Elasticity:
+    """Linear elasticity on a vector space ``V`` (``cdim = 3``):
+
+        a(u, v) = inner(sigma(u), grad(v))*dx + beta*inner(u, v)*dx,
+        sigma(u) = 2*mu*sym(grad(u)) + lmbda*tr(sym(grad(u)))*Identity(3)
+
+    A symmetric bilinear form whose element matrices couple the three components.  It works with
+    ``assemble(F, u=w)`` (action, degrees 1..4), ``assemble(F)`` (a blocked aij Mat of block size 3,
+    degrees 1..3), ``assemble(F, mat_type="matfree")`` and :func:`solve` with ``pc_type`` "none",
+    "jacobi" or "mg" (the coarse operators are ``Elasticity(W, mu, lmbda, beta)`` on the coarser
+    levels).  Dirichlet conditions constrain every component of their nodes."""
+    V: FunctionSpace
+    mu: float
+    lmbda: float
+    beta: float = 0.0
+    symmetric = True
+
+    def coefficient_args(self):
+        return []
+
+    def kernel(self, rank, diagonal=False):
+        if self.V.cdim != 3:
+            raise ValueError("elasticity needs a vector space with 3 components")
+        return op2.Kernel("elasticity", degree=self.V.degree, mu=self.mu, lmbda=self.lmbda, beta=self.beta,
+                          rank=rank, diagonal=diagonal, cdim=3)
+
+
 def poisson(V):
     return Form(V, 1.0, 0.0)
 
@@ -689,8 +835,9 @@ class ImplicitMatrixContext:
         """``assemble(a, diagonal=True)`` then 1 on the constrained rows
         (matrix_free/operators.py:199-205; firedrake/assemble.py:1226-1241)."""
         V = self.form.V
-        if self.form.coefficient_args():
-            # coefficient forms (kappa, a Jacobian's linearisation point) have their own diagonal kernel
+        if self.form.coefficient_args() or not isinstance(self.form, Form):
+            # coefficient forms (kappa, a Jacobian's linearisation point) and elasticity have their own
+            # diagonal kernel
             k = self.form.kernel(1, diagonal=True)
         else:
             k = op2.Kernel("helmholtz", degree=V.degree, alpha=self.form.alpha, beta=self.form.beta,
@@ -1008,7 +1155,8 @@ def solve_nonlinear(F: NonlinearDiffusion, L: op2.Dat, u: op2.Dat, bcs=(), solve
 def solve(form: Form, L: op2.Dat, u: op2.Dat, bcs=(), solver_parameters=None, hierarchy=None, allreduce=None):
     """``solve(a == L, u, bcs=bcs, solver_parameters=...)`` for the supported forms
     (firedrake/solving.py:128-260 -> LinearVariationalSolver; SURVEY.md section 3.5): assemble the
-    operator, lift the Dirichlet values, run the Krylov solver on the device.
+    operator, lift the Dirichlet values, run the Krylov solver on the device.  ``form``: a
+    :class:`Form` or an :class:`Elasticity` form (vector space; Dirichlet values on every component).
 
     ``L``: the assembled right-hand side (a Dat, e.g. ``assemble(mass(V), u=f)``).
     ``solver_parameters`` (PETSc option names, the subset that makes sense here):
@@ -1049,8 +1197,7 @@ def solve(form: Form, L: op2.Dat, u: op2.Dat, bcs=(), solver_parameters=None, hi
         if pc == "jacobi":
             ctx = A if isinstance(A, ImplicitMatrixContext) else ImplicitMatrixContext(form, bcs)
             d = ctx.getDiagonal(V.dat())
-            op2.par_loop(op2.Kernel("static void recip(double *w) { *w = 1.0 / *w; }", "recip"), V.node_set,
-                         d(op2.RW))
+            op2.par_loop(_mg.reciprocal_kernel(V.cdim), V.node_set, d(op2.RW))
 
             def M(r, z):
                 _lib.check(lib.fdb_vec_pointwise_mult(n, r.device_ptr, d.device_ptr, z.device_ptr))
@@ -1061,9 +1208,18 @@ def solve(form: Form, L: op2.Dat, u: op2.Dat, bcs=(), solver_parameters=None, hi
             # with a coefficient field, every coarser level gets the injection of the next finer
             # level's kappa (VCycle's ``kappa``), as Firedrake coarsens coefficients for rediscretised
             # multigrid
-            vc = _mg.VCycle(hierarchy, V.degree, lambda W, k=None: Form(W, form.alpha, form.beta, k),
+            # elasticity: the Jacobi smoother's damping is 0.6, not 0.8.  The spectrum of D^-1 A of the coupled
+            # operator reaches past 2 / 0.8, so 0.8 amplifies its highest modes: CG1 at nu = 0.3 took 16 and
+            # 97 iterations on 8^3 and 16^3 with 0.8, 8 and 9 with 0.6 (DESIGN.md section 4.8)
+            if isinstance(form, Elasticity):
+                make = lambda W, k=None: Elasticity(W, form.mu, form.lmbda, form.beta)
+                omega = 0.6
+            else:
+                make = lambda W, k=None: Form(W, form.alpha, form.beta, k)
+                omega = 0.8
+            vc = _mg.VCycle(hierarchy, V.degree, make,
                             bc_domains=tuple(s for bc in bcs for s in bc.sub_domains), allreduce=allreduce,
-                            kappa=form.kappa)
+                            kappa=getattr(form, "kappa", None), cdim=V.cdim, omega=omega)
             top = len(hierarchy) - 1
             M = lambda r, z: vc.apply(top, r, z)
         else:

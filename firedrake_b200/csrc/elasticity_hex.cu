@@ -1,0 +1,422 @@
+// FDB_FORM_ELASTICITY: linear elasticity on vector (cdim = 3) Q_p (x) P_p hexahedra,
+//     a(u, v) = inner(sigma(u), grad v)*dx + beta*inner(u, v)*dx,
+//     sigma(u) = mu (grad u + grad u^T) + lmbda tr(grad u) I
+// (mu = desc.alpha, lmbda = desc.lmbda).  The first form of the engine whose element tensor couples
+// the components: the stress at a Gauss point needs the full 3 x 3 physical gradient, so the three
+// components cannot run through the slab-thread pipeline of action_hex.cu one after the other.
+//
+// Layout (DESIGN.md section 4.8): one thread per Gauss point, CPB cells ("slots") per CTA.  Per slot the
+// CTA keeps in shared memory the 8 vertices, the three components' values at the points (S_U), a work
+// buffer (S_T) and the nine reference fluxes (S_F, also the second work buffer of the sum-factorised
+// passes).  Per unit:
+//   gather u (AoS, three components)  ->  B (x) B (x) B, one axis per pass (three passes through S_T/S_F)
+//   point: reference gradients of the three components by collocated differentiation (Dt = D B^{-1})
+//          of S_U, geometry from the trilinear vertex field, G = ghat J^{-1}, sigma, the fluxes
+//          fhat_d = w |det J| J^{-1} sigma_d into S_F and the mass term beta w |det J| u_d
+//   Dt^T of the fluxes plus the mass term at the points, then B^T along each axis, and the scatter.
+// The point stage holds the geometry once for the three components.
+//
+// MATRIX: one unit per trial dof (node j, component b) of a cell (3 N^3 units per cell); its gathered
+// values are the unit vector e_(j,b), and the thread of test node i scatters entries (i, a; j, b),
+// a = 0..2, into the 3 x 3 block at the node pair's CSR position (row-major inside the block).  Entries
+// whose dof-level lgmap index is negative are dropped.  With vals == NULL the kernel adds the
+// diagonal entry (j, b; j, b) into diag[3 j + b] instead.
+#include "common.cuh"
+
+namespace {
+
+template <int N>
+struct ElasParams {
+    double *y;                   // action / diagonal output (AoS, 3 per node)
+    const double *x;             // action input (AoS)
+    const double *coords;        // AoS, 3 per vertex
+    const fdb_int *map0, *map1;  // node map (ND per column / cell), vertex map (8)
+    const fdb_int *off0, *off1;  // layer offsets (zeros for native hexes)
+    const fdb_int *collist;      // columns to visit (subset / colour) or NULL = col0 + i
+    int col0, ncols;
+    int nlay_items, lay_first, lay_step;   // layers lay_first + lay_step * k, k < nlay_items
+    double mu, lmbda, beta;
+    double B[N * N], Dt[N * N], wq[N];
+    double xq[N];
+    // MATRIX
+    const long long *rowptr;
+    const fdb_int *colidx;
+    double *vals;                // NULL: diagonal into y
+    const fdb_int *row_lg, *col_lg;   // dof-level, NULL = identity
+    const unsigned short *rank_tab;
+    int nvar, nlay_total;
+};
+
+template <int N>
+struct ElasShape {
+    static constexpr int ND = N * N * N;
+    static constexpr int CPB = (256 / ND) > 0 ? 256 / ND : 1;          // cells (slots) per CTA
+    static constexpr int THREADS = ((CPB * ND + 31) / 32) * 32;
+    // doubles per slot: vertices, values at the points, work buffer, fluxes (9 per point)
+    static constexpr int SLOT = 24 + 3 * ND + 3 * ND + 9 * ND;
+    static constexpr size_t SMEM = (size_t)CPB * SLOT * sizeof(double) + (size_t)CPB * ND * sizeof(int);
+};
+
+// out[i][j][k] (one value per thread, the thread's (i, j, k)) = sum_a T[a-index along `axis`] in[...]:
+// tr = false: T[q][a] applied to the a-index (dofs -> points); tr = true: T^T (points -> dofs)
+template <int N, int AXIS, bool TR>
+__device__ __forceinline__ double pass1(const double *__restrict__ T, const double *in, int i, int j, int k)
+{
+    constexpr int ST = AXIS == 0 ? N * N : (AXIS == 1 ? N : 1);
+    const int o = AXIS == 0 ? i : (AXIS == 1 ? j : k);
+    const int base = (i * N + j) * N + k - o * ST;
+    double s = 0.0;
+#pragma unroll
+    for (int a = 0; a < N; a++) s = fma(TR ? T[a * N + o] : T[o * N + a], in[base + a * ST], s);
+    return s;
+}
+
+template <int N, bool MATRIX, bool ATOMIC>
+__global__ void __launch_bounds__(ElasShape<N>::THREADS)
+elasticity_kernel(const __grid_constant__ ElasParams<N> P)
+{
+    using S = ElasShape<N>;
+    constexpr int ND = S::ND;
+    constexpr int CPB = S::CPB;
+    extern __shared__ __align__(16) unsigned char smem_raw[];
+    const int slot = threadIdx.x / ND;
+    const int l = threadIdx.x - slot * ND;                 // this thread's dof / point in the cell
+    const bool in_cta = slot < CPB;
+    const int sl = in_cta ? slot : 0;
+    double *sb = reinterpret_cast<double *>(smem_raw) + (size_t)sl * S::SLOT;
+    double *s_x = sb;                                      // [8][3]
+    double *s_u = s_x + 24;                                // [3][ND]
+    double *s_t = s_u + 3 * ND;                            // [3][ND]
+    double *s_f = s_t + 3 * ND;                            // [3 d][3 m][ND]
+    int *s_idx = reinterpret_cast<int *>(reinterpret_cast<double *>(smem_raw) + (size_t)CPB * S::SLOT) + sl * ND;
+    const int qi = l / (N * N), qj = (l / N) % N, qk = l % N;
+
+    const long long ncells = (long long)P.ncols * P.nlay_items;
+    const long long nunits = MATRIX ? ncells * 3 * ND : ncells;
+    for (long long base = (long long)blockIdx.x * CPB; base < nunits; base += (long long)gridDim.x * CPB) {
+        const long long unit = base + slot;
+        const bool valid = in_cta && unit < nunits;
+        const long long cell = MATRIX ? unit / (3 * ND) : unit;
+        const int jb = MATRIX ? (int)(unit - cell * 3 * ND) : 0;   // trial dof: node jb / 3, component jb % 3
+        int col = 0, layer = 0;
+        if (valid) {
+            const int ci = (int)(cell / P.nlay_items);
+            layer = P.lay_first + P.lay_step * (int)(cell - (long long)ci * P.nlay_items);
+            col = P.collist ? __ldg(P.collist + ci) : P.col0 + ci;
+        }
+        // ---- gather: node index, values (or the unit vector), vertices
+        int g = 0;
+        if (valid) {
+            g = __ldg(P.map0 + (long long)col * ND + l) + __ldg(P.off0 + l) * layer;
+            s_idx[l] = g;
+#pragma unroll
+            for (int d = 0; d < 3; d++)
+                s_u[d * ND + l] = MATRIX ? ((jb == 3 * l + d) ? 1.0 : 0.0) : __ldg(P.x + (long long)g * 3 + d);
+            for (int i = l; i < 24; i += ND) {
+                const int v = i / 3, a = i - 3 * v;
+                const int gv = __ldg(P.map1 + (long long)col * 8 + v) + __ldg(P.off1 + v) * layer;
+                s_x[i] = __ldg(P.coords + (long long)gv * 3 + a);
+            }
+        } else if (in_cta) {
+            // idle slot: the unit cube with zero values keeps the point stage finite
+#pragma unroll
+            for (int d = 0; d < 3; d++) s_u[d * ND + l] = 0.0;
+            for (int i = l; i < 24; i += ND) s_x[i] = (double)(((i / 3) >> (2 - i % 3)) & 1);
+        }
+        __syncthreads();
+        // ---- forward: values at the points, x then y then z (S_U -> S_T -> S_F -> S_U)
+        if (in_cta) {
+#pragma unroll
+            for (int d = 0; d < 3; d++) s_t[d * ND + l] = pass1<N, 0, false>(P.B, s_u + d * ND, qi, qj, qk);
+        }
+        __syncthreads();
+        if (in_cta) {
+#pragma unroll
+            for (int d = 0; d < 3; d++) s_f[d * ND + l] = pass1<N, 1, false>(P.B, s_t + d * ND, qi, qj, qk);
+        }
+        __syncthreads();
+        if (in_cta) {
+#pragma unroll
+            for (int d = 0; d < 3; d++) s_u[d * ND + l] = pass1<N, 2, false>(P.B, s_f + d * ND, qi, qj, qk);
+        }
+        __syncthreads();
+        // ---- point stage
+        double mres[3] = {0.0, 0.0, 0.0};
+        if (in_cta) {
+            double gh[3][3];                               // gh[d][m] = d u_d / d xi_m
+#pragma unroll
+            for (int d = 0; d < 3; d++) {
+                gh[d][0] = pass1<N, 0, false>(P.Dt, s_u + d * ND, qi, qj, qk);
+                gh[d][1] = pass1<N, 1, false>(P.Dt, s_u + d * ND, qi, qj, qk);
+                gh[d][2] = pass1<N, 2, false>(P.Dt, s_u + d * ND, qi, qj, qk);
+            }
+            // J[c][r] = d x_c / d xi_r of the trilinear vertex field (vertex (bx*2 + by)*2 + bz)
+            const double xi[3] = {P.xq[qi], P.xq[qj], P.xq[qk]};
+            double J[3][3];
+#pragma unroll
+            for (int c = 0; c < 3; c++)
+#pragma unroll
+                for (int r = 0; r < 3; r++) J[c][r] = 0.0;
+#pragma unroll
+            for (int v = 0; v < 8; v++) {
+                const int b[3] = {(v >> 2) & 1, (v >> 1) & 1, v & 1};
+                double dphi[3];
+#pragma unroll
+                for (int r = 0; r < 3; r++) {
+                    double s = b[r] ? 1.0 : -1.0;
+#pragma unroll
+                    for (int e = 0; e < 3; e++)
+                        if (e != r) s *= b[e] ? xi[e] : 1.0 - xi[e];
+                    dphi[r] = s;
+                }
+#pragma unroll
+                for (int c = 0; c < 3; c++) {
+                    const double X = s_x[v * 3 + c];
+#pragma unroll
+                    for (int r = 0; r < 3; r++) J[c][r] = fma(X, dphi[r], J[c][r]);
+                }
+            }
+            // cofactor rows: R[m] . J[:, r] = det * delta_mr, so J^{-1}[m][c] = R[m][c] / det
+            double R[3][3];
+            R[0][0] = J[1][1] * J[2][2] - J[2][1] * J[1][2];
+            R[0][1] = J[2][1] * J[0][2] - J[0][1] * J[2][2];
+            R[0][2] = J[0][1] * J[1][2] - J[1][1] * J[0][2];
+            R[1][0] = J[1][2] * J[2][0] - J[2][2] * J[1][0];
+            R[1][1] = J[2][2] * J[0][0] - J[0][2] * J[2][0];
+            R[1][2] = J[0][2] * J[1][0] - J[1][2] * J[0][0];
+            R[2][0] = J[1][0] * J[2][1] - J[2][0] * J[1][1];
+            R[2][1] = J[2][0] * J[0][1] - J[0][0] * J[2][1];
+            R[2][2] = J[0][0] * J[1][1] - J[1][0] * J[0][1];
+            const double det = J[0][0] * R[0][0] + J[1][0] * R[0][1] + J[2][0] * R[0][2];
+            const double rdet = 1.0 / det;
+            const double w = P.wq[qi] * P.wq[qj] * P.wq[qk];
+            // physical gradient G[d][k] = sum_m gh[d][m] J^{-1}[m][k]
+            double G[3][3];
+#pragma unroll
+            for (int d = 0; d < 3; d++)
+#pragma unroll
+                for (int k = 0; k < 3; k++)
+                    G[d][k] = (gh[d][0] * R[0][k] + gh[d][1] * R[1][k] + gh[d][2] * R[2][k]) * rdet;
+            const double ltr = P.lmbda * (G[0][0] + G[1][1] + G[2][2]);
+            // fhat_d[m] = w |det| sum_k J^{-1}[m][k] sigma[d][k] = (w |det| / det) sum_k R[m][k] sigma[d][k]
+            const double sw = w * fabs(det) * rdet;
+#pragma unroll
+            for (int d = 0; d < 3; d++) {
+                double sg[3];
+#pragma unroll
+                for (int k = 0; k < 3; k++) sg[k] = P.mu * (G[d][k] + G[k][d]) + (k == d ? ltr : 0.0);
+#pragma unroll
+                for (int m = 0; m < 3; m++)
+                    s_f[(d * 3 + m) * ND + l] = sw * (R[m][0] * sg[0] + R[m][1] * sg[1] + R[m][2] * sg[2]);
+                mres[d] = P.beta * w * fabs(det) * s_u[d * ND + l];
+            }
+        }
+        __syncthreads();
+        // ---- backward: Dt^T of the fluxes plus the mass term at the points, then B^T along z, y, x
+        if (in_cta) {
+#pragma unroll
+            for (int d = 0; d < 3; d++) {
+                const double *f = s_f + d * 3 * ND;
+                s_t[d * ND + l] = mres[d] + pass1<N, 0, true>(P.Dt, f, qi, qj, qk) +
+                                  pass1<N, 1, true>(P.Dt, f + ND, qi, qj, qk) +
+                                  pass1<N, 2, true>(P.Dt, f + 2 * ND, qi, qj, qk);
+            }
+        }
+        __syncthreads();
+        if (in_cta) {
+#pragma unroll
+            for (int d = 0; d < 3; d++) s_u[d * ND + l] = pass1<N, 2, true>(P.B, s_t + d * ND, qi, qj, qk);
+        }
+        __syncthreads();
+        if (in_cta) {
+#pragma unroll
+            for (int d = 0; d < 3; d++) s_t[d * ND + l] = pass1<N, 1, true>(P.B, s_u + d * ND, qi, qj, qk);
+        }
+        __syncthreads();
+        double out[3];
+        if (in_cta) {
+#pragma unroll
+            for (int d = 0; d < 3; d++) out[d] = pass1<N, 0, true>(P.B, s_t + d * ND, qi, qj, qk);
+        }
+        // ---- scatter (this thread's node, three components)
+        if (valid) {
+            if (!MATRIX) {
+                double *dst = P.y + (long long)g * 3;
+#pragma unroll
+                for (int a = 0; a < 3; a++) {
+                    if (ATOMIC) atomicAdd(dst + a, out[a]);
+                    else dst[a] += out[a];
+                }
+            } else {
+                const int j = jb / 3, b = jb - 3 * (jb / 3);
+                if (P.vals == nullptr) {
+                    if (l == j) atomicAdd(P.y + (long long)g * 3 + b, b == 0 ? out[0] : (b == 1 ? out[1] : out[2]));
+                } else {
+                    const int gj = s_idx[j];
+                    if (!P.col_lg || __ldg(P.col_lg + (long long)gj * 3 + b) >= 0) {
+                        long long lo = __ldg(P.rowptr + g);
+                        if (P.rank_tab) {
+                            const int v = P.nlay_total < 3 ? layer
+                                                           : (layer == 0 ? 0 : (layer == P.nlay_total - 1 ? 2 : 1));
+                            lo += __ldg(P.rank_tab + (((long long)col * P.nvar + v) * ND + j) * ND + l);
+                        } else {
+                            long long hi = __ldg(P.rowptr + g + 1);
+                            while (hi - lo > 1) {
+                                const long long mid = (lo + hi) >> 1;
+                                if (__ldg(P.colidx + mid) <= gj) lo = mid; else hi = mid;
+                            }
+                        }
+#pragma unroll
+                        for (int a = 0; a < 3; a++) {
+                            if (P.row_lg && __ldg(P.row_lg + (long long)g * 3 + a) < 0) continue;
+                            atomicAdd(P.vals + (lo * 3 + a) * 3 + b, out[a]);
+                        }
+                    }
+                }
+            }
+        }
+        __syncthreads();          // the slot's buffers are refilled by the next unit
+    }
+}
+
+template <int N, bool MATRIX, bool ATOMIC>
+int launch(cudaStream_t st, const ElasParams<N> &P, int sm_count)
+{
+    using S = ElasShape<N>;
+    auto kern = elasticity_kernel<N, MATRIX, ATOMIC>;
+    static bool attr = false;
+    if (!attr) {
+        FDB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)S::SMEM));
+        attr = true;
+    }
+    int per_sm = 0;
+    FDB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, S::THREADS, S::SMEM));
+    const long long ncells = (long long)P.ncols * P.nlay_items;
+    const long long nunits = MATRIX ? ncells * 3 * S::ND : ncells;
+    long long grid = (nunits + S::CPB - 1) / S::CPB;
+    const long long cap = (long long)sm_count * (per_sm > 0 ? per_sm : 1);
+    if (grid > cap) grid = cap;
+    if (grid < 1) return 0;
+    kern<<<(int)grid, S::THREADS, S::SMEM, st>>>(P);
+    FDB_LAUNCH_CHECK();
+    return 0;
+}
+
+template <int N>
+void fill_tables(const fdb_kernel_s *k, ElasParams<N> &P)
+{
+    P.off0 = k->d_off0;
+    P.off1 = k->d_off1;
+    P.mu = k->desc.alpha;
+    P.lmbda = k->desc.lmbda;
+    P.beta = k->desc.beta;
+    for (int i = 0; i < N * N; i++) {
+        P.B[i] = k->desc.B[i];
+        P.Dt[i] = k->Dt[i];
+    }
+    for (int i = 0; i < N; i++) {
+        P.wq[i] = k->desc.wq[i];
+        P.xq[i] = k->desc.xq[i];
+    }
+}
+
+template <int N>
+int action_n(fdb_kernel_s *k, fdb_int start, fdb_int end, int nlay, const fdb_int *subset, double *y,
+             const double *coords, const double *x, const fdb_int *map0, const fdb_int *map1)
+{
+    fdb::Context &c = fdb::ctx();
+    ElasParams<N> P;
+    memset(&P, 0, sizeof(P));
+    fill_tables(k, P);
+    P.y = y;
+    P.x = x;
+    P.coords = coords;
+    P.map0 = map0;
+    P.map1 = map1;
+    if (k->desc.scatter == FDB_SCATTER_ATOMIC) {
+        P.collist = subset;
+        P.col0 = start;
+        P.ncols = end - start;
+        P.nlay_items = nlay;
+        P.lay_first = 0;
+        P.lay_step = 1;
+        if (P.ncols <= 0 || nlay <= 0) return 0;
+        return launch<N, false, true>(c.stream, P, c.sm_count);
+    }
+    // deterministic: one launch per (colour, layer parity), no two cells of a launch share a node
+    if (subset) {
+        fdb::set_error("coloured scatter does not support subsets yet");
+        return 1;
+    }
+    for (int col = 0; col < k->ncolours; col++) {
+        P.collist = k->d_colour_cols + k->colour_start[col];
+        P.col0 = 0;
+        P.ncols = k->colour_start[col + 1] - k->colour_start[col];
+        for (int par = 0; par < (nlay > 1 ? 2 : 1); par++) {
+            P.lay_first = par;
+            P.lay_step = 2;
+            P.nlay_items = (nlay - par + 1) / 2;
+            if (P.ncols <= 0 || P.nlay_items <= 0) continue;
+            if (launch<N, false, false>(c.stream, P, c.sm_count)) return 1;
+        }
+    }
+    return 0;
+}
+
+template <int N>
+int matrix_n(fdb_kernel_s *k, fdb_int start, fdb_int end, int nlay, const fdb_int *subset, fdb_mat_t mat,
+             const double *coords, const fdb_int *map0, const fdb_int *map1, double *diag_out)
+{
+    fdb::Context &c = fdb::ctx();
+    ElasParams<N> P;
+    memset(&P, 0, sizeof(P));
+    fill_tables(k, P);
+    P.coords = coords;
+    P.map0 = map0;
+    P.map1 = map1;
+    if (mat) {
+        if (fdb_mat_device_view(mat, &P.rowptr, &P.colidx, &P.vals, &P.row_lg, &P.col_lg)) return 1;
+        fdb_mat_rank_table(mat, &P.rank_tab, &P.nvar);
+    } else {
+        P.y = diag_out;
+    }
+    P.nlay_total = nlay;
+    if (subset || k->desc.cell != FDB_CELL_HEX_EXTRUDED) P.rank_tab = nullptr;   // table is per column of the full set
+    P.collist = subset;
+    P.col0 = start;
+    P.ncols = end - start;
+    P.nlay_items = nlay;
+    P.lay_first = 0;
+    P.lay_step = 1;
+    if (P.ncols <= 0 || nlay <= 0) return 0;
+    return launch<N, true, true>(c.stream, P, c.sm_count);
+}
+
+}  // namespace
+
+int fdb_launch_elasticity_action(fdb_kernel_s *k, fdb_int start, fdb_int end, int nlay, const fdb_int *subset,
+                                 double *y, const double *coords, const double *x, const fdb_int *map0,
+                                 const fdb_int *map1)
+{
+    switch (k->n1d) {
+    case 2: return action_n<2>(k, start, end, nlay, subset, y, coords, x, map0, map1);
+    case 3: return action_n<3>(k, start, end, nlay, subset, y, coords, x, map0, map1);
+    case 4: return action_n<4>(k, start, end, nlay, subset, y, coords, x, map0, map1);
+    case 5: return action_n<5>(k, start, end, nlay, subset, y, coords, x, map0, map1);
+    }
+    fdb::set_error("elasticity action: degree %d not instantiated (1..4)", k->n1d - 1);
+    return 1;
+}
+
+int fdb_launch_elasticity_matrix(fdb_kernel_s *k, fdb_int start, fdb_int end, int nlay, const fdb_int *subset,
+                                 fdb_mat_t mat, const double *coords, const fdb_int *map0, const fdb_int *map1,
+                                 double *diag_out)
+{
+    switch (k->n1d) {
+    case 2: return matrix_n<2>(k, start, end, nlay, subset, mat, coords, map0, map1, diag_out);
+    case 3: return matrix_n<3>(k, start, end, nlay, subset, mat, coords, map0, map1, diag_out);
+    case 4: return matrix_n<4>(k, start, end, nlay, subset, mat, coords, map0, map1, diag_out);
+    }
+    fdb::set_error("elasticity matrix: degree %d not instantiated (1..3)", k->n1d - 1);
+    return 1;
+}

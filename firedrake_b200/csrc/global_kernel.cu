@@ -302,6 +302,31 @@ int fdb_kernel_create(const fdb_kernel_desc *d, fdb_kernel_t *out)
                       d->rank == 2 ? "matrix" : (d->diagonal ? "diagonal" : "action"), d->degree, maxdeg);
             return 1;
         }
+    } else if (d->form == FDB_FORM_ELASTICITY) {
+        // coupled vector form: elasticity_hex.cu (never the DMMA element-matrix kernels)
+        if (d->cell != FDB_CELL_HEX_EXTRUDED && d->cell != FDB_CELL_HEX) {
+            set_error("fdb_kernel_create: elasticity needs hex cells (extruded or native), got cell %d", d->cell);
+            return 1;
+        }
+        if (d->cdim != 3) {
+            set_error("fdb_kernel_create: elasticity needs a vector space of value size 3 (cdim %d)", d->cdim);
+            return 1;
+        }
+        if (d->affine_cells) {
+            set_error("fdb_kernel_create: elasticity has no affine-cell variant (affine_cells must be 0)");
+            return 1;
+        }
+        if (d->nq != d->degree + 1) {
+            set_error("fdb_kernel_create: elasticity needs nq == degree+1 Gauss points per axis (got nq=%d for "
+                      "degree %d)", d->nq, d->degree);
+            return 1;
+        }
+        const int maxdeg = (d->rank == 2 || d->diagonal) ? 3 : 4;
+        if (d->degree < 1 || d->degree > maxdeg) {
+            set_error("fdb_kernel_create: elasticity %s: degree %d outside 1..%d",
+                      d->rank == 2 ? "matrix" : (d->diagonal ? "diagonal" : "action"), d->degree, maxdeg);
+            return 1;
+        }
     } else if (d->form != FDB_FORM_HELMHOLTZ) {
         set_error("fdb_kernel_create: form %d is not in the supported set", d->form);
         return 1;
@@ -444,6 +469,7 @@ int fdb_kernel_call(fdb_kernel_t k, const fdb_call_args *a)
     const bool nl_jac = k->desc.form == FDB_FORM_NONLINEAR_DIFFUSION_JACOBIAN;
     const bool coef = k->desc.form == FDB_FORM_HELMHOLTZ_COEF || nl_jac;
     const bool nl_res = k->desc.form == FDB_FORM_NONLINEAR_DIFFUSION;
+    const bool elas = k->desc.form == FDB_FORM_ELASTICITY;
     const char *cname = nl_jac ? "nonlinear_diffusion_jacobian" : "helmholtz_coef";
     const char *cvar = nl_jac ? "u" : "kappa";
     if (coef && k->desc.rank == 2) {
@@ -537,6 +563,9 @@ int fdb_kernel_call(fdb_kernel_t k, const fdb_call_args *a)
             dm[0] = a->maps[0];
             dm[1] = a->maps[1];
         }
+        if (elas)
+            return fdb_launch_elasticity_matrix(k, a->start, a->end, nlay, dsub, target, dcoords, dm[0], dm[1],
+                                                nullptr);
         if (mat_bs == 1)
             return fdb_launch_helmholtz_matrix(k, a->start, a->end, nlay, dsub, target, dcoords, dm[0], dm[1],
                                                nullptr);
@@ -558,6 +587,16 @@ int fdb_kernel_call(fdb_kernel_t k, const fdb_call_args *a)
         return fdb_launch_helmholtz_coef_matrix(k, a->start, a->end, nlay, a->subset, nullptr,
                                                 (const double *)a->args[1], (const double *)a->args[2],
                                                 a->maps[0], a->maps[1], (double *)a->args[0]);
+    }
+    if (elas && k->desc.diagonal) {
+        // args = [d (INC, 3 values per node), coords]; device-resident only
+        if (a->nargs != 2 || a->nmaps != 2 || a->location != FDB_LOC_DEVICE) {
+            set_error("fdb_kernel_call: elasticity diagonal expects 2 device args (d, coords) and 2 maps");
+            return 1;
+        }
+        return fdb_launch_elasticity_matrix(k, a->start, a->end, nlay, a->subset, nullptr,
+                                            (const double *)a->args[1], a->maps[0], a->maps[1],
+                                            (double *)a->args[0]);
     }
     if (k->desc.diagonal) {
         // args = [d (INC), coords]; device-resident only
@@ -583,8 +622,8 @@ int fdb_kernel_call(fdb_kernel_t k, const fdb_call_args *a)
         return 1;
     }
     // the pipelined host action moves x and y only and runs the constant-coefficient kernels: the
-    // coefficient and nonlinear forms take the monolithic path
-    if (!coef && !nl_res && a->location == FDB_LOC_HOST && a->arg_versions && a->arg_bytes && a->map_bytes &&
+    // coefficient, nonlinear and elasticity forms take the monolithic path
+    if (!coef && !nl_res && !elas && a->location == FDB_LOC_HOST && a->arg_versions && a->arg_bytes && a->map_bytes &&
         a->writeback && a->output_is_zero && !a->subset && extruded &&
         k->desc.scatter == FDB_SCATTER_ATOMIC) {
         int rc = pipelined_host_action(k, a, nlay);
@@ -646,7 +685,10 @@ int fdb_kernel_call(fdb_kernel_t k, const fdb_call_args *a)
         return 1;
     }
     // (the residual: the coefficient entry point without a coefficient, see action_hex.cu)
-    int rc = (coef || nl_res)
+    int rc = elas ? fdb_launch_elasticity_action(k, a->start, a->end, nlay, dsubset, (double *)dargs[0],
+                                                 (const double *)dargs[1], (const double *)dargs[2], dmaps[0],
+                                                 dmaps[1])
+             : (coef || nl_res)
                  ? fdb_launch_helmholtz_coef_action(k, a->start, a->end, nlay, dsubset, (double *)dargs[0],
                                                     (const double *)dargs[1], (const double *)dargs[2],
                                                     coef ? (const double *)dargs[3] : nullptr, dmaps[0], dmaps[1])

@@ -237,6 +237,15 @@ def inject(fine, coarse, manager):
     return manager.inject(fine, coarse)
 
 
+def reciprocal_kernel(cdim=1):
+    """Node kernel inverting every one of the ``cdim`` components of a RW Dat in place (the Jacobi
+    preconditioner's inverse diagonal)."""
+    if cdim == 1:
+        return CStringKernel("static void recip(double *w) { *w = 1.0 / *w; }", "recip")
+    return CStringKernel(f"static void recip{cdim}(double *w) {{ for (int c = 0; c < {cdim}; ++c) w[c] = 1.0 / w[c]; }}",
+                         f"recip{cdim}")
+
+
 def _touched(*dats):
     """Vector algebra ran over the local entries: owned rows are right, ghost rows are not
     (pyop2/types/dat.py:622-678: any write invalidates the halo)."""
@@ -293,18 +302,19 @@ class VCycle:
     coarsest level solved by CG.  Everything stays on the device."""
 
     def __init__(self, hierarchy, degree, make_form, bc_domains=(), nu=2, omega=0.8,
-                 coarse_rtol=1e-2, coarse_maxit=200, allreduce=None, kappa=None):
+                 coarse_rtol=1e-2, coarse_maxit=200, allreduce=None, kappa=None, cdim=1):
         """``allreduce``: callable summing a float over the ranks (partitioned hierarchies).
         ``kappa``: coefficient field on the finest level (a scalar Dat laid out like this V-cycle's
         finest space); it is copied there, each coarser level gets the injection of the next finer
-        level's field, and the operators are ``make_form(V, kappa_l)``."""
+        level's field, and the operators are ``make_form(V, kappa_l)``.  ``cdim``: value size of the
+        level spaces (3 for elasticity); Dirichlet conditions constrain every component."""
         from .assemble import DirichletBC, FunctionSpace, assemble
         self.allreduce = allreduce
         if hierarchy.partitions is None:
-            self.spaces = [FunctionSpace(m, degree) for m in hierarchy.meshes]
+            self.spaces = [FunctionSpace(m, degree, cdim) for m in hierarchy.meshes]
         else:
             parts = [hierarchy.partition(l, degree) for l in range(len(hierarchy))]
-            self.spaces = [FunctionSpace(pt.mesh, degree, partition=pt) for pt in parts]
+            self.spaces = [FunctionSpace(pt.mesh, degree, cdim, partition=pt) for pt in parts]
         self.bcs = [[DirichletBC(V, 0.0, s) for s in bc_domains] for V in self.spaces]
         self.transfers = [TransferManager(self.spaces[l], self.spaces[l + 1]) for l in range(len(self.spaces) - 1)]
         if kappa is None:
@@ -318,8 +328,7 @@ class VCycle:
         self.invdiag = []
         for V, A in zip(self.spaces, self.ops):
             d = A.getDiagonal(V.dat())
-            op2.par_loop(CStringKernel("static void recip(double *w) { *w = 1.0 / *w; }", "recip"),
-                         V.node_set, d(op2.RW))
+            op2.par_loop(reciprocal_kernel(cdim), V.node_set, d(op2.RW))
             self.invdiag.append(d)
         # per level: r residual, t smoother scratch, e prolonged correction; as a COARSE level also
         # b (restricted residual = its right-hand side) and x (its solution) -- x and e must be

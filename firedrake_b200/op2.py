@@ -1367,6 +1367,12 @@ class Kernel:
     derivative at u, ``alpha*inner(D(u)*grad w + D'(u)*w*grad u, grad v)*dx + beta*inner(w, v)*dx``,
     with u as the LAST argument like kappa: action (output, coordinates, w, u), diagonal and rank 2
     (output, coordinates, u).  Its matrix is not symmetric.
+
+    "elasticity" is linear elasticity on a vector space (``cdim=3``), ``inner(sigma(u), grad(v))*dx +
+    beta*inner(u, v)*dx`` with ``sigma(u) = 2*mu*sym(grad(u)) + lmbda*tr(sym(grad(u)))*Identity(3)``
+    (``mu``, ``lmbda``; ``alpha`` is not used).  Its arguments are those of the constant-coefficient
+    form: action (INC, READ, READ), diagonal and rank 2 (INC, READ); the rank-2 target is a Mat of block
+    size 3, every 3 x 3 block filled.
     """
     form: str = "helmholtz"
     degree: int = 1
@@ -1384,6 +1390,8 @@ class Kernel:
     # tabulation: a fiat_lite.Interval1D, or None for the default GLL/Gauss pair
     element: object = field(default=None, compare=False, hash=False)
     d: tuple = (1.0, 0.0, 0.0)      # nonlinear diffusion: D(s) = d[0] + d[1] s + d[2] s^2
+    mu: float = 1.0                 # elasticity: Lame parameters
+    lmbda: float = 0.0
 
     def __new__(cls, *args, **kwargs):
         # ``op2.Kernel(code, name)`` with C source (pyop2/local_kernel.py:33-43) builds the
@@ -1428,7 +1436,8 @@ class Kernel:
 
 _FORMS = {"helmholtz": _lib.FORM_HELMHOLTZ, "dg_advection": _lib.FORM_DG_ADVECTION,
           "helmholtz_coef": _lib.FORM_HELMHOLTZ_COEF, "nonlinear_diffusion": _lib.FORM_NONLINEAR_DIFFUSION,
-          "nonlinear_diffusion_jacobian": _lib.FORM_NONLINEAR_DIFFUSION_JACOBIAN}
+          "nonlinear_diffusion_jacobian": _lib.FORM_NONLINEAR_DIFFUSION_JACOBIAN,
+          "elasticity": _lib.FORM_ELASTICITY}
 _INTEGRALS = {"cell": _lib.INTEGRAL_CELL, "exterior_facet": _lib.INTEGRAL_EXTERIOR_FACET,
               "interior_facet": _lib.INTEGRAL_INTERIOR_FACET, "fused": _lib.INTEGRAL_FUSED}
 
@@ -1514,6 +1523,8 @@ class GlobalKernel:
         d.affine_cells = int(lk.affine and lk.rank == 1 and not lk.diagonal)
         for i in range(3):
             d.dcoef[i] = lk.d[i]
+        if lk.form == "elasticity":
+            d.alpha, d.lmbda = lk.mu, lk.lmbda
         for q in range(el.nq):
             d.wq[q] = el.wq[q]
             d.xq[q] = el.xq[q]

@@ -128,7 +128,7 @@ enum fdb_form {
                                    2, not diagonal):  [y INC, coords, u].  Hex cells, cdim == 1,
                                    nq == degree+1, affine_cells == 0, degrees 1..5; atomic or
                                    coloured scatter, device or host mode (host mode monolithic).   */
-    FDB_FORM_NONLINEAR_DIFFUSION_JACOBIAN = 5
+    FDB_FORM_NONLINEAR_DIFFUSION_JACOBIAN = 5,
                                 /* its Gateaux derivative at u (exact Newton Jacobian, NOT symmetric):
                                      J(u)[w; v] = alpha*inner(D(u) grad w + D'(u) w grad u, grad v)*dx
                                                   + beta*inner(w, v)*dx
@@ -139,6 +139,22 @@ enum fdb_form {
                                      diagonal  [d INC, coords, u]      (device mode)
                                      rank 2    [Mat, coords, u]  (row = test dof, column = trial dof)
                                    Never the DMMA element-matrix kernels (they assume symmetry).  */
+    FDB_FORM_ELASTICITY = 6
+                                /* linear elasticity on a vector space (value size 3, AoS):
+                                     a(u, v) = inner(sigma(u), grad v)*dx + beta*inner(u, v)*dx,
+                                     sigma(u) = mu (grad u + grad u^T) + lmbda tr(grad u) I
+                                   mu = alpha, beta = beta, lmbda = the field lmbda (dcoef unused).
+                                   The components couple: every 3 x 3 block of the element matrix is
+                                   filled, and the matrix is symmetric.  Hex cells (extruded or
+                                   native), cdim == 3, nq == degree+1, affine_cells == 0; degrees 1..4
+                                   (action), 1..3 (rank 2 and diagonal):
+                                     action    [y INC, coords, u]  (atomic or coloured; device or host
+                                               mode, host mode monolithic)
+                                     diagonal  [d INC, coords]     (device mode; 3 values per node)
+                                     rank 2    [Mat (block size 3), coords]  (row = test dof,
+                                               column = trial dof; dof-level lgmaps)
+                                   Never the DMMA element-matrix kernels ("matrix_kernel" does not
+                                   apply).                                                          */
 };
 
 enum fdb_cell {
@@ -201,6 +217,8 @@ typedef struct fdb_kernel_desc {
     /* FDB_FORM_NONLINEAR_DIFFUSION[_JACOBIAN]: D(s) = dcoef[0] + dcoef[1] s + dcoef[2] s^2.
      * Ignored by every other form (a zeroed descriptor stays valid for them). */
     double dcoef[3];
+    /* FDB_FORM_ELASTICITY: the Lame parameter lambda (mu is alpha).  Ignored by every other form. */
+    double lmbda;
 } fdb_kernel_desc;
 
 typedef struct fdb_kernel_s *fdb_kernel_t;
