@@ -20,6 +20,8 @@ FORM_HELMHOLTZ_COEF = 3
 FORM_NONLINEAR_DIFFUSION = 4
 FORM_NONLINEAR_DIFFUSION_JACOBIAN = 5
 FORM_ELASTICITY = 6
+FORM_HYPERELASTICITY = 7
+FORM_HYPERELASTICITY_JACOBIAN = 8
 CELL_HEX_EXTRUDED = 1
 CELL_HEX = 2
 CELL_TRIANGLE = 3

@@ -11,8 +11,8 @@ Mirrors (same names / call protocol, thin Python over the engine):
 * ``firedrake.matrix_free.operators.ImplicitMatrixContext`` (operators.py:74-242)
 
 Forms are described by :class:`Form` (the Helmholtz family on a
-:class:`FunctionSpace`), :class:`NonlinearDiffusion` and :class:`Elasticity` (linear elasticity on a
-vector space) instead of UFL: UFL/TSFC are not available here, and the
+:class:`FunctionSpace`), :class:`NonlinearDiffusion`, :class:`Elasticity` (linear elasticity on a
+vector space) and :class:`HyperElasticity` (its Neo-Hookean counterpart) instead of UFL: UFL/TSFC are not available here, and the
 engine keys its kernels on a form descriptor (DESIGN.md section 1).
 """
 from __future__ import annotations
@@ -366,19 +366,15 @@ def assemble_variable_coefficient(V: "FunctionSpace", kappa: op2.Dat, u: op2.Dat
     return tensor
 
 
-def elasticity_kernel(degree, mu, lmbda, beta=0.0, name="elasticity_action"):
-    """C source of the 1-form ``action(inner(sigma(u), grad(v))*dx + beta*inner(u, v)*dx, u)`` of linear
-    elasticity, ``sigma(u) = 2*mu*sym(grad(u)) + lmbda*tr(sym(grad(u)))*Identity(3)``, on the vector
-    Q_p (x) P_p space (3 components, AoS), written the way TSFC's spectral mode would and run through the
-    generic wrapper builder: the independent statement of the hand-written FDB_FORM_ELASTICITY kernel.
-    Arguments: y (INC), coords, u."""
+def _vector_hex_tables(degree):
+    """C preamble of the generic-path vector (3 component) hex kernels: the 1-D tables of the Q_p (x) P_p
+    element and the sum-factorised tensor contraction ``el_tensor``."""
     from .fiat_lite import interval_element
-    from .codegen import CStringKernel
     el = interval_element(degree)
     n = degree + 1
     tab = lambda a: "{" + ", ".join("{" + ", ".join(repr(float(v)) for v in r) + "}" for r in a) + "}"
     vec = lambda a: "{" + ", ".join(repr(float(v)) for v in a) + "}"
-    code = f"""
+    return f"""
 #define EN {n}
 #define END (EN * EN * EN)
 static const double EB[EN][EN] = {tab(el.B)};      /* EB[q][a] */
@@ -404,7 +400,17 @@ static inline void el_tensor(const double (*T0)[EN], const double (*T1)[EN], con
     el_apply(T1, 1, tr, t1, t2);
     el_apply(T2, 2, tr, t2, out);
 }}
-static void {name}(double *y, const double *X, const double *u)
+"""
+
+
+def elasticity_kernel(degree, mu, lmbda, beta=0.0, name="elasticity_action"):
+    """C source of the 1-form ``action(inner(sigma(u), grad(v))*dx + beta*inner(u, v)*dx, u)`` of linear
+    elasticity, ``sigma(u) = 2*mu*sym(grad(u)) + lmbda*tr(sym(grad(u)))*Identity(3)``, on the vector
+    Q_p (x) P_p space (3 components, AoS), written the way TSFC's spectral mode would and run through the
+    generic wrapper builder: the independent statement of the hand-written FDB_FORM_ELASTICITY kernel.
+    Arguments: y (INC), coords, u."""
+    from .codegen import CStringKernel
+    code = _vector_hex_tables(degree) + f"""static void {name}(double *y, const double *X, const double *u)
 {{
     double U[3][END], G[3][3][END], c[END], t[END];
     for (int d = 0; d < 3; ++d) {{
@@ -480,6 +486,137 @@ def assemble_elasticity_generic(V: "FunctionSpace", u: op2.Dat, mu, lmbda, beta=
     tensor.device_ptr
     op2.par_loop(elasticity_kernel(V.degree, mu, lmbda, beta), V.cell_set, tensor(op2.INC, V.cell_node_map),
                  V.coordinates(op2.READ, V.coord_map), u(op2.READ, V.cell_node_map))
+    return tensor
+
+
+def hyperelasticity_kernel(degree, mu, lmbda, beta=0.0, jacobian=False, name=None):
+    """C source of the residual of compressible Neo-Hookean hyperelasticity,
+    ``inner(P(F), grad(v))*dx + beta*inner(u, v)*dx`` with ``F = I + grad(u)``, ``J = det(F)`` and
+    ``P(F) = mu*(F - F^{-T}) + lmbda*ln(J)*F^{-T}`` (arguments: y (INC), coords, u), or with ``jacobian``
+    of its Gateaux derivative's action at u, ``inner(dP[grad(w)], grad(v))*dx + beta*inner(w, v)*dx``
+    (arguments: y (INC), coords, w, u).  Written the way TSFC's spectral mode would, with the inverse of F
+    formed explicitly, and run through the generic wrapper builder: the independent statement of the
+    hand-written FDB_FORM_HYPERELASTICITY[_JACOBIAN] kernels."""
+    from .codegen import CStringKernel
+    if name is None:
+        name = "hyperelasticity_jacobian_action" if jacobian else "hyperelasticity_residual"
+    args = "double *y, const double *X, const double *w, const double *u" if jacobian else \
+        "double *y, const double *X, const double *u"
+    mu, lmbda, beta = repr(float(mu)), repr(float(lmbda)), repr(float(beta))
+    # the point stress: P(F) or dP[H] with H the gradient of w
+    if jacobian:
+        stress = f"""
+        double A[3][3], C[3][3], trA = 0.0;
+        for (int i = 0; i < 3; ++i)
+            for (int j = 0; j < 3; ++j)
+                A[i][j] = Finv[i][0] * H[0][j] + Finv[i][1] * H[1][j] + Finv[i][2] * H[2][j];
+        for (int i = 0; i < 3; ++i) trA += A[i][i];
+        for (int i = 0; i < 3; ++i)
+            for (int j = 0; j < 3; ++j)
+                C[i][j] = A[i][0] * Finv[0][j] + A[i][1] * Finv[1][j] + A[i][2] * Finv[2][j];
+        for (int d = 0; d < 3; ++d)
+            for (int k = 0; k < 3; ++k)
+                S[d][k] = {mu} * H[d][k] + ({mu} - {lmbda} * lnJ) * C[k][d] + {lmbda} * trA * Finv[k][d];"""
+    else:
+        stress = f"""
+        for (int d = 0; d < 3; ++d)
+            for (int k = 0; k < 3; ++k)
+                S[d][k] = {mu} * (Fd[d][k] - Finv[k][d]) + {lmbda} * lnJ * Finv[k][d];"""
+    wv = "w" if jacobian else "u"
+    code = _vector_hex_tables(degree) + f"""static void {name}({args})
+{{
+    double U[3][END], G[3][3][END], GU[3][3][END], c[END], t[END];
+    for (int d = 0; d < 3; ++d) {{
+        for (int i = 0; i < END; ++i) c[i] = {wv}[i * 3 + d];
+        el_tensor(EB, EB, EB, 0, c, U[d]);
+        el_tensor(ED, EB, EB, 0, c, G[d][0]);
+        el_tensor(EB, ED, EB, 0, c, G[d][1]);
+        el_tensor(EB, EB, ED, 0, c, G[d][2]);
+        for (int i = 0; i < END; ++i) c[i] = u[i * 3 + d];
+        el_tensor(ED, EB, EB, 0, c, GU[d][0]);
+        el_tensor(EB, ED, EB, 0, c, GU[d][1]);
+        el_tensor(EB, EB, ED, 0, c, GU[d][2]);
+    }}
+    for (int qx = 0; qx < EN; ++qx) for (int qy = 0; qy < EN; ++qy) for (int qz = 0; qz < EN; ++qz) {{
+        const int q = (qx * EN + qy) * EN + qz;
+        const double xi[3] = {{EX[qx], EX[qy], EX[qz]}};
+        double J[3][3] = {{{{0}}}};
+        for (int v = 0; v < 8; ++v) {{
+            const int b[3] = {{(v >> 2) & 1, (v >> 1) & 1, v & 1}};
+            for (int r = 0; r < 3; ++r) {{
+                double g = b[r] ? 1.0 : -1.0;
+                for (int e = 0; e < 3; ++e) if (e != r) g *= b[e] ? xi[e] : 1.0 - xi[e];
+                for (int k = 0; k < 3; ++k) J[k][r] += X[v * 3 + k] * g;
+            }}
+        }}
+        const double det = J[0][0] * (J[1][1] * J[2][2] - J[1][2] * J[2][1])
+                         - J[0][1] * (J[1][0] * J[2][2] - J[1][2] * J[2][0])
+                         + J[0][2] * (J[1][0] * J[2][1] - J[1][1] * J[2][0]);
+        double Jinv[3][3];
+        Jinv[0][0] = (J[1][1] * J[2][2] - J[1][2] * J[2][1]) / det;
+        Jinv[0][1] = (J[0][2] * J[2][1] - J[0][1] * J[2][2]) / det;
+        Jinv[0][2] = (J[0][1] * J[1][2] - J[0][2] * J[1][1]) / det;
+        Jinv[1][0] = (J[1][2] * J[2][0] - J[1][0] * J[2][2]) / det;
+        Jinv[1][1] = (J[0][0] * J[2][2] - J[0][2] * J[2][0]) / det;
+        Jinv[1][2] = (J[0][2] * J[1][0] - J[0][0] * J[1][2]) / det;
+        Jinv[2][0] = (J[1][0] * J[2][1] - J[1][1] * J[2][0]) / det;
+        Jinv[2][1] = (J[0][1] * J[2][0] - J[0][0] * J[2][1]) / det;
+        Jinv[2][2] = (J[0][0] * J[1][1] - J[0][1] * J[1][0]) / det;
+        const double wd = EW[qx] * EW[qy] * EW[qz] * fabs(det);
+        double H[3][3], Fd[3][3], Finv[3][3], S[3][3];
+        for (int d = 0; d < 3; ++d)
+            for (int k = 0; k < 3; ++k) {{
+                H[d][k] = G[d][0][q] * Jinv[0][k] + G[d][1][q] * Jinv[1][k] + G[d][2][q] * Jinv[2][k];
+                Fd[d][k] = (d == k ? 1.0 : 0.0)
+                         + GU[d][0][q] * Jinv[0][k] + GU[d][1][q] * Jinv[1][k] + GU[d][2][q] * Jinv[2][k];
+            }}
+        const double dF = Fd[0][0] * (Fd[1][1] * Fd[2][2] - Fd[1][2] * Fd[2][1])
+                        - Fd[0][1] * (Fd[1][0] * Fd[2][2] - Fd[1][2] * Fd[2][0])
+                        + Fd[0][2] * (Fd[1][0] * Fd[2][1] - Fd[1][1] * Fd[2][0]);
+        Finv[0][0] = (Fd[1][1] * Fd[2][2] - Fd[1][2] * Fd[2][1]) / dF;
+        Finv[0][1] = (Fd[0][2] * Fd[2][1] - Fd[0][1] * Fd[2][2]) / dF;
+        Finv[0][2] = (Fd[0][1] * Fd[1][2] - Fd[0][2] * Fd[1][1]) / dF;
+        Finv[1][0] = (Fd[1][2] * Fd[2][0] - Fd[1][0] * Fd[2][2]) / dF;
+        Finv[1][1] = (Fd[0][0] * Fd[2][2] - Fd[0][2] * Fd[2][0]) / dF;
+        Finv[1][2] = (Fd[0][2] * Fd[1][0] - Fd[0][0] * Fd[1][2]) / dF;
+        Finv[2][0] = (Fd[1][0] * Fd[2][1] - Fd[1][1] * Fd[2][0]) / dF;
+        Finv[2][1] = (Fd[0][1] * Fd[2][0] - Fd[0][0] * Fd[2][1]) / dF;
+        Finv[2][2] = (Fd[0][0] * Fd[1][1] - Fd[0][1] * Fd[1][0]) / dF;
+        const double lnJ = log(dF);{stress}
+        for (int d = 0; d < 3; ++d) {{
+            for (int m = 0; m < 3; ++m)
+                G[d][m][q] = wd * (Jinv[m][0] * S[d][0] + Jinv[m][1] * S[d][1] + Jinv[m][2] * S[d][2]);
+            U[d][q] *= {beta} * wd;
+        }}
+    }}
+    for (int d = 0; d < 3; ++d) {{
+        el_tensor(EB, EB, EB, 1, U[d], c);
+        el_tensor(ED, EB, EB, 1, G[d][0], t);  for (int i = 0; i < END; ++i) c[i] += t[i];
+        el_tensor(EB, ED, EB, 1, G[d][1], t);  for (int i = 0; i < END; ++i) c[i] += t[i];
+        el_tensor(EB, EB, ED, 1, G[d][2], t);  for (int i = 0; i < END; ++i) c[i] += t[i];
+        for (int i = 0; i < END; ++i) y[i * 3 + d] += c[i];
+    }}
+}}
+#undef END
+#undef EN
+"""
+    return CStringKernel(code, name)
+
+
+def assemble_hyperelasticity_generic(V: "FunctionSpace", u: op2.Dat, mu, lmbda, beta=0.0, w: op2.Dat = None,
+                                     tensor=None):
+    """The residual R(u) of :class:`HyperElasticity` (``w`` None) or the Jacobian action J(u) w through the
+    generic wrapper path (:func:`hyperelasticity_kernel`): the cross-check and the baseline of the
+    hand-written kernels."""
+    if V.cdim != 3:
+        raise ValueError("hyperelasticity needs a vector space with 3 components")
+    if tensor is None:
+        tensor = V.dat()
+    tensor.zero()
+    tensor.device_ptr
+    ins = ([w(op2.READ, V.cell_node_map)] if w is not None else []) + [u(op2.READ, V.cell_node_map)]
+    op2.par_loop(hyperelasticity_kernel(V.degree, mu, lmbda, beta, jacobian=w is not None), V.cell_set,
+                 tensor(op2.INC, V.cell_node_map), V.coordinates(op2.READ, V.coord_map), *ins)
     return tensor
 
 
@@ -709,6 +846,72 @@ class Elasticity:
             raise ValueError("elasticity needs a vector space with 3 components")
         return op2.Kernel("elasticity", degree=self.V.degree, mu=self.mu, lmbda=self.lmbda, beta=self.beta,
                           rank=rank, diagonal=diagonal, cdim=3)
+
+
+@dataclass
+class HyperElasticity:
+    """The residual of compressible Neo-Hookean hyperelasticity on a vector space ``V`` (``cdim = 3``),
+    without its load term:
+
+        F = I + grad(u),  J = det(F),
+        psi = mu/2*(tr(F^T F) - 3) - mu*ln(J) + lmbda/2*ln(J)**2,
+        R(u; v) = inner(P(F), grad(v))*dx + beta*inner(u, v)*dx,  P = dpsi/dF = mu*(F - F^{-T}) + lmbda*ln(J)*F^{-T}
+
+    ``assemble(F, u=u)`` is the vector R(u) (degrees 1..4); the problem R(u; v) = inner(f, v)*dx is
+    solved by :func:`solve_nonlinear`.  At u = 0 its Jacobian is ``Elasticity(V, mu, lmbda, beta)``.  A
+    point with J <= 0 (an inverted element) makes ln(J) and the residual NaN, as in Firedrake."""
+    V: FunctionSpace
+    mu: float
+    lmbda: float
+    beta: float = 0.0
+    symmetric = True
+
+    def coefficient_args(self):
+        return []
+
+    def kernel(self, rank, diagonal=False):
+        if rank != 1 or diagonal:
+            raise ValueError("the residual is a 1-form: its matrix and diagonal are those of F.jacobian(u)")
+        if self.V.cdim != 3:
+            raise ValueError("hyperelasticity needs a vector space with 3 components")
+        return op2.Kernel("hyperelasticity", degree=self.V.degree, mu=self.mu, lmbda=self.lmbda, beta=self.beta,
+                          cdim=3)
+
+    def jacobian(self, u0: op2.Dat):
+        """The Gateaux derivative at ``u0`` (the exact Newton Jacobian, a symmetric bilinear form)."""
+        return HyperElasticityJacobian(self.V, self.mu, self.lmbda, self.beta, u0)
+
+
+@dataclass
+class HyperElasticityJacobian:
+    """J(u0)[w; v] = inner(dP[grad(w)], grad(v))*dx + beta*inner(w, v)*dx with
+    dP[H] = mu*H + (mu - lmbda*ln(J))*F^{-T} H^T F^{-T} + lmbda*tr(F^{-1} H)*F^{-T} at F = I + grad(u0):
+    a symmetric bilinear form (``assemble(J, u=w)``, ``assemble(J)`` as a blocked aij Mat,
+    ``assemble(J, mat_type="matfree")``).  ``u0`` is read through the argument map."""
+    V: FunctionSpace
+    mu: float
+    lmbda: float
+    beta: float
+    u0: op2.Dat
+    symmetric = True
+
+    def coefficient_args(self):
+        return [self.u0(op2.READ, self.V.cell_node_map)]
+
+    def kernel(self, rank, diagonal=False):
+        if self.V.cdim != 3:
+            raise ValueError("hyperelasticity needs a vector space with 3 components")
+        return op2.Kernel("hyperelasticity_jacobian", degree=self.V.degree, mu=self.mu, lmbda=self.lmbda,
+                          beta=self.beta, rank=rank, diagonal=diagonal, cdim=3)
+
+
+class ConvergenceError(RuntimeError):
+    """A nonlinear solve that cannot go on (firedrake.exceptions.ConvergenceError); ``reason`` is the
+    SNES converged reason, e.g. "DIVERGED_FNORM_NAN"."""
+
+    def __init__(self, msg, reason):
+        super().__init__(msg)
+        self.reason = reason
 
 
 def poisson(V):
@@ -1058,10 +1261,10 @@ def gmres(A, b: op2.Dat, x: op2.Dat, M=None, rtol=1e-5, atol=0.0, restart=30, ma
     return it, hist
 
 
-def solve_nonlinear(F: NonlinearDiffusion, L: op2.Dat, u: op2.Dat, bcs=(), solver_parameters=None,
-                    hierarchy=None, allreduce=None):
-    """``solve(F == 0, u, bcs=bcs, solver_parameters=...)`` for nonlinear diffusion with the source
-    ``L`` (the assembled right-hand side, e.g. ``assemble(mass(V), u=f)``): Newton's method with the
+def solve_nonlinear(F, L: op2.Dat, u: op2.Dat, bcs=(), solver_parameters=None, hierarchy=None, allreduce=None):
+    """``solve(F == 0, u, bcs=bcs, solver_parameters=...)`` for nonlinear diffusion (``F`` a
+    :class:`NonlinearDiffusion`) or hyperelasticity (a :class:`HyperElasticity` on a vector space) with the
+    source ``L`` (the assembled right-hand side, e.g. ``assemble(mass(V), u=f)``): Newton's method with the
     full step (``snes_type newtonls``, ``snes_linesearch_type basic``) on the residual R(u) = F(u) - L,
     each step solved by GMRES with the exact Jacobian ``F.jacobian(u)``.  ``u`` is the initial guess
     and is overwritten with the solution.
@@ -1070,10 +1273,14 @@ def solve_nonlinear(F: NonlinearDiffusion, L: op2.Dat, u: op2.Dat, bcs=(), solve
     and the Newton update vanishes there.  ``solver_parameters``: ``snes_rtol`` (1e-8), ``snes_atol``
     (1e-50), ``snes_max_it`` (50); ``ksp_type`` "gmres", ``ksp_gmres_restart`` (30), ``ksp_rtol``
     (1e-5), ``ksp_max_it`` (10000); ``mat_type`` "matfree" (default) | "aij"; ``pc_type`` "none"
-    (default) | "jacobi" (the Jacobian's exact diagonal) | "mg" (a V-cycle of the SPD operator
-    ``Form(V, alpha, beta, kappa=D(u))``, rebuilt at every Newton step; needs ``hierarchy``).
-    Converged when ||R(u)|| <= max(snes_rtol * ||R(u_0)||, snes_atol).  Returns (Newton residual
-    norms, Krylov iterations per Newton step)."""
+    (default) | "jacobi" (the Jacobian's exact diagonal) | "mg" (needs ``hierarchy``; nonlinear
+    diffusion: a V-cycle of the SPD operator ``Form(V, alpha, beta, kappa=D(u))``, rebuilt at every
+    Newton step; hyperelasticity: a V-cycle of ``Elasticity(V, mu, lmbda, beta)``, the Jacobian at u = 0,
+    built once per solve, with Jacobi smoothing damped by 0.6 as in :func:`solve`).
+    Converged when ||R(u)|| <= max(snes_rtol * ||R(u_0)||, snes_atol).  For hyperelasticity a
+    non-finite residual norm (an inverted element: ln J of J <= 0) ends the solve with a
+    :class:`ConvergenceError` whose reason is "DIVERGED_FNORM_NAN".  Returns (Newton residual norms,
+    Krylov iterations per Newton step)."""
     from . import _lib
     from . import mg as _mg
     sp = {"snes_rtol": 1e-8, "snes_atol": 1e-50, "snes_max_it": 50, "ksp_type": "gmres",
@@ -1081,7 +1288,7 @@ def solve_nonlinear(F: NonlinearDiffusion, L: op2.Dat, u: op2.Dat, bcs=(), solve
           "pc_type": "none"}
     sp.update(solver_parameters or {})
     if sp["ksp_type"] != "gmres":
-        raise NotImplementedError("ksp_type gmres only (the Newton Jacobian is not symmetric)")
+        raise NotImplementedError("ksp_type gmres only (a Newton Jacobian need not be symmetric or definite)")
     if sp["mat_type"] not in ("matfree", "aij"):
         raise NotImplementedError(f"mat_type {sp['mat_type']!r}")
     V = F.V
@@ -1105,8 +1312,17 @@ def solve_nonlinear(F: NonlinearDiffusion, L: op2.Dat, u: op2.Dat, bcs=(), solve
         _lib.check(lib.fdb_vec_dot(n_owned, R.device_ptr, R.device_ptr, C.byref(out)))
         return float(np.sqrt(allreduce(out.value) if allreduce else out.value))
 
+    hyper = isinstance(F, HyperElasticity)
+
+    def check_finite():
+        if hyper and not np.isfinite(hist[-1]):
+            raise ConvergenceError(f"nonlinear solve diverged: the residual norm is {hist[-1]} after "
+                                   f"{len(kits)} Newton steps (DIVERGED_FNORM_NAN; an inverted element "
+                                   f"has det F <= 0)", "DIVERGED_FNORM_NAN")
+
     hist = [residual()]
     kits = []
+    check_finite()
     tol = max(sp["snes_rtol"] * hist[0], sp["snes_atol"])
     # J reads u in place: the matrix-free operator and the diagonal's context follow every update,
     # an assembled matrix is assembled again at every step
@@ -1114,6 +1330,7 @@ def solve_nonlinear(F: NonlinearDiffusion, L: op2.Dat, u: op2.Dat, bcs=(), solve
     pc = sp["pc_type"]
     A = ctx = None
     d = V.dat() if pc == "jacobi" else None
+    vc = None
     while hist[-1] > tol and len(kits) < sp["snes_max_it"]:
         if A is None or sp["mat_type"] != "matfree":
             A = assemble(J, bcs=bcs, mat_type=sp["mat_type"])
@@ -1123,8 +1340,7 @@ def solve_nonlinear(F: NonlinearDiffusion, L: op2.Dat, u: op2.Dat, bcs=(), solve
             if ctx is None:
                 ctx = A if isinstance(A, ImplicitMatrixContext) else ImplicitMatrixContext(J, bcs)
             ctx.getDiagonal(d)
-            op2.par_loop(op2.Kernel("static void recip(double *w) { *w = 1.0 / *w; }", "recip"), V.node_set,
-                         d(op2.RW))
+            op2.par_loop(_mg.reciprocal_kernel(V.cdim), V.node_set, d(op2.RW))
 
             def M(r, z, d=d):
                 _lib.check(lib.fdb_vec_pointwise_mult(n, r.device_ptr, d.device_ptr, z.device_ptr))
@@ -1132,10 +1348,16 @@ def solve_nonlinear(F: NonlinearDiffusion, L: op2.Dat, u: op2.Dat, bcs=(), solve
         elif pc == "mg":
             if hierarchy is None:
                 raise ValueError("pc_type mg needs the mesh hierarchy")
-            kap = F.diffusivity(u)
-            vc = _mg.VCycle(hierarchy, V.degree, lambda W, k=None: Form(W, F.alpha, F.beta, k),
-                            bc_domains=tuple(s for bc in bcs for s in bc.sub_domains), allreduce=allreduce,
-                            kappa=kap)
+            domains = tuple(s for bc in bcs for s in bc.sub_domains)
+            if hyper:
+                # J(0) = Elasticity: the same operator at every Newton step, so one V-cycle per solve
+                if vc is None:
+                    vc = _mg.VCycle(hierarchy, V.degree, lambda W, k=None: Elasticity(W, F.mu, F.lmbda, F.beta),
+                                    bc_domains=domains, allreduce=allreduce, cdim=3, omega=0.6)
+            else:
+                kap = F.diffusivity(u)
+                vc = _mg.VCycle(hierarchy, V.degree, lambda W, k=None: Form(W, F.alpha, F.beta, k),
+                                bc_domains=domains, allreduce=allreduce, kappa=kap)
             top = len(hierarchy) - 1
             M = lambda r, z, vc=vc: vc.apply(top, r, z)
         else:
@@ -1149,6 +1371,7 @@ def solve_nonlinear(F: NonlinearDiffusion, L: op2.Dat, u: op2.Dat, bcs=(), solve
         u.axpy(-1.0, du)
         kits.append(its)
         hist.append(residual())
+        check_finite()
     return hist, kits
 
 

@@ -128,11 +128,12 @@ int fdb_launch_helmholtz_coef_matrix(fdb_kernel_s *k, fdb_int start, fdb_int end
                                      const fdb_int *subset, fdb_mat_t mat, const double *coords,
                                      const double *kappa, const fdb_int *map0, const fdb_int *map1,
                                      double *diag_out);
-// FDB_FORM_ELASTICITY (elasticity_hex.cu): x, y and diag_out are AoS with 3 values per node; mat has
-// block size 3 (diag_out is used when mat is NULL)
+// FDB_FORM_ELASTICITY and FDB_FORM_HYPERELASTICITY[_JACOBIAN] (elasticity_hex.cu): x, y, u and diag_out are
+// AoS with 3 values per node; mat has block size 3 (diag_out is used when mat is NULL).  u is the
+// Jacobian's linearisation point (NULL for the other forms; the residual's u is x)
 int fdb_launch_elasticity_action(fdb_kernel_s *k, fdb_int start, fdb_int end, int nlay, const fdb_int *subset,
-                                 double *y, const double *coords, const double *x, const fdb_int *map0,
-                                 const fdb_int *map1);
+                                 double *y, const double *coords, const double *x, const double *u,
+                                 const fdb_int *map0, const fdb_int *map1);
 int fdb_launch_elasticity_matrix(fdb_kernel_s *k, fdb_int start, fdb_int end, int nlay, const fdb_int *subset,
-                                 fdb_mat_t mat, const double *coords, const fdb_int *map0, const fdb_int *map1,
-                                 double *diag_out);
+                                 fdb_mat_t mat, const double *coords, const double *u, const fdb_int *map0,
+                                 const fdb_int *map1, double *diag_out);

@@ -21,6 +21,18 @@
 // a = 0..2, into the 3 x 3 block at the node pair's CSR position (row-major inside the block).  Entries
 // whose dof-level lgmap index is negative are dropped.  With vals == NULL the kernel adds the
 // diagonal entry (j, b; j, b) into diag[3 j + b] instead.
+//
+// FDB_FORM_HYPERELASTICITY[_JACOBIAN] (DESIGN.md section 4.9) run through the same kernel with MODE
+// EL_RESIDUAL / EL_JACOBIAN: the compressible Neo-Hookean residual and its exact Gateaux derivative,
+//     F = I + grad u,  J = det F,  P(F) = mu (F - F^{-T}) + lmbda ln(J) F^{-T}
+//     R(u; v)    = inner(P(F(u)), grad v)*dx + beta*inner(u, v)*dx
+//     J(u)[w; v] = inner(dP[grad w], grad v)*dx + beta*inner(w, v)*dx,
+//     dP[H] = mu H + (mu - lmbda ln J) F^{-T} H^T F^{-T} + lmbda tr(F^{-1} H) F^{-T}.
+// Only the point stage differs: P (or dP) goes into the nine fluxes where sigma goes.  The residual's
+// gathered values are u itself.  The Jacobian also gathers u (through the same node map, again for every
+// trial-dof unit in MATRIX mode) into a fourth per-slot buffer S_V; its forward passes share S_T/S_F
+// with those of w, and F comes from the collocated derivative of S_V.  J <= 0 at a point gives NaN
+// (ln of a negative number), as in Firedrake: the kernel does not guard it.
 #include "common.cuh"
 
 namespace {
@@ -45,15 +57,19 @@ struct ElasParams {
     const fdb_int *row_lg, *col_lg;   // dof-level, NULL = identity
     const unsigned short *rank_tab;
     int nvar, nlay_total;
+    const double *u;             // EL_JACOBIAN: the linearisation point (AoS, node map)
 };
 
-template <int N>
+enum { EL_LINEAR = 0, EL_RESIDUAL = 1, EL_JACOBIAN = 2 };
+
+template <int N, int MODE = EL_LINEAR>
 struct ElasShape {
     static constexpr int ND = N * N * N;
     static constexpr int CPB = (256 / ND) > 0 ? 256 / ND : 1;          // cells (slots) per CTA
     static constexpr int THREADS = ((CPB * ND + 31) / 32) * 32;
-    // doubles per slot: vertices, values at the points, work buffer, fluxes (9 per point)
-    static constexpr int SLOT = 24 + 3 * ND + 3 * ND + 9 * ND;
+    // doubles per slot: vertices, values at the points, work buffer, fluxes (9 per point); the Jacobian
+    // also holds u's values (S_V)
+    static constexpr int SLOT = 24 + 3 * ND + 3 * ND + 9 * ND + (MODE == EL_JACOBIAN ? 3 * ND : 0);
     static constexpr size_t SMEM = (size_t)CPB * SLOT * sizeof(double) + (size_t)CPB * ND * sizeof(int);
 };
 
@@ -71,13 +87,29 @@ __device__ __forceinline__ double pass1(const double *__restrict__ T, const doub
     return s;
 }
 
-template <int N, bool MATRIX, bool ATOMIC>
+// cof[i][j] = cofactor of F[i][j]: F^{-T} = cof / det F, F^{-1}[i][j] = cof[j][i] / det F; returns det F
+__device__ __forceinline__ double cofactors(const double F[3][3], double cof[3][3])
+{
+    cof[0][0] = F[1][1] * F[2][2] - F[1][2] * F[2][1];
+    cof[0][1] = F[1][2] * F[2][0] - F[1][0] * F[2][2];
+    cof[0][2] = F[1][0] * F[2][1] - F[1][1] * F[2][0];
+    cof[1][0] = F[0][2] * F[2][1] - F[0][1] * F[2][2];
+    cof[1][1] = F[0][0] * F[2][2] - F[0][2] * F[2][0];
+    cof[1][2] = F[0][1] * F[2][0] - F[0][0] * F[2][1];
+    cof[2][0] = F[0][1] * F[1][2] - F[0][2] * F[1][1];
+    cof[2][1] = F[0][2] * F[1][0] - F[0][0] * F[1][2];
+    cof[2][2] = F[0][0] * F[1][1] - F[0][1] * F[1][0];
+    return F[0][0] * cof[0][0] + F[0][1] * cof[0][1] + F[0][2] * cof[0][2];
+}
+
+template <int N, bool MATRIX, bool ATOMIC, int MODE = EL_LINEAR>
 __global__ void __launch_bounds__(ElasShape<N>::THREADS)
 elasticity_kernel(const __grid_constant__ ElasParams<N> P)
 {
-    using S = ElasShape<N>;
+    using S = ElasShape<N, MODE>;
     constexpr int ND = S::ND;
     constexpr int CPB = S::CPB;
+    constexpr bool JAC = MODE == EL_JACOBIAN;
     extern __shared__ __align__(16) unsigned char smem_raw[];
     const int slot = threadIdx.x / ND;
     const int l = threadIdx.x - slot * ND;                 // this thread's dof / point in the cell
@@ -88,6 +120,7 @@ elasticity_kernel(const __grid_constant__ ElasParams<N> P)
     double *s_u = s_x + 24;                                // [3][ND]
     double *s_t = s_u + 3 * ND;                            // [3][ND]
     double *s_f = s_t + 3 * ND;                            // [3 d][3 m][ND]
+    double *s_v = s_f + 9 * ND;                            // [3][ND], EL_JACOBIAN only
     int *s_idx = reinterpret_cast<int *>(reinterpret_cast<double *>(smem_raw) + (size_t)CPB * S::SLOT) + sl * ND;
     const int qi = l / (N * N), qj = (l / N) % N, qk = l % N;
 
@@ -112,6 +145,10 @@ elasticity_kernel(const __grid_constant__ ElasParams<N> P)
 #pragma unroll
             for (int d = 0; d < 3; d++)
                 s_u[d * ND + l] = MATRIX ? ((jb == 3 * l + d) ? 1.0 : 0.0) : __ldg(P.x + (long long)g * 3 + d);
+            if (JAC) {
+#pragma unroll
+                for (int d = 0; d < 3; d++) s_v[d * ND + l] = __ldg(P.u + (long long)g * 3 + d);
+            }
             for (int i = l; i < 24; i += ND) {
                 const int v = i / 3, a = i - 3 * v;
                 const int gv = __ldg(P.map1 + (long long)col * 8 + v) + __ldg(P.off1 + v) * layer;
@@ -121,23 +158,43 @@ elasticity_kernel(const __grid_constant__ ElasParams<N> P)
             // idle slot: the unit cube with zero values keeps the point stage finite
 #pragma unroll
             for (int d = 0; d < 3; d++) s_u[d * ND + l] = 0.0;
+            if (JAC) {
+#pragma unroll
+                for (int d = 0; d < 3; d++) s_v[d * ND + l] = 0.0;
+            }
             for (int i = l; i < 24; i += ND) s_x[i] = (double)(((i / 3) >> (2 - i % 3)) & 1);
         }
         __syncthreads();
-        // ---- forward: values at the points, x then y then z (S_U -> S_T -> S_F -> S_U)
+        // ---- forward: values at the points, x then y then z (S_U -> S_T -> S_F -> S_U; the Jacobian's u:
+        //      S_V -> S_F[3..6) -> S_F[6..9) -> S_V)
         if (in_cta) {
 #pragma unroll
             for (int d = 0; d < 3; d++) s_t[d * ND + l] = pass1<N, 0, false>(P.B, s_u + d * ND, qi, qj, qk);
+            if (JAC) {
+#pragma unroll
+                for (int d = 0; d < 3; d++)
+                    s_f[(3 + d) * ND + l] = pass1<N, 0, false>(P.B, s_v + d * ND, qi, qj, qk);
+            }
         }
         __syncthreads();
         if (in_cta) {
 #pragma unroll
             for (int d = 0; d < 3; d++) s_f[d * ND + l] = pass1<N, 1, false>(P.B, s_t + d * ND, qi, qj, qk);
+            if (JAC) {
+#pragma unroll
+                for (int d = 0; d < 3; d++)
+                    s_f[(6 + d) * ND + l] = pass1<N, 1, false>(P.B, s_f + (3 + d) * ND, qi, qj, qk);
+            }
         }
         __syncthreads();
         if (in_cta) {
 #pragma unroll
             for (int d = 0; d < 3; d++) s_u[d * ND + l] = pass1<N, 2, false>(P.B, s_f + d * ND, qi, qj, qk);
+            if (JAC) {
+#pragma unroll
+                for (int d = 0; d < 3; d++)
+                    s_v[d * ND + l] = pass1<N, 2, false>(P.B, s_f + (6 + d) * ND, qi, qj, qk);
+            }
         }
         __syncthreads();
         // ---- point stage
@@ -197,6 +254,7 @@ elasticity_kernel(const __grid_constant__ ElasParams<N> P)
 #pragma unroll
                 for (int k = 0; k < 3; k++)
                     G[d][k] = (gh[d][0] * R[0][k] + gh[d][1] * R[1][k] + gh[d][2] * R[2][k]) * rdet;
+            if (MODE == EL_LINEAR) {
             const double ltr = P.lmbda * (G[0][0] + G[1][1] + G[2][2]);
             // fhat_d[m] = w |det| sum_k J^{-1}[m][k] sigma[d][k] = (w |det| / det) sum_k R[m][k] sigma[d][k]
             const double sw = w * fabs(det) * rdet;
@@ -209,6 +267,70 @@ elasticity_kernel(const __grid_constant__ ElasParams<N> P)
                 for (int m = 0; m < 3; m++)
                     s_f[(d * 3 + m) * ND + l] = sw * (R[m][0] * sg[0] + R[m][1] * sg[1] + R[m][2] * sg[2]);
                 mres[d] = P.beta * w * fabs(det) * s_u[d * ND + l];
+            }
+            } else {
+                // deformation gradient Fd = I + grad u: u's gradient is G (residual) or comes from S_V
+                double Fd[3][3];
+                if (JAC) {
+#pragma unroll
+                    for (int d = 0; d < 3; d++) {
+                        const double g0 = pass1<N, 0, false>(P.Dt, s_v + d * ND, qi, qj, qk);
+                        const double g1 = pass1<N, 1, false>(P.Dt, s_v + d * ND, qi, qj, qk);
+                        const double g2 = pass1<N, 2, false>(P.Dt, s_v + d * ND, qi, qj, qk);
+#pragma unroll
+                        for (int k = 0; k < 3; k++)
+                            Fd[d][k] = (k == d ? 1.0 : 0.0) + (g0 * R[0][k] + g1 * R[1][k] + g2 * R[2][k]) * rdet;
+                    }
+                } else {
+#pragma unroll
+                    for (int d = 0; d < 3; d++)
+#pragma unroll
+                        for (int k = 0; k < 3; k++) Fd[d][k] = (k == d ? 1.0 : 0.0) + G[d][k];
+                }
+                double cof[3][3];
+                const double detF = cofactors(Fd, cof);
+                const double rJ = 1.0 / detF;
+                const double lnJ = log(detF);
+                // Pk[d][k]: the first Piola-Kirchhoff stress (residual) or dP[H] with H = G (Jacobian)
+                double Pk[3][3];
+                if (JAC) {
+                    // tr(F^{-1} H) = cof : H / J;  C = F^{-1} H F^{-1}, C^T = F^{-T} H^T F^{-T}
+                    double trA = 0.0;
+#pragma unroll
+                    for (int a = 0; a < 3; a++)
+#pragma unroll
+                        for (int b = 0; b < 3; b++) trA = fma(cof[a][b], G[a][b], trA);
+                    trA *= rJ;
+                    double T[3][3];                        // T = H F^{-1} * J
+#pragma unroll
+                    for (int a = 0; a < 3; a++)
+#pragma unroll
+                        for (int d = 0; d < 3; d++)
+                            T[a][d] = G[a][0] * cof[d][0] + G[a][1] * cof[d][1] + G[a][2] * cof[d][2];
+                    const double c1 = (P.mu - P.lmbda * lnJ) * rJ * rJ;
+                    const double c2 = P.lmbda * trA * rJ;
+#pragma unroll
+                    for (int d = 0; d < 3; d++)
+#pragma unroll
+                        for (int k = 0; k < 3; k++)   // C[k][d] = sum_a F^{-1}[k][a] T[a][d] / J
+                            Pk[d][k] = P.mu * G[d][k] +
+                                       c1 * (cof[0][k] * T[0][d] + cof[1][k] * T[1][d] + cof[2][k] * T[2][d]) +
+                                       c2 * cof[d][k];
+                } else {
+                    const double c = (P.lmbda * lnJ - P.mu) * rJ;
+#pragma unroll
+                    for (int d = 0; d < 3; d++)
+#pragma unroll
+                        for (int k = 0; k < 3; k++) Pk[d][k] = P.mu * Fd[d][k] + c * cof[d][k];
+                }
+                const double sw = w * fabs(det) * rdet;
+#pragma unroll
+                for (int d = 0; d < 3; d++) {
+#pragma unroll
+                    for (int m = 0; m < 3; m++)
+                        s_f[(d * 3 + m) * ND + l] = sw * (R[m][0] * Pk[d][0] + R[m][1] * Pk[d][1] + R[m][2] * Pk[d][2]);
+                    mres[d] = P.beta * w * fabs(det) * s_u[d * ND + l];
+                }
             }
         }
         __syncthreads();
@@ -279,11 +401,11 @@ elasticity_kernel(const __grid_constant__ ElasParams<N> P)
     }
 }
 
-template <int N, bool MATRIX, bool ATOMIC>
+template <int N, bool MATRIX, bool ATOMIC, int MODE>
 int launch(cudaStream_t st, const ElasParams<N> &P, int sm_count)
 {
-    using S = ElasShape<N>;
-    auto kern = elasticity_kernel<N, MATRIX, ATOMIC>;
+    using S = ElasShape<N, MODE>;
+    auto kern = elasticity_kernel<N, MATRIX, ATOMIC, MODE>;
     static bool attr = false;
     if (!attr) {
         FDB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)S::SMEM));
@@ -320,9 +442,9 @@ void fill_tables(const fdb_kernel_s *k, ElasParams<N> &P)
     }
 }
 
-template <int N>
+template <int N, int MODE>
 int action_n(fdb_kernel_s *k, fdb_int start, fdb_int end, int nlay, const fdb_int *subset, double *y,
-             const double *coords, const double *x, const fdb_int *map0, const fdb_int *map1)
+             const double *coords, const double *x, const double *u, const fdb_int *map0, const fdb_int *map1)
 {
     fdb::Context &c = fdb::ctx();
     ElasParams<N> P;
@@ -330,6 +452,7 @@ int action_n(fdb_kernel_s *k, fdb_int start, fdb_int end, int nlay, const fdb_in
     fill_tables(k, P);
     P.y = y;
     P.x = x;
+    P.u = u;
     P.coords = coords;
     P.map0 = map0;
     P.map1 = map1;
@@ -341,7 +464,7 @@ int action_n(fdb_kernel_s *k, fdb_int start, fdb_int end, int nlay, const fdb_in
         P.lay_first = 0;
         P.lay_step = 1;
         if (P.ncols <= 0 || nlay <= 0) return 0;
-        return launch<N, false, true>(c.stream, P, c.sm_count);
+        return launch<N, false, true, MODE>(c.stream, P, c.sm_count);
     }
     // deterministic: one launch per (colour, layer parity), no two cells of a launch share a node
     if (subset) {
@@ -357,21 +480,22 @@ int action_n(fdb_kernel_s *k, fdb_int start, fdb_int end, int nlay, const fdb_in
             P.lay_step = 2;
             P.nlay_items = (nlay - par + 1) / 2;
             if (P.ncols <= 0 || P.nlay_items <= 0) continue;
-            if (launch<N, false, false>(c.stream, P, c.sm_count)) return 1;
+            if (launch<N, false, false, MODE>(c.stream, P, c.sm_count)) return 1;
         }
     }
     return 0;
 }
 
-template <int N>
+template <int N, int MODE>
 int matrix_n(fdb_kernel_s *k, fdb_int start, fdb_int end, int nlay, const fdb_int *subset, fdb_mat_t mat,
-             const double *coords, const fdb_int *map0, const fdb_int *map1, double *diag_out)
+             const double *coords, const double *u, const fdb_int *map0, const fdb_int *map1, double *diag_out)
 {
     fdb::Context &c = fdb::ctx();
     ElasParams<N> P;
     memset(&P, 0, sizeof(P));
     fill_tables(k, P);
     P.coords = coords;
+    P.u = u;
     P.map0 = map0;
     P.map1 = map1;
     if (mat) {
@@ -389,34 +513,64 @@ int matrix_n(fdb_kernel_s *k, fdb_int start, fdb_int end, int nlay, const fdb_in
     P.lay_first = 0;
     P.lay_step = 1;
     if (P.ncols <= 0 || nlay <= 0) return 0;
-    return launch<N, true, true>(c.stream, P, c.sm_count);
+    return launch<N, true, true, MODE>(c.stream, P, c.sm_count);
 }
 
-}  // namespace
-
-int fdb_launch_elasticity_action(fdb_kernel_s *k, fdb_int start, fdb_int end, int nlay, const fdb_int *subset,
-                                 double *y, const double *coords, const double *x, const fdb_int *map0,
-                                 const fdb_int *map1)
+template <int MODE>
+int action_mode(fdb_kernel_s *k, fdb_int start, fdb_int end, int nlay, const fdb_int *subset, double *y,
+                const double *coords, const double *x, const double *u, const fdb_int *map0, const fdb_int *map1)
 {
     switch (k->n1d) {
-    case 2: return action_n<2>(k, start, end, nlay, subset, y, coords, x, map0, map1);
-    case 3: return action_n<3>(k, start, end, nlay, subset, y, coords, x, map0, map1);
-    case 4: return action_n<4>(k, start, end, nlay, subset, y, coords, x, map0, map1);
-    case 5: return action_n<5>(k, start, end, nlay, subset, y, coords, x, map0, map1);
+    case 2: return action_n<2, MODE>(k, start, end, nlay, subset, y, coords, x, u, map0, map1);
+    case 3: return action_n<3, MODE>(k, start, end, nlay, subset, y, coords, x, u, map0, map1);
+    case 4: return action_n<4, MODE>(k, start, end, nlay, subset, y, coords, x, u, map0, map1);
+    case 5: return action_n<5, MODE>(k, start, end, nlay, subset, y, coords, x, u, map0, map1);
     }
     fdb::set_error("elasticity action: degree %d not instantiated (1..4)", k->n1d - 1);
     return 1;
 }
 
-int fdb_launch_elasticity_matrix(fdb_kernel_s *k, fdb_int start, fdb_int end, int nlay, const fdb_int *subset,
-                                 fdb_mat_t mat, const double *coords, const fdb_int *map0, const fdb_int *map1,
-                                 double *diag_out)
+template <int MODE>
+int matrix_mode(fdb_kernel_s *k, fdb_int start, fdb_int end, int nlay, const fdb_int *subset, fdb_mat_t mat,
+                const double *coords, const double *u, const fdb_int *map0, const fdb_int *map1, double *diag_out)
 {
     switch (k->n1d) {
-    case 2: return matrix_n<2>(k, start, end, nlay, subset, mat, coords, map0, map1, diag_out);
-    case 3: return matrix_n<3>(k, start, end, nlay, subset, mat, coords, map0, map1, diag_out);
-    case 4: return matrix_n<4>(k, start, end, nlay, subset, mat, coords, map0, map1, diag_out);
+    case 2: return matrix_n<2, MODE>(k, start, end, nlay, subset, mat, coords, u, map0, map1, diag_out);
+    case 3: return matrix_n<3, MODE>(k, start, end, nlay, subset, mat, coords, u, map0, map1, diag_out);
+    case 4: return matrix_n<4, MODE>(k, start, end, nlay, subset, mat, coords, u, map0, map1, diag_out);
     }
     fdb::set_error("elasticity matrix: degree %d not instantiated (1..3)", k->n1d - 1);
+    return 1;
+}
+
+}  // namespace
+
+int fdb_launch_elasticity_action(fdb_kernel_s *k, fdb_int start, fdb_int end, int nlay, const fdb_int *subset,
+                                 double *y, const double *coords, const double *x, const double *u,
+                                 const fdb_int *map0, const fdb_int *map1)
+{
+    switch (k->desc.form) {
+    case FDB_FORM_ELASTICITY:
+        return action_mode<EL_LINEAR>(k, start, end, nlay, subset, y, coords, x, nullptr, map0, map1);
+    case FDB_FORM_HYPERELASTICITY:
+        return action_mode<EL_RESIDUAL>(k, start, end, nlay, subset, y, coords, x, nullptr, map0, map1);
+    case FDB_FORM_HYPERELASTICITY_JACOBIAN:
+        return action_mode<EL_JACOBIAN>(k, start, end, nlay, subset, y, coords, x, u, map0, map1);
+    }
+    fdb::set_error("elasticity action: form %d is not an elasticity form", k->desc.form);
+    return 1;
+}
+
+int fdb_launch_elasticity_matrix(fdb_kernel_s *k, fdb_int start, fdb_int end, int nlay, const fdb_int *subset,
+                                 fdb_mat_t mat, const double *coords, const double *u, const fdb_int *map0,
+                                 const fdb_int *map1, double *diag_out)
+{
+    switch (k->desc.form) {
+    case FDB_FORM_ELASTICITY:
+        return matrix_mode<EL_LINEAR>(k, start, end, nlay, subset, mat, coords, nullptr, map0, map1, diag_out);
+    case FDB_FORM_HYPERELASTICITY_JACOBIAN:
+        return matrix_mode<EL_JACOBIAN>(k, start, end, nlay, subset, mat, coords, u, map0, map1, diag_out);
+    }
+    fdb::set_error("elasticity matrix: form %d has no element matrix", k->desc.form);
     return 1;
 }

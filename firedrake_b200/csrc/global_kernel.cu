@@ -302,28 +302,37 @@ int fdb_kernel_create(const fdb_kernel_desc *d, fdb_kernel_t *out)
                       d->rank == 2 ? "matrix" : (d->diagonal ? "diagonal" : "action"), d->degree, maxdeg);
             return 1;
         }
-    } else if (d->form == FDB_FORM_ELASTICITY) {
-        // coupled vector form: elasticity_hex.cu (never the DMMA element-matrix kernels)
+    } else if (d->form == FDB_FORM_ELASTICITY || d->form == FDB_FORM_HYPERELASTICITY ||
+               d->form == FDB_FORM_HYPERELASTICITY_JACOBIAN) {
+        // coupled vector forms: elasticity_hex.cu (never the DMMA element-matrix kernels)
+        const char *name = d->form == FDB_FORM_ELASTICITY
+                               ? "elasticity"
+                               : (d->form == FDB_FORM_HYPERELASTICITY ? "hyperelasticity" : "hyperelasticity_jacobian");
         if (d->cell != FDB_CELL_HEX_EXTRUDED && d->cell != FDB_CELL_HEX) {
-            set_error("fdb_kernel_create: elasticity needs hex cells (extruded or native), got cell %d", d->cell);
+            set_error("fdb_kernel_create: %s needs hex cells (extruded or native), got cell %d", name, d->cell);
             return 1;
         }
         if (d->cdim != 3) {
-            set_error("fdb_kernel_create: elasticity needs a vector space of value size 3 (cdim %d)", d->cdim);
+            set_error("fdb_kernel_create: %s needs a vector space of value size 3 (cdim %d)", name, d->cdim);
             return 1;
         }
         if (d->affine_cells) {
-            set_error("fdb_kernel_create: elasticity has no affine-cell variant (affine_cells must be 0)");
+            set_error("fdb_kernel_create: %s has no affine-cell variant (affine_cells must be 0)", name);
             return 1;
         }
         if (d->nq != d->degree + 1) {
-            set_error("fdb_kernel_create: elasticity needs nq == degree+1 Gauss points per axis (got nq=%d for "
-                      "degree %d)", d->nq, d->degree);
+            set_error("fdb_kernel_create: %s needs nq == degree+1 Gauss points per axis (got nq=%d for "
+                      "degree %d)", name, d->nq, d->degree);
+            return 1;
+        }
+        if (d->form == FDB_FORM_HYPERELASTICITY && (d->rank != 1 || d->diagonal)) {
+            set_error("fdb_kernel_create: hyperelasticity is the residual, a 1-form action only: its matrix and "
+                      "diagonal are those of hyperelasticity_jacobian");
             return 1;
         }
         const int maxdeg = (d->rank == 2 || d->diagonal) ? 3 : 4;
         if (d->degree < 1 || d->degree > maxdeg) {
-            set_error("fdb_kernel_create: elasticity %s: degree %d outside 1..%d",
+            set_error("fdb_kernel_create: %s %s: degree %d outside 1..%d", name,
                       d->rank == 2 ? "matrix" : (d->diagonal ? "diagonal" : "action"), d->degree, maxdeg);
             return 1;
         }
@@ -469,7 +478,9 @@ int fdb_kernel_call(fdb_kernel_t k, const fdb_call_args *a)
     const bool nl_jac = k->desc.form == FDB_FORM_NONLINEAR_DIFFUSION_JACOBIAN;
     const bool coef = k->desc.form == FDB_FORM_HELMHOLTZ_COEF || nl_jac;
     const bool nl_res = k->desc.form == FDB_FORM_NONLINEAR_DIFFUSION;
-    const bool elas = k->desc.form == FDB_FORM_ELASTICITY;
+    // the elasticity kernel's forms; the hyperelastic Jacobian has a trailing u
+    const bool hyper_jac = k->desc.form == FDB_FORM_HYPERELASTICITY_JACOBIAN;
+    const bool elas = k->desc.form == FDB_FORM_ELASTICITY || k->desc.form == FDB_FORM_HYPERELASTICITY || hyper_jac;
     const char *cname = nl_jac ? "nonlinear_diffusion_jacobian" : "helmholtz_coef";
     const char *cvar = nl_jac ? "u" : "kappa";
     if (coef && k->desc.rank == 2) {
@@ -525,7 +536,11 @@ int fdb_kernel_call(fdb_kernel_t k, const fdb_call_args *a)
         // 2-form: args = [Mat handle (INC), coords (READ)], maps = [V map, coord map]
         // (the reference passes the PETSc Mat handle in the same slot:
         // pyop2/types/mat.py:621-623)
-        if (a->nargs != 2 || a->nmaps != 2) {
+        if (hyper_jac && (a->nargs != 3 || a->nmaps != 2)) {
+            set_error("fdb_kernel_call: hyperelasticity_jacobian 2-form expects 3 args (mat, coords, u) and 2 maps");
+            return 1;
+        }
+        if (!hyper_jac && (a->nargs != 2 || a->nmaps != 2)) {
             set_error("fdb_kernel_call: 2-form expects 2 args (mat, coords) and 2 maps");
             return 1;
         }
@@ -542,6 +557,7 @@ int fdb_kernel_call(fdb_kernel_t k, const fdb_call_args *a)
             return 1;
         }
         const double *dcoords;
+        const double *du = hyper_jac ? (const double *)a->args[2] : nullptr;
         const fdb_int *dm[2];
         const fdb_int *dsub = a->subset;
         if (a->location == FDB_LOC_HOST) {
@@ -550,6 +566,12 @@ int fdb_kernel_call(fdb_kernel_t k, const fdb_call_args *a)
             if (!a->arg_versions) fdb_mirror_drop(a->args[1]);
             if (fdb_mirror_acquire(a->args[1], a->arg_bytes[1], ver, 1, &p)) return 1;
             dcoords = (const double *)p;
+            if (hyper_jac) {
+                if (!a->arg_versions) fdb_mirror_drop(a->args[2]);
+                if (fdb_mirror_acquire(a->args[2], a->arg_bytes[2], a->arg_versions ? a->arg_versions[2] : 0, 1, &p))
+                    return 1;
+                du = (const double *)p;
+            }
             for (int i = 0; i < 2; i++) {
                 if (fdb_mirror_acquire(a->maps[i], a->map_bytes[i], map_ver(a, i), 1, &p)) return 1;
                 dm[i] = (const fdb_int *)p;
@@ -564,8 +586,8 @@ int fdb_kernel_call(fdb_kernel_t k, const fdb_call_args *a)
             dm[1] = a->maps[1];
         }
         if (elas)
-            return fdb_launch_elasticity_matrix(k, a->start, a->end, nlay, dsub, target, dcoords, dm[0], dm[1],
-                                                nullptr);
+            return fdb_launch_elasticity_matrix(k, a->start, a->end, nlay, dsub, target, dcoords, du, dm[0],
+                                                dm[1], nullptr);
         if (mat_bs == 1)
             return fdb_launch_helmholtz_matrix(k, a->start, a->end, nlay, dsub, target, dcoords, dm[0], dm[1],
                                                nullptr);
@@ -589,13 +611,17 @@ int fdb_kernel_call(fdb_kernel_t k, const fdb_call_args *a)
                                                 a->maps[0], a->maps[1], (double *)a->args[0]);
     }
     if (elas && k->desc.diagonal) {
-        // args = [d (INC, 3 values per node), coords]; device-resident only
-        if (a->nargs != 2 || a->nmaps != 2 || a->location != FDB_LOC_DEVICE) {
-            set_error("fdb_kernel_call: elasticity diagonal expects 2 device args (d, coords) and 2 maps");
+        // args = [d (INC, 3 values per node), coords] (hyperelasticity_jacobian: [d, coords, u]); device-resident
+        // only
+        if (a->nargs != (hyper_jac ? 3 : 2) || a->nmaps != 2 || a->location != FDB_LOC_DEVICE) {
+            set_error(hyper_jac ? "fdb_kernel_call: hyperelasticity_jacobian diagonal expects 3 device args (d, "
+                                  "coords, u) and 2 maps"
+                                : "fdb_kernel_call: elasticity diagonal expects 2 device args (d, coords) and 2 maps");
             return 1;
         }
         return fdb_launch_elasticity_matrix(k, a->start, a->end, nlay, a->subset, nullptr,
-                                            (const double *)a->args[1], a->maps[0], a->maps[1],
+                                            (const double *)a->args[1],
+                                            hyper_jac ? (const double *)a->args[2] : nullptr, a->maps[0], a->maps[1],
                                             (double *)a->args[0]);
     }
     if (k->desc.diagonal) {
@@ -616,13 +642,18 @@ int fdb_kernel_call(fdb_kernel_t k, const fdb_call_args *a)
                   cname, cvar, a->nargs, a->nmaps);
         return 1;
     }
-    if (!coef && (a->nargs != 3 || a->nmaps != 2)) {
+    if (hyper_jac && (a->nargs != 4 || a->nmaps != 2)) {
+        set_error("fdb_kernel_call: hyperelasticity_jacobian 1-form expects 4 args (y, coords, w, u) and 2 maps, "
+                  "got %d/%d", a->nargs, a->nmaps);
+        return 1;
+    }
+    if (!coef && !hyper_jac && (a->nargs != 3 || a->nmaps != 2)) {
         set_error("fdb_kernel_call: 1-form expects 3 args (y, coords, x) and 2 maps, got %d/%d",
                   a->nargs, a->nmaps);
         return 1;
     }
     // the pipelined host action moves x and y only and runs the constant-coefficient kernels: the
-    // coefficient, nonlinear and elasticity forms take the monolithic path
+    // coefficient, nonlinear and elasticity-kernel forms take the monolithic path
     if (!coef && !nl_res && !elas && a->location == FDB_LOC_HOST && a->arg_versions && a->arg_bytes && a->map_bytes &&
         a->writeback && a->output_is_zero && !a->subset && extruded &&
         k->desc.scatter == FDB_SCATTER_ATOMIC) {
@@ -686,7 +717,8 @@ int fdb_kernel_call(fdb_kernel_t k, const fdb_call_args *a)
     }
     // (the residual: the coefficient entry point without a coefficient, see action_hex.cu)
     int rc = elas ? fdb_launch_elasticity_action(k, a->start, a->end, nlay, dsubset, (double *)dargs[0],
-                                                 (const double *)dargs[1], (const double *)dargs[2], dmaps[0],
+                                                 (const double *)dargs[1], (const double *)dargs[2],
+                                                 hyper_jac ? (const double *)dargs[3] : nullptr, dmaps[0],
                                                  dmaps[1])
              : (coef || nl_res)
                  ? fdb_launch_helmholtz_coef_action(k, a->start, a->end, nlay, dsubset, (double *)dargs[0],

@@ -1373,6 +1373,13 @@ class Kernel:
     (``mu``, ``lmbda``; ``alpha`` is not used).  Its arguments are those of the constant-coefficient
     form: action (INC, READ, READ), diagonal and rank 2 (INC, READ); the rank-2 target is a Mat of block
     size 3, every 3 x 3 block filled.
+
+    "hyperelasticity" is the residual of compressible Neo-Hookean hyperelasticity on a vector space
+    (``cdim=3``), ``inner(P(F), grad(v))*dx + beta*inner(u, v)*dx`` with ``F = I + grad(u)``, ``J =
+    det(F)`` and ``P(F) = mu*(F - F^{-T}) + lmbda*ln(J)*F^{-T}``: a rank-1 action only (INC, READ, READ:
+    output, coordinates, u).  "hyperelasticity_jacobian" is its Gateaux derivative at u, with u as the
+    LAST argument: action (output, coordinates, w, u), diagonal and rank 2 (output, coordinates, u).
+    Its matrix is symmetric.
     """
     form: str = "helmholtz"
     degree: int = 1
@@ -1390,7 +1397,7 @@ class Kernel:
     # tabulation: a fiat_lite.Interval1D, or None for the default GLL/Gauss pair
     element: object = field(default=None, compare=False, hash=False)
     d: tuple = (1.0, 0.0, 0.0)      # nonlinear diffusion: D(s) = d[0] + d[1] s + d[2] s^2
-    mu: float = 1.0                 # elasticity: Lame parameters
+    mu: float = 1.0                 # (hyper)elasticity: Lame parameters
     lmbda: float = 0.0
 
     def __new__(cls, *args, **kwargs):
@@ -1407,9 +1414,9 @@ class Kernel:
             object.__setattr__(self, "d", tuple(float(c) for c in self.d))
             if len(self.d) != 3:
                 raise ValueError("d holds the three coefficients of D(s) = d0 + d1 s + d2 s^2")
-        if self.form == "nonlinear_diffusion":
+        if self.form in ("nonlinear_diffusion", "hyperelasticity"):
             return                       # residual: (INC, READ, READ), like the constant-coefficient action
-        if self.form in ("helmholtz_coef", "nonlinear_diffusion_jacobian"):
+        if self.form in ("helmholtz_coef", "nonlinear_diffusion_jacobian", "hyperelasticity_jacobian"):
             acc = (INC, READ, READ) if (self.diagonal or self.rank == 2) else (INC, READ, READ, READ)
             object.__setattr__(self, "accesses", acc)
             if self.rank == 2 and self.name == "form0_cell_integral":
@@ -1437,7 +1444,8 @@ class Kernel:
 _FORMS = {"helmholtz": _lib.FORM_HELMHOLTZ, "dg_advection": _lib.FORM_DG_ADVECTION,
           "helmholtz_coef": _lib.FORM_HELMHOLTZ_COEF, "nonlinear_diffusion": _lib.FORM_NONLINEAR_DIFFUSION,
           "nonlinear_diffusion_jacobian": _lib.FORM_NONLINEAR_DIFFUSION_JACOBIAN,
-          "elasticity": _lib.FORM_ELASTICITY}
+          "elasticity": _lib.FORM_ELASTICITY, "hyperelasticity": _lib.FORM_HYPERELASTICITY,
+          "hyperelasticity_jacobian": _lib.FORM_HYPERELASTICITY_JACOBIAN}
 _INTEGRALS = {"cell": _lib.INTEGRAL_CELL, "exterior_facet": _lib.INTEGRAL_EXTERIOR_FACET,
               "interior_facet": _lib.INTEGRAL_INTERIOR_FACET, "fused": _lib.INTEGRAL_FUSED}
 
@@ -1523,7 +1531,7 @@ class GlobalKernel:
         d.affine_cells = int(lk.affine and lk.rank == 1 and not lk.diagonal)
         for i in range(3):
             d.dcoef[i] = lk.d[i]
-        if lk.form == "elasticity":
+        if lk.form in ("elasticity", "hyperelasticity", "hyperelasticity_jacobian"):
             d.alpha, d.lmbda = lk.mu, lk.lmbda
         for q in range(el.nq):
             d.wq[q] = el.wq[q]
@@ -1682,7 +1690,7 @@ class Parloop:
                     it._dev_idx = DeviceArray.from_host(it.indices)
                 subset = it._dev_idx.ptr
             # coordinates, then the coefficient field of a helmholtz_coef form (the linearisation
-            # point of a nonlinear_diffusion_jacobian)
+            # point of a nonlinear_diffusion_jacobian or hyperelasticity_jacobian)
             ins = [a.data.device_ptr for a in self.args[1:]]
             try:
                 gk(start, end, layers, subset, [out.handle.value] + ins, None, None,

@@ -139,7 +139,7 @@ enum fdb_form {
                                      diagonal  [d INC, coords, u]      (device mode)
                                      rank 2    [Mat, coords, u]  (row = test dof, column = trial dof)
                                    Never the DMMA element-matrix kernels (they assume symmetry).  */
-    FDB_FORM_ELASTICITY = 6
+    FDB_FORM_ELASTICITY = 6,
                                 /* linear elasticity on a vector space (value size 3, AoS):
                                      a(u, v) = inner(sigma(u), grad v)*dx + beta*inner(u, v)*dx,
                                      sigma(u) = mu (grad u + grad u^T) + lmbda tr(grad u) I
@@ -155,6 +155,26 @@ enum fdb_form {
                                                column = trial dof; dof-level lgmaps)
                                    Never the DMMA element-matrix kernels ("matrix_kernel" does not
                                    apply).                                                          */
+    FDB_FORM_HYPERELASTICITY = 7,
+                                /* residual of compressible Neo-Hookean hyperelasticity (value size 3):
+                                     F = I + grad u,  J = det F,
+                                     P(F) = mu (F - F^{-T}) + lmbda ln(J) F^{-T}
+                                     R(u; v) = inner(P(F), grad v)*dx + beta*inner(u, v)*dx
+                                   mu = alpha, lmbda and beta as for FDB_FORM_ELASTICITY.  J <= 0 at
+                                   a Gauss point gives NaN, as ln J does.  Same cells and restrictions
+                                   as FDB_FORM_ELASTICITY; rank 1 action only (not rank 2, not
+                                   diagonal), degrees 1..4:  [y INC, coords, u]  (atomic or coloured;
+                                   device or host mode, host mode monolithic).                      */
+    FDB_FORM_HYPERELASTICITY_JACOBIAN = 8
+                                /* its Gateaux derivative at u (exact Newton Jacobian, symmetric):
+                                     J(u)[w; v] = inner(dP[grad w], grad v)*dx + beta*inner(w, v)*dx
+                                     dP[H] = mu H + (mu - lmbda ln J) F^{-T} H^T F^{-T}
+                                             + lmbda tr(F^{-1} H) F^{-T}
+                                   Degrees 1..4 (action), 1..3 (rank 2 and diagonal).  u is always
+                                   the LAST argument, gathered through maps[0]:
+                                     action    [y INC, coords, w, u]  (device or host mode)
+                                     diagonal  [d INC, coords, u]     (device mode)
+                                     rank 2    [Mat (block size 3), coords, u]                      */
 };
 
 enum fdb_cell {
@@ -217,7 +237,8 @@ typedef struct fdb_kernel_desc {
     /* FDB_FORM_NONLINEAR_DIFFUSION[_JACOBIAN]: D(s) = dcoef[0] + dcoef[1] s + dcoef[2] s^2.
      * Ignored by every other form (a zeroed descriptor stays valid for them). */
     double dcoef[3];
-    /* FDB_FORM_ELASTICITY: the Lame parameter lambda (mu is alpha).  Ignored by every other form. */
+    /* FDB_FORM_ELASTICITY, FDB_FORM_HYPERELASTICITY[_JACOBIAN]: the Lame parameter lambda (mu is
+     * alpha).  Ignored by every other form. */
     double lmbda;
 } fdb_kernel_desc;
 
