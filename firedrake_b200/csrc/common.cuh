@@ -54,6 +54,7 @@ int require_init();
 extern int fdb_opt_matrix_kernel;   // fdb_set_option("matrix_kernel", ...)
 
 struct fdb_jit_s;   // NVRTC-compiled generic wrapper (wrapper_jit.cu)
+struct fdb_hex_form;   // a form of the hand-written hex kernels (global_kernel.cu)
 
 // kernel object behind fdb_kernel_t
 struct fdb_kernel_s {
@@ -76,6 +77,8 @@ struct fdb_kernel_s {
     double *d_bdb_table = nullptr;
     // non-NULL: this handle is a generated wrapper around an arbitrary local kernel
     fdb_jit_s *jit = nullptr;
+    // the form's row for the hex kernels; NULL for DG advection, P1 triangles and generated wrappers
+    const fdb_hex_form *hex = nullptr;
 };
 
 int fdb_jit_call(fdb_kernel_s *k, const fdb_call_args *a);

@@ -233,7 +233,81 @@ static int pipelined_host_action(fdb_kernel_s *k, const fdb_call_args *a, int nl
     return 0;
 }
 
+// The call's pointers on the device.  Device mode passes them through.  Host mode mirrors every Dat
+// argument (not the Mat handle in args[0] of a matrix call), both maps and the subset; an output the
+// caller has just zeroed is zero-filled on the device instead of uploaded.
+static int device_pointers(const fdb_call_args *a, bool mat, void **args, const fdb_int **maps,
+                           const fdb_int **subset)
+{
+    for (int i = 0; i < a->nargs; i++) args[i] = a->args[i];
+    for (int i = 0; i < 2; i++) maps[i] = a->maps[i];
+    *subset = a->subset;
+    if (a->location != FDB_LOC_HOST) return 0;
+    if (!a->arg_bytes || !a->map_bytes) {
+        set_error("fdb_kernel_call: host mode needs arg_bytes and map_bytes");
+        return 1;
+    }
+    for (int i = mat ? 1 : 0; i < a->nargs; i++) {
+        // without versions every call re-uploads (drop-in default: the
+        // reference hands over live NumPy buffers)
+        if (!a->arg_versions) fdb_mirror_drop(a->args[i]);
+        const bool zero_out = (i == 0 && a->output_is_zero);
+        if (fdb_mirror_acquire(a->args[i], a->arg_bytes[i], a->arg_versions ? a->arg_versions[i] : 0,
+                               zero_out ? 0 : 1, &args[i]))
+            return 1;
+        if (zero_out) FDB_CUDA(cudaMemsetAsync(args[i], 0, a->arg_bytes[i], ctx().stream));
+    }
+    void *p;
+    for (int i = 0; i < 2; i++) {
+        if (fdb_mirror_acquire(a->maps[i], a->map_bytes[i], map_ver(a, i), 1, &p)) return 1;
+        maps[i] = (const fdb_int *)p;
+    }
+    if (a->subset) {
+        if (fdb_mirror_acquire(a->subset, sizeof(fdb_int) * (size_t)a->end, a->subset_version, 1, &p)) return 1;
+        *subset = (const fdb_int *)p;
+    }
+    return 0;
+}
+
 }  // namespace
+
+// The forms of the hand-written hex kernels: what fdb_kernel_create accepts for each and how
+// fdb_kernel_call hands its arguments to the launchers.
+enum { MODE_ACTION, MODE_MATRIX, MODE_DIAGONAL };
+enum { LAUNCH_HELMHOLTZ, LAUNCH_HELMHOLTZ_COEF, LAUNCH_ELASTICITY };
+
+struct fdb_hex_form {
+    int form;                 // enum fdb_form
+    const char *name;
+    int cdim;                 // value size of the argument space; 0: any of 1..3, the diagonal scalar only
+    bool affine;              // has the affine_cells variant
+    const char *coef;         // the trailing coefficient argument, or NULL
+    bool residual;            // a 1-form action only
+    int launcher;             // fdb_launch_helmholtz_*, fdb_launch_helmholtz_coef_* (which also run the
+                              // nonlinear diffusion forms) or fdb_launch_elasticity_*
+    int max_degree[3];        // per mode: action, matrix, diagonal
+};
+
+static const fdb_hex_form hex_forms[] = {
+    {FDB_FORM_HELMHOLTZ, "helmholtz", 0, true, nullptr, false, LAUNCH_HELMHOLTZ, {5, 4, 3}},
+    {FDB_FORM_HELMHOLTZ_COEF, "helmholtz_coef", 1, false, "kappa", false, LAUNCH_HELMHOLTZ_COEF, {5, 4, 3}},
+    {FDB_FORM_NONLINEAR_DIFFUSION, "nonlinear_diffusion", 1, false, nullptr, true, LAUNCH_HELMHOLTZ_COEF,
+     {5, 0, 0}},
+    {FDB_FORM_NONLINEAR_DIFFUSION_JACOBIAN, "nonlinear_diffusion_jacobian", 1, false, "u", false,
+     LAUNCH_HELMHOLTZ_COEF, {5, 4, 3}},
+    {FDB_FORM_ELASTICITY, "elasticity", 3, false, nullptr, false, LAUNCH_ELASTICITY, {4, 3, 3}},
+    {FDB_FORM_HYPERELASTICITY, "hyperelasticity", 3, false, nullptr, true, LAUNCH_ELASTICITY, {4, 0, 0}},
+    {FDB_FORM_HYPERELASTICITY_JACOBIAN, "hyperelasticity_jacobian", 3, false, "u", false, LAUNCH_ELASTICITY,
+     {4, 3, 3}},
+};
+
+static const char *const mode_name[] = {"action", "matrix", "diagonal"};
+
+// rank 2 is the matrix whatever the diagonal flag says
+static int hex_mode(const fdb_kernel_desc *d)
+{
+    return d->rank == 2 ? MODE_MATRIX : (d->diagonal ? MODE_DIAGONAL : MODE_ACTION);
+}
 
 extern "C" {
 
@@ -273,97 +347,51 @@ int fdb_kernel_create(const fdb_kernel_desc *d, fdb_kernel_t *out)
         *out = k;
         return 0;
     }
-    const bool nl_res = d->form == FDB_FORM_NONLINEAR_DIFFUSION;
-    const bool nl_jac = d->form == FDB_FORM_NONLINEAR_DIFFUSION_JACOBIAN;
-    if (d->form == FDB_FORM_HELMHOLTZ_COEF || nl_res || nl_jac) {
-        // kappa (or the nonlinear diffusion's u) in the scalar argument space: the slab-thread kernel
-        // with its coefficient stage, or the residual's D(u) weight
-        const char *name = nl_res ? "nonlinear_diffusion" : (nl_jac ? "nonlinear_diffusion_jacobian" : "helmholtz_coef");
-        if (d->cell != FDB_CELL_HEX_EXTRUDED && d->cell != FDB_CELL_HEX) {
-            set_error("fdb_kernel_create: %s needs hex cells (extruded or native), got cell %d", name, d->cell);
-            return 1;
-        }
-        if (d->cdim != 1) {
-            set_error("fdb_kernel_create: %s takes scalar spaces only (cdim %d)", name, d->cdim);
-            return 1;
-        }
-        if (d->affine_cells) {
-            set_error("fdb_kernel_create: %s has no affine-cell variant (affine_cells must be 0)", name);
-            return 1;
-        }
-        if (nl_res && (d->rank != 1 || d->diagonal)) {
-            set_error("fdb_kernel_create: nonlinear_diffusion is the residual, a 1-form action only: its matrix "
-                      "and diagonal are those of nonlinear_diffusion_jacobian");
-            return 1;
-        }
-        const int maxdeg = d->rank == 2 ? 4 : (d->diagonal ? 3 : 5);
-        if (d->degree < 1 || d->degree > maxdeg) {
-            set_error("fdb_kernel_create: %s %s: degree %d outside 1..%d", name,
-                      d->rank == 2 ? "matrix" : (d->diagonal ? "diagonal" : "action"), d->degree, maxdeg);
-            return 1;
-        }
-    } else if (d->form == FDB_FORM_ELASTICITY || d->form == FDB_FORM_HYPERELASTICITY ||
-               d->form == FDB_FORM_HYPERELASTICITY_JACOBIAN) {
-        // coupled vector forms: elasticity_hex.cu (never the DMMA element-matrix kernels)
-        const char *name = d->form == FDB_FORM_ELASTICITY
-                               ? "elasticity"
-                               : (d->form == FDB_FORM_HYPERELASTICITY ? "hyperelasticity" : "hyperelasticity_jacobian");
-        if (d->cell != FDB_CELL_HEX_EXTRUDED && d->cell != FDB_CELL_HEX) {
-            set_error("fdb_kernel_create: %s needs hex cells (extruded or native), got cell %d", name, d->cell);
-            return 1;
-        }
-        if (d->cdim != 3) {
-            set_error("fdb_kernel_create: %s needs a vector space of value size 3 (cdim %d)", name, d->cdim);
-            return 1;
-        }
-        if (d->affine_cells) {
-            set_error("fdb_kernel_create: %s has no affine-cell variant (affine_cells must be 0)", name);
-            return 1;
-        }
-        if (d->nq != d->degree + 1) {
-            set_error("fdb_kernel_create: %s needs nq == degree+1 Gauss points per axis (got nq=%d for "
-                      "degree %d)", name, d->nq, d->degree);
-            return 1;
-        }
-        if (d->form == FDB_FORM_HYPERELASTICITY && (d->rank != 1 || d->diagonal)) {
-            set_error("fdb_kernel_create: hyperelasticity is the residual, a 1-form action only: its matrix and "
-                      "diagonal are those of hyperelasticity_jacobian");
-            return 1;
-        }
-        const int maxdeg = (d->rank == 2 || d->diagonal) ? 3 : 4;
-        if (d->degree < 1 || d->degree > maxdeg) {
-            set_error("fdb_kernel_create: %s %s: degree %d outside 1..%d", name,
-                      d->rank == 2 ? "matrix" : (d->diagonal ? "diagonal" : "action"), d->degree, maxdeg);
-            return 1;
-        }
-    } else if (d->form != FDB_FORM_HELMHOLTZ) {
+    const fdb_hex_form *f = nullptr;
+    for (const fdb_hex_form &row : hex_forms)
+        if (row.form == d->form) f = &row;
+    if (!f) {
         set_error("fdb_kernel_create: form %d is not in the supported set", d->form);
         return 1;
     }
+    const int mode = hex_mode(d);
     if (d->cell != FDB_CELL_HEX_EXTRUDED && d->cell != FDB_CELL_HEX) {
-        set_error("fdb_kernel_create: cell type %d not supported for form %d", d->cell, d->form);
+        set_error("fdb_kernel_create: %s needs hex cells (extruded or native), got cell %d", f->name, d->cell);
         return 1;
     }
-    if (d->integral != FDB_INTEGRAL_CELL) {
-        set_error("fdb_kernel_create: Helmholtz-family forms only have cell integrals");
+    const int cdim = f->cdim ? f->cdim : (mode == MODE_DIAGONAL ? 1 : 0);
+    if (cdim ? d->cdim != cdim : (d->cdim < 1 || d->cdim > 3)) {
+        set_error("fdb_kernel_create: %s %s takes %s (cdim %d)", f->name, mode_name[mode],
+                  cdim == 1 ? "scalar spaces only"
+                            : (cdim == 3 ? "a vector space of value size 3 only" : "value sizes 1..3"),
+                  d->cdim);
         return 1;
     }
-    if (d->degree < 1 || d->degree > 5) {
-        set_error("fdb_kernel_create: degree %d outside 1..5", d->degree);
+    if (d->affine_cells && !f->affine) {
+        set_error("fdb_kernel_create: %s has no affine-cell variant (affine_cells must be 0)", f->name);
         return 1;
     }
     if (d->nq != d->degree + 1) {
-        set_error("fdb_kernel_create: hex kernels need nq == degree+1 Gauss points per axis "
-                  "(got nq=%d for degree %d); pin the rule with dx(degree=2*p)",
-                  d->nq, d->degree);
+        set_error("fdb_kernel_create: %s needs nq == degree+1 Gauss points per axis (got nq=%d for degree %d); "
+                  "pin the rule with dx(degree=2*p)", f->name, d->nq, d->degree);
+        return 1;
+    }
+    if (f->residual && mode != MODE_ACTION) {
+        set_error("fdb_kernel_create: %s is the residual, a 1-form action only: its matrix and diagonal are those "
+                  "of %s_jacobian", f->name, f->name);
+        return 1;
+    }
+    if (d->degree < 1 || d->degree > f->max_degree[mode]) {
+        set_error("fdb_kernel_create: %s %s: degree %d outside 1..%d", f->name, mode_name[mode], d->degree,
+                  f->max_degree[mode]);
+        return 1;
+    }
+    if (d->integral != FDB_INTEGRAL_CELL) {
+        set_error("fdb_kernel_create: %s has cell integrals only", f->name);
         return 1;
     }
     if (d->rank != 1 && d->rank != 2) {
         set_error("fdb_kernel_create: rank must be 1 or 2");
-        return 1;
-    }
-    if (d->cdim < 1 || d->cdim > 3) {
-        set_error("fdb_kernel_create: cdim %d outside 1..3", d->cdim);
         return 1;
     }
     if (d->cell == FDB_CELL_HEX_EXTRUDED && (!d->offset0 || !d->offset1)) {
@@ -372,6 +400,7 @@ int fdb_kernel_create(const fdb_kernel_desc *d, fdb_kernel_t *out)
     }
     fdb_kernel_s *k = new fdb_kernel_s;
     k->desc = *d;
+    k->hex = f;
     k->n1d = d->degree + 1;
     k->arity = k->n1d * k->n1d * k->n1d;
     memset(k->h_off0, 0, sizeof(k->h_off0));
@@ -473,80 +502,23 @@ int fdb_kernel_call(fdb_kernel_t k, const fdb_call_args *a)
         set_error("fdb_kernel_call: iteration set too large for IntType");
         return 1;
     }
-    // forms with a trailing coefficient argument (kappa; the nonlinear diffusion Jacobian's u), and the
-    // nonlinear diffusion residual, whose args are those of the constant-coefficient action
-    const bool nl_jac = k->desc.form == FDB_FORM_NONLINEAR_DIFFUSION_JACOBIAN;
-    const bool coef = k->desc.form == FDB_FORM_HELMHOLTZ_COEF || nl_jac;
-    const bool nl_res = k->desc.form == FDB_FORM_NONLINEAR_DIFFUSION;
-    // the elasticity kernel's forms; the hyperelastic Jacobian has a trailing u
-    const bool hyper_jac = k->desc.form == FDB_FORM_HYPERELASTICITY_JACOBIAN;
-    const bool elas = k->desc.form == FDB_FORM_ELASTICITY || k->desc.form == FDB_FORM_HYPERELASTICITY || hyper_jac;
-    const char *cname = nl_jac ? "nonlinear_diffusion_jacobian" : "helmholtz_coef";
-    const char *cvar = nl_jac ? "u" : "kappa";
-    if (coef && k->desc.rank == 2) {
-        // args = [Mat handle (INC), coords (READ), kappa (READ)], maps = [V map, coord map]
-        if (a->nargs != 3 || a->nmaps != 2) {
-            set_error("fdb_kernel_call: %s 2-form expects 3 args (mat, coords, %s) and 2 maps", cname, cvar);
-            return 1;
-        }
-        fdb_mat_t target = (fdb_mat_t)a->args[0];
-        int mat_bs = 1;
-        fdb_mat_block_size(target, &mat_bs);
-        if (mat_bs != 1) {
-            set_error("fdb_kernel_call: %s assembles scalar matrices only (block size %d)", cname, mat_bs);
-            return 1;
-        }
-        if (k->desc.scatter != FDB_SCATTER_ATOMIC) {
-            set_error("fdb_kernel_call: coloured scatter is not implemented for matrices");
-            return 1;
-        }
-        const void *din[2];
-        const fdb_int *dm[2];
-        const fdb_int *dsub = a->subset;
-        if (a->location == FDB_LOC_HOST) {
-            if (!a->arg_bytes || !a->map_bytes) {
-                set_error("fdb_kernel_call: host mode needs arg_bytes and map_bytes");
-                return 1;
-            }
-            void *p;
-            for (int i = 0; i < 2; i++) {
-                uint64_t ver = a->arg_versions ? a->arg_versions[i + 1] : 0;
-                if (!a->arg_versions) fdb_mirror_drop(a->args[i + 1]);
-                if (fdb_mirror_acquire(a->args[i + 1], a->arg_bytes[i + 1], ver, 1, &p)) return 1;
-                din[i] = p;
-            }
-            for (int i = 0; i < 2; i++) {
-                if (fdb_mirror_acquire(a->maps[i], a->map_bytes[i], map_ver(a, i), 1, &p)) return 1;
-                dm[i] = (const fdb_int *)p;
-            }
-            if (a->subset) {
-                if (fdb_mirror_acquire(a->subset, sizeof(fdb_int) * (size_t)a->end, a->subset_version, 1, &p)) return 1;
-                dsub = (const fdb_int *)p;
-            }
-        } else {
-            din[0] = a->args[1];
-            din[1] = a->args[2];
-            dm[0] = a->maps[0];
-            dm[1] = a->maps[1];
-        }
-        return fdb_launch_helmholtz_coef_matrix(k, a->start, a->end, nlay, dsub, target, (const double *)din[0],
-                                                (const double *)din[1], dm[0], dm[1], nullptr);
+    // args = [y (INC), coords, x] (action), [Mat handle (INC), coords] (matrix: the reference passes the
+    // PETSc Mat handle in the same slot, pyop2/types/mat.py:621-623) or [d (INC), coords] (diagonal), then
+    // the form's trailing coefficient; maps = [V map, coord map]
+    const fdb_hex_form *f = k->hex;
+    const int mode = hex_mode(&k->desc);
+    const int want = (mode == MODE_ACTION ? 3 : 2) + (f->coef ? 1 : 0);
+    if (a->nargs != want || a->nmaps != 2 || (mode == MODE_DIAGONAL && a->location != FDB_LOC_DEVICE)) {
+        static const char *const args[] = {"y, coords, x", "mat, coords", "d, coords"};
+        set_error("fdb_kernel_call: %s %s expects %d %sargs (%s%s%s) and 2 maps, got %d/%d", f->name,
+                  mode_name[mode], want, mode == MODE_DIAGONAL ? "device " : "", args[mode], f->coef ? ", " : "",
+                  f->coef ? f->coef : "", a->nargs, a->nmaps);
+        return 1;
     }
-    if (k->desc.rank == 2) {
-        // 2-form: args = [Mat handle (INC), coords (READ)], maps = [V map, coord map]
-        // (the reference passes the PETSc Mat handle in the same slot:
-        // pyop2/types/mat.py:621-623)
-        if (hyper_jac && (a->nargs != 3 || a->nmaps != 2)) {
-            set_error("fdb_kernel_call: hyperelasticity_jacobian 2-form expects 3 args (mat, coords, u) and 2 maps");
-            return 1;
-        }
-        if (!hyper_jac && (a->nargs != 2 || a->nmaps != 2)) {
-            set_error("fdb_kernel_call: 2-form expects 2 args (mat, coords) and 2 maps");
-            return 1;
-        }
-        fdb_mat_t target = (fdb_mat_t)a->args[0];
+    const fdb_mat_t mat = mode == MODE_MATRIX ? (fdb_mat_t)a->args[0] : nullptr;
+    if (mat) {
         int mat_bs = 1;
-        fdb_mat_block_size(target, &mat_bs);
+        fdb_mat_block_size(mat, &mat_bs);
         if (mat_bs != k->desc.cdim) {
             set_error("fdb_kernel_call: Mat block size %d != value size %d of the argument space", mat_bs,
                       k->desc.cdim);
@@ -556,143 +528,45 @@ int fdb_kernel_call(fdb_kernel_t k, const fdb_call_args *a)
             set_error("fdb_kernel_call: coloured scatter is not implemented for matrices");
             return 1;
         }
-        const double *dcoords;
-        const double *du = hyper_jac ? (const double *)a->args[2] : nullptr;
-        const fdb_int *dm[2];
-        const fdb_int *dsub = a->subset;
-        if (a->location == FDB_LOC_HOST) {
-            void *p;
-            uint64_t ver = a->arg_versions ? a->arg_versions[1] : 0;
-            if (!a->arg_versions) fdb_mirror_drop(a->args[1]);
-            if (fdb_mirror_acquire(a->args[1], a->arg_bytes[1], ver, 1, &p)) return 1;
-            dcoords = (const double *)p;
-            if (hyper_jac) {
-                if (!a->arg_versions) fdb_mirror_drop(a->args[2]);
-                if (fdb_mirror_acquire(a->args[2], a->arg_bytes[2], a->arg_versions ? a->arg_versions[2] : 0, 1, &p))
-                    return 1;
-                du = (const double *)p;
-            }
-            for (int i = 0; i < 2; i++) {
-                if (fdb_mirror_acquire(a->maps[i], a->map_bytes[i], map_ver(a, i), 1, &p)) return 1;
-                dm[i] = (const fdb_int *)p;
-            }
-            if (a->subset) {
-                if (fdb_mirror_acquire(a->subset, sizeof(fdb_int) * (size_t)a->end, a->subset_version, 1, &p)) return 1;
-                dsub = (const fdb_int *)p;
-            }
-        } else {
-            dcoords = (const double *)a->args[1];
-            dm[0] = a->maps[0];
-            dm[1] = a->maps[1];
-        }
-        if (elas)
-            return fdb_launch_elasticity_matrix(k, a->start, a->end, nlay, dsub, target, dcoords, du, dm[0],
-                                                dm[1], nullptr);
-        if (mat_bs == 1)
-            return fdb_launch_helmholtz_matrix(k, a->start, a->end, nlay, dsub, target, dcoords, dm[0], dm[1],
-                                               nullptr);
-        // vector-valued space: the element tensor of the Helmholtz family is A_scalar (x) I_cdim
-        // (off-diagonal component blocks vanish identically), so the scalar kernel assembles into
-        // a scalar view of the blocked pattern, which is then added to the block diagonals
-        fdb_mat_t view = nullptr;
-        if (fdb_mat_scalar_view_begin(target, &view)) return 1;
-        int rc = fdb_launch_helmholtz_matrix(k, a->start, a->end, nlay, dsub, view, dcoords, dm[0], dm[1], nullptr);
-        int rc2 = fdb_mat_scalar_view_end(target, view);
-        return rc ? rc : rc2;
-    }
-    if (coef && k->desc.diagonal) {
-        // args = [d (INC), coords, kappa]; device-resident only
-        if (a->nargs != 3 || a->nmaps != 2 || a->location != FDB_LOC_DEVICE) {
-            set_error("fdb_kernel_call: %s diagonal expects 3 device args (d, coords, %s) and 2 maps", cname, cvar);
-            return 1;
-        }
-        return fdb_launch_helmholtz_coef_matrix(k, a->start, a->end, nlay, a->subset, nullptr,
-                                                (const double *)a->args[1], (const double *)a->args[2],
-                                                a->maps[0], a->maps[1], (double *)a->args[0]);
-    }
-    if (elas && k->desc.diagonal) {
-        // args = [d (INC, 3 values per node), coords] (hyperelasticity_jacobian: [d, coords, u]); device-resident
-        // only
-        if (a->nargs != (hyper_jac ? 3 : 2) || a->nmaps != 2 || a->location != FDB_LOC_DEVICE) {
-            set_error(hyper_jac ? "fdb_kernel_call: hyperelasticity_jacobian diagonal expects 3 device args (d, "
-                                  "coords, u) and 2 maps"
-                                : "fdb_kernel_call: elasticity diagonal expects 2 device args (d, coords) and 2 maps");
-            return 1;
-        }
-        return fdb_launch_elasticity_matrix(k, a->start, a->end, nlay, a->subset, nullptr,
-                                            (const double *)a->args[1],
-                                            hyper_jac ? (const double *)a->args[2] : nullptr, a->maps[0], a->maps[1],
-                                            (double *)a->args[0]);
-    }
-    if (k->desc.diagonal) {
-        // args = [d (INC), coords]; device-resident only
-        if (a->nargs != 2 || a->nmaps != 2 || a->location != FDB_LOC_DEVICE || k->desc.cdim != 1 ||
-            k->n1d > 4) {
-            set_error("fdb_kernel_call: diagonal assembly expects 2 device args, 2 maps, scalar CG1..3");
-            return 1;
-        }
-        return fdb_launch_helmholtz_matrix(k, a->start, a->end, nlay, a->subset, nullptr,
-                                           (const double *)a->args[1], a->maps[0], a->maps[1],
-                                           (double *)a->args[0]);
-    }
-    // 1-form: args = [y (INC), coords (READ), x (READ)], maps = [V map, coord map]
-    // (helmholtz_coef: [y, coords, x, kappa (READ)])
-    if (coef && (a->nargs != 4 || a->nmaps != 2)) {
-        set_error("fdb_kernel_call: %s 1-form expects 4 args (y, coords, x, %s) and 2 maps, got %d/%d",
-                  cname, cvar, a->nargs, a->nmaps);
-        return 1;
-    }
-    if (hyper_jac && (a->nargs != 4 || a->nmaps != 2)) {
-        set_error("fdb_kernel_call: hyperelasticity_jacobian 1-form expects 4 args (y, coords, w, u) and 2 maps, "
-                  "got %d/%d", a->nargs, a->nmaps);
-        return 1;
-    }
-    if (!coef && !hyper_jac && (a->nargs != 3 || a->nmaps != 2)) {
-        set_error("fdb_kernel_call: 1-form expects 3 args (y, coords, x) and 2 maps, got %d/%d",
-                  a->nargs, a->nmaps);
-        return 1;
     }
     // the pipelined host action moves x and y only and runs the constant-coefficient kernels: the
     // coefficient, nonlinear and elasticity-kernel forms take the monolithic path
-    if (!coef && !nl_res && !elas && a->location == FDB_LOC_HOST && a->arg_versions && a->arg_bytes && a->map_bytes &&
-        a->writeback && a->output_is_zero && !a->subset && extruded &&
+    if (f->launcher == LAUNCH_HELMHOLTZ && mode == MODE_ACTION && a->location == FDB_LOC_HOST && a->arg_versions &&
+        a->arg_bytes && a->map_bytes && a->writeback && a->output_is_zero && !a->subset && extruded &&
         k->desc.scatter == FDB_SCATTER_ATOMIC) {
         int rc = pipelined_host_action(k, a, nlay);
         if (rc >= 0) return rc;      // -1: not applicable, fall through to the monolithic path
     }
-    const int nin = a->nargs;
     void *dargs[4];
     const fdb_int *dmaps[2];
-    const fdb_int *dsubset = a->subset;
-    if (a->location == FDB_LOC_HOST) {
-        if (!a->arg_bytes || !a->map_bytes) {
-            set_error("fdb_kernel_call: host mode needs arg_bytes and map_bytes");
-            return 1;
+    const fdb_int *dsubset;
+    if (device_pointers(a, mat != nullptr, dargs, dmaps, &dsubset)) return 1;
+    const double *coords = (const double *)dargs[1];
+    const double *coef = f->coef ? (const double *)dargs[want - 1] : nullptr;
+    double *out = mat ? nullptr : (double *)dargs[0];     // the action's y or the diagonal
+    if (mode != MODE_ACTION) {
+        switch (f->launcher) {
+        case LAUNCH_HELMHOLTZ:
+            if (mat && k->desc.cdim > 1) {
+                // vector-valued space: the element tensor of the Helmholtz family is A_scalar (x) I_cdim
+                // (off-diagonal component blocks vanish identically), so the scalar kernel assembles into
+                // a scalar view of the blocked pattern, which is then added to the block diagonals
+                fdb_mat_t view = nullptr;
+                if (fdb_mat_scalar_view_begin(mat, &view)) return 1;
+                int rc = fdb_launch_helmholtz_matrix(k, a->start, a->end, nlay, dsubset, view, coords, dmaps[0],
+                                                     dmaps[1], nullptr);
+                int rc2 = fdb_mat_scalar_view_end(mat, view);
+                return rc ? rc : rc2;
+            }
+            return fdb_launch_helmholtz_matrix(k, a->start, a->end, nlay, dsubset, mat, coords, dmaps[0], dmaps[1],
+                                               out);
+        case LAUNCH_HELMHOLTZ_COEF:
+            return fdb_launch_helmholtz_coef_matrix(k, a->start, a->end, nlay, dsubset, mat, coords, coef, dmaps[0],
+                                                    dmaps[1], out);
+        default:
+            return fdb_launch_elasticity_matrix(k, a->start, a->end, nlay, dsubset, mat, coords, coef, dmaps[0],
+                                                dmaps[1], out);
         }
-        for (int i = 0; i < nin; i++) {
-            uint64_t ver = a->arg_versions ? a->arg_versions[i] : 0;
-            // without versions every call re-uploads (drop-in default: the
-            // reference hands over live NumPy buffers)
-            if (!a->arg_versions) fdb_mirror_drop(a->args[i]);
-            const bool zero_out = (i == 0 && a->output_is_zero);
-            if (fdb_mirror_acquire(a->args[i], a->arg_bytes[i], ver, zero_out ? 0 : 1, &dargs[i]))
-                return 1;
-            if (zero_out)
-                FDB_CUDA(cudaMemsetAsync(dargs[i], 0, a->arg_bytes[i], ctx().stream));
-        }
-        for (int i = 0; i < 2; i++) {
-            void *p;
-            if (fdb_mirror_acquire(a->maps[i], a->map_bytes[i], map_ver(a, i), 1, &p)) return 1;
-            dmaps[i] = (const fdb_int *)p;
-        }
-        if (a->subset) {
-            void *p;
-            if (fdb_mirror_acquire(a->subset, sizeof(fdb_int) * (size_t)a->end, a->subset_version, 1, &p)) return 1;
-            dsubset = (const fdb_int *)p;
-        }
-    } else {
-        for (int i = 0; i < nin; i++) dargs[i] = a->args[i];
-        for (int i = 0; i < 2; i++) dmaps[i] = a->maps[i];
     }
     if (k->desc.scatter == FDB_SCATTER_COLOURED &&
         (k->colour_map_key != (const void *)a->maps[0] || k->colour_map_gen != map_ver(a, 0) ||
@@ -715,18 +589,21 @@ int fdb_kernel_call(fdb_kernel_t k, const fdb_call_args *a)
         set_error("fdb_kernel_call: coloured scatter needs start == 0");
         return 1;
     }
-    // (the residual: the coefficient entry point without a coefficient, see action_hex.cu)
-    int rc = elas ? fdb_launch_elasticity_action(k, a->start, a->end, nlay, dsubset, (double *)dargs[0],
-                                                 (const double *)dargs[1], (const double *)dargs[2],
-                                                 hyper_jac ? (const double *)dargs[3] : nullptr, dmaps[0],
-                                                 dmaps[1])
-             : (coef || nl_res)
-                 ? fdb_launch_helmholtz_coef_action(k, a->start, a->end, nlay, dsubset, (double *)dargs[0],
-                                                    (const double *)dargs[1], (const double *)dargs[2],
-                                                    coef ? (const double *)dargs[3] : nullptr, dmaps[0], dmaps[1])
-                  : fdb_launch_helmholtz_action(k, a->start, a->end, nlay, dsubset, (double *)dargs[0],
-                                                (const double *)dargs[1], (const double *)dargs[2],
-                                                dmaps[0], dmaps[1]);
+    // (a residual's coefficient is NULL: its u is x, see action_hex.cu and elasticity_hex.cu)
+    const double *x = (const double *)dargs[2];
+    int rc;
+    switch (f->launcher) {
+    case LAUNCH_HELMHOLTZ:
+        rc = fdb_launch_helmholtz_action(k, a->start, a->end, nlay, dsubset, out, coords, x, dmaps[0], dmaps[1]);
+        break;
+    case LAUNCH_HELMHOLTZ_COEF:
+        rc = fdb_launch_helmholtz_coef_action(k, a->start, a->end, nlay, dsubset, out, coords, x, coef, dmaps[0],
+                                              dmaps[1]);
+        break;
+    default:
+        rc = fdb_launch_elasticity_action(k, a->start, a->end, nlay, dsubset, out, coords, x, coef, dmaps[0],
+                                          dmaps[1]);
+    }
     if (rc) return rc;
     if (a->location == FDB_LOC_HOST && a->writeback) {
         // the output mirror now differs from the host copy: write it back

@@ -36,6 +36,7 @@ import enum
 import itertools
 import weakref
 from dataclasses import dataclass, field
+from typing import NamedTuple
 
 import numpy as np
 
@@ -1414,9 +1415,10 @@ class Kernel:
             object.__setattr__(self, "d", tuple(float(c) for c in self.d))
             if len(self.d) != 3:
                 raise ValueError("d holds the three coefficients of D(s) = d0 + d1 s + d2 s^2")
-        if self.form in ("nonlinear_diffusion", "hyperelasticity"):
-            return                       # residual: (INC, READ, READ), like the constant-coefficient action
-        if self.form in ("helmholtz_coef", "nonlinear_diffusion_jacobian", "hyperelasticity_jacobian"):
+        spec = _FORMS.get(self.form)
+        if spec and spec.residual:
+            return          # (INC, READ, READ) whatever rank and diagonal say: the engine refuses them
+        if spec and spec.coefficient:
             acc = (INC, READ, READ) if (self.diagonal or self.rank == 2) else (INC, READ, READ, READ)
             object.__setattr__(self, "accesses", acc)
             if self.rank == 2 and self.name == "form0_cell_integral":
@@ -1441,11 +1443,21 @@ class Kernel:
         return 2 * 6 * n ** 4 * 2 + 130 * n ** 3
 
 
-_FORMS = {"helmholtz": _lib.FORM_HELMHOLTZ, "dg_advection": _lib.FORM_DG_ADVECTION,
-          "helmholtz_coef": _lib.FORM_HELMHOLTZ_COEF, "nonlinear_diffusion": _lib.FORM_NONLINEAR_DIFFUSION,
-          "nonlinear_diffusion_jacobian": _lib.FORM_NONLINEAR_DIFFUSION_JACOBIAN,
-          "elasticity": _lib.FORM_ELASTICITY, "hyperelasticity": _lib.FORM_HYPERELASTICITY,
-          "hyperelasticity_jacobian": _lib.FORM_HYPERELASTICITY_JACOBIAN}
+class _Form(NamedTuple):
+    enum: int                   # fdb_kernel_desc.form
+    coefficient: bool = False   # a trailing coefficient argument (kappa, or a Jacobian's u)
+    residual: bool = False      # a rank-1 action only
+    lame: bool = False          # takes mu and lmbda
+
+
+_FORMS = {"helmholtz": _Form(_lib.FORM_HELMHOLTZ),
+          "dg_advection": _Form(_lib.FORM_DG_ADVECTION),
+          "helmholtz_coef": _Form(_lib.FORM_HELMHOLTZ_COEF, coefficient=True),
+          "nonlinear_diffusion": _Form(_lib.FORM_NONLINEAR_DIFFUSION, residual=True),
+          "nonlinear_diffusion_jacobian": _Form(_lib.FORM_NONLINEAR_DIFFUSION_JACOBIAN, coefficient=True),
+          "elasticity": _Form(_lib.FORM_ELASTICITY, lame=True),
+          "hyperelasticity": _Form(_lib.FORM_HYPERELASTICITY, residual=True, lame=True),
+          "hyperelasticity_jacobian": _Form(_lib.FORM_HYPERELASTICITY_JACOBIAN, coefficient=True, lame=True)}
 _INTEGRALS = {"cell": _lib.INTEGRAL_CELL, "exterior_facet": _lib.INTEGRAL_EXTERIOR_FACET,
               "interior_facet": _lib.INTEGRAL_INTERIOR_FACET, "fused": _lib.INTEGRAL_FUSED}
 
@@ -1480,7 +1492,7 @@ class GlobalKernel:
         if lk.form == "dg_advection":
             nq = lk.nq or 3
             d = _lib.KernelDesc()
-            d.form, d.rank, d.cell = _FORMS[lk.form], 1, _lib.CELL_QUAD
+            d.form, d.rank, d.cell = _FORMS[lk.form].enum, 1, _lib.CELL_QUAD
             d.integral = _INTEGRALS[lk.integral]
             d.degree, d.nq, d.cdim, d.scatter = 1, nq, 1, _lib.SCATTER_ATOMIC
             xq, wq = gauss_legendre(nq)
@@ -1500,7 +1512,7 @@ class GlobalKernel:
             # P1 on affine triangles, FIAT basis order (1-x-y, x, y), 3-point
             # edge-midpoint rule (degree 2, exact for the P1 mass matrix)
             d = _lib.KernelDesc()
-            d.form, d.rank, d.cell = _FORMS[lk.form], lk.rank, _lib.CELL_TRIANGLE
+            d.form, d.rank, d.cell = _FORMS[lk.form].enum, lk.rank, _lib.CELL_TRIANGLE
             d.integral, d.degree, d.nq, d.cdim, d.scatter = _lib.INTEGRAL_CELL, 1, 3, 1, _lib.SCATTER_ATOMIC
             d.alpha, d.beta = lk.alpha, lk.beta
             pts = [(0.5, 0.0), (0.5, 0.5), (0.0, 0.5)]
@@ -1518,7 +1530,8 @@ class GlobalKernel:
         if el.ndof != n:
             raise ValueError("element degree does not match the kernel")
         d = _lib.KernelDesc()
-        d.form = _FORMS[lk.form]
+        spec = _FORMS[lk.form]
+        d.form = spec.enum
         d.rank = lk.rank
         d.cell = _lib.CELL_HEX_EXTRUDED if self.extruded else _lib.CELL_HEX
         d.integral = _lib.INTEGRAL_CELL
@@ -1531,7 +1544,7 @@ class GlobalKernel:
         d.affine_cells = int(lk.affine and lk.rank == 1 and not lk.diagonal)
         for i in range(3):
             d.dcoef[i] = lk.d[i]
-        if lk.form in ("elasticity", "hyperelasticity", "hyperelasticity_jacobian"):
+        if spec.lame:
             d.alpha, d.lmbda = lk.mu, lk.lmbda
         for q in range(el.nq):
             d.wq[q] = el.wq[q]
