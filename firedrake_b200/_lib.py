@@ -22,6 +22,7 @@ FORM_NONLINEAR_DIFFUSION_JACOBIAN = 5
 FORM_ELASTICITY = 6
 FORM_HYPERELASTICITY = 7
 FORM_HYPERELASTICITY_JACOBIAN = 8
+FORM_ADVECTION_DIFFUSION = 9
 CELL_HEX_EXTRUDED = 1
 CELL_HEX = 2
 CELL_TRIANGLE = 3

@@ -55,6 +55,19 @@ class FunctionSpace:
     def dat(self, data=None, pinned=False):
         return op2.Dat(self.dof_dset, data, pinned=pinned)
 
+    def vector_dset(self, dim=3):
+        """``op2.DataSet(V.node_set, dim)``: ``dim`` values per node of this space (AoS), e.g. the velocity
+        of :class:`AdvectionDiffusion` on a scalar space.  On a partitioned space its ghost rows are
+        exchanged with the same neighbours as the space's own."""
+        if dim == self.cdim:
+            return self.dof_dset
+        cache = self.__dict__.setdefault("_vector_dsets", {})
+        if dim not in cache:
+            h = self.dof_dset.halo
+            cache[dim] = op2.DataSet(self.node_set, dim,
+                                     halo=Halo(h.neighbours, max_cdim=dim) if h is not None else None)
+        return cache[dim]
+
     def cells_are_affine(self):
         """True iff every cell is a parallelepiped (checked on the device, cached per version of
         the coordinate Dat): lets the assembler pick the per-cell-metric kernel variant."""
@@ -489,6 +502,90 @@ def assemble_elasticity_generic(V: "FunctionSpace", u: op2.Dat, mu, lmbda, beta=
     return tensor
 
 
+def advection_diffusion_kernel(degree, alpha=1.0, beta=0.0, name="advection_diffusion_action"):
+    """C source of the 1-form ``action(alpha*inner(grad(u), grad(v))*dx + inner(dot(b, grad(u)), v)*dx +
+    beta*inner(u, v)*dx, u)`` on the scalar Q_p (x) P_p space, with the velocity b of 3 values per node
+    (AoS), written the way TSFC's spectral mode would, with J^{-1} formed explicitly, and run through the
+    generic wrapper builder: the independent statement of the hand-written FDB_FORM_ADVECTION_DIFFUSION
+    kernel.  Arguments: y (INC), coords, u, b.  Degrees 1..3: at degree 4 the NVRTC build of this statement
+    reads b at a cell's first node as u there (its host build is exact), so it is refused (DESIGN.md
+    section 4.10)."""
+    from .codegen import CStringKernel
+    if not 1 <= degree <= 3:
+        raise NotImplementedError(f"advection_diffusion_kernel: degree {degree} outside 1..3 (the device build of "
+                                  f"the degree-4 statement is wrong at a cell's first node, DESIGN.md section 4.10)")
+    code = _vector_hex_tables(degree) + f"""static void {name}(double *y, const double *X, const double *u,
+                                 const double *b)
+{{
+    double U[END], G[3][END], Bq[3][END], c[END], t[END];
+    for (int d = 0; d < 3; ++d) {{
+        for (int i = 0; i < END; ++i) c[i] = b[i * 3 + d];
+        el_tensor(EB, EB, EB, 0, c, Bq[d]);
+    }}
+    el_tensor(EB, EB, EB, 0, u, U);
+    el_tensor(ED, EB, EB, 0, u, G[0]);
+    el_tensor(EB, ED, EB, 0, u, G[1]);
+    el_tensor(EB, EB, ED, 0, u, G[2]);
+    for (int qx = 0; qx < EN; ++qx) for (int qy = 0; qy < EN; ++qy) for (int qz = 0; qz < EN; ++qz) {{
+        const int q = (qx * EN + qy) * EN + qz;
+        const double xi[3] = {{EX[qx], EX[qy], EX[qz]}};
+        double J[3][3] = {{{{0}}}};
+        for (int v = 0; v < 8; ++v) {{
+            const int bv[3] = {{(v >> 2) & 1, (v >> 1) & 1, v & 1}};
+            for (int r = 0; r < 3; ++r) {{
+                double g = bv[r] ? 1.0 : -1.0;
+                for (int e = 0; e < 3; ++e) if (e != r) g *= bv[e] ? xi[e] : 1.0 - xi[e];
+                for (int k = 0; k < 3; ++k) J[k][r] += X[v * 3 + k] * g;
+            }}
+        }}
+        /* Jinv[m][k] = dxi_m/dx_k */
+        const double det = J[0][0] * (J[1][1] * J[2][2] - J[1][2] * J[2][1])
+                         - J[0][1] * (J[1][0] * J[2][2] - J[1][2] * J[2][0])
+                         + J[0][2] * (J[1][0] * J[2][1] - J[1][1] * J[2][0]);
+        double Jinv[3][3];
+        Jinv[0][0] = (J[1][1] * J[2][2] - J[1][2] * J[2][1]) / det;
+        Jinv[0][1] = (J[0][2] * J[2][1] - J[0][1] * J[2][2]) / det;
+        Jinv[0][2] = (J[0][1] * J[1][2] - J[0][2] * J[1][1]) / det;
+        Jinv[1][0] = (J[1][2] * J[2][0] - J[1][0] * J[2][2]) / det;
+        Jinv[1][1] = (J[0][0] * J[2][2] - J[0][2] * J[2][0]) / det;
+        Jinv[1][2] = (J[0][2] * J[1][0] - J[0][0] * J[1][2]) / det;
+        Jinv[2][0] = (J[1][0] * J[2][1] - J[1][1] * J[2][0]) / det;
+        Jinv[2][1] = (J[0][1] * J[2][0] - J[0][0] * J[2][1]) / det;
+        Jinv[2][2] = (J[0][0] * J[1][1] - J[0][1] * J[1][0]) / det;
+        const double wd = EW[qx] * EW[qy] * EW[qz] * fabs(det);
+        double gp[3];                                /* grad u */
+        for (int k = 0; k < 3; ++k) gp[k] = G[0][q] * Jinv[0][k] + G[1][q] * Jinv[1][k] + G[2][q] * Jinv[2][k];
+        for (int m = 0; m < 3; ++m)
+            G[m][q] = {float(alpha)!r} * wd * (Jinv[m][0] * gp[0] + Jinv[m][1] * gp[1] + Jinv[m][2] * gp[2]);
+        U[q] = wd * ({float(beta)!r} * U[q] + Bq[0][q] * gp[0] + Bq[1][q] * gp[1] + Bq[2][q] * gp[2]);
+    }}
+    el_tensor(EB, EB, EB, 1, U, c);
+    el_tensor(ED, EB, EB, 1, G[0], t);  for (int i = 0; i < END; ++i) c[i] += t[i];
+    el_tensor(EB, ED, EB, 1, G[1], t);  for (int i = 0; i < END; ++i) c[i] += t[i];
+    el_tensor(EB, EB, ED, 1, G[2], t);  for (int i = 0; i < END; ++i) c[i] += t[i];
+    for (int i = 0; i < END; ++i) y[i] += c[i];
+}}
+#undef END
+#undef EN
+"""
+    return CStringKernel(code, name)
+
+
+def assemble_advection_diffusion_generic(V: "FunctionSpace", u: op2.Dat, b: op2.Dat, alpha=1.0, beta=0.0,
+                                         tensor=None):
+    """``assemble(action(a, u))`` of advection-diffusion through the generic wrapper path
+    (:func:`advection_diffusion_kernel`): the cross-check and the baseline of :class:`AdvectionDiffusion`."""
+    if V.cdim != 1:
+        raise ValueError("advection-diffusion takes scalar spaces only")
+    if tensor is None:
+        tensor = V.dat()
+    tensor.zero()
+    tensor.device_ptr
+    op2.par_loop(advection_diffusion_kernel(V.degree, alpha, beta), V.cell_set, tensor(op2.INC, V.cell_node_map),
+                 V.coordinates(op2.READ, V.coord_map), u(op2.READ, V.cell_node_map), b(op2.READ, V.cell_node_map))
+    return tensor
+
+
 def hyperelasticity_kernel(degree, mu, lmbda, beta=0.0, jacobian=False, name=None):
     """C source of the residual of compressible Neo-Hookean hyperelasticity,
     ``inner(P(F), grad(v))*dx + beta*inner(u, v)*dx`` with ``F = I + grad(u)``, ``J = det(F)`` and
@@ -905,6 +1002,37 @@ class HyperElasticityJacobian:
                           beta=self.beta, rank=rank, diagonal=diagonal, cdim=3)
 
 
+@dataclass
+class AdvectionDiffusion:
+    """Advection-diffusion of a scalar on ``V`` (``cdim = 1``):
+
+        a(u, v) = alpha*inner(grad(u), grad(v))*dx + inner(dot(b, grad(u)), v)*dx + beta*inner(u, v)*dx
+
+    with the velocity ``b`` a Dat of 3 values per node of ``V`` (``V.vector_dset(3)``, i.e.
+    ``op2.DataSet(V.node_set, 3)``), read through the argument map.  beta = 1/dt gives an implicit
+    Euler step of a transported scalar.  The form is NOT symmetric: it works with ``assemble(F, u=w)``
+    (action, degrees 1..4), ``assemble(F)`` (aij, degrees 1..3), ``assemble(F, mat_type="matfree")``
+    (``multTranspose`` is not implemented) and :func:`solve`, whose default Krylov method for it is GMRES."""
+    V: FunctionSpace
+    b: op2.Dat
+    alpha: float = 1.0
+    beta: float = 0.0
+    symmetric = False
+
+    def __post_init__(self):
+        if self.b.cdim != 3:
+            raise ValueError(f"the velocity b has 3 values per node (V.vector_dset(3)), got {self.b.cdim}")
+
+    def coefficient_args(self):
+        return [self.b(op2.READ, self.V.cell_node_map)]
+
+    def kernel(self, rank, diagonal=False):
+        if self.V.cdim != 1:
+            raise NotImplementedError("advection-diffusion takes scalar spaces only")
+        return op2.Kernel("advection_diffusion", degree=self.V.degree, alpha=self.alpha, beta=self.beta,
+                          rank=rank, diagonal=diagonal)
+
+
 class ConvergenceError(RuntimeError):
     """A nonlinear solve that cannot go on (firedrake.exceptions.ConvergenceError); ``reason`` is the
     SNES converged reason, e.g. "DIVERGED_FNORM_NAN"."""
@@ -1076,9 +1204,12 @@ class ImplicitMatrixContext:
         """``Y = A^T X`` (matrix_free/operators.py:245-330: the action of ``adjoint(a)`` with the
         row and column conditions exchanged).  Every form of the supported family is
         symmetric and row/column DirichletBCs coincide here (no EquationBC), so A^T = A.  The
-        Jacobian of nonlinear diffusion is not symmetric, and its transpose is not implemented."""
+        Jacobian of nonlinear diffusion and advection-diffusion are not symmetric, and their transpose
+        is not implemented."""
         if not getattr(self.form, "symmetric", True):
-            raise NotImplementedError("multTranspose of a nonsymmetric form (the nonlinear diffusion Jacobian)")
+            which = "advection-diffusion" if isinstance(self.form, AdvectionDiffusion) else \
+                "the nonlinear diffusion Jacobian"
+            raise NotImplementedError(f"multTranspose of a nonsymmetric form ({which})")
         return self.mult(X, Y)
 
     def mult(self, X: op2.Dat, Y: op2.Dat):
@@ -1379,18 +1510,26 @@ def solve(form: Form, L: op2.Dat, u: op2.Dat, bcs=(), solver_parameters=None, hi
     """``solve(a == L, u, bcs=bcs, solver_parameters=...)`` for the supported forms
     (firedrake/solving.py:128-260 -> LinearVariationalSolver; SURVEY.md section 3.5): assemble the
     operator, lift the Dirichlet values, run the Krylov solver on the device.  ``form``: a
-    :class:`Form` or an :class:`Elasticity` form (vector space; Dirichlet values on every component).
+    :class:`Form`, an :class:`Elasticity` form (vector space; Dirichlet values on every component) or an
+    :class:`AdvectionDiffusion` form.
 
     ``L``: the assembled right-hand side (a Dat, e.g. ``assemble(mass(V), u=f)``).
     ``solver_parameters`` (PETSc option names, the subset that makes sense here):
-    ``mat_type`` "matfree" (default) | "aij" | "is"; ``ksp_type`` "cg"; ``pc_type`` "none" (default) |
-    "jacobi" | "mg" (needs ``hierarchy``, a mg.MeshHierarchy whose finest mesh is ``form.V.mesh``);
-    ``ksp_rtol`` (1e-8), ``ksp_max_it`` (1000).  Returns (iterations, residual history)."""
+    ``mat_type`` "matfree" (default) | "aij" | "is"; ``ksp_type`` "cg" (the default for symmetric forms) |
+    "gmres" (:func:`gmres`, right-preconditioned and flexible; the default for nonsymmetric forms, which
+    cg refuses), ``ksp_gmres_restart`` (30); ``pc_type`` "none" (default) | "jacobi" | "mg" (needs
+    ``hierarchy``, a mg.MeshHierarchy whose finest mesh is ``form.V.mesh``; for advection-diffusion a
+    V-cycle of its symmetric part ``Form(W, alpha, beta)``); ``ksp_rtol`` (1e-8), ``ksp_max_it`` (1000).
+    Returns (iterations, residual history)."""
     from . import _lib
-    sp = {"mat_type": "matfree", "ksp_type": "cg", "pc_type": "none", "ksp_rtol": 1e-8, "ksp_max_it": 1000}
+    symmetric = getattr(form, "symmetric", True)
+    sp = {"mat_type": "matfree", "ksp_type": "cg" if symmetric else "gmres", "pc_type": "none", "ksp_rtol": 1e-8,
+          "ksp_max_it": 1000, "ksp_gmres_restart": 30}
     sp.update(solver_parameters or {})
-    if sp["ksp_type"] != "cg":
-        raise NotImplementedError("ksp_type cg only (the supported forms are symmetric positive definite)")
+    if sp["ksp_type"] not in ("cg", "gmres"):
+        raise NotImplementedError(f"ksp_type {sp['ksp_type']!r}: cg or gmres")
+    if sp["ksp_type"] == "cg" and not symmetric:
+        raise ValueError(f"ksp_type cg needs a symmetric operator, and {type(form).__name__} is not: use gmres")
     V = form.V
     bcs = tuple(bcs)
     lib = _lib.lib()
@@ -1413,9 +1552,8 @@ def solve(form: Form, L: op2.Dat, u: op2.Dat, bcs=(), solver_parameters=None, hi
     u.zero()
     u.device_ptr
     pc = sp["pc_type"]
-    if pc == "none":
-        its, hist = cg(A, b, u, rtol=sp["ksp_rtol"], maxit=sp["ksp_max_it"], allreduce=allreduce)
-    else:
+    M = None
+    if pc != "none":
         from . import mg as _mg
         if pc == "jacobi":
             ctx = A if isinstance(A, ImplicitMatrixContext) else ImplicitMatrixContext(form, bcs)
@@ -1434,6 +1572,8 @@ def solve(form: Form, L: op2.Dat, u: op2.Dat, bcs=(), solver_parameters=None, hi
             # elasticity: the Jacobi smoother's damping is 0.6, not 0.8.  The spectrum of D^-1 A of the coupled
             # operator reaches past 2 / 0.8, so 0.8 amplifies its highest modes: CG1 at nu = 0.3 took 16 and
             # 97 iterations on 8^3 and 16^3 with 0.8, 8 and 9 with 0.6 (DESIGN.md section 4.8)
+            # advection-diffusion: a V-cycle of its symmetric part Form(W, alpha, beta) on every level (the
+            # convective term is left to the outer GMRES, DESIGN.md section 4.10)
             if isinstance(form, Elasticity):
                 make = lambda W, k=None: Elasticity(W, form.mu, form.lmbda, form.beta)
                 omega = 0.6
@@ -1447,6 +1587,12 @@ def solve(form: Form, L: op2.Dat, u: op2.Dat, bcs=(), solver_parameters=None, hi
             M = lambda r, z: vc.apply(top, r, z)
         else:
             raise NotImplementedError(f"pc_type {pc!r}")
+    if sp["ksp_type"] == "gmres":
+        its, hist = gmres(A, b, u, M, rtol=sp["ksp_rtol"], restart=sp["ksp_gmres_restart"], maxit=sp["ksp_max_it"],
+                          allreduce=allreduce)
+    elif M is None:
+        its, hist = cg(A, b, u, rtol=sp["ksp_rtol"], maxit=sp["ksp_max_it"], allreduce=allreduce)
+    else:
         its, hist = _mg.pcg(A, b, u, M, rtol=sp["ksp_rtol"], maxit=sp["ksp_max_it"], allreduce=allreduce)
     if lift:
         u.axpy(1.0, g)

@@ -30,6 +30,8 @@
 // nonlinear_residual_kernel and nonlinear_jacobian_kernel are the same body with NL = 1 / 2: the
 // residual and the exact Newton Jacobian of alpha*inner(D(u) grad u, grad v)*dx + beta*inner(u, v)*dx
 // (FDB_FORM_NONLINEAR_DIFFUSION[_JACOBIAN], DESIGN.md section 4.6).
+// advection_diffusion_kernel is the same body with ADV set: the velocity b (3 values per node) in three
+// kappa buffers adds inner(dot(b, grad u), v)*dx (FDB_FORM_ADVECTION_DIFFUSION, DESIGN.md section 4.10).
 //
 // Arithmetic: the basis is first interpolated to the N Gauss points per axis
 // (B (x) B (x) B), gradients are then taken with the collocated derivative
@@ -158,6 +160,35 @@ __device__ __forceinline__ void apply_second(const double *M, const double (&in)
         }
 }
 
+// A field's dof values in a cell-strided buffer (this lane's layout-Z slots) to its values at the
+// quadrature points (B (x) B (x) B, this lane's layout-Y slots), in place: the kappa interpolation of
+// action_hex_body.cuh, for the second and third components of the advection velocity
+template <int N>
+__device__ __forceinline__ void to_points_in_place(const double *B, double *sk, bool valid, int t)
+{
+    double kz[N][N], kt[N][N];
+#pragma unroll
+    for (int x = 0; x < N; x++)
+#pragma unroll
+        for (int yy = 0; yy < N; yy++) kz[x][yy] = valid ? sk[(x * N + yy) * N + t] : 0.0;
+    apply_first<N, false>(B, kz, kt);
+    apply_second<N, false>(B, kt, kz);
+#pragma unroll
+    for (int x = 0; x < N; x++)
+#pragma unroll
+        for (int yy = 0; yy < N; yy++) sk[(x * N + yy) * N + t] = kz[x][yy];
+    __syncwarp();
+#pragma unroll
+    for (int x = 0; x < N; x++)
+#pragma unroll
+        for (int z = 0; z < N; z++) kt[x][z] = sk[(x * N + t) * N + z];
+    apply_second<N, false>(B, kt, kz);
+#pragma unroll
+    for (int x = 0; x < N; x++)
+#pragma unroll
+        for (int z = 0; z < N; z++) sk[(x * N + t) * N + z] = kz[x][z];
+}
+
 // Shared-memory tile used to re-orient slabs.  For N == 4 the (y, z) position
 // is rotated by the cell's index in the warp so that both the layout-Z and the
 // layout-Y access patterns touch all 32 banks exactly once per half-warp.
@@ -273,8 +304,9 @@ __device__ __forceinline__ void cp_async4(void *smem, const void *gmem)
 // column has at least 32/N layers) instead of one per cell, triple-buffered over
 // the three items in flight (compute / value prefetch / row prefetch).
 // COEF: one more cell-strided buffer for kappa, first its gathered dof values (layout Z), then,
-// overwritten in place, its values at the quadrature points (layout Y: [qx][qy][qz] at qy = lane)
-template <int N, bool SLIM = false, bool COEF = false>
+// overwritten in place, its values at the quadrature points (layout Y: [qx][qy][qz] at qy = lane);
+// NKAP such buffers (3 for the advection velocity b, one per component)
+template <int N, bool SLIM = false, bool COEF = false, int NKAP = 1>
 struct WarpSmem {
     static constexpr int CW = 32 / N;
     static constexpr int CWS = (32 % N == 0) ? CW : CW + 1;   // idle lanes get a scratch slot
@@ -289,7 +321,7 @@ struct WarpSmem {
 #endif
     static constexpr int GS = FDB_STASH_STRIDE;                // stash stride: c2 c4 c5 c7 (12) + A1 of 4 lanes (4 apart)
     static constexpr int STASH = (OPT_STASH && N == 4 && !SLIM) ? CWS * GS : 0;   // doubles
-    static constexpr int KAPPA = COEF ? CWS * US : 0;          // doubles: kappa (single buffer)
+    static constexpr int KAPPA = COEF ? NKAP * CWS * US : 0;   // doubles: kappa (single buffer)
     static constexpr int IDX = SLIM ? 0 : 2 * CWS * US;        // ints: global dof index per local dof
     static constexpr int MAPRAW = SLIM ? 3 * 2 * US : CWS * US;   // ints: bottom-cell map row(s)
     static constexpr int VIDX = SLIM ? 3 * 2 * 8 : 2 * CWS * 8;   // ints: bottom-cell vertex row(s)
@@ -321,7 +353,7 @@ template <int N, bool MASS, bool ATOMIC, int MINB, bool MATRIX = false, bool SLI
 __global__ void __launch_bounds__(WPC<N, SLIM>::value * 32, MINB)
 helmholtz_action_kernel(const __grid_constant__ HelmParams<N> P)
 {
-    constexpr bool COEF = false;
+    constexpr bool COEF = false, ADV = false;
     constexpr int NL = 0;
     [[maybe_unused]] const double *kappa = nullptr;
     [[maybe_unused]] const double *dcoef = nullptr;
@@ -333,7 +365,7 @@ template <int N, bool MASS, bool ATOMIC, int MINB, bool MATRIX = false, bool SLI
 __global__ void __launch_bounds__(WPC<N, SLIM, true>::value * 32, MINB)
 helmholtz_coef_kernel(const __grid_constant__ HelmCoefParams<N> P)
 {
-    constexpr bool COEF = true, AFFINE = false;
+    constexpr bool COEF = true, AFFINE = false, ADV = false;
     constexpr int NL = 0;
     const double *kappa = P.kappa;
     [[maybe_unused]] const double *dcoef = nullptr;
@@ -346,7 +378,7 @@ template <int N, bool MASS, bool ATOMIC, int MINB, bool SLIM = false>
 __global__ void __launch_bounds__(WPC<N, SLIM>::value * 32, MINB)
 nonlinear_residual_kernel(const __grid_constant__ HelmNlParams<N> P)
 {
-    constexpr bool COEF = false, MATRIX = false, AFFINE = false;
+    constexpr bool COEF = false, MATRIX = false, AFFINE = false, ADV = false;
     constexpr int NL = 1;
     [[maybe_unused]] const double *kappa = nullptr;
     const double *dcoef = P.dcoef;
@@ -359,25 +391,40 @@ template <int N, bool MASS, bool ATOMIC, int MINB, bool MATRIX = false, bool SLI
 __global__ void __launch_bounds__(WPC<N, SLIM, true>::value * 32, MINB)
 nonlinear_jacobian_kernel(const __grid_constant__ HelmNlParams<N> P)
 {
-    constexpr bool COEF = true, AFFINE = false;
+    constexpr bool COEF = true, AFFINE = false, ADV = false;
     constexpr int NL = 2;
     const double *kappa = P.kappa;
     const double *dcoef = P.dcoef;
 #include "action_hex_body.cuh"
 }
 
+// FDB_FORM_ADVECTION_DIFFUSION (action, element matrix, diagonal): the coefficient layout with three
+// kappa buffers, b's components, reused across the N^3 units of a cell in matrix mode
+template <int N, bool MASS, bool ATOMIC, int MINB, bool MATRIX = false>
+__global__ void __launch_bounds__(WPC<N, false, true>::value * 32, MINB)
+advection_diffusion_kernel(const __grid_constant__ HelmCoefParams<N> P)
+{
+    constexpr bool COEF = true, AFFINE = false, SLIM = false, ADV = true;
+    constexpr int NL = 0;
+    const double *kappa = P.kappa;   // b, 3 values per node
+    [[maybe_unused]] const double *dcoef = nullptr;
+#include "action_hex_body.cuh"
+}
+
 #include "action_hex_ws.cuh"
 
 template <int N, bool MASS, bool ATOMIC, int MINB, bool MATRIX = false, bool SLIM = false, bool AFFINE = false,
-          bool COEF = false, int NL = 0>
+          bool COEF = false, int NL = 0, bool ADV = false>
 int launch_one(int grid_cap_per_sm, cudaStream_t st, HelmNlParams<N> &P, int sm_count)
 {
     static_assert(NL == 0 || COEF == (NL == 2), "the Jacobian takes the coefficient layout, the residual not");
-    using WS = WarpSmem<N, SLIM, COEF>;
+    static_assert(!ADV || (COEF && NL == 0 && !SLIM), "advection-diffusion takes the coefficient layout");
+    using WS = WarpSmem<N, SLIM, COEF, ADV ? 3 : 1>;
     constexpr int WARPS_PER_CTA = WPC<N, SLIM, COEF>::value;
     constexpr int T = WARPS_PER_CTA * 32;
     auto kern = [] {
-        if constexpr (NL == 1) return nonlinear_residual_kernel<N, MASS, ATOMIC, MINB, SLIM>;
+        if constexpr (ADV) return advection_diffusion_kernel<N, MASS, ATOMIC, MINB, MATRIX>;
+        else if constexpr (NL == 1) return nonlinear_residual_kernel<N, MASS, ATOMIC, MINB, SLIM>;
         else if constexpr (NL == 2) return nonlinear_jacobian_kernel<N, MASS, ATOMIC, MINB, MATRIX, SLIM>;
         else if constexpr (COEF) return helmholtz_coef_kernel<N, MASS, ATOMIC, MINB, MATRIX, SLIM>;
         else return helmholtz_action_kernel<N, MASS, ATOMIC, MINB, MATRIX, SLIM, AFFINE>;
@@ -474,6 +521,23 @@ int launch_nl(int nl, bool mass, int cap, cudaStream_t st, HelmNlParams<N> &P, i
     if (mass) return launch_one<N, true, ATOMIC, MB, false, false, false, true, 2>(cap, st, P, sm_count);
     return launch_one<N, false, ATOMIC, MB, false, false, false, true, 2>(cap, st, P, sm_count);
 }
+
+// advection-diffusion (action, element matrix or diagonal: MATRIX): the slab-thread kernel with b in three
+// kappa buffers, degrees 1..4 (no slim staging, no thread-per-cell, warp-specialised, affine or DMMA variant);
+// the register bound is the coefficient kernel's
+template <int N, bool ATOMIC, bool MATRIX = false>
+int launch_adv(bool mass, int cap, cudaStream_t st, HelmNlParams<N> &P, int sm_count)
+{
+    if constexpr (N <= (MATRIX ? 4 : 5)) {
+        constexpr int MB = CoefMinB<N>::value;
+        if (mass) return launch_one<N, true, ATOMIC, MB, MATRIX, false, false, true, 0, true>(cap, st, P, sm_count);
+        return launch_one<N, false, ATOMIC, MB, MATRIX, false, false, true, 0, true>(cap, st, P, sm_count);
+    }
+    fdb::set_error("advection_diffusion %s: degree %d not instantiated", MATRIX ? "matrix" : "action", N - 1);
+    return 1;
+}
+
+inline bool is_adv(const fdb_kernel_s *k) { return k->desc.form == FDB_FORM_ADVECTION_DIFFUSION; }
 
 // nonlinear mode of a kernel: 1 residual, 2 Jacobian, 0 any other form
 inline int nl_mode(const fdb_kernel_s *k)
@@ -575,6 +639,7 @@ int launch_n(fdb_kernel_s *k, fdb_int start, fdb_int end, int nlay, const fdb_in
         P.lay_first = 0;
         P.lay_step = 1;
         if (P.ncols <= 0 || nlay <= 0) return 0;
+        if (is_adv(k)) return launch_adv<N, true>(mass, cap, c.stream, P, c.sm_count);
         if (kappa && !nl) return launch_coef<N, true>(mass, cap, c.stream, P, c.sm_count);
         if (nl) return launch_nl<N, true>(nl, mass, cap, c.stream, P, c.sm_count);
         if constexpr (N == 4) {
@@ -611,7 +676,8 @@ int launch_n(fdb_kernel_s *k, fdb_int start, fdb_int end, int nlay, const fdb_in
             P.lay_step = 2;
             P.nlay_items = (nlay - par + 1) / 2;
             if (P.ncols <= 0 || P.nlay_items <= 0) continue;
-            if (kappa && !nl ? launch_coef<N, false>(mass, cap, c.stream, P, c.sm_count)
+            if (is_adv(k)      ? launch_adv<N, false>(mass, cap, c.stream, P, c.sm_count)
+                : kappa && !nl ? launch_coef<N, false>(mass, cap, c.stream, P, c.sm_count)
                 : nl         ? launch_nl<N, false>(nl, mass, cap, c.stream, P, c.sm_count)
                              : launch_variant<N, false>(mass, minb, cap, c.stream, P, c.sm_count))
                 return 1;
@@ -669,6 +735,7 @@ int launch_matrix_n(fdb_kernel_s *k, fdb_int start, fdb_int end, int nlay, const
     P.lay_first = 0;
     P.lay_step = 1;
     if (P.ncols <= 0 || nlay <= 0) return 0;
+    if (is_adv(k)) return launch_adv<N, true, true>(k->desc.beta != 0.0, 0, c.stream, P, c.sm_count);
     if (kappa && nl_mode(k) == 0) {
         constexpr int MB = CoefMinB<N>::value;
         if (k->desc.beta != 0.0)
@@ -738,8 +805,9 @@ int fdb_launch_helmholtz_action(fdb_kernel_s *k, fdb_int start, fdb_int end, int
 
 // FDB_FORM_HELMHOLTZ_COEF: the slab-thread kernel for every degree (1..5 action, 1..4 matrix and
 // diagonal); never the thread-per-cell, warp-specialised, affine or DMMA kernels.  The nonlinear
-// diffusion forms take the same entry points (launch_n / launch_matrix_n pick the mode from the
-// form): the residual with kappa = NULL, the Jacobian with kappa = the linearisation point u.
+// diffusion and advection-diffusion forms take the same entry points (launch_n / launch_matrix_n pick
+// the mode from the form): the residual with kappa = NULL, the Jacobian with kappa = the linearisation
+// point u, advection-diffusion with kappa = b (3 values per node).
 int fdb_launch_helmholtz_coef_action(fdb_kernel_s *k, fdb_int start, fdb_int end, int nlay,
                                      const fdb_int *subset, double *y, const double *coords,
                                      const double *x, const double *kappa, const fdb_int *map0,

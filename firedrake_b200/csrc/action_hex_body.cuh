@@ -1,8 +1,8 @@
 // Body of the slab-thread kernels of action_hex.cu (helmholtz_action_kernel, helmholtz_coef_kernel,
-// nonlinear_residual_kernel, nonlinear_jacobian_kernel), included inside each __global__ function: the
-// template parameters N, MASS, ATOMIC, MATRIX, SLIM, AFFINE, the parameter block P and, from the
-// including kernel, `constexpr bool COEF`, `constexpr int NL`, `const double *kappa` and
-// `const double *dcoef` are in scope.  A textual include rather than a __forceinline__ function taking
+// nonlinear_residual_kernel, nonlinear_jacobian_kernel, advection_diffusion_kernel), included inside each
+// __global__ function: the template parameters N, MASS, ATOMIC, MATRIX, SLIM, AFFINE, the parameter block P
+// and, from the including kernel, `constexpr bool COEF`, `constexpr int NL`, `constexpr bool ADV`,
+// `const double *kappa` and `const double *dcoef` are in scope.  A textual include rather than a __forceinline__ function taking
 // P by reference: the reference changes the register allocation of the existing matrix-mode kernels,
 // whose machine code this layout keeps exactly as it was before the coefficient form existed.
 //
@@ -11,12 +11,18 @@
 //   2  Jacobian: x is w, u is gathered into the kappa buffer (COEF layout) and interpolated to the
 //      points there; the reference gradient g of w becomes D(u_q) g + D'(u_q) w_q ghat(u)_q, with
 //      ghat(u)_q taken by collocated differentiation (Dt) of the buffer's quadrature values
+//
+// ADV (advection-diffusion, alpha*inner(grad u, grad v)*dx + inner(dot(b, grad u), v)*dx + beta*inner(u, v)*dx):
+//   the COEF layout with three kappa buffers, one per component of b (AoS, gathered at 3 g + c with x's
+//   indices g) and interpolated to the points in place like kappa; the stiffness weight stays w, and
+//   w sign(det J) (b_q . h) -- h = sum_m r_m ghat_m = det J grad u -- goes to the value slot with the mass
     static_assert(!(SLIM && MATRIX), "matrix mode keeps the per-cell index buffer");
     static_assert(!(AFFINE && MATRIX), "the affine variant exists for 1-forms only");
     static_assert(!(AFFINE && COEF), "the coefficient form has no affine variant");
     static_assert(NL != 1 || (!COEF && !MATRIX && !AFFINE), "the residual is a 1-form without a kappa buffer");
     static_assert(NL != 2 || (COEF && !AFFINE), "the Jacobian keeps u in the kappa buffer");
-    using WS = WarpSmem<N, SLIM, COEF>;
+    static_assert(!ADV || (COEF && NL == 0 && !SLIM && !AFFINE), "b takes the coefficient layout, three times");
+    using WS = WarpSmem<N, SLIM, COEF, ADV ? 3 : 1>;
     constexpr int CW = WS::CW;
     constexpr int CWS = WS::CWS;
     constexpr int ND = N * N * N;
@@ -30,7 +36,7 @@
     double *s_coord = s_u + WS::UBUF;                // [CWS][CS]   (single buffer)
     double *s_stash = s_coord + WS::COORD;           // [CWS][GS]   (geometry coefficients, if STASH)
     constexpr bool STASH = WS::STASH > 0 && !MATRIX && !AFFINE;
-    double *s_kap = s_stash + WS::STASH;             // [CWS][US]   (kappa, if COEF)
+    double *s_kap = s_stash + WS::STASH;             // [NKAP][CWS][US]   (kappa, if COEF; b's components if ADV)
     int *s_idx = reinterpret_cast<int *>(s_kap + WS::KAPPA);   // [2][CWS][US]  (empty if SLIM)
     int *s_mapraw = s_idx + WS::IDX;                 // [CWS][US], or [3][2][US] if SLIM
     int *s_vidx = s_mapraw + WS::MAPRAW;             // [2][CWS][8], or [3][2][8] if SLIM
@@ -197,7 +203,12 @@
             for (int j = 0; j < N * N; j++) {
                 const int loc = j * N + t;
                 const int g = SLIM ? sm[loc] + s_off0[loc] * u.layer : si[loc];
-                cp_async8(sk + loc, kappa + g);
+                if constexpr (ADV) {
+#pragma unroll
+                    for (int c = 0; c < 3; c++) cp_async8(sk + c * WS::UBUF + loc, kappa + 3ll * g + c);
+                } else {
+                    cp_async8(sk + loc, kappa + g);
+                }
             }
         }
     };
@@ -322,6 +333,15 @@
                 for (int x = 0; x < N; x++)
 #pragma unroll
                     for (int z = 0; z < N; z++) sk[(x * N + t) * N + z] = kz[x][z];
+            }
+        }
+        if constexpr (ADV) {
+            // b's second and third components, the same way on their own buffers (the first is in the
+            // kappa buffer proper, done above; that block stays as it is, with the machine code of the
+            // existing coefficient kernels)
+            if (cur.comp == 0) {
+                to_points_in_place<N>(P.B, s_kap + WS::UBUF + cw * US, valid, t);
+                to_points_in_place<N>(P.B, s_kap + 2 * WS::UBUF + cw * US, valid, t);
             }
         }
         const int comp = cur.comp;
@@ -454,8 +474,9 @@
                     r2[2] = ca[0] * cb[1] - ca[1] * cb[0];
                     const double det = ca[0] * r0[0] + ca[1] * r0[1] + ca[2] * r0[2];
                     const double adet = fabs(det);
-                    const double s = stiff_weight<COEF, NL>(wyz_a * P.wq[qx], s_kap + cw * US, (qx * N + t) * N + qz,
-                                                            U[qx][0], dcoef) * fast_rcp(adet);
+                    const double s = stiff_weight<COEF && !ADV, NL>(wyz_a * P.wq[qx], s_kap + cw * US,
+                                                                    (qx * N + t) * N + qz, U[qx][0], dcoef) *
+                                     fast_rcp(adet);
                     double h[3];
                     if constexpr (NL == 2) {
                         // u and its reference gradient at (qx, qy = t, qz) from the buffer's quadrature
@@ -490,6 +511,13 @@
                     for (int q = 0; q < N; q++) {
                         Vp[q][0] = fma(P.Dt[qx * N + q], fx, Vp[q][0]);
                         Vp[qx][q] = fma(dz[q], fz, Vp[qx][q]);
+                    }
+                    if constexpr (ADV) {
+                        // w |det J| b . grad u = w sign(det J) (b . h), whatever beta is
+                        const double *sb = s_kap + cw * US + (qx * N + t) * N + qz;
+                        const double bh = sb[0] * h[0] + sb[WS::UBUF] * h[1] + sb[2 * WS::UBUF] * h[2];
+                        const double w = P.wq[lane_active ? t : 0] * P.wq[qz] * P.wq[qx];
+                        Vp[qx][0] = fma(copysign(w, det), bh, Vp[qx][0]);
                     }
                     if (MASS) Vp[qx][0] = fma(wyz_b * P.wq[qx] * adet, U[qx][0], Vp[qx][0]);
                 }

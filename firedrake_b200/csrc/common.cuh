@@ -93,6 +93,7 @@ int fdb_mat_device_view(fdb_mat_t m, const long long **rowptr, const fdb_int **c
                         const fdb_int **row_lg, const fdb_int **col_lg);
 int fdb_mat_rank_table(fdb_mat_t m, const unsigned short **rank, int *nvar);
 int fdb_mat_block_size(fdb_mat_t m, int *bs);
+int fdb_mat_rows(fdb_mat_t m, fdb_int *nrows);      // node rows (block rows if blocked)
 int fdb_mat_scalar_view_begin(fdb_mat_t blocked, fdb_mat_t *view);
 int fdb_mat_scalar_view_end(fdb_mat_t blocked, fdb_mat_t view);
 int fdb_launch_helmholtz_matrix(fdb_kernel_s *k, fdb_int start, fdb_int end, int nlay,

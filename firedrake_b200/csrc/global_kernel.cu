@@ -282,22 +282,25 @@ struct fdb_hex_form {
     int cdim;                 // value size of the argument space; 0: any of 1..3, the diagonal scalar only
     bool affine;              // has the affine_cells variant
     const char *coef;         // the trailing coefficient argument, or NULL
+    int coef_cdim;            // its values per node (0 without one): the argument space's, or 3 for b
     bool residual;            // a 1-form action only
     int launcher;             // fdb_launch_helmholtz_*, fdb_launch_helmholtz_coef_* (which also run the
-                              // nonlinear diffusion forms) or fdb_launch_elasticity_*
+                              // nonlinear diffusion and advection-diffusion forms) or fdb_launch_elasticity_*
     int max_degree[3];        // per mode: action, matrix, diagonal
 };
 
 static const fdb_hex_form hex_forms[] = {
-    {FDB_FORM_HELMHOLTZ, "helmholtz", 0, true, nullptr, false, LAUNCH_HELMHOLTZ, {5, 4, 3}},
-    {FDB_FORM_HELMHOLTZ_COEF, "helmholtz_coef", 1, false, "kappa", false, LAUNCH_HELMHOLTZ_COEF, {5, 4, 3}},
-    {FDB_FORM_NONLINEAR_DIFFUSION, "nonlinear_diffusion", 1, false, nullptr, true, LAUNCH_HELMHOLTZ_COEF,
+    {FDB_FORM_HELMHOLTZ, "helmholtz", 0, true, nullptr, 0, false, LAUNCH_HELMHOLTZ, {5, 4, 3}},
+    {FDB_FORM_HELMHOLTZ_COEF, "helmholtz_coef", 1, false, "kappa", 1, false, LAUNCH_HELMHOLTZ_COEF, {5, 4, 3}},
+    {FDB_FORM_NONLINEAR_DIFFUSION, "nonlinear_diffusion", 1, false, nullptr, 0, true, LAUNCH_HELMHOLTZ_COEF,
      {5, 0, 0}},
-    {FDB_FORM_NONLINEAR_DIFFUSION_JACOBIAN, "nonlinear_diffusion_jacobian", 1, false, "u", false,
+    {FDB_FORM_NONLINEAR_DIFFUSION_JACOBIAN, "nonlinear_diffusion_jacobian", 1, false, "u", 1, false,
      LAUNCH_HELMHOLTZ_COEF, {5, 4, 3}},
-    {FDB_FORM_ELASTICITY, "elasticity", 3, false, nullptr, false, LAUNCH_ELASTICITY, {4, 3, 3}},
-    {FDB_FORM_HYPERELASTICITY, "hyperelasticity", 3, false, nullptr, true, LAUNCH_ELASTICITY, {4, 0, 0}},
-    {FDB_FORM_HYPERELASTICITY_JACOBIAN, "hyperelasticity_jacobian", 3, false, "u", false, LAUNCH_ELASTICITY,
+    {FDB_FORM_ELASTICITY, "elasticity", 3, false, nullptr, 0, false, LAUNCH_ELASTICITY, {4, 3, 3}},
+    {FDB_FORM_HYPERELASTICITY, "hyperelasticity", 3, false, nullptr, 0, true, LAUNCH_ELASTICITY, {4, 0, 0}},
+    {FDB_FORM_HYPERELASTICITY_JACOBIAN, "hyperelasticity_jacobian", 3, false, "u", 3, false, LAUNCH_ELASTICITY,
+     {4, 3, 3}},
+    {FDB_FORM_ADVECTION_DIFFUSION, "advection_diffusion", 1, false, "b", 3, false, LAUNCH_HELMHOLTZ_COEF,
      {4, 3, 3}},
 };
 
@@ -526,6 +529,24 @@ int fdb_kernel_call(fdb_kernel_t k, const fdb_call_args *a)
         }
         if (k->desc.scatter != FDB_SCATTER_ATOMIC) {
             set_error("fdb_kernel_call: coloured scatter is not implemented for matrices");
+            return 1;
+        }
+    }
+    if (f->coef && f->coef_cdim != k->desc.cdim && a->location == FDB_LOC_HOST && a->arg_bytes && mode != MODE_DIAGONAL) {
+        // a coefficient with another value size than the argument space (advection-diffusion's b): host mode
+        // mirrors it by its byte size, which must cover every node that x (action) or the Mat's rows (matrix)
+        // cover.  Device mode has no sizes to check; op2.Parloop checks the Dat's value size there.
+        size_t nodes;
+        if (mat) {
+            fdb_int rows = 0;
+            fdb_mat_rows(mat, &rows);
+            nodes = (size_t)rows;
+        } else {
+            nodes = a->arg_bytes[2] / (sizeof(double) * k->desc.cdim);
+        }
+        if (a->arg_bytes[want - 1] < nodes * f->coef_cdim * sizeof(double)) {
+            set_error("fdb_kernel_call: %s %s: %s has %d values per node, %zu bytes are too few for %zu nodes",
+                      f->name, mode_name[mode], f->coef, f->coef_cdim, a->arg_bytes[want - 1], nodes);
             return 1;
         }
     }

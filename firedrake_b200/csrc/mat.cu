@@ -275,6 +275,12 @@ int fdb_mat_block_size(fdb_mat_t m, int *bs)
     return 0;
 }
 
+int fdb_mat_rows(fdb_mat_t m, fdb_int *nrows)
+{
+    *nrows = m->nrows;
+    return 0;
+}
+
 // Scalar view of a blocked matrix for forms whose element tensor is A_scalar (x) I
 // (inner(grad u, grad v) + inner(u, v) on a vector space: the off-diagonal
 // component blocks vanish identically, SURVEY.md section 8d).  The view shares the

@@ -1381,6 +1381,11 @@ class Kernel:
     output, coordinates, u).  "hyperelasticity_jacobian" is its Gateaux derivative at u, with u as the
     LAST argument: action (output, coordinates, w, u), diagonal and rank 2 (output, coordinates, u).
     Its matrix is symmetric.
+
+    "advection_diffusion" is ``alpha*inner(grad u, grad v)*dx + inner(dot(b, grad u), v)*dx +
+    beta*inner(u, v)*dx`` on a scalar space, with the velocity b a Dat of 3 values per node of the argument
+    space (``op2.DataSet(V.node_set, 3)``), passed as the LAST argument like kappa: action (output,
+    coordinates, u, b), diagonal and rank 2 (output, coordinates, b).  Its matrix is not symmetric.
     """
     form: str = "helmholtz"
     degree: int = 1
@@ -1448,6 +1453,7 @@ class _Form(NamedTuple):
     coefficient: bool = False   # a trailing coefficient argument (kappa, or a Jacobian's u)
     residual: bool = False      # a rank-1 action only
     lame: bool = False          # takes mu and lmbda
+    coef_cdim: int = 0          # values per node of the trailing coefficient when they differ from the space's
 
 
 _FORMS = {"helmholtz": _Form(_lib.FORM_HELMHOLTZ),
@@ -1457,7 +1463,8 @@ _FORMS = {"helmholtz": _Form(_lib.FORM_HELMHOLTZ),
           "nonlinear_diffusion_jacobian": _Form(_lib.FORM_NONLINEAR_DIFFUSION_JACOBIAN, coefficient=True),
           "elasticity": _Form(_lib.FORM_ELASTICITY, lame=True),
           "hyperelasticity": _Form(_lib.FORM_HYPERELASTICITY, residual=True, lame=True),
-          "hyperelasticity_jacobian": _Form(_lib.FORM_HYPERELASTICITY_JACOBIAN, coefficient=True, lame=True)}
+          "hyperelasticity_jacobian": _Form(_lib.FORM_HYPERELASTICITY_JACOBIAN, coefficient=True, lame=True),
+          "advection_diffusion": _Form(_lib.FORM_ADVECTION_DIFFUSION, coefficient=True, coef_cdim=3)}
 _INTEGRALS = {"cell": _lib.INTEGRAL_CELL, "exterior_facet": _lib.INTEGRAL_EXTERIOR_FACET,
               "interior_facet": _lib.INTEGRAL_INTERIOR_FACET, "fused": _lib.INTEGRAL_FUSED}
 
@@ -1665,6 +1672,12 @@ class Parloop:
         lk = self.global_kernel.local_kernel
         if len(self.args) != len(lk.accesses):
             raise ValueError(f"kernel takes {len(lk.accesses)} arguments, got {len(self.args)}")
+        spec = _FORMS.get(getattr(lk, "form", None))
+        if spec and spec.coef_cdim and self.args[-1].data.cdim != spec.coef_cdim:
+            # the kernel reads coef_cdim values per node (e.g. advection-diffusion's b at 3 node + c): a Dat with
+            # fewer would be read past its end
+            raise ValueError(f"{lk.form}: the trailing coefficient has {spec.coef_cdim} values per node, "
+                             f"{self.args[-1].data.name} has {self.args[-1].data.cdim}")
         for a, acc in zip(self.args, lk.accesses):
             if a.access != acc:
                 raise ValueError(f"argument {a.data.name}: access {a.access.name} != kernel's {acc.name}")

@@ -165,7 +165,7 @@ enum fdb_form {
                                    as FDB_FORM_ELASTICITY; rank 1 action only (not rank 2, not
                                    diagonal), degrees 1..4:  [y INC, coords, u]  (atomic or coloured;
                                    device or host mode, host mode monolithic).                      */
-    FDB_FORM_HYPERELASTICITY_JACOBIAN = 8
+    FDB_FORM_HYPERELASTICITY_JACOBIAN = 8,
                                 /* its Gateaux derivative at u (exact Newton Jacobian, symmetric):
                                      J(u)[w; v] = inner(dP[grad w], grad v)*dx + beta*inner(w, v)*dx
                                      dP[H] = mu H + (mu - lmbda ln J) F^{-T} H^T F^{-T}
@@ -175,6 +175,20 @@ enum fdb_form {
                                      action    [y INC, coords, w, u]  (device or host mode)
                                      diagonal  [d INC, coords, u]     (device mode)
                                      rank 2    [Mat (block size 3), coords, u]                      */
+    FDB_FORM_ADVECTION_DIFFUSION = 9
+                                /* advection-diffusion of a scalar (NOT symmetric):
+                                     a(u, v) = alpha*inner(grad u, grad v)*dx
+                                               + inner(dot(b, grad u), v)*dx + beta*inner(u, v)*dx
+                                   b is a vector FIELD of 3 components on the nodes of the scalar
+                                   argument space, AoS (node i holds b[3 i + c]), gathered through
+                                   maps[0].  Hex cells (extruded or native), cdim == 1, nq ==
+                                   degree+1, affine_cells == 0; degrees 1..4 (action), 1..3 (rank 2
+                                   and diagonal).  b is always the LAST argument:
+                                     action    [y INC, coords, u, b]  (atomic or coloured; device or
+                                               host mode, host mode monolithic)
+                                     diagonal  [d INC, coords, b]     (device mode)
+                                     rank 2    [Mat, coords, b]  (row = test dof, column = trial dof)
+                                   Never the DMMA element-matrix kernels (they assume symmetry).  */
 };
 
 enum fdb_cell {
