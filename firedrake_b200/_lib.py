@@ -23,6 +23,7 @@ FORM_ELASTICITY = 6
 FORM_HYPERELASTICITY = 7
 FORM_HYPERELASTICITY_JACOBIAN = 8
 FORM_ADVECTION_DIFFUSION = 9
+FORM_STOKES = 10
 CELL_HEX_EXTRUDED = 1
 CELL_HEX = 2
 CELL_TRIANGLE = 3
@@ -53,6 +54,15 @@ class KernelDesc(C.Structure):
         ("diagonal", C.c_int32), ("affine_cells", C.c_int32),
         ("dcoef", C.c_double * 3),
         ("lmbda", C.c_double),
+    ]
+
+
+class Space2Desc(C.Structure):
+    """fdb_space2_desc: the second space of a form on two spaces (fdb_kernel_create_mixed)."""
+    _fields_ = [
+        ("degree", C.c_int32),
+        ("B", C.c_double * (MAX_1D * MAX_1D)),
+        ("offset", C.POINTER(C.c_int32)),
     ]
 
 
@@ -130,6 +140,7 @@ SIGNATURES = {
     "fdb_mirror_drop": (C.c_int, [C.c_void_p]),
     "fdb_mirror_drop_all": (C.c_int, []),
     "fdb_kernel_create": (C.c_int, [C.POINTER(KernelDesc), C.POINTER(C.c_void_p)]),
+    "fdb_kernel_create_mixed": (C.c_int, [C.POINTER(KernelDesc), C.POINTER(Space2Desc), C.POINTER(C.c_void_p)]),
     "fdb_kernel_destroy": (C.c_int, [C.c_void_p]),
     "fdb_cells_are_affine": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int,
                                        C.POINTER(C.c_int)]),

@@ -502,6 +502,113 @@ def assemble_elasticity_generic(V: "FunctionSpace", u: op2.Dat, mu, lmbda, beta=
     return tensor
 
 
+def stokes_kernel(degree, mu=1.0, beta=0.0, name="stokes_action"):
+    """C source of the Stokes action ``mu*inner(grad u, grad v)*dx + beta*inner(u, v)*dx - p*div(v)*dx -
+    q*div(u)*dx`` on Taylor-Hood Q_p-Q_(p-1) hexahedra, run through the generic wrapper builder with MixedDat
+    arguments: the independent statement of the hand-written FDB_FORM_STOKES kernel.  Arguments: y (INC) and
+    up, each the velocity's 3 END values (AoS) followed by the pressure's (EN-1)^3, and the coordinates.
+    The pressure is held in an EN^3 block, zero at every dof index EN-1, with its table padded by a zero
+    column, so the square contractions of the velocity serve it too."""
+    from .codegen import CStringKernel
+    from .fiat_lite import interval_element
+    if not 2 <= degree <= 4:
+        raise NotImplementedError(f"the generic-path Stokes statement covers degrees 2..4, got degree {degree}")
+    elq = interval_element(degree - 1, degree + 1)
+    n = degree + 1
+    bq = [[float(elq.B[q, a]) if a < n - 1 else 0.0 for a in range(n)] for q in range(n)]
+    tab = "{" + ", ".join("{" + ", ".join(repr(v) for v in r) + "}" for r in bq) + "}"
+    code = _vector_hex_tables(degree) + f"""#define ENP (EN - 1)
+static const double EQ[EN][EN] = {tab};      /* EQ[q][a]: pressure basis, zero last column */
+static void {name}(double *y, const double *X, const double *up)
+{{
+    double U[3][END], G[3][3][END], c[END], t[END], P[END], T[END];
+    const double *pin = up + 3 * END;
+    for (int d = 0; d < 3; ++d) {{
+        for (int i = 0; i < END; ++i) c[i] = up[i * 3 + d];
+        el_tensor(EB, EB, EB, 0, c, U[d]);
+        el_tensor(ED, EB, EB, 0, c, G[d][0]);
+        el_tensor(EB, ED, EB, 0, c, G[d][1]);
+        el_tensor(EB, EB, ED, 0, c, G[d][2]);
+    }}
+    for (int i = 0; i < END; ++i) {{
+        const int a = i / (EN * EN), b = (i / EN) % EN, e = i % EN;
+        c[i] = (a < ENP && b < ENP && e < ENP) ? pin[(a * ENP + b) * ENP + e] : 0.0;
+    }}
+    el_tensor(EQ, EQ, EQ, 0, c, P);
+    for (int qx = 0; qx < EN; ++qx) for (int qy = 0; qy < EN; ++qy) for (int qz = 0; qz < EN; ++qz) {{
+        const int q = (qx * EN + qy) * EN + qz;
+        const double xi[3] = {{EX[qx], EX[qy], EX[qz]}};
+        double J[3][3] = {{{{0}}}};
+        for (int v = 0; v < 8; ++v) {{
+            const int b[3] = {{(v >> 2) & 1, (v >> 1) & 1, v & 1}};
+            for (int r = 0; r < 3; ++r) {{
+                double g = b[r] ? 1.0 : -1.0;
+                for (int e = 0; e < 3; ++e) if (e != r) g *= b[e] ? xi[e] : 1.0 - xi[e];
+                for (int k = 0; k < 3; ++k) J[k][r] += X[v * 3 + k] * g;
+            }}
+        }}
+        const double det = J[0][0] * (J[1][1] * J[2][2] - J[1][2] * J[2][1])
+                         - J[0][1] * (J[1][0] * J[2][2] - J[1][2] * J[2][0])
+                         + J[0][2] * (J[1][0] * J[2][1] - J[1][1] * J[2][0]);
+        double Jinv[3][3];
+        Jinv[0][0] = (J[1][1] * J[2][2] - J[1][2] * J[2][1]) / det;
+        Jinv[0][1] = (J[0][2] * J[2][1] - J[0][1] * J[2][2]) / det;
+        Jinv[0][2] = (J[0][1] * J[1][2] - J[0][2] * J[1][1]) / det;
+        Jinv[1][0] = (J[1][2] * J[2][0] - J[1][0] * J[2][2]) / det;
+        Jinv[1][1] = (J[0][0] * J[2][2] - J[0][2] * J[2][0]) / det;
+        Jinv[1][2] = (J[0][2] * J[1][0] - J[0][0] * J[1][2]) / det;
+        Jinv[2][0] = (J[1][0] * J[2][1] - J[1][1] * J[2][0]) / det;
+        Jinv[2][1] = (J[0][1] * J[2][0] - J[0][0] * J[2][1]) / det;
+        Jinv[2][2] = (J[0][0] * J[1][1] - J[0][1] * J[1][0]) / det;
+        const double wd = EW[qx] * EW[qy] * EW[qz] * fabs(det);
+        double Gp[3][3], S[3][3];
+        for (int d = 0; d < 3; ++d)
+            for (int k = 0; k < 3; ++k)
+                Gp[d][k] = G[d][0][q] * Jinv[0][k] + G[d][1][q] * Jinv[1][k] + G[d][2][q] * Jinv[2][k];
+        for (int d = 0; d < 3; ++d)
+            for (int k = 0; k < 3; ++k)
+                S[d][k] = {float(mu)!r} * Gp[d][k] - (d == k ? P[q] : 0.0);
+        for (int d = 0; d < 3; ++d) {{
+            for (int m = 0; m < 3; ++m)
+                G[d][m][q] = wd * (Jinv[m][0] * S[d][0] + Jinv[m][1] * S[d][1] + Jinv[m][2] * S[d][2]);
+            U[d][q] *= {float(beta)!r} * wd;
+        }}
+        T[q] = -wd * (Gp[0][0] + Gp[1][1] + Gp[2][2]);
+    }}
+    for (int d = 0; d < 3; ++d) {{
+        el_tensor(EB, EB, EB, 1, U[d], c);
+        el_tensor(ED, EB, EB, 1, G[d][0], t);  for (int i = 0; i < END; ++i) c[i] += t[i];
+        el_tensor(EB, ED, EB, 1, G[d][1], t);  for (int i = 0; i < END; ++i) c[i] += t[i];
+        el_tensor(EB, EB, ED, 1, G[d][2], t);  for (int i = 0; i < END; ++i) c[i] += t[i];
+        for (int i = 0; i < END; ++i) y[i * 3 + d] += c[i];
+    }}
+    el_tensor(EQ, EQ, EQ, 1, T, c);
+    for (int a = 0; a < ENP; ++a) for (int b = 0; b < ENP; ++b) for (int e = 0; e < ENP; ++e)
+        y[3 * END + (a * ENP + b) * ENP + e] += c[(a * EN + b) * EN + e];
+}}
+#undef ENP
+#undef END
+#undef EN
+"""
+    return CStringKernel(code, name)
+
+
+def assemble_stokes_generic(F: "Stokes", up: op2.MixedDat, tensor=None):
+    """``assemble(action(a, up))`` of :class:`Stokes` through the generic wrapper path (:func:`stokes_kernel`,
+    MixedDat arguments over the velocity and pressure maps): the cross-check and the baseline of the
+    hand-written kernel."""
+    V = F.V
+    if tensor is None:
+        tensor = F.dat()
+    tensor.zero()
+    for d in tensor:
+        d.device_ptr
+    mm = op2.MixedMap([V.cell_node_map, F.pressure_map])
+    op2.par_loop(stokes_kernel(V.degree, F.mu, F.beta), V.cell_set, tensor(op2.INC, mm),
+                 V.coordinates(op2.READ, V.coord_map), up(op2.READ, mm))
+    return tensor
+
+
 def advection_diffusion_kernel(degree, alpha=1.0, beta=0.0, name="advection_diffusion_action"):
     """C source of the 1-form ``action(alpha*inner(grad(u), grad(v))*dx + inner(dot(b, grad(u)), v)*dx +
     beta*inner(u, v)*dx, u)`` on the scalar Q_p (x) P_p space, with the velocity b of 3 values per node
@@ -1033,6 +1140,113 @@ class AdvectionDiffusion:
                           rank=rank, diagonal=diagonal)
 
 
+@dataclass
+class Stokes:
+    """Stokes flow on Taylor-Hood hexahedra: velocity in the vector space ``V`` (CG_p, ``cdim = 3``) and
+    pressure in the scalar space ``Q`` (CG_{p-1}) on the same mesh, p = 2..4 (Q2-Q1, Q3-Q2, Q4-Q3):
+
+        a((u, p), (v, q)) = mu*inner(grad(u), grad(v))*dx + beta*inner(u, v)*dx - p*div(v)*dx - q*div(u)*dx
+
+    beta = 0 is steady Stokes, beta = 1/dt an implicit Euler step of unsteady Stokes.  The form is symmetric
+    and indefinite.  Firedrake's Stokes demo writes ``+ q*div(u)``: that is the same system with the pressure
+    rows negated; the symmetric sign here makes the transpose the operator itself.
+
+    Vectors are :class:`op2.MixedDat` (velocity, pressure), e.g. ``F.dat()``.  It works with
+    ``assemble(F, u=up)`` (the action, a MixedDat), ``assemble(F, mat_type="matfree")`` and :func:`solve`
+    (GMRES, optionally with a diagonal Schur-complement fieldsplit preconditioner).  There is no assembled
+    matrix.  Dirichlet conditions are on the velocity space ``V``."""
+    V: FunctionSpace
+    Q: FunctionSpace
+    mu: float = 1.0
+    beta: float = 0.0
+    symmetric = True
+
+    def __post_init__(self):
+        V, Q = self.V, self.Q
+        if V.cdim != 3:
+            raise ValueError(f"the Stokes velocity space is a vector space with 3 components, got cdim {V.cdim}")
+        if Q.cdim != 1:
+            raise ValueError(f"the Stokes pressure space is scalar, got cdim {Q.cdim}")
+        if V.mesh is not Q.mesh:
+            raise ValueError("the Stokes velocity and pressure spaces must be on the same mesh")
+        if not 2 <= V.degree <= 4 or Q.degree != V.degree - 1:
+            raise ValueError(f"Taylor-Hood Q_p-Q_(p-1) with p = 2..4: got velocity degree {V.degree}, pressure "
+                             f"degree {Q.degree}")
+        if any(W.dof_dset.halo is not None or W.cell_set.owner_computes for W in (V, Q)):
+            raise NotImplementedError("Stokes on a partitioned mesh is not implemented: the velocity and pressure "
+                                      "node sets need their own halo design")
+        # the pressure map on the velocity space's cell set (the parloop iterates over one set)
+        self.pressure_map = op2.Map(V.cell_set, Q.node_set, Q.V.arity, Q.V.cell_node_map, offset=Q.V.offset)
+
+    def dat(self, u=None, p=None):
+        """A (velocity, pressure) vector: ``op2.MixedDat([V.dat(u), Q.dat(p)])``."""
+        return op2.MixedDat([self.V.dat(u), self.Q.dat(p)])
+
+    def kernel(self, rank=1, diagonal=False):
+        if rank != 1 or diagonal:
+            raise NotImplementedError("Stokes is an action only: there is no assembled matrix or diagonal "
+                                      "(use mat_type='matfree')")
+        return op2.Kernel("stokes", degree=self.V.degree, mu=self.mu, beta=self.beta)
+
+
+class StokesAssembler:
+    """Cached assembler of the Stokes action (velocity, pressure) -> (y_u, y_p) on MixedDats, the
+    counterpart of :class:`OneFormAssembler`: the parloop is built once and re-run."""
+
+    def __init__(self, form: Stokes, up: op2.MixedDat, bcs=(), scatter="atomic"):
+        self.form, self.up, self.bcs = form, up, tuple(bcs)
+        V = form.V
+        self._gk = op2.GlobalKernel(form.kernel(1), [V.cell_node_map, V.coord_map, form.pressure_map],
+                                    extruded=True, scatter=scatter)
+        self._loop = None
+
+    def assemble(self, tensor=None):
+        F = self.form
+        V = F.V
+        if tensor is None:
+            tensor = F.dat()
+        if self._loop is None or self._tensor is not tensor:
+            self._tensor = tensor
+            u, p = self.up
+            yu, yp = tensor
+            self._loop = op2.Parloop(self._gk, V.cell_set,
+                                     [yu(op2.INC, V.cell_node_map), V.coordinates(op2.READ, V.coord_map),
+                                      u(op2.READ, V.cell_node_map), yp(op2.INC, F.pressure_map),
+                                      p(op2.READ, F.pressure_map)], location="device")
+        tensor.zero()
+        self._loop()
+        for bc in self.bcs:
+            bc.zero(tensor[0])
+        return tensor
+
+
+class StokesMatrixContext:
+    """Matrix-free Stokes operator on MixedDats: ``mult`` zeroes the velocity-BC entries of x, applies the
+    saddle-point action and writes x back on the constrained velocity rows (identity there).  The operator
+    is symmetric, so ``multTranspose`` is ``mult``."""
+
+    def __init__(self, form: Stokes, bcs=()):
+        self.form, self.bcs = form, tuple(bcs)
+        self._x = form.dat()
+        self._assembler = StokesAssembler(form, self._x, ())
+
+    def mult(self, X: op2.MixedDat, Y: op2.MixedDat):
+        from . import _lib
+        L = _lib.lib()
+        for a, b in zip(self._x, X):
+            _lib.check(L.fdb_memcpy_d2d(a.device_ptr, b.device_ptr, b.nbytes))
+            a._device_written()
+        for bc in self.bcs:
+            bc.zero(self._x[0])
+        self._assembler.assemble(tensor=Y)
+        for bc in self.bcs:
+            bc.set(Y[0], X[0])
+        return Y
+
+    def multTranspose(self, X: op2.MixedDat, Y: op2.MixedDat):
+        return self.mult(X, Y)
+
+
 class ConvergenceError(RuntimeError):
     """A nonlinear solve that cannot go on (firedrake.exceptions.ConvergenceError); ``reason`` is the
     SNES converged reason, e.g. "DIVERGED_FNORM_NAN"."""
@@ -1089,6 +1303,13 @@ def assemble(form: Form, u=None, tensor=None, bcs=(), mat_type="aij"):
     unassembled), ``"matfree"`` -> :class:`ImplicitMatrixContext`."""
     V = form.V
     bcs = tuple(bcs)
+    if isinstance(form, Stokes):
+        if u is not None:
+            return StokesAssembler(form, u, bcs).assemble(tensor)
+        if mat_type != "matfree":
+            raise NotImplementedError(f"mat_type {mat_type!r}: Stokes has no assembled matrix, use mat_type "
+                                      f"'matfree'")
+        return StokesMatrixContext(form, bcs)
     if u is not None:
         return OneFormAssembler(form, u, bcs).assemble(tensor)
     if mat_type == "matfree":
@@ -1312,30 +1533,52 @@ def gmres(A, b: op2.Dat, x: op2.Dat, M=None, rtol=1e-5, atol=0.0, restart=30, ma
     z)`` writes z from z = 0 (None: no preconditioner).  Inner products run over the owned dofs,
     summed over the ranks by ``allreduce``; the (restart + 1) x restart Hessenberg least-squares
     problem is solved on the host with Givens rotations.  Converged when the residual norm is at most
-    max(rtol * ||b - A x0||, atol).  Returns (iterations, residual norms)."""
+    max(rtol * ||b - A x0||, atol).  Returns (iterations, residual norms).
+
+    The vectors may be :class:`op2.MixedDat` (e.g. velocity and pressure of :class:`Stokes`): every vector
+    operation then runs block by block, and an inner product is the sum of the blocks' inner products."""
     import ctypes as C
     from . import _lib
     from .mg import _touched
     L = _lib.lib()
-    Vd = b.dataset
-    n = b._data.size
-    n_owned = b.dataset.set.size * b.cdim
+    mixed = isinstance(b, op2.MixedDat)
+    blocks = (lambda v: tuple(v)) if mixed else (lambda v: (v,))
+    sizes = [(d._data.size, d.dataset.set.size * d.cdim) for d in blocks(b)]
     m = max(1, int(restart))
-    Vs = [op2.Dat(Vd) for _ in range(m + 1)]
-    Zs = [op2.Dat(Vd) for _ in range(m)] if M is not None else Vs
-    w = op2.Dat(Vd)
+    new = (lambda: op2.MixedDat([op2.Dat(d.dataset) for d in b])) if mixed else (lambda: op2.Dat(b.dataset))
+    Vs = [new() for _ in range(m + 1)]
+    Zs = [new() for _ in range(m)] if M is not None else Vs
+    w = new()
 
     def dot(u, v):
-        out = C.c_double()
-        _lib.check(L.fdb_vec_dot(n_owned, u.device_ptr, v.device_ptr, C.byref(out)))
-        return allreduce(out.value) if allreduce else out.value
+        s = 0.0
+        for (_, n_owned), ub, vb in zip(sizes, blocks(u), blocks(v)):
+            out = C.c_double()
+            _lib.check(L.fdb_vec_dot(n_owned, ub.device_ptr, vb.device_ptr, C.byref(out)))
+            s += out.value
+        return allreduce(s) if allreduce else s
+
+    def axpy(a, xv, yv):
+        for (n, _), xb, yb in zip(sizes, blocks(xv), blocks(yv)):
+            _lib.check(L.fdb_vec_axpy(n, a, xb.device_ptr, yb.device_ptr))
+
+    def scale(a, xv):
+        for (n, _), xb in zip(sizes, blocks(xv)):
+            _lib.check(L.fdb_vec_scale(n, a, xb.device_ptr))
+
+    def copy(dst, src):
+        for db, sb in zip(blocks(dst), blocks(src)):
+            _lib.check(L.fdb_memcpy_d2d(db.device_ptr, sb.device_ptr, sb.nbytes))
+
+    def touched(v):
+        _touched(*blocks(v))
 
     def residual(r):
         """r = b - A x, returns ||r||"""
         A.mult(x, w)
-        _lib.check(L.fdb_memcpy_d2d(r.device_ptr, b.device_ptr, b.nbytes))
-        _lib.check(L.fdb_vec_axpy(n, -1.0, w.device_ptr, r.device_ptr))
-        _touched(r)
+        copy(r, b)
+        axpy(-1.0, w, r)
+        touched(r)
         return float(np.sqrt(dot(r, r)))
 
     beta = residual(Vs[0])
@@ -1343,8 +1586,8 @@ def gmres(A, b: op2.Dat, x: op2.Dat, M=None, rtol=1e-5, atol=0.0, restart=30, ma
     tol = max(rtol * beta, atol)
     it = 0
     while beta > tol and it < maxit:
-        _lib.check(L.fdb_vec_scale(n, 1.0 / beta, Vs[0].device_ptr))
-        _touched(Vs[0])
+        scale(1.0 / beta, Vs[0])
+        touched(Vs[0])
         H = np.zeros((m + 1, m))
         cs, sn = np.zeros(m), np.zeros(m)
         g = np.zeros(m + 1)
@@ -1353,18 +1596,19 @@ def gmres(A, b: op2.Dat, x: op2.Dat, M=None, rtol=1e-5, atol=0.0, restart=30, ma
         for j in range(m):
             if M is not None:
                 Zs[j].zero()
-                Zs[j].device_ptr
+                for zb in blocks(Zs[j]):
+                    zb.device_ptr
                 M(Vs[j], Zs[j])
             A.mult(Zs[j], w)
             for i in range(j + 1):                      # modified Gram-Schmidt
                 H[i, j] = dot(w, Vs[i])
-                _lib.check(L.fdb_vec_axpy(n, -H[i, j], Vs[i].device_ptr, w.device_ptr))
-            _touched(w)
+                axpy(-H[i, j], Vs[i], w)
+            touched(w)
             H[j + 1, j] = np.sqrt(max(dot(w, w), 0.0))
             if H[j + 1, j] > 0.0:
-                _lib.check(L.fdb_memcpy_d2d(Vs[j + 1].device_ptr, w.device_ptr, w.nbytes))
-                _lib.check(L.fdb_vec_scale(n, 1.0 / H[j + 1, j], Vs[j + 1].device_ptr))
-                _touched(Vs[j + 1])
+                copy(Vs[j + 1], w)
+                scale(1.0 / H[j + 1, j], Vs[j + 1])
+                touched(Vs[j + 1])
             for i in range(j):                          # previous rotations on the new column
                 t = cs[i] * H[i, j] + sn[i] * H[i + 1, j]
                 H[i + 1, j] = -sn[i] * H[i, j] + cs[i] * H[i + 1, j]
@@ -1385,8 +1629,8 @@ def gmres(A, b: op2.Dat, x: op2.Dat, M=None, rtol=1e-5, atol=0.0, restart=30, ma
         for i in range(k - 1, -1, -1):
             y[i] = (g[i] - H[i, i + 1:k] @ y[i + 1:k]) / H[i, i] if H[i, i] != 0.0 else 0.0
         for i in range(k):
-            _lib.check(L.fdb_vec_axpy(n, y[i], Zs[i].device_ptr, x.device_ptr))
-        _touched(x)
+            axpy(y[i], Zs[i], x)
+        touched(x)
         beta = residual(Vs[0])                          # the true residual at every restart
         hist[-1] = beta
     return it, hist
@@ -1506,7 +1750,8 @@ def solve_nonlinear(F, L: op2.Dat, u: op2.Dat, bcs=(), solver_parameters=None, h
     return hist, kits
 
 
-def solve(form: Form, L: op2.Dat, u: op2.Dat, bcs=(), solver_parameters=None, hierarchy=None, allreduce=None):
+def solve(form: Form, L: op2.Dat, u: op2.Dat, bcs=(), solver_parameters=None, hierarchy=None, allreduce=None,
+          nullspace=None):
     """``solve(a == L, u, bcs=bcs, solver_parameters=...)`` for the supported forms
     (firedrake/solving.py:128-260 -> LinearVariationalSolver; SURVEY.md section 3.5): assemble the
     operator, lift the Dirichlet values, run the Krylov solver on the device.  ``form``: a
@@ -1520,8 +1765,13 @@ def solve(form: Form, L: op2.Dat, u: op2.Dat, bcs=(), solver_parameters=None, hi
     cg refuses), ``ksp_gmres_restart`` (30); ``pc_type`` "none" (default) | "jacobi" | "mg" (needs
     ``hierarchy``, a mg.MeshHierarchy whose finest mesh is ``form.V.mesh``; for advection-diffusion a
     V-cycle of its symmetric part ``Form(W, alpha, beta)``); ``ksp_rtol`` (1e-8), ``ksp_max_it`` (1000).
-    Returns (iterations, residual history)."""
+    A :class:`Stokes` form takes MixedDats and its own options (:func:`_solve_stokes`), and the only form
+    that takes ``nullspace``.  Returns (iterations, residual history)."""
     from . import _lib
+    if isinstance(form, Stokes):
+        return _solve_stokes(form, L, u, bcs, solver_parameters, hierarchy, nullspace)
+    if nullspace is not None:
+        raise NotImplementedError("nullspace is implemented for Stokes forms only")
     symmetric = getattr(form, "symmetric", True)
     sp = {"mat_type": "matfree", "ksp_type": "cg" if symmetric else "gmres", "pc_type": "none", "ksp_rtol": 1e-8,
           "ksp_max_it": 1000, "ksp_gmres_restart": 30}
@@ -1599,6 +1849,152 @@ def solve(form: Form, L: op2.Dat, u: op2.Dat, bcs=(), solver_parameters=None, hi
     else:
         for bc in bcs:
             bc.apply(u)
+    return its, hist
+
+
+def _solve_stokes(form: Stokes, L: op2.MixedDat, up: op2.MixedDat, bcs=(), solver_parameters=None,
+                  hierarchy=None, nullspace=None):
+    """``solve(a == L, up, bcs=bcs, solver_parameters=..., nullspace=...)`` for :class:`Stokes`, with the option
+    names of Firedrake's matrix-free Stokes demo:
+
+    - ``mat_type`` "matfree" (the only one); ``ksp_type`` "gmres" (default; "cg" is refused, the operator is
+      indefinite), ``ksp_gmres_restart`` (30), ``ksp_rtol`` (1e-8), ``ksp_max_it`` (1000).
+    - ``pc_type`` "none" (default) or "fieldsplit" with ``pc_fieldsplit_type`` "schur" and
+      ``pc_fieldsplit_schur_fact_type`` "diag": z_u = P_0(r_u), z_p = P_1(r_p).
+      ``fieldsplit_0_pc_type`` "jacobi" (default: the inverse diagonal of the velocity block) or "mg" (one
+      V-cycle of ``Form(W, mu, beta)`` on the vector spaces of ``hierarchy``, with the velocity conditions'
+      sub-domains); ``fieldsplit_1_pc_type`` "jacobi" (default): the inverse diagonal of the Schur complement
+      approximation (1/mu) M_p, as Firedrake's MassInvPC with the viscosity.  Only one application of each
+      (``fieldsplit_*_ksp_type`` "preonly").
+    - ``nullspace`` "constant": the pressure is determined up to a constant
+      (``MixedVectorSpaceBasis(Z, [Z.sub(0), VectorSpaceBasis(constant=True)])``).  The dof-mean of the
+      pressure block is removed from the right-hand side, from every preconditioned vector and from the
+      final pressure.
+
+    Dirichlet conditions are on the velocity; their values are lifted with the full Stokes action on
+    (g, 0), so the pressure rows receive -q div g.  ``up`` is overwritten with the solution.  Returns
+    (iterations, residual history)."""
+    from . import _lib
+    from . import mg as _mg
+    sp = {"mat_type": "matfree", "ksp_type": "gmres", "pc_type": "none", "ksp_rtol": 1e-8, "ksp_max_it": 1000,
+          "ksp_gmres_restart": 30, "fieldsplit_0_pc_type": "jacobi", "fieldsplit_1_pc_type": "jacobi",
+          "fieldsplit_0_ksp_type": "preonly", "fieldsplit_1_ksp_type": "preonly"}
+    sp.update(solver_parameters or {})
+    if sp["ksp_type"] == "cg":
+        raise ValueError("ksp_type cg needs a positive definite operator, and the Stokes operator is indefinite: "
+                         "use gmres")
+    if sp["ksp_type"] != "gmres":
+        raise NotImplementedError(f"ksp_type {sp['ksp_type']!r}: Stokes solves with gmres")
+    if sp["mat_type"] != "matfree":
+        raise NotImplementedError(f"mat_type {sp['mat_type']!r}: Stokes has no assembled matrix, use mat_type "
+                                  f"'matfree'")
+    if nullspace not in (None, "constant"):
+        raise NotImplementedError(f"nullspace {nullspace!r}: None or 'constant' (constant pressures)")
+    pc = sp["pc_type"]
+    if pc not in ("none", "fieldsplit"):
+        raise NotImplementedError(f"pc_type {pc!r}: 'none' or 'fieldsplit'")
+    if pc == "fieldsplit":
+        if sp.get("pc_fieldsplit_type") != "schur":
+            raise NotImplementedError(f"pc_fieldsplit_type {sp.get('pc_fieldsplit_type')!r}: 'schur' only")
+        if sp.get("pc_fieldsplit_schur_fact_type") != "diag":
+            raise NotImplementedError(f"pc_fieldsplit_schur_fact_type {sp.get('pc_fieldsplit_schur_fact_type')!r}: "
+                                      f"'diag' only")
+        for f in ("0", "1"):
+            if sp[f"fieldsplit_{f}_ksp_type"] != "preonly":
+                raise NotImplementedError(f"fieldsplit_{f}_ksp_type {sp[f'fieldsplit_{f}_ksp_type']!r}: 'preonly' "
+                                          f"only")
+        if sp["fieldsplit_0_pc_type"] not in ("jacobi", "mg"):
+            raise NotImplementedError(f"fieldsplit_0_pc_type {sp['fieldsplit_0_pc_type']!r}: 'jacobi' or 'mg'")
+        if sp["fieldsplit_1_pc_type"] != "jacobi":
+            raise NotImplementedError(f"fieldsplit_1_pc_type {sp['fieldsplit_1_pc_type']!r}: 'jacobi' (the "
+                                      f"inverse diagonal of the pressure mass matrix over mu)")
+        if sp["fieldsplit_0_pc_type"] == "mg" and hierarchy is None:
+            raise ValueError("fieldsplit_0_pc_type mg needs the mesh hierarchy")
+    V, Q = form.V, form.Q
+    bcs = tuple(bcs)
+    lib = _lib.lib()
+
+    ones = Q.dat(np.ones(Q.node_count)) if nullspace else None
+
+    def remove_pressure_mean(v):
+        v[1].axpy(-v[1].inner(ones) / Q.node_count, ones)
+
+    # lifting: A (up - (g, 0)) = L - A (g, 0) with homogeneous conditions
+    g = form.dat()
+    g.zero()
+    g[0].device_ptr
+    for bc in bcs:
+        bc.apply(g[0])
+    lift = any(not (np.isscalar(bc.g) and bc.g == 0.0) for bc in bcs)
+    b = form.dat()
+    L.copy(b)
+    if lift:
+        b.axpy(-1.0, StokesAssembler(form, g).assemble())
+    for bc in bcs:
+        bc.zero(b[0])
+    if nullspace:
+        remove_pressure_mean(b)
+    A = StokesMatrixContext(form, bcs)
+    up.zero()
+    for d in up:
+        d.device_ptr
+    M = None
+    if pc == "fieldsplit":
+        n_u, n_p = up[0]._data.size, up[1]._data.size
+        # pressure: the inverse diagonal of (1/mu) M_p
+        dp = ImplicitMatrixContext(Form(Q, 0.0, 1.0 / form.mu)).getDiagonal(Q.dat())
+        op2.par_loop(_mg.reciprocal_kernel(1), Q.node_set, dp(op2.RW))
+        if sp["fieldsplit_0_pc_type"] == "jacobi":
+            # the velocity block is mu * (vector Laplacian) + beta * mass: the scalar diagonal on every component
+            Vs = FunctionSpace(V.mesh, V.degree)
+            ds = ImplicitMatrixContext(Form(Vs, form.mu, form.beta)).getDiagonal(Vs.dat()).data_ro
+            du = V.dat(np.repeat(ds, 3).reshape(-1, 3))
+            for bc in bcs:
+                bc.set(du, 1.0)
+            op2.par_loop(_mg.reciprocal_kernel(3), V.node_set, du(op2.RW))
+
+            def Mu(r, z):
+                _lib.check(lib.fdb_vec_pointwise_mult(n_u, r.device_ptr, du.device_ptr, z.device_ptr))
+                z._device_written()
+        else:
+            # the velocity block is three uncoupled copies of the scalar Form(W, mu, beta): one scalar V-cycle
+            # per component (the Helmholtz diagonal kernel that the smoother needs is scalar)
+            vc = _mg.VCycle(hierarchy, V.degree, lambda W, k=None: Form(W, form.mu, form.beta),
+                            bc_domains=tuple(s for bc in bcs for s in bc.sub_domains))
+            top = len(hierarchy) - 1
+            nn = V.node_count
+            comp = [op2.DeviceArray.from_host(np.ascontiguousarray(3 * np.arange(nn, dtype=np.int32) + c))
+                    for c in range(3)]
+            rs, zs = vc.spaces[-1].dat(), vc.spaces[-1].dat()
+
+            def Mu(r, z):
+                for c in range(3):
+                    _lib.check(lib.fdb_vec_gather(nn, comp[c].ptr, r.device_ptr, rs.device_ptr))
+                    _mg._touched(rs)
+                    zs.zero()
+                    zs.device_ptr
+                    vc.apply(top, rs, zs)
+                    _lib.check(lib.fdb_vec_scatter(nn, comp[c].ptr, zs.device_ptr, z.device_ptr))
+                z._device_written()
+
+        def M(r, z):
+            Mu(r[0], z[0])
+            _lib.check(lib.fdb_vec_pointwise_mult(n_p, r[1].device_ptr, dp.device_ptr, z[1].device_ptr))
+            z[1]._device_written()
+            if nullspace:
+                remove_pressure_mean(z)
+    elif nullspace:
+        def M(r, z):
+            r.copy(z)
+            remove_pressure_mean(z)
+    its, hist = gmres(A, b, up, M, rtol=sp["ksp_rtol"], restart=sp["ksp_gmres_restart"], maxit=sp["ksp_max_it"])
+    if nullspace:
+        remove_pressure_mean(up)
+    if lift:
+        up[0].axpy(1.0, g[0])
+    else:
+        for bc in bcs:
+            bc.apply(up[0])
     return its, hist
 
 

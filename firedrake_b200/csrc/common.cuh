@@ -65,6 +65,9 @@ struct fdb_kernel_s {
     fdb_int *d_off1 = nullptr;
     fdb_int h_off0[512];
     fdb_int h_off1[8];
+    fdb_int *d_off2 = nullptr;   // a form on two spaces (FDB_FORM_STOKES): the second map's layer offsets
+    fdb_int h_off2[512];
+    double B2[FDB_MAX_1D * FDB_MAX_1D];   // and the second space's basis at the points, (nq, degree2 + 1)
     double Dt[FDB_MAX_1D * FDB_MAX_1D];   // collocated derivative D * B^{-1}
     // colouring plan for FDB_SCATTER_COLOURED, built lazily per map
     const void *colour_map_key = nullptr;   // plan is valid for (map pointer, generation, end)
@@ -141,3 +144,8 @@ int fdb_launch_elasticity_action(fdb_kernel_s *k, fdb_int start, fdb_int end, in
 int fdb_launch_elasticity_matrix(fdb_kernel_s *k, fdb_int start, fdb_int end, int nlay, const fdb_int *subset,
                                  fdb_mat_t mat, const double *coords, const double *u, const fdb_int *map0,
                                  const fdb_int *map1, double *diag_out);
+// FDB_FORM_STOKES (elasticity_hex.cu): yu and u AoS with 3 values per node of map0, yp and p one value per
+// node of map2 (the pressure map)
+int fdb_launch_stokes_action(fdb_kernel_s *k, fdb_int start, fdb_int end, int nlay, const fdb_int *subset,
+                             double *yu, const double *coords, const double *u, double *yp, const double *p,
+                             const fdb_int *map0, const fdb_int *map1, const fdb_int *map2);

@@ -33,6 +33,15 @@
 // trial-dof unit in MATRIX mode) into a fourth per-slot buffer S_V; its forward passes share S_T/S_F
 // with those of w, and F comes from the collocated derivative of S_V.  J <= 0 at a point gives NaN
 // (ln of a negative number), as in Firedrake: the kernel does not guard it.
+//
+// FDB_FORM_STOKES (DESIGN.md section 4.11) runs with MODE EL_STOKES: the Taylor-Hood saddle-point action
+// on velocity u (vector CG_p, the node map) and pressure p (scalar CG_{p-1}, a second map map2),
+//     a((u, p), (v, q)) = mu inner(grad u, grad v)*dx + beta inner(u, v)*dx - p div(v)*dx - q div(u)*dx.
+// p's (N-1)^3 values are gathered into a fifth per-slot buffer laid out as an N^3 block whose entries
+// with a dof index N-1 along any axis are zero, so the rectangular (N, N-1) table Bq runs through the
+// same square passes as B: Bq is padded with a zero last column.  The point stage puts mu G - p I into
+// the fluxes where sigma goes and replaces p by its test value -w |det J| tr G, which goes back through
+// Bq^T along z, y, x; the threads of the (N-1)^3 pressure dofs scatter it into yp.
 #include "common.cuh"
 
 namespace {
@@ -58,9 +67,14 @@ struct ElasParams {
     const unsigned short *rank_tab;
     int nvar, nlay_total;
     const double *u;             // EL_JACOBIAN: the linearisation point (AoS, node map)
+    // EL_STOKES: the pressure action output and input (one value per node of map2, (N-1)^3 per cell)
+    double *yp;
+    const double *xp;
+    const fdb_int *map2, *off2;
+    double Bq[N * N];            // pressure basis at the points, (N, N-1) padded with a zero last column
 };
 
-enum { EL_LINEAR = 0, EL_RESIDUAL = 1, EL_JACOBIAN = 2 };
+enum { EL_LINEAR = 0, EL_RESIDUAL = 1, EL_JACOBIAN = 2, EL_STOKES = 3 };
 
 template <int N, int MODE = EL_LINEAR>
 struct ElasShape {
@@ -68,8 +82,9 @@ struct ElasShape {
     static constexpr int CPB = (256 / ND) > 0 ? 256 / ND : 1;          // cells (slots) per CTA
     static constexpr int THREADS = ((CPB * ND + 31) / 32) * 32;
     // doubles per slot: vertices, values at the points, work buffer, fluxes (9 per point); the Jacobian
-    // also holds u's values (S_V)
-    static constexpr int SLOT = 24 + 3 * ND + 3 * ND + 9 * ND + (MODE == EL_JACOBIAN ? 3 * ND : 0);
+    // also holds u's values (S_V), Stokes the pressure and its work buffer (S_P, S_Q)
+    static constexpr int SLOT = 24 + 3 * ND + 3 * ND + 9 * ND + (MODE == EL_JACOBIAN ? 3 * ND : 0) +
+                                (MODE == EL_STOKES ? 2 * ND : 0);
     static constexpr size_t SMEM = (size_t)CPB * SLOT * sizeof(double) + (size_t)CPB * ND * sizeof(int);
 };
 
@@ -110,6 +125,8 @@ elasticity_kernel(const __grid_constant__ ElasParams<N> P)
     constexpr int ND = S::ND;
     constexpr int CPB = S::CPB;
     constexpr bool JAC = MODE == EL_JACOBIAN;
+    constexpr bool STK = MODE == EL_STOKES;
+    constexpr int NP = N - 1;                              // pressure dofs per axis (EL_STOKES)
     extern __shared__ __align__(16) unsigned char smem_raw[];
     const int slot = threadIdx.x / ND;
     const int l = threadIdx.x - slot * ND;                 // this thread's dof / point in the cell
@@ -121,8 +138,13 @@ elasticity_kernel(const __grid_constant__ ElasParams<N> P)
     double *s_t = s_u + 3 * ND;                            // [3][ND]
     double *s_f = s_t + 3 * ND;                            // [3 d][3 m][ND]
     double *s_v = s_f + 9 * ND;                            // [3][ND], EL_JACOBIAN only
+    double *s_p = s_f + 9 * ND;                            // [ND], EL_STOKES only: pressure
+    double *s_q = s_p + ND;                                // [ND], EL_STOKES only: its work buffer
     int *s_idx = reinterpret_cast<int *>(reinterpret_cast<double *>(smem_raw) + (size_t)CPB * S::SLOT) + sl * ND;
     const int qi = l / (N * N), qj = (l / N) % N, qk = l % N;
+    // EL_STOKES: this thread's pressure dof, if its (i, j, k) is one
+    const bool pdof = STK && qi < NP && qj < NP && qk < NP;
+    const int lp = (qi * NP + qj) * NP + qk;
 
     const long long ncells = (long long)P.ncols * P.nlay_items;
     const long long nunits = MATRIX ? ncells * 3 * ND : ncells;
@@ -138,7 +160,7 @@ elasticity_kernel(const __grid_constant__ ElasParams<N> P)
             col = P.collist ? __ldg(P.collist + ci) : P.col0 + ci;
         }
         // ---- gather: node index, values (or the unit vector), vertices
-        int g = 0;
+        int g = 0, gp = 0;
         if (valid) {
             g = __ldg(P.map0 + (long long)col * ND + l) + __ldg(P.off0 + l) * layer;
             s_idx[l] = g;
@@ -148,6 +170,10 @@ elasticity_kernel(const __grid_constant__ ElasParams<N> P)
             if (JAC) {
 #pragma unroll
                 for (int d = 0; d < 3; d++) s_v[d * ND + l] = __ldg(P.u + (long long)g * 3 + d);
+            }
+            if (STK) {
+                if (pdof) gp = __ldg(P.map2 + (long long)col * (NP * NP * NP) + lp) + __ldg(P.off2 + lp) * layer;
+                s_p[l] = pdof ? __ldg(P.xp + gp) : 0.0;
             }
             for (int i = l; i < 24; i += ND) {
                 const int v = i / 3, a = i - 3 * v;
@@ -162,6 +188,7 @@ elasticity_kernel(const __grid_constant__ ElasParams<N> P)
 #pragma unroll
                 for (int d = 0; d < 3; d++) s_v[d * ND + l] = 0.0;
             }
+            if (STK) s_p[l] = 0.0;
             for (int i = l; i < 24; i += ND) s_x[i] = (double)(((i / 3) >> (2 - i % 3)) & 1);
         }
         __syncthreads();
@@ -175,6 +202,7 @@ elasticity_kernel(const __grid_constant__ ElasParams<N> P)
                 for (int d = 0; d < 3; d++)
                     s_f[(3 + d) * ND + l] = pass1<N, 0, false>(P.B, s_v + d * ND, qi, qj, qk);
             }
+            if (STK) s_q[l] = pass1<N, 0, false>(P.Bq, s_p, qi, qj, qk);
         }
         __syncthreads();
         if (in_cta) {
@@ -185,6 +213,7 @@ elasticity_kernel(const __grid_constant__ ElasParams<N> P)
                 for (int d = 0; d < 3; d++)
                     s_f[(6 + d) * ND + l] = pass1<N, 1, false>(P.B, s_f + (3 + d) * ND, qi, qj, qk);
             }
+            if (STK) s_p[l] = pass1<N, 1, false>(P.Bq, s_q, qi, qj, qk);
         }
         __syncthreads();
         if (in_cta) {
@@ -195,6 +224,7 @@ elasticity_kernel(const __grid_constant__ ElasParams<N> P)
                 for (int d = 0; d < 3; d++)
                     s_v[d * ND + l] = pass1<N, 2, false>(P.B, s_f + (6 + d) * ND, qi, qj, qk);
             }
+            if (STK) s_q[l] = pass1<N, 2, false>(P.Bq, s_p, qi, qj, qk);
         }
         __syncthreads();
         // ---- point stage
@@ -268,6 +298,21 @@ elasticity_kernel(const __grid_constant__ ElasParams<N> P)
                     s_f[(d * 3 + m) * ND + l] = sw * (R[m][0] * sg[0] + R[m][1] * sg[1] + R[m][2] * sg[2]);
                 mres[d] = P.beta * w * fabs(det) * s_u[d * ND + l];
             }
+            } else if (STK) {
+                // flux mu G - p I; the pressure's test value -w |det| div u replaces p in S_P
+                const double pv = s_q[l];
+                const double sw = w * fabs(det) * rdet;
+#pragma unroll
+                for (int d = 0; d < 3; d++) {
+                    double sg[3];
+#pragma unroll
+                    for (int k = 0; k < 3; k++) sg[k] = P.mu * G[d][k] - (k == d ? pv : 0.0);
+#pragma unroll
+                    for (int m = 0; m < 3; m++)
+                        s_f[(d * 3 + m) * ND + l] = sw * (R[m][0] * sg[0] + R[m][1] * sg[1] + R[m][2] * sg[2]);
+                    mres[d] = P.beta * w * fabs(det) * s_u[d * ND + l];
+                }
+                s_p[l] = -w * fabs(det) * (G[0][0] + G[1][1] + G[2][2]);
             } else {
                 // deformation gradient Fd = I + grad u: u's gradient is G (residual) or comes from S_V
                 double Fd[3][3];
@@ -343,11 +388,13 @@ elasticity_kernel(const __grid_constant__ ElasParams<N> P)
                                   pass1<N, 1, true>(P.Dt, f + ND, qi, qj, qk) +
                                   pass1<N, 2, true>(P.Dt, f + 2 * ND, qi, qj, qk);
             }
+            if (STK) s_q[l] = pass1<N, 2, true>(P.Bq, s_p, qi, qj, qk);
         }
         __syncthreads();
         if (in_cta) {
 #pragma unroll
             for (int d = 0; d < 3; d++) s_u[d * ND + l] = pass1<N, 2, true>(P.B, s_t + d * ND, qi, qj, qk);
+            if (STK) s_p[l] = pass1<N, 1, true>(P.Bq, s_q, qi, qj, qk);
         }
         __syncthreads();
         if (in_cta) {
@@ -355,10 +402,11 @@ elasticity_kernel(const __grid_constant__ ElasParams<N> P)
             for (int d = 0; d < 3; d++) s_t[d * ND + l] = pass1<N, 1, true>(P.B, s_u + d * ND, qi, qj, qk);
         }
         __syncthreads();
-        double out[3];
+        double out[3], outp = 0.0;
         if (in_cta) {
 #pragma unroll
             for (int d = 0; d < 3; d++) out[d] = pass1<N, 0, true>(P.B, s_t + d * ND, qi, qj, qk);
+            if (STK) outp = pass1<N, 0, true>(P.Bq, s_p, qi, qj, qk);
         }
         // ---- scatter (this thread's node, three components)
         if (valid) {
@@ -368,6 +416,10 @@ elasticity_kernel(const __grid_constant__ ElasParams<N> P)
                 for (int a = 0; a < 3; a++) {
                     if (ATOMIC) atomicAdd(dst + a, out[a]);
                     else dst[a] += out[a];
+                }
+                if (pdof) {
+                    if (ATOMIC) atomicAdd(P.yp + gp, outp);
+                    else P.yp[gp] += outp;
                 }
             } else {
                 const int j = jb / 3, b = jb - 3 * (jb / 3);
@@ -440,11 +492,17 @@ void fill_tables(const fdb_kernel_s *k, ElasParams<N> &P)
         P.wq[i] = k->desc.wq[i];
         P.xq[i] = k->desc.xq[i];
     }
+    if (k->desc.form == FDB_FORM_STOKES) {
+        P.off2 = k->d_off2;
+        for (int q = 0; q < N; q++)
+            for (int a = 0; a < N; a++) P.Bq[q * N + a] = a < N - 1 ? k->B2[q * (N - 1) + a] : 0.0;
+    }
 }
 
 template <int N, int MODE>
 int action_n(fdb_kernel_s *k, fdb_int start, fdb_int end, int nlay, const fdb_int *subset, double *y,
-             const double *coords, const double *x, const double *u, const fdb_int *map0, const fdb_int *map1)
+             const double *coords, const double *x, const double *u, const fdb_int *map0, const fdb_int *map1,
+             double *yp, const double *xp, const fdb_int *map2)
 {
     fdb::Context &c = fdb::ctx();
     ElasParams<N> P;
@@ -456,6 +514,9 @@ int action_n(fdb_kernel_s *k, fdb_int start, fdb_int end, int nlay, const fdb_in
     P.coords = coords;
     P.map0 = map0;
     P.map1 = map1;
+    P.yp = yp;
+    P.xp = xp;
+    P.map2 = map2;
     if (k->desc.scatter == FDB_SCATTER_ATOMIC) {
         P.collist = subset;
         P.col0 = start;
@@ -518,13 +579,18 @@ int matrix_n(fdb_kernel_s *k, fdb_int start, fdb_int end, int nlay, const fdb_in
 
 template <int MODE>
 int action_mode(fdb_kernel_s *k, fdb_int start, fdb_int end, int nlay, const fdb_int *subset, double *y,
-                const double *coords, const double *x, const double *u, const fdb_int *map0, const fdb_int *map1)
+                const double *coords, const double *x, const double *u, const fdb_int *map0, const fdb_int *map1,
+                double *yp = nullptr, const double *xp = nullptr, const fdb_int *map2 = nullptr)
 {
+    // Stokes has no degree-1 instantiation (its pressure space would be CG_0)
     switch (k->n1d) {
-    case 2: return action_n<2, MODE>(k, start, end, nlay, subset, y, coords, x, u, map0, map1);
-    case 3: return action_n<3, MODE>(k, start, end, nlay, subset, y, coords, x, u, map0, map1);
-    case 4: return action_n<4, MODE>(k, start, end, nlay, subset, y, coords, x, u, map0, map1);
-    case 5: return action_n<5, MODE>(k, start, end, nlay, subset, y, coords, x, u, map0, map1);
+    case 2:
+        if constexpr (MODE != EL_STOKES)
+            return action_n<2, MODE>(k, start, end, nlay, subset, y, coords, x, u, map0, map1, yp, xp, map2);
+        break;
+    case 3: return action_n<3, MODE>(k, start, end, nlay, subset, y, coords, x, u, map0, map1, yp, xp, map2);
+    case 4: return action_n<4, MODE>(k, start, end, nlay, subset, y, coords, x, u, map0, map1, yp, xp, map2);
+    case 5: return action_n<5, MODE>(k, start, end, nlay, subset, y, coords, x, u, map0, map1, yp, xp, map2);
     }
     fdb::set_error("elasticity action: degree %d not instantiated (1..4)", k->n1d - 1);
     return 1;
@@ -559,6 +625,13 @@ int fdb_launch_elasticity_action(fdb_kernel_s *k, fdb_int start, fdb_int end, in
     }
     fdb::set_error("elasticity action: form %d is not an elasticity form", k->desc.form);
     return 1;
+}
+
+int fdb_launch_stokes_action(fdb_kernel_s *k, fdb_int start, fdb_int end, int nlay, const fdb_int *subset,
+                             double *yu, const double *coords, const double *u, double *yp, const double *p,
+                             const fdb_int *map0, const fdb_int *map1, const fdb_int *map2)
+{
+    return action_mode<EL_STOKES>(k, start, end, nlay, subset, yu, coords, u, nullptr, map0, map1, yp, p, map2);
 }
 
 int fdb_launch_elasticity_matrix(fdb_kernel_s *k, fdb_int start, fdb_int end, int nlay, const fdb_int *subset,

@@ -240,7 +240,7 @@ static int device_pointers(const fdb_call_args *a, bool mat, void **args, const 
                            const fdb_int **subset)
 {
     for (int i = 0; i < a->nargs; i++) args[i] = a->args[i];
-    for (int i = 0; i < 2; i++) maps[i] = a->maps[i];
+    for (int i = 0; i < a->nmaps; i++) maps[i] = a->maps[i];
     *subset = a->subset;
     if (a->location != FDB_LOC_HOST) return 0;
     if (!a->arg_bytes || !a->map_bytes) {
@@ -274,7 +274,7 @@ static int device_pointers(const fdb_call_args *a, bool mat, void **args, const 
 // The forms of the hand-written hex kernels: what fdb_kernel_create accepts for each and how
 // fdb_kernel_call hands its arguments to the launchers.
 enum { MODE_ACTION, MODE_MATRIX, MODE_DIAGONAL };
-enum { LAUNCH_HELMHOLTZ, LAUNCH_HELMHOLTZ_COEF, LAUNCH_ELASTICITY };
+enum { LAUNCH_HELMHOLTZ, LAUNCH_HELMHOLTZ_COEF, LAUNCH_ELASTICITY, LAUNCH_STOKES };
 
 struct fdb_hex_form {
     int form;                 // enum fdb_form
@@ -285,23 +285,31 @@ struct fdb_hex_form {
     int coef_cdim;            // its values per node (0 without one): the argument space's, or 3 for b
     bool residual;            // a 1-form action only
     int launcher;             // fdb_launch_helmholtz_*, fdb_launch_helmholtz_coef_* (which also run the
-                              // nonlinear diffusion and advection-diffusion forms) or fdb_launch_elasticity_*
+                              // nonlinear diffusion and advection-diffusion forms), fdb_launch_elasticity_*
+                              // or fdb_launch_stokes_action
     int max_degree[3];        // per mode: action, matrix, diagonal
+    int min_degree;
+    const char *space2;       // the arguments on a second space (output and input, through a third map), or
+                              // NULL: such a form is an action only, in device mode
 };
 
 static const fdb_hex_form hex_forms[] = {
-    {FDB_FORM_HELMHOLTZ, "helmholtz", 0, true, nullptr, 0, false, LAUNCH_HELMHOLTZ, {5, 4, 3}},
-    {FDB_FORM_HELMHOLTZ_COEF, "helmholtz_coef", 1, false, "kappa", 1, false, LAUNCH_HELMHOLTZ_COEF, {5, 4, 3}},
+    {FDB_FORM_HELMHOLTZ, "helmholtz", 0, true, nullptr, 0, false, LAUNCH_HELMHOLTZ, {5, 4, 3}, 1, nullptr},
+    {FDB_FORM_HELMHOLTZ_COEF, "helmholtz_coef", 1, false, "kappa", 1, false, LAUNCH_HELMHOLTZ_COEF, {5, 4, 3}, 1,
+     nullptr},
     {FDB_FORM_NONLINEAR_DIFFUSION, "nonlinear_diffusion", 1, false, nullptr, 0, true, LAUNCH_HELMHOLTZ_COEF,
-     {5, 0, 0}},
+     {5, 0, 0}, 1, nullptr},
     {FDB_FORM_NONLINEAR_DIFFUSION_JACOBIAN, "nonlinear_diffusion_jacobian", 1, false, "u", 1, false,
-     LAUNCH_HELMHOLTZ_COEF, {5, 4, 3}},
-    {FDB_FORM_ELASTICITY, "elasticity", 3, false, nullptr, 0, false, LAUNCH_ELASTICITY, {4, 3, 3}},
-    {FDB_FORM_HYPERELASTICITY, "hyperelasticity", 3, false, nullptr, 0, true, LAUNCH_ELASTICITY, {4, 0, 0}},
+     LAUNCH_HELMHOLTZ_COEF, {5, 4, 3}, 1, nullptr},
+    {FDB_FORM_ELASTICITY, "elasticity", 3, false, nullptr, 0, false, LAUNCH_ELASTICITY, {4, 3, 3}, 1, nullptr},
+    {FDB_FORM_HYPERELASTICITY, "hyperelasticity", 3, false, nullptr, 0, true, LAUNCH_ELASTICITY, {4, 0, 0}, 1,
+     nullptr},
     {FDB_FORM_HYPERELASTICITY_JACOBIAN, "hyperelasticity_jacobian", 3, false, "u", 3, false, LAUNCH_ELASTICITY,
-     {4, 3, 3}},
+     {4, 3, 3}, 1, nullptr},
     {FDB_FORM_ADVECTION_DIFFUSION, "advection_diffusion", 1, false, "b", 3, false, LAUNCH_HELMHOLTZ_COEF,
-     {4, 3, 3}},
+     {4, 3, 3}, 1, nullptr},
+    // velocity CG_p with pressure CG_{p-1}: p >= 2
+    {FDB_FORM_STOKES, "stokes", 3, false, nullptr, 0, false, LAUNCH_STOKES, {4, 0, 0}, 2, "y_p, p"},
 };
 
 static const char *const mode_name[] = {"action", "matrix", "diagonal"};
@@ -312,9 +320,8 @@ static int hex_mode(const fdb_kernel_desc *d)
     return d->rank == 2 ? MODE_MATRIX : (d->diagonal ? MODE_DIAGONAL : MODE_ACTION);
 }
 
-extern "C" {
-
-int fdb_kernel_create(const fdb_kernel_desc *d, fdb_kernel_t *out)
+// fdb_kernel_create (s2 == NULL) and fdb_kernel_create_mixed (s2: the second space of a form on two spaces)
+static int kernel_create(const fdb_kernel_desc *d, const fdb_space2_desc *s2, fdb_kernel_t *out)
 {
     if (require_init()) return 1;
     if (!d || !out) {
@@ -357,6 +364,11 @@ int fdb_kernel_create(const fdb_kernel_desc *d, fdb_kernel_t *out)
         set_error("fdb_kernel_create: form %d is not in the supported set", d->form);
         return 1;
     }
+    if (f->space2 && !s2) {
+        set_error("fdb_kernel_create: %s is a form on two spaces: create it with fdb_kernel_create_mixed and the "
+                  "second space's fdb_space2_desc", f->name);
+        return 1;
+    }
     const int mode = hex_mode(d);
     if (d->cell != FDB_CELL_HEX_EXTRUDED && d->cell != FDB_CELL_HEX) {
         set_error("fdb_kernel_create: %s needs hex cells (extruded or native), got cell %d", f->name, d->cell);
@@ -384,9 +396,14 @@ int fdb_kernel_create(const fdb_kernel_desc *d, fdb_kernel_t *out)
                   "of %s_jacobian", f->name, f->name);
         return 1;
     }
-    if (d->degree < 1 || d->degree > f->max_degree[mode]) {
-        set_error("fdb_kernel_create: %s %s: degree %d outside 1..%d", f->name, mode_name[mode], d->degree,
-                  f->max_degree[mode]);
+    if (f->space2 && mode != MODE_ACTION) {
+        set_error("fdb_kernel_create: %s is a mixed form, a rank-1 action only: it has no assembled matrix or "
+                  "diagonal", f->name);
+        return 1;
+    }
+    if (d->degree < f->min_degree || d->degree > f->max_degree[mode]) {
+        set_error("fdb_kernel_create: %s %s: degree %d outside %d..%d", f->name, mode_name[mode], d->degree,
+                  f->min_degree, f->max_degree[mode]);
         return 1;
     }
     if (d->integral != FDB_INTEGRAL_CELL) {
@@ -401,6 +418,17 @@ int fdb_kernel_create(const fdb_kernel_desc *d, fdb_kernel_t *out)
         set_error("fdb_kernel_create: extruded cells need offset0/offset1");
         return 1;
     }
+    // the second space: CG_{p-1} with p^3 dofs per cell (Stokes' pressure)
+    if (f->space2 && s2->degree != d->degree - 1) {
+        set_error("fdb_kernel_create_mixed: %s of degree %d needs a second space of degree %d, got %d", f->name,
+                  d->degree, d->degree - 1, s2->degree);
+        return 1;
+    }
+    if (f->space2 && d->cell == FDB_CELL_HEX_EXTRUDED && !s2->offset) {
+        set_error("fdb_kernel_create_mixed: %s on extruded cells needs the layer offsets of the second map "
+                  "(fdb_space2_desc.offset)", f->name);
+        return 1;
+    }
     fdb_kernel_s *k = new fdb_kernel_s;
     k->desc = *d;
     k->hex = f;
@@ -412,6 +440,14 @@ int fdb_kernel_create(const fdb_kernel_desc *d, fdb_kernel_t *out)
     if (d->offset1) memcpy(k->h_off1, d->offset1, sizeof(fdb_int) * 8);
     k->desc.offset0 = k->h_off0;
     k->desc.offset1 = k->h_off1;
+    // the second space's map: CG_{p-1}, p^3 dofs per cell
+    const int arity2 = d->degree * d->degree * d->degree;
+    memset(k->h_off2, 0, sizeof(k->h_off2));
+    memset(k->B2, 0, sizeof(k->B2));
+    if (f->space2) {
+        if (s2->offset) memcpy(k->h_off2, s2->offset, sizeof(fdb_int) * arity2);
+        memcpy(k->B2, s2->B, sizeof(k->B2));
+    }
     if (collocated_derivative(k->n1d, d->B, d->D, k->Dt)) {
         set_error("fdb_kernel_create: basis table B is singular");
         delete k;
@@ -423,9 +459,35 @@ int fdb_kernel_create(const fdb_kernel_desc *d, fdb_kernel_t *out)
                              cudaMemcpyHostToDevice, ctx().stream));
     FDB_CUDA(cudaMemcpyAsync(k->d_off1, k->h_off1, sizeof(fdb_int) * 8, cudaMemcpyHostToDevice,
                              ctx().stream));
+    if (f->space2) {
+        FDB_CUDA(cudaMalloc(&k->d_off2, sizeof(fdb_int) * arity2));
+        FDB_CUDA(cudaMemcpyAsync(k->d_off2, k->h_off2, sizeof(fdb_int) * arity2, cudaMemcpyHostToDevice,
+                                 ctx().stream));
+    }
     FDB_CUDA(cudaStreamSynchronize(ctx().stream));
     *out = k;
     return 0;
+}
+
+extern "C" {
+
+int fdb_kernel_create(const fdb_kernel_desc *d, fdb_kernel_t *out)
+{
+    return kernel_create(d, nullptr, out);
+}
+
+int fdb_kernel_create_mixed(const fdb_kernel_desc *d, const fdb_space2_desc *s2, fdb_kernel_t *out)
+{
+    if (require_init()) return 1;
+    if (!d || !s2 || !out) {
+        set_error("fdb_kernel_create_mixed: NULL argument");
+        return 1;
+    }
+    for (const fdb_hex_form &row : hex_forms)
+        if (row.form == d->form && row.space2) return kernel_create(d, s2, out);
+    set_error("fdb_kernel_create_mixed: form %d is not a form on two spaces: create it with fdb_kernel_create",
+              d->form);
+    return 1;
 }
 
 int fdb_kernel_destroy(fdb_kernel_t k)
@@ -436,6 +498,7 @@ int fdb_kernel_destroy(fdb_kernel_t k)
     if (ctx().ready) {
         if (k->d_off0) cudaFree(k->d_off0);
         if (k->d_off1) cudaFree(k->d_off1);
+        if (k->d_off2) cudaFree(k->d_off2);
         if (k->d_colour_cols) cudaFree(k->d_colour_cols);
         if (k->d_bdb_table) cudaFree(k->d_bdb_table);
     }
@@ -507,15 +570,20 @@ int fdb_kernel_call(fdb_kernel_t k, const fdb_call_args *a)
     }
     // args = [y (INC), coords, x] (action), [Mat handle (INC), coords] (matrix: the reference passes the
     // PETSc Mat handle in the same slot, pyop2/types/mat.py:621-623) or [d (INC), coords] (diagonal), then
-    // the form's trailing coefficient; maps = [V map, coord map]
+    // the form's trailing coefficient; maps = [V map, coord map].  A form on two spaces (Stokes) has the
+    // output and input of the second space after x and a third map: [y, coords, x, y2, x2], [V map, coord
+    // map, second map]
     const fdb_hex_form *f = k->hex;
     const int mode = hex_mode(&k->desc);
-    const int want = (mode == MODE_ACTION ? 3 : 2) + (f->coef ? 1 : 0);
-    if (a->nargs != want || a->nmaps != 2 || (mode == MODE_DIAGONAL && a->location != FDB_LOC_DEVICE)) {
+    const int want = (mode == MODE_ACTION ? 3 : 2) + (f->coef ? 1 : 0) + (f->space2 ? 2 : 0);
+    const int want_maps = f->space2 ? 3 : 2;
+    const bool device_only = mode == MODE_DIAGONAL || f->space2;
+    if (a->nargs != want || a->nmaps != want_maps || (device_only && a->location != FDB_LOC_DEVICE)) {
         static const char *const args[] = {"y, coords, x", "mat, coords", "d, coords"};
-        set_error("fdb_kernel_call: %s %s expects %d %sargs (%s%s%s) and 2 maps, got %d/%d", f->name,
-                  mode_name[mode], want, mode == MODE_DIAGONAL ? "device " : "", args[mode], f->coef ? ", " : "",
-                  f->coef ? f->coef : "", a->nargs, a->nmaps);
+        set_error("fdb_kernel_call: %s %s expects %d %sargs (%s%s%s%s%s) and %d maps, got %d/%d", f->name,
+                  mode_name[mode], want, device_only ? "device " : "", args[mode], f->coef ? ", " : "",
+                  f->coef ? f->coef : "", f->space2 ? ", " : "", f->space2 ? f->space2 : "", want_maps, a->nargs,
+                  a->nmaps);
         return 1;
     }
     const fdb_mat_t mat = mode == MODE_MATRIX ? (fdb_mat_t)a->args[0] : nullptr;
@@ -558,8 +626,8 @@ int fdb_kernel_call(fdb_kernel_t k, const fdb_call_args *a)
         int rc = pipelined_host_action(k, a, nlay);
         if (rc >= 0) return rc;      // -1: not applicable, fall through to the monolithic path
     }
-    void *dargs[4];
-    const fdb_int *dmaps[2];
+    void *dargs[5];
+    const fdb_int *dmaps[3];
     const fdb_int *dsubset;
     if (device_pointers(a, mat != nullptr, dargs, dmaps, &dsubset)) return 1;
     const double *coords = (const double *)dargs[1];
@@ -621,9 +689,13 @@ int fdb_kernel_call(fdb_kernel_t k, const fdb_call_args *a)
         rc = fdb_launch_helmholtz_coef_action(k, a->start, a->end, nlay, dsubset, out, coords, x, coef, dmaps[0],
                                               dmaps[1]);
         break;
-    default:
+    case LAUNCH_ELASTICITY:
         rc = fdb_launch_elasticity_action(k, a->start, a->end, nlay, dsubset, out, coords, x, coef, dmaps[0],
                                           dmaps[1]);
+        break;
+    default:
+        rc = fdb_launch_stokes_action(k, a->start, a->end, nlay, dsubset, out, coords, x, (double *)dargs[3],
+                                      (const double *)dargs[4], dmaps[0], dmaps[1], dmaps[2]);
     }
     if (rc) return rc;
     if (a->location == FDB_LOC_HOST && a->writeback) {

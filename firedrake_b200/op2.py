@@ -1386,6 +1386,11 @@ class Kernel:
     beta*inner(u, v)*dx`` on a scalar space, with the velocity b a Dat of 3 values per node of the argument
     space (``op2.DataSet(V.node_set, 3)``), passed as the LAST argument like kappa: action (output,
     coordinates, u, b), diagonal and rank 2 (output, coordinates, b).  Its matrix is not symmetric.
+
+    "stokes" is the Taylor-Hood saddle-point action ``mu*inner(grad u, grad v)*dx + beta*inner(u, v)*dx -
+    p*div(v)*dx - q*div(u)*dx`` with the velocity in vector CG_p (``degree`` = p, 2..4; ``cdim`` 3) and the
+    pressure in scalar CG_{p-1}, read and written through a second map: a rank-1 action only, (INC, READ,
+    READ, INC, READ) = (velocity output, coordinates, u, pressure output, p).
     """
     form: str = "helmholtz"
     degree: int = 1
@@ -1421,6 +1426,13 @@ class Kernel:
             if len(self.d) != 3:
                 raise ValueError("d holds the three coefficients of D(s) = d0 + d1 s + d2 s^2")
         spec = _FORMS.get(self.form)
+        if spec and spec.pressure:
+            # the velocity space is always a vector space: cdim is 3 unless given otherwise (which the engine
+            # refuses)
+            if self.cdim == 1:
+                object.__setattr__(self, "cdim", 3)
+            object.__setattr__(self, "accesses", (INC, READ, READ, INC, READ))
+            return
         if spec and spec.residual:
             return          # (INC, READ, READ) whatever rank and diagonal say: the engine refuses them
         if spec and spec.coefficient:
@@ -1454,6 +1466,7 @@ class _Form(NamedTuple):
     residual: bool = False      # a rank-1 action only
     lame: bool = False          # takes mu and lmbda
     coef_cdim: int = 0          # values per node of the trailing coefficient when they differ from the space's
+    pressure: bool = False      # also reads and writes a scalar pressure space through a third map (Stokes)
 
 
 _FORMS = {"helmholtz": _Form(_lib.FORM_HELMHOLTZ),
@@ -1464,7 +1477,8 @@ _FORMS = {"helmholtz": _Form(_lib.FORM_HELMHOLTZ),
           "elasticity": _Form(_lib.FORM_ELASTICITY, lame=True),
           "hyperelasticity": _Form(_lib.FORM_HYPERELASTICITY, residual=True, lame=True),
           "hyperelasticity_jacobian": _Form(_lib.FORM_HYPERELASTICITY_JACOBIAN, coefficient=True, lame=True),
-          "advection_diffusion": _Form(_lib.FORM_ADVECTION_DIFFUSION, coefficient=True, coef_cdim=3)}
+          "advection_diffusion": _Form(_lib.FORM_ADVECTION_DIFFUSION, coefficient=True, coef_cdim=3),
+          "stokes": _Form(_lib.FORM_STOKES, pressure=True)}
 _INTEGRALS = {"cell": _lib.INTEGRAL_CELL, "exterior_facet": _lib.INTEGRAL_EXTERIOR_FACET,
               "interior_facet": _lib.INTEGRAL_INTERIOR_FACET, "fused": _lib.INTEGRAL_FUSED}
 
@@ -1553,13 +1567,24 @@ class GlobalKernel:
             d.dcoef[i] = lk.d[i]
         if spec.lame:
             d.alpha, d.lmbda = lk.mu, lk.lmbda
+        s2 = None
+        if spec.pressure:
+            d.alpha = lk.mu
+            # the pressure space CG_{p-1} (fdb_space2_desc): its basis at the velocity's Gauss points, (nq, p)
+            s2 = _lib.Space2Desc()
+            s2.degree = lk.degree - 1
+            if lk.degree >= 2:
+                elq = interval_element(lk.degree - 1, el.nq)
+                for q in range(el.nq):
+                    for a in range(lk.degree):
+                        s2.B[q * lk.degree + a] = elq.B[q, a]
         for q in range(el.nq):
             d.wq[q] = el.wq[q]
             d.xq[q] = el.xq[q]
             for a in range(n):
                 d.B[q * n + a] = el.B[q, a]
                 d.D[q * n + a] = el.D[q, a]
-        m0, m1 = self.arguments
+        m0, m1 = self.arguments[:2]
         keep = []
         if self.extruded:
             if m0.offset is None or m1.offset is None:
@@ -1569,8 +1594,16 @@ class GlobalKernel:
             keep = [o0, o1]
             d.offset0 = o0.ctypes.data_as(C.POINTER(C.c_int32))
             d.offset1 = o1.ctypes.data_as(C.POINTER(C.c_int32))
+            if spec.pressure and len(self.arguments) > 2 and self.arguments[2].offset is not None:
+                o2 = np.ascontiguousarray(self.arguments[2].offset, dtype=IntType)
+                keep.append(o2)
+                s2.offset = o2.ctypes.data_as(C.POINTER(C.c_int32))
         h = C.c_void_p()
-        _lib.check(_lib.lib().fdb_kernel_create(C.byref(d), C.byref(h)), "fdb_kernel_create")
+        if s2 is not None:
+            _lib.check(_lib.lib().fdb_kernel_create_mixed(C.byref(d), C.byref(s2), C.byref(h)),
+                       "fdb_kernel_create_mixed")
+        else:
+            _lib.check(_lib.lib().fdb_kernel_create(C.byref(d), C.byref(h)), "fdb_kernel_create")
         del keep
         self._handle = h
         return h
@@ -1678,6 +1711,13 @@ class Parloop:
             # fewer would be read past its end
             raise ValueError(f"{lk.form}: the trailing coefficient has {spec.coef_cdim} values per node, "
                              f"{self.args[-1].data.name} has {self.args[-1].data.cdim}")
+        if spec and spec.pressure:
+            # the kernel reads and writes one pressure value per node of the third map: a Dat with more
+            # values per node would be misread, one with fewer nodes read past its end
+            for a in self.args[3:5]:
+                if a.data.cdim != 1:
+                    raise ValueError(f"{lk.form}: the pressure Dats have 1 value per node, {a.data.name} has "
+                                     f"{a.data.cdim}")
         for a, acc in zip(self.args, lk.accesses):
             if a.access != acc:
                 raise ValueError(f"argument {a.data.name}: access {a.access.name} != kernel's {acc.name}")
@@ -1737,6 +1777,9 @@ class Parloop:
             gk(start, end, layers, subset, ptrs, None, None, [m.device_ptr for m in maps], None,
                _lib.LOC_DEVICE, False, False)
             out._device_written()
+            for a in self.args[1:]:
+                if a.access == INC:          # a second output (Stokes' pressure)
+                    a.data._device_written()
         else:
             subset = it.indices.ctypes.data if isinstance(it, Subset) else None
             lazy_zero = out._is_zero and not out._host_valid

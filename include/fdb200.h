@@ -175,7 +175,7 @@ enum fdb_form {
                                      action    [y INC, coords, w, u]  (device or host mode)
                                      diagonal  [d INC, coords, u]     (device mode)
                                      rank 2    [Mat (block size 3), coords, u]                      */
-    FDB_FORM_ADVECTION_DIFFUSION = 9
+    FDB_FORM_ADVECTION_DIFFUSION = 9,
                                 /* advection-diffusion of a scalar (NOT symmetric):
                                      a(u, v) = alpha*inner(grad u, grad v)*dx
                                                + inner(dot(b, grad u), v)*dx + beta*inner(u, v)*dx
@@ -189,6 +189,25 @@ enum fdb_form {
                                      diagonal  [d INC, coords, b]     (device mode)
                                      rank 2    [Mat, coords, b]  (row = test dof, column = trial dof)
                                    Never the DMMA element-matrix kernels (they assume symmetry).  */
+    FDB_FORM_STOKES = 10
+                                /* Stokes flow on Taylor-Hood hexahedra: velocity u in vector CG_p
+                                   (value size 3, AoS, maps[0]) and pressure p in scalar CG_{p-1}
+                                   (one value per node, maps[2]) on the same cells,
+                                     a((u, p), (v, q)) = mu*inner(grad u, grad v)*dx
+                                                         + beta*inner(u, v)*dx
+                                                         - p*div(v)*dx - q*div(u)*dx
+                                   mu = alpha, beta = beta (beta = 1/dt: an implicit Euler step of
+                                   unsteady Stokes).  Symmetric and indefinite; the pressure rows carry
+                                   -q div u (Firedrake's Stokes demo writes +q div u: the same system
+                                   with the pressure rows negated).  degree = p (2..4), cdim == 3,
+                                   nq == p+1, affine_cells == 0, B/D the velocity tables.  A form on
+                                   two spaces: created by fdb_kernel_create_mixed, whose
+                                   fdb_space2_desc gives the pressure space (degree p-1, its basis at
+                                   the nq Gauss points and, on extruded cells, the pressure map's
+                                   layer offsets).  Rank 1 action only (not rank 2, not diagonal),
+                                   device mode only, atomic or coloured scatter:
+                                     action  [y_u INC, coords, u, y_p INC, p]
+                                             maps [V map, coord map, Q map]                       */
 };
 
 enum fdb_cell {
@@ -256,12 +275,27 @@ typedef struct fdb_kernel_desc {
     double lmbda;
 } fdb_kernel_desc;
 
+/* The second space of a form on two spaces (FDB_FORM_STOKES: the pressure space), passed to
+ * fdb_kernel_create_mixed next to the descriptor of the first (argument) space, which keeps its
+ * layout.  degree: the second space's polynomial degree (Stokes: the velocity degree minus 1);
+ * B: its basis at the descriptor's nq Gauss points, row-major (nq, degree+1), 1-D dof numbering;
+ * offset: the extruded layer offsets of the second space's map, (degree+1)^3 entries, NULL for
+ * native hexes, copied at creation. */
+typedef struct fdb_space2_desc {
+    int32_t degree;
+    double B[FDB_MAX_1D * FDB_MAX_1D];
+    const fdb_int *offset;
+} fdb_space2_desc;
+
 typedef struct fdb_kernel_s *fdb_kernel_t;
 
 /* Replaces pyop2.global_kernel.compile_global_kernel (global_kernel.py:426-456):
  * "compile" = validate the descriptor, precompute tables, pick the sm_90a
  * kernel instantiation.  Fails (nonzero) for forms outside the supported set. */
 int fdb_kernel_create(const fdb_kernel_desc *desc, fdb_kernel_t *out);
+/* The same for a form on two spaces (FDB_FORM_STOKES), which fdb_kernel_create refuses; a form on one
+ * space is refused here. */
+int fdb_kernel_create_mixed(const fdb_kernel_desc *desc, const fdb_space2_desc *space2, fdb_kernel_t *out);
 int fdb_kernel_destroy(fdb_kernel_t k);
 
 /* 1 in *result iff every hex cell of columns [start, end) x nlay layers is a parallelepiped,
