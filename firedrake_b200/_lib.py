@@ -24,6 +24,8 @@ FORM_HYPERELASTICITY = 7
 FORM_HYPERELASTICITY_JACOBIAN = 8
 FORM_ADVECTION_DIFFUSION = 9
 FORM_STOKES = 10
+FORM_NAVIER_STOKES = 11
+FORM_NAVIER_STOKES_JACOBIAN = 12
 CELL_HEX_EXTRUDED = 1
 CELL_HEX = 2
 CELL_TRIANGLE = 3

@@ -609,6 +609,136 @@ def assemble_stokes_generic(F: "Stokes", up: op2.MixedDat, tensor=None):
     return tensor
 
 
+def navier_stokes_kernel(degree, nu=1.0, beta=0.0, jacobian=False, name=None):
+    """C source of the steady Navier-Stokes residual ``nu*inner(grad u, grad v)*dx + beta*inner(u, v)*dx +
+    inner(dot(grad u, u), v)*dx - p*div(v)*dx - q*div(u)*dx`` on Taylor-Hood Q_p-Q_(p-1) hexahedra (arguments: y
+    (INC) and up as in :func:`stokes_kernel`, and the coordinates), or with ``jacobian`` of its Gateaux
+    derivative's action at u on (w, r), the Stokes action on (w, r) plus ``inner(dot(grad w, u), v)*dx +
+    inner(dot(grad u, w), v)*dx`` (arguments: y (INC), coords, wr, u with u the velocity's 3 END values).  The
+    independent statement of the hand-written FDB_FORM_NAVIER_STOKES[_JACOBIAN] kernels, run through the
+    generic wrapper builder."""
+    from .codegen import CStringKernel
+    from .fiat_lite import interval_element
+    if not 2 <= degree <= 4:
+        raise NotImplementedError(f"the generic-path Navier-Stokes statement covers degrees 2..4, got degree {degree}")
+    if name is None:
+        name = "navier_stokes_jacobian_action" if jacobian else "navier_stokes_residual"
+    elq = interval_element(degree - 1, degree + 1)
+    n = degree + 1
+    bq = [[float(elq.B[q, a]) if a < n - 1 else 0.0 for a in range(n)] for q in range(n)]
+    tab = "{" + ", ".join("{" + ", ".join(repr(v) for v in r) + "}" for r in bq) + "}"
+    args = "double *y, const double *X, const double *up, const double *u" if jacobian else \
+        "double *y, const double *X, const double *up"
+    # the linearisation velocity's values UL and physical gradient GL at the point: u itself for the residual
+    lin = """
+        double GL[3][3];
+        for (int d = 0; d < 3; ++d)
+            for (int k = 0; k < 3; ++k)
+                GL[d][k] = GU[d][0][q] * Jinv[0][k] + GU[d][1][q] * Jinv[1][k] + GU[d][2][q] * Jinv[2][k];
+        for (int d = 0; d < 3; ++d)
+            cv[d] = Gp[d][0] * UL[0][q] + Gp[d][1] * UL[1][q] + Gp[d][2] * UL[2][q]
+                  + GL[d][0] * U[0][q] + GL[d][1] * U[1][q] + GL[d][2] * U[2][q];""" if jacobian else """
+        for (int d = 0; d < 3; ++d) cv[d] = Gp[d][0] * U[0][q] + Gp[d][1] * U[1][q] + Gp[d][2] * U[2][q];"""
+    gather_u = """
+        for (int i = 0; i < END; ++i) c[i] = u[i * 3 + d];
+        el_tensor(EB, EB, EB, 0, c, UL[d]);
+        el_tensor(ED, EB, EB, 0, c, GU[d][0]);
+        el_tensor(EB, ED, EB, 0, c, GU[d][1]);
+        el_tensor(EB, EB, ED, 0, c, GU[d][2]);""" if jacobian else ""
+    decl_u = "double UL[3][END], GU[3][3][END];" if jacobian else ""
+    code = _vector_hex_tables(degree) + f"""#define ENP (EN - 1)
+static const double EQ[EN][EN] = {tab};      /* EQ[q][a]: pressure basis, zero last column */
+static void {name}({args})
+{{
+    double U[3][END], G[3][3][END], c[END], t[END], P[END], T[END];
+    {decl_u}
+    const double *pin = up + 3 * END;
+    for (int d = 0; d < 3; ++d) {{
+        for (int i = 0; i < END; ++i) c[i] = up[i * 3 + d];
+        el_tensor(EB, EB, EB, 0, c, U[d]);
+        el_tensor(ED, EB, EB, 0, c, G[d][0]);
+        el_tensor(EB, ED, EB, 0, c, G[d][1]);
+        el_tensor(EB, EB, ED, 0, c, G[d][2]);{gather_u}
+    }}
+    for (int i = 0; i < END; ++i) {{
+        const int a = i / (EN * EN), b = (i / EN) % EN, e = i % EN;
+        c[i] = (a < ENP && b < ENP && e < ENP) ? pin[(a * ENP + b) * ENP + e] : 0.0;
+    }}
+    el_tensor(EQ, EQ, EQ, 0, c, P);
+    for (int qx = 0; qx < EN; ++qx) for (int qy = 0; qy < EN; ++qy) for (int qz = 0; qz < EN; ++qz) {{
+        const int q = (qx * EN + qy) * EN + qz;
+        const double xi[3] = {{EX[qx], EX[qy], EX[qz]}};
+        double J[3][3] = {{{{0}}}};
+        for (int v = 0; v < 8; ++v) {{
+            const int b[3] = {{(v >> 2) & 1, (v >> 1) & 1, v & 1}};
+            for (int r = 0; r < 3; ++r) {{
+                double g = b[r] ? 1.0 : -1.0;
+                for (int e = 0; e < 3; ++e) if (e != r) g *= b[e] ? xi[e] : 1.0 - xi[e];
+                for (int k = 0; k < 3; ++k) J[k][r] += X[v * 3 + k] * g;
+            }}
+        }}
+        const double det = J[0][0] * (J[1][1] * J[2][2] - J[1][2] * J[2][1])
+                         - J[0][1] * (J[1][0] * J[2][2] - J[1][2] * J[2][0])
+                         + J[0][2] * (J[1][0] * J[2][1] - J[1][1] * J[2][0]);
+        double Jinv[3][3];
+        Jinv[0][0] = (J[1][1] * J[2][2] - J[1][2] * J[2][1]) / det;
+        Jinv[0][1] = (J[0][2] * J[2][1] - J[0][1] * J[2][2]) / det;
+        Jinv[0][2] = (J[0][1] * J[1][2] - J[0][2] * J[1][1]) / det;
+        Jinv[1][0] = (J[1][2] * J[2][0] - J[1][0] * J[2][2]) / det;
+        Jinv[1][1] = (J[0][0] * J[2][2] - J[0][2] * J[2][0]) / det;
+        Jinv[1][2] = (J[0][2] * J[1][0] - J[0][0] * J[1][2]) / det;
+        Jinv[2][0] = (J[1][0] * J[2][1] - J[1][1] * J[2][0]) / det;
+        Jinv[2][1] = (J[0][1] * J[2][0] - J[0][0] * J[2][1]) / det;
+        Jinv[2][2] = (J[0][0] * J[1][1] - J[0][1] * J[1][0]) / det;
+        const double wd = EW[qx] * EW[qy] * EW[qz] * fabs(det);
+        double Gp[3][3], S[3][3], cv[3];
+        for (int d = 0; d < 3; ++d)
+            for (int k = 0; k < 3; ++k)
+                Gp[d][k] = G[d][0][q] * Jinv[0][k] + G[d][1][q] * Jinv[1][k] + G[d][2][q] * Jinv[2][k];{lin}
+        for (int d = 0; d < 3; ++d)
+            for (int k = 0; k < 3; ++k)
+                S[d][k] = {float(nu)!r} * Gp[d][k] - (d == k ? P[q] : 0.0);
+        for (int d = 0; d < 3; ++d)
+            for (int m = 0; m < 3; ++m)
+                G[d][m][q] = wd * (Jinv[m][0] * S[d][0] + Jinv[m][1] * S[d][1] + Jinv[m][2] * S[d][2]);
+        for (int d = 0; d < 3; ++d) U[d][q] = wd * ({float(beta)!r} * U[d][q] + cv[d]);
+        T[q] = -wd * (Gp[0][0] + Gp[1][1] + Gp[2][2]);
+    }}
+    for (int d = 0; d < 3; ++d) {{
+        el_tensor(EB, EB, EB, 1, U[d], c);
+        el_tensor(ED, EB, EB, 1, G[d][0], t);  for (int i = 0; i < END; ++i) c[i] += t[i];
+        el_tensor(EB, ED, EB, 1, G[d][1], t);  for (int i = 0; i < END; ++i) c[i] += t[i];
+        el_tensor(EB, EB, ED, 1, G[d][2], t);  for (int i = 0; i < END; ++i) c[i] += t[i];
+        for (int i = 0; i < END; ++i) y[i * 3 + d] += c[i];
+    }}
+    el_tensor(EQ, EQ, EQ, 1, T, c);
+    for (int a = 0; a < ENP; ++a) for (int b = 0; b < ENP; ++b) for (int e = 0; e < ENP; ++e)
+        y[3 * END + (a * ENP + b) * ENP + e] += c[(a * EN + b) * EN + e];
+}}
+#undef ENP
+#undef END
+#undef EN
+"""
+    return CStringKernel(code, name)
+
+
+def assemble_navier_stokes_generic(F: "NavierStokes", up: op2.MixedDat, w: op2.MixedDat = None, tensor=None):
+    """The residual R(up) of :class:`NavierStokes` (``w`` None) or the Jacobian action J(up[0]) w through the
+    generic wrapper path (:func:`navier_stokes_kernel`): the cross-check and the baseline of the hand-written
+    kernels."""
+    V = F.V
+    if tensor is None:
+        tensor = F.dat()
+    tensor.zero()
+    for d in tensor:
+        d.device_ptr
+    mm = op2.MixedMap([V.cell_node_map, F.pressure_map])
+    k = navier_stokes_kernel(V.degree, F.nu, F.beta, jacobian=w is not None)
+    ins = [w(op2.READ, mm), up[0](op2.READ, V.cell_node_map)] if w is not None else [up(op2.READ, mm)]
+    op2.par_loop(k, V.cell_set, tensor(op2.INC, mm), V.coordinates(op2.READ, V.coord_map), *ins)
+    return tensor
+
+
 def advection_diffusion_kernel(degree, alpha=1.0, beta=0.0, name="advection_diffusion_action"):
     """C source of the 1-form ``action(alpha*inner(grad(u), grad(v))*dx + inner(dot(b, grad(u)), v)*dx +
     beta*inner(u, v)*dx, u)`` on the scalar Q_p (x) P_p space, with the velocity b of 3 values per node
@@ -1162,25 +1292,14 @@ class Stokes:
     symmetric = True
 
     def __post_init__(self):
-        V, Q = self.V, self.Q
-        if V.cdim != 3:
-            raise ValueError(f"the Stokes velocity space is a vector space with 3 components, got cdim {V.cdim}")
-        if Q.cdim != 1:
-            raise ValueError(f"the Stokes pressure space is scalar, got cdim {Q.cdim}")
-        if V.mesh is not Q.mesh:
-            raise ValueError("the Stokes velocity and pressure spaces must be on the same mesh")
-        if not 2 <= V.degree <= 4 or Q.degree != V.degree - 1:
-            raise ValueError(f"Taylor-Hood Q_p-Q_(p-1) with p = 2..4: got velocity degree {V.degree}, pressure "
-                             f"degree {Q.degree}")
-        if any(W.dof_dset.halo is not None or W.cell_set.owner_computes for W in (V, Q)):
-            raise NotImplementedError("Stokes on a partitioned mesh is not implemented: the velocity and pressure "
-                                      "node sets need their own halo design")
-        # the pressure map on the velocity space's cell set (the parloop iterates over one set)
-        self.pressure_map = op2.Map(V.cell_set, Q.node_set, Q.V.arity, Q.V.cell_node_map, offset=Q.V.offset)
+        self.pressure_map = _taylor_hood_pressure_map(self.V, self.Q, "Stokes")
 
     def dat(self, u=None, p=None):
         """A (velocity, pressure) vector: ``op2.MixedDat([V.dat(u), Q.dat(p)])``."""
         return op2.MixedDat([self.V.dat(u), self.Q.dat(p)])
+
+    def coefficient_args(self):
+        return []
 
     def kernel(self, rank=1, diagonal=False):
         if rank != 1 or diagonal:
@@ -1189,9 +1308,102 @@ class Stokes:
         return op2.Kernel("stokes", degree=self.V.degree, mu=self.mu, beta=self.beta)
 
 
+def _taylor_hood_pressure_map(V, Q, what):
+    """Check a Taylor-Hood pair (vector CG_p, scalar CG_{p-1}, p = 2..4, one unpartitioned mesh) and return the
+    pressure map on the velocity space's cell set (the parloop iterates over one set)."""
+    if V.cdim != 3:
+        raise ValueError(f"the {what} velocity space is a vector space with 3 components, got cdim {V.cdim}")
+    if Q.cdim != 1:
+        raise ValueError(f"the {what} pressure space is scalar, got cdim {Q.cdim}")
+    if V.mesh is not Q.mesh:
+        raise ValueError(f"the {what} velocity and pressure spaces must be on the same mesh")
+    if not 2 <= V.degree <= 4 or Q.degree != V.degree - 1:
+        raise ValueError(f"Taylor-Hood Q_p-Q_(p-1) with p = 2..4: got velocity degree {V.degree}, pressure "
+                         f"degree {Q.degree}")
+    if any(W.dof_dset.halo is not None or W.cell_set.owner_computes for W in (V, Q)):
+        raise NotImplementedError(f"{what} on a partitioned mesh is not implemented: the velocity and pressure "
+                                  f"node sets need their own halo design")
+    return op2.Map(V.cell_set, Q.node_set, Q.V.arity, Q.V.cell_node_map, offset=Q.V.offset)
+
+
+@dataclass
+class NavierStokes:
+    """The residual of steady incompressible Navier-Stokes on the Taylor-Hood spaces of :class:`Stokes`
+    (velocity ``V``, vector CG_p; pressure ``Q``, CG_{p-1}; p = 2..4), without its source term:
+
+        R((u, p); (v, q)) = nu*inner(grad(u), grad(v))*dx + beta*inner(u, v)*dx + inner(dot(grad(u), u), v)*dx
+                            - p*div(v)*dx - q*div(u)*dx
+
+    with the Stokes sign convention, so that R at u = 0 is the Stokes action and the Jacobian at u = 0 is
+    ``Stokes(V, Q, mu=nu, beta)``.  nu is the kinematic viscosity (1/Re on the unit cavity).  ``assemble(F,
+    u=up)`` is R(up), a MixedDat; ``F.jacobian(up)`` the exact Newton Jacobian; :func:`solve_nonlinear` runs
+    Newton with matrix-free GMRES and the fieldsplit preconditioner of :func:`_solve_stokes`.  The (p+1)-point
+    Gauss rule integrates the div terms exactly, the convective term not."""
+    V: FunctionSpace
+    Q: FunctionSpace
+    nu: float = 1.0
+    beta: float = 0.0
+    symmetric = False
+
+    def __post_init__(self):
+        self.pressure_map = _taylor_hood_pressure_map(self.V, self.Q, "Navier-Stokes")
+
+    def dat(self, u=None, p=None):
+        """A (velocity, pressure) vector: ``op2.MixedDat([V.dat(u), Q.dat(p)])``."""
+        return op2.MixedDat([self.V.dat(u), self.Q.dat(p)])
+
+    def coefficient_args(self):
+        return []
+
+    def kernel(self, rank=1, diagonal=False):
+        if rank != 1 or diagonal:
+            raise ValueError("the residual is a 1-form: its operator is F.jacobian(up), a matrix-free action")
+        return op2.Kernel("navier_stokes", degree=self.V.degree, mu=self.nu, beta=self.beta)
+
+    def jacobian(self, up: op2.MixedDat):
+        """The Gateaux derivative at the velocity ``up[0]``, read in place (a nonsymmetric bilinear form)."""
+        return NavierStokesJacobian(self.V, self.Q, self.nu, self.beta, up[0], self.pressure_map)
+
+
+@dataclass
+class NavierStokesJacobian:
+    """J(u0)[(w, r); (v, q)] = nu*inner(grad(w), grad(v))*dx + beta*inner(w, v)*dx + inner(dot(grad(w), u0), v)*dx
+    + inner(dot(grad(u0), w), v)*dx - r*div(v)*dx - q*div(w)*dx: a nonsymmetric bilinear form on MixedDats
+    (``assemble(J, u=wr)``, ``assemble(J, mat_type="matfree")``; no assembled matrix).  ``u0``, a Dat of the
+    velocity space, is read through the velocity map."""
+    V: FunctionSpace
+    Q: FunctionSpace
+    nu: float
+    beta: float
+    u0: op2.Dat
+    pressure_map: op2.Map = None
+    symmetric = False
+
+    def __post_init__(self):
+        if self.pressure_map is None:
+            self.pressure_map = _taylor_hood_pressure_map(self.V, self.Q, "Navier-Stokes")
+
+    def dat(self, u=None, p=None):
+        return op2.MixedDat([self.V.dat(u), self.Q.dat(p)])
+
+    def coefficient_args(self):
+        return [self.u0(op2.READ, self.V.cell_node_map)]
+
+    def kernel(self, rank=1, diagonal=False):
+        if rank != 1 or diagonal:
+            raise NotImplementedError("the Navier-Stokes Jacobian is an action only: there is no assembled matrix "
+                                      "or diagonal (use mat_type='matfree')")
+        return op2.Kernel("navier_stokes_jacobian", degree=self.V.degree, mu=self.nu, beta=self.beta)
+
+
+_TAYLOR_HOOD_FORMS = (Stokes, NavierStokes, NavierStokesJacobian)
+
+
 class StokesAssembler:
-    """Cached assembler of the Stokes action (velocity, pressure) -> (y_u, y_p) on MixedDats, the
-    counterpart of :class:`OneFormAssembler`: the parloop is built once and re-run."""
+    """Cached assembler of the action (velocity, pressure) -> (y_u, y_p) on MixedDats of a form on the
+    Taylor-Hood pair (:class:`Stokes`, :class:`NavierStokes`, :class:`NavierStokesJacobian`), the counterpart
+    of :class:`OneFormAssembler`: the parloop is built once and re-run; the form's coefficients (the Jacobian's
+    u) follow the pressure."""
 
     def __init__(self, form: Stokes, up: op2.MixedDat, bcs=(), scatter="atomic"):
         self.form, self.up, self.bcs = form, up, tuple(bcs)
@@ -1212,7 +1424,7 @@ class StokesAssembler:
             self._loop = op2.Parloop(self._gk, V.cell_set,
                                      [yu(op2.INC, V.cell_node_map), V.coordinates(op2.READ, V.coord_map),
                                       u(op2.READ, V.cell_node_map), yp(op2.INC, F.pressure_map),
-                                      p(op2.READ, F.pressure_map)], location="device")
+                                      p(op2.READ, F.pressure_map)] + F.coefficient_args(), location="device")
         tensor.zero()
         self._loop()
         for bc in self.bcs:
@@ -1221,9 +1433,10 @@ class StokesAssembler:
 
 
 class StokesMatrixContext:
-    """Matrix-free Stokes operator on MixedDats: ``mult`` zeroes the velocity-BC entries of x, applies the
-    saddle-point action and writes x back on the constrained velocity rows (identity there).  The operator
-    is symmetric, so ``multTranspose`` is ``mult``."""
+    """Matrix-free operator of a Taylor-Hood form (:class:`Stokes`, :class:`NavierStokesJacobian`) on
+    MixedDats: ``mult`` zeroes the velocity-BC entries of x, applies the saddle-point action and writes x back
+    on the constrained velocity rows (identity there).  The Stokes operator is symmetric, so ``multTranspose``
+    is ``mult``; for a nonsymmetric form it raises."""
 
     def __init__(self, form: Stokes, bcs=()):
         self.form, self.bcs = form, tuple(bcs)
@@ -1244,6 +1457,9 @@ class StokesMatrixContext:
         return Y
 
     def multTranspose(self, X: op2.MixedDat, Y: op2.MixedDat):
+        if not self.form.symmetric:
+            raise NotImplementedError(f"multTranspose: {type(self.form).__name__} is not symmetric, and its "
+                                      f"transpose action is not implemented")
         return self.mult(X, Y)
 
 
@@ -1303,11 +1519,15 @@ def assemble(form: Form, u=None, tensor=None, bcs=(), mat_type="aij"):
     unassembled), ``"matfree"`` -> :class:`ImplicitMatrixContext`."""
     V = form.V
     bcs = tuple(bcs)
-    if isinstance(form, Stokes):
+    if isinstance(form, _TAYLOR_HOOD_FORMS):
         if u is not None:
             return StokesAssembler(form, u, bcs).assemble(tensor)
+        if isinstance(form, NavierStokes):
+            raise ValueError("the Navier-Stokes residual is a 1-form: assemble(F, u=up), or its operator "
+                             "assemble(F.jacobian(up), mat_type='matfree')")
         if mat_type != "matfree":
-            raise NotImplementedError(f"mat_type {mat_type!r}: Stokes has no assembled matrix, use mat_type "
+            what = "Stokes" if isinstance(form, Stokes) else "the Navier-Stokes Jacobian"
+            raise NotImplementedError(f"mat_type {mat_type!r}: {what} has no assembled matrix, use mat_type "
                                       f"'matfree'")
         return StokesMatrixContext(form, bcs)
     if u is not None:
@@ -1636,7 +1856,8 @@ def gmres(A, b: op2.Dat, x: op2.Dat, M=None, rtol=1e-5, atol=0.0, restart=30, ma
     return it, hist
 
 
-def solve_nonlinear(F, L: op2.Dat, u: op2.Dat, bcs=(), solver_parameters=None, hierarchy=None, allreduce=None):
+def solve_nonlinear(F, L: op2.Dat, u: op2.Dat, bcs=(), solver_parameters=None, hierarchy=None, allreduce=None,
+                    nullspace=None):
     """``solve(F == 0, u, bcs=bcs, solver_parameters=...)`` for nonlinear diffusion (``F`` a
     :class:`NonlinearDiffusion`) or hyperelasticity (a :class:`HyperElasticity` on a vector space) with the
     source ``L`` (the assembled right-hand side, e.g. ``assemble(mass(V), u=f)``): Newton's method with the
@@ -1655,9 +1876,22 @@ def solve_nonlinear(F, L: op2.Dat, u: op2.Dat, bcs=(), solver_parameters=None, h
     Converged when ||R(u)|| <= max(snes_rtol * ||R(u_0)||, snes_atol).  For hyperelasticity a
     non-finite residual norm (an inverted element: ln J of J <= 0) ends the solve with a
     :class:`ConvergenceError` whose reason is "DIVERGED_FNORM_NAN".  Returns (Newton residual norms,
-    Krylov iterations per Newton step)."""
+    Krylov iterations per Newton step).
+
+    Navier-Stokes (``F`` a :class:`NavierStokes`): ``L`` and ``u`` are MixedDats (velocity, pressure), the
+    Dirichlet conditions are on the velocity, and the residual norm runs over both blocks.  Each step is
+    matrix-free GMRES on ``F.jacobian(u)`` with the options of :func:`_solve_stokes`: ``mat_type`` "matfree",
+    ``pc_type`` "none" (default) or "fieldsplit" (schur, diag; ``fieldsplit_0_pc_type`` "jacobi" or "mg" on
+    ``Form(W, nu, beta)`` per component, ``fieldsplit_1_pc_type`` "jacobi", the pressure mass over nu), built
+    once per solve.  ``nullspace`` "constant" removes the pressure mean from the residual, from every
+    preconditioned vector and from the final pressure.  A non-finite residual norm ends the solve with a
+    :class:`ConvergenceError` ("DIVERGED_FNORM_NAN").  The other forms take no ``nullspace``."""
     from . import _lib
     from . import mg as _mg
+    if isinstance(F, NavierStokes):
+        return _solve_navier_stokes(F, L, u, bcs, solver_parameters, hierarchy, nullspace)
+    if nullspace is not None:
+        raise NotImplementedError("nullspace is implemented for Navier-Stokes forms only")
     sp = {"snes_rtol": 1e-8, "snes_atol": 1e-50, "snes_max_it": 50, "ksp_type": "gmres",
           "ksp_gmres_restart": 30, "ksp_rtol": 1e-5, "ksp_max_it": 10000, "mat_type": "matfree",
           "pc_type": "none"}
@@ -1874,8 +2108,6 @@ def _solve_stokes(form: Stokes, L: op2.MixedDat, up: op2.MixedDat, bcs=(), solve
     Dirichlet conditions are on the velocity; their values are lifted with the full Stokes action on
     (g, 0), so the pressure rows receive -q div g.  ``up`` is overwritten with the solution.  Returns
     (iterations, residual history)."""
-    from . import _lib
-    from . import mg as _mg
     sp = {"mat_type": "matfree", "ksp_type": "gmres", "pc_type": "none", "ksp_rtol": 1e-8, "ksp_max_it": 1000,
           "ksp_gmres_restart": 30, "fieldsplit_0_pc_type": "jacobi", "fieldsplit_1_pc_type": "jacobi",
           "fieldsplit_0_ksp_type": "preonly", "fieldsplit_1_ksp_type": "preonly"}
@@ -1890,34 +2122,10 @@ def _solve_stokes(form: Stokes, L: op2.MixedDat, up: op2.MixedDat, bcs=(), solve
                                   f"'matfree'")
     if nullspace not in (None, "constant"):
         raise NotImplementedError(f"nullspace {nullspace!r}: None or 'constant' (constant pressures)")
-    pc = sp["pc_type"]
-    if pc not in ("none", "fieldsplit"):
-        raise NotImplementedError(f"pc_type {pc!r}: 'none' or 'fieldsplit'")
-    if pc == "fieldsplit":
-        if sp.get("pc_fieldsplit_type") != "schur":
-            raise NotImplementedError(f"pc_fieldsplit_type {sp.get('pc_fieldsplit_type')!r}: 'schur' only")
-        if sp.get("pc_fieldsplit_schur_fact_type") != "diag":
-            raise NotImplementedError(f"pc_fieldsplit_schur_fact_type {sp.get('pc_fieldsplit_schur_fact_type')!r}: "
-                                      f"'diag' only")
-        for f in ("0", "1"):
-            if sp[f"fieldsplit_{f}_ksp_type"] != "preonly":
-                raise NotImplementedError(f"fieldsplit_{f}_ksp_type {sp[f'fieldsplit_{f}_ksp_type']!r}: 'preonly' "
-                                          f"only")
-        if sp["fieldsplit_0_pc_type"] not in ("jacobi", "mg"):
-            raise NotImplementedError(f"fieldsplit_0_pc_type {sp['fieldsplit_0_pc_type']!r}: 'jacobi' or 'mg'")
-        if sp["fieldsplit_1_pc_type"] != "jacobi":
-            raise NotImplementedError(f"fieldsplit_1_pc_type {sp['fieldsplit_1_pc_type']!r}: 'jacobi' (the "
-                                      f"inverse diagonal of the pressure mass matrix over mu)")
-        if sp["fieldsplit_0_pc_type"] == "mg" and hierarchy is None:
-            raise ValueError("fieldsplit_0_pc_type mg needs the mesh hierarchy")
+    _check_fieldsplit(sp, hierarchy)
     V, Q = form.V, form.Q
     bcs = tuple(bcs)
-    lib = _lib.lib()
-
-    ones = Q.dat(np.ones(Q.node_count)) if nullspace else None
-
-    def remove_pressure_mean(v):
-        v[1].axpy(-v[1].inner(ones) / Q.node_count, ones)
+    remove_pressure_mean = _pressure_mean_remover(Q) if nullspace else None
 
     # lifting: A (up - (g, 0)) = L - A (g, 0) with homogeneous conditions
     g = form.dat()
@@ -1938,16 +2146,72 @@ def _solve_stokes(form: Stokes, L: op2.MixedDat, up: op2.MixedDat, bcs=(), solve
     up.zero()
     for d in up:
         d.device_ptr
-    M = None
+    M = _fieldsplit_pc(V, Q, form.mu, form.beta, up, bcs, sp, hierarchy, remove_pressure_mean)
+    its, hist = gmres(A, b, up, M, rtol=sp["ksp_rtol"], restart=sp["ksp_gmres_restart"], maxit=sp["ksp_max_it"])
+    if nullspace:
+        remove_pressure_mean(up)
+    if lift:
+        up[0].axpy(1.0, g[0])
+    else:
+        for bc in bcs:
+            bc.apply(up[0])
+    return its, hist
+
+
+def _check_fieldsplit(sp, hierarchy):
+    """The preconditioner options of the Taylor-Hood solves (:func:`_solve_stokes`, Newton on
+    :class:`NavierStokes`): ``pc_type`` "none" or the diagonal Schur fieldsplit."""
+    pc = sp["pc_type"]
+    if pc not in ("none", "fieldsplit"):
+        raise NotImplementedError(f"pc_type {pc!r}: 'none' or 'fieldsplit'")
     if pc == "fieldsplit":
+        if sp.get("pc_fieldsplit_type") != "schur":
+            raise NotImplementedError(f"pc_fieldsplit_type {sp.get('pc_fieldsplit_type')!r}: 'schur' only")
+        if sp.get("pc_fieldsplit_schur_fact_type") != "diag":
+            raise NotImplementedError(f"pc_fieldsplit_schur_fact_type {sp.get('pc_fieldsplit_schur_fact_type')!r}: "
+                                      f"'diag' only")
+        for f in ("0", "1"):
+            if sp[f"fieldsplit_{f}_ksp_type"] != "preonly":
+                raise NotImplementedError(f"fieldsplit_{f}_ksp_type {sp[f'fieldsplit_{f}_ksp_type']!r}: 'preonly' "
+                                          f"only")
+        if sp["fieldsplit_0_pc_type"] not in ("jacobi", "mg"):
+            raise NotImplementedError(f"fieldsplit_0_pc_type {sp['fieldsplit_0_pc_type']!r}: 'jacobi' or 'mg'")
+        if sp["fieldsplit_1_pc_type"] != "jacobi":
+            raise NotImplementedError(f"fieldsplit_1_pc_type {sp['fieldsplit_1_pc_type']!r}: 'jacobi' (the "
+                                      f"inverse diagonal of the pressure mass matrix over mu)")
+        if sp["fieldsplit_0_pc_type"] == "mg" and hierarchy is None:
+            raise ValueError("fieldsplit_0_pc_type mg needs the mesh hierarchy")
+
+
+def _pressure_mean_remover(Q):
+    """v -> v with the dof-mean of its pressure block removed (the constant-pressure nullspace)."""
+    ones = Q.dat(np.ones(Q.node_count))
+
+    def remove_pressure_mean(v):
+        v[1].axpy(-v[1].inner(ones) / Q.node_count, ones)
+    return remove_pressure_mean
+
+
+def _fieldsplit_pc(V, Q, mu, beta, up, bcs, sp, hierarchy, remove_pressure_mean=None):
+    """The preconditioner ``M(r, z)`` of the Taylor-Hood GMRES solves (None: none), from the options that
+    :func:`_check_fieldsplit` accepted.  The diagonal Schur fieldsplit preconditions the velocity with Jacobi
+    or one V-cycle per component of ``Form(W, mu, beta)`` and the pressure with the inverse diagonal of
+    (1/mu) M_p.  It does not depend on the velocity, so one is built per solve.  ``remove_pressure_mean``
+    (the constant nullspace) is applied to every preconditioned vector."""
+    from . import _lib
+    from . import mg as _mg
+    lib = _lib.lib()
+    nullspace = remove_pressure_mean is not None
+    M = None
+    if sp["pc_type"] == "fieldsplit":
         n_u, n_p = up[0]._data.size, up[1]._data.size
         # pressure: the inverse diagonal of (1/mu) M_p
-        dp = ImplicitMatrixContext(Form(Q, 0.0, 1.0 / form.mu)).getDiagonal(Q.dat())
+        dp = ImplicitMatrixContext(Form(Q, 0.0, 1.0 / mu)).getDiagonal(Q.dat())
         op2.par_loop(_mg.reciprocal_kernel(1), Q.node_set, dp(op2.RW))
         if sp["fieldsplit_0_pc_type"] == "jacobi":
             # the velocity block is mu * (vector Laplacian) + beta * mass: the scalar diagonal on every component
             Vs = FunctionSpace(V.mesh, V.degree)
-            ds = ImplicitMatrixContext(Form(Vs, form.mu, form.beta)).getDiagonal(Vs.dat()).data_ro
+            ds = ImplicitMatrixContext(Form(Vs, mu, beta)).getDiagonal(Vs.dat()).data_ro
             du = V.dat(np.repeat(ds, 3).reshape(-1, 3))
             for bc in bcs:
                 bc.set(du, 1.0)
@@ -1959,7 +2223,7 @@ def _solve_stokes(form: Stokes, L: op2.MixedDat, up: op2.MixedDat, bcs=(), solve
         else:
             # the velocity block is three uncoupled copies of the scalar Form(W, mu, beta): one scalar V-cycle
             # per component (the Helmholtz diagonal kernel that the smoother needs is scalar)
-            vc = _mg.VCycle(hierarchy, V.degree, lambda W, k=None: Form(W, form.mu, form.beta),
+            vc = _mg.VCycle(hierarchy, V.degree, lambda W, k=None: Form(W, mu, beta),
                             bc_domains=tuple(s for bc in bcs for s in bc.sub_domains))
             top = len(hierarchy) - 1
             nn = V.node_count
@@ -1987,15 +2251,73 @@ def _solve_stokes(form: Stokes, L: op2.MixedDat, up: op2.MixedDat, bcs=(), solve
         def M(r, z):
             r.copy(z)
             remove_pressure_mean(z)
-    its, hist = gmres(A, b, up, M, rtol=sp["ksp_rtol"], restart=sp["ksp_gmres_restart"], maxit=sp["ksp_max_it"])
+    return M
+
+
+def _solve_navier_stokes(F: NavierStokes, L: op2.MixedDat, up: op2.MixedDat, bcs=(), solver_parameters=None,
+                         hierarchy=None, nullspace=None):
+    """Newton's method for :class:`NavierStokes` (``snes_type newtonls``, ``snes_linesearch_type basic``) on
+    R(up) = F(up) - L over MixedDats; see :func:`solve_nonlinear`."""
+    sp = {"snes_rtol": 1e-8, "snes_atol": 1e-50, "snes_max_it": 50, "ksp_type": "gmres",
+          "ksp_gmres_restart": 30, "ksp_rtol": 1e-5, "ksp_max_it": 10000, "mat_type": "matfree",
+          "pc_type": "none", "fieldsplit_0_pc_type": "jacobi", "fieldsplit_1_pc_type": "jacobi",
+          "fieldsplit_0_ksp_type": "preonly", "fieldsplit_1_ksp_type": "preonly"}
+    sp.update(solver_parameters or {})
+    if sp["ksp_type"] != "gmres":
+        raise NotImplementedError(f"ksp_type {sp['ksp_type']!r}: the Navier-Stokes Jacobian is nonsymmetric and "
+                                  f"indefinite, Newton solves with gmres")
+    if sp["mat_type"] != "matfree":
+        raise NotImplementedError(f"mat_type {sp['mat_type']!r}: the Navier-Stokes Jacobian has no assembled "
+                                  f"matrix, use mat_type 'matfree'")
+    if nullspace not in (None, "constant"):
+        raise NotImplementedError(f"nullspace {nullspace!r}: None or 'constant' (constant pressures)")
+    _check_fieldsplit(sp, hierarchy)
+    V, Q = F.V, F.Q
+    bcs = tuple(bcs)
+    remove_pressure_mean = _pressure_mean_remover(Q) if nullspace else None
+    for d in up:
+        d.device_ptr
+    for bc in bcs:
+        bc.apply(up[0])
+    R, du = F.dat(), F.dat()
+    res = StokesAssembler(F, up)
+
+    def residual():
+        res.assemble(tensor=R)
+        R.axpy(-1.0, L)
+        for bc in bcs:
+            bc.zero(R[0])
+        if nullspace:
+            remove_pressure_mean(R)
+        return R.norm()
+
+    def check_finite():
+        if not np.isfinite(hist[-1]):
+            raise ConvergenceError(f"Newton diverged: the residual norm is {hist[-1]} after {len(kits)} steps "
+                                   f"(DIVERGED_FNORM_NAN)", "DIVERGED_FNORM_NAN")
+
+    hist = [residual()]
+    kits = []
+    check_finite()
+    tol = max(sp["snes_rtol"] * hist[0], sp["snes_atol"])
+    # J reads up[0] in place, so one matrix-free operator serves every step; the preconditioner does not
+    # depend on u
+    A = StokesMatrixContext(F.jacobian(up), bcs)
+    M = _fieldsplit_pc(V, Q, F.nu, F.beta, up, bcs, sp, hierarchy, remove_pressure_mean)
+    while hist[-1] > tol and len(kits) < sp["snes_max_it"]:
+        du.zero()
+        for d in du:
+            d.device_ptr
+        its, _ = gmres(A, R, du, M, rtol=sp["ksp_rtol"], restart=sp["ksp_gmres_restart"], maxit=sp["ksp_max_it"])
+        for bc in bcs:
+            bc.zero(du[0])
+        up.axpy(-1.0, du)
+        kits.append(its)
+        hist.append(residual())
+        check_finite()
     if nullspace:
         remove_pressure_mean(up)
-    if lift:
-        up[0].axpy(1.0, g[0])
-    else:
-        for bc in bcs:
-            bc.apply(up[0])
-    return its, hist
+    return hist, kits
 
 
 class DGAdvection:

@@ -145,7 +145,8 @@ int fdb_launch_elasticity_matrix(fdb_kernel_s *k, fdb_int start, fdb_int end, in
                                  fdb_mat_t mat, const double *coords, const double *u, const fdb_int *map0,
                                  const fdb_int *map1, double *diag_out);
 // FDB_FORM_STOKES (elasticity_hex.cu): yu and u AoS with 3 values per node of map0, yp and p one value per
-// node of map2 (the pressure map)
+// node of map2 (the pressure map).  FDB_FORM_NAVIER_STOKES[_JACOBIAN] run through it too: ulin is the
+// Jacobian's linearisation velocity (AoS through map0), NULL for the other two forms
 int fdb_launch_stokes_action(fdb_kernel_s *k, fdb_int start, fdb_int end, int nlay, const fdb_int *subset,
                              double *yu, const double *coords, const double *u, double *yp, const double *p,
-                             const fdb_int *map0, const fdb_int *map1, const fdb_int *map2);
+                             const double *ulin, const fdb_int *map0, const fdb_int *map1, const fdb_int *map2);

@@ -42,6 +42,15 @@
 // same square passes as B: Bq is padded with a zero last column.  The point stage puts mu G - p I into
 // the fluxes where sigma goes and replaces p by its test value -w |det J| tr G, which goes back through
 // Bq^T along z, y, x; the threads of the (N-1)^3 pressure dofs scatter it into yp.
+//
+// FDB_FORM_NAVIER_STOKES[_JACOBIAN] (DESIGN.md section 4.12) run with MODE EL_NS_RESIDUAL / EL_NS_JACOBIAN:
+// steady incompressible Navier-Stokes on the same spaces and its exact Newton Jacobian at u,
+//     R((u, p); (v, q))      = Stokes((u, p); (v, q)) + inner(dot(grad u, u), v)*dx
+//     J(u)[(w, r); (v, q)]   = Stokes((w, r); (v, q)) + inner(dot(grad w, u), v)*dx + inner(dot(grad u, w), v)*dx
+// (mu = nu).  Gather, passes and scatter are those of EL_STOKES; only the value slot of the point stage
+// gains the convective term, w |det J| sum_k G[d][k] u_k (residual) or w |det J| sum_k (G_w[d][k] u_k +
+// G_u[d][k] w_k) (Jacobian).  The Jacobian gathers u into S_V as EL_JACOBIAN does (its forward passes share
+// S_F[3..9)), takes G_u from the collocated derivative of S_V, and keeps S_P / S_Q after S_V.
 #include "common.cuh"
 
 namespace {
@@ -66,25 +75,32 @@ struct ElasParams {
     const fdb_int *row_lg, *col_lg;   // dof-level, NULL = identity
     const unsigned short *rank_tab;
     int nvar, nlay_total;
-    const double *u;             // EL_JACOBIAN: the linearisation point (AoS, node map)
-    // EL_STOKES: the pressure action output and input (one value per node of map2, (N-1)^3 per cell)
+    const double *u;             // EL_JACOBIAN, EL_NS_JACOBIAN: the linearisation point (AoS, node map)
+    // EL_STOKES, EL_NS_*: the pressure action output and input (one value per node of map2, (N-1)^3 per cell)
     double *yp;
     const double *xp;
     const fdb_int *map2, *off2;
     double Bq[N * N];            // pressure basis at the points, (N, N-1) padded with a zero last column
 };
 
-enum { EL_LINEAR = 0, EL_RESIDUAL = 1, EL_JACOBIAN = 2, EL_STOKES = 3 };
+enum { EL_LINEAR = 0, EL_RESIDUAL = 1, EL_JACOBIAN = 2, EL_STOKES = 3, EL_NS_RESIDUAL = 4, EL_NS_JACOBIAN = 5 };
+
+// the modes that also gather u into S_V (a Jacobian's linearisation point), and those on the Taylor-Hood pair
+__host__ __device__ constexpr bool el_holds_u(int mode) { return mode == EL_JACOBIAN || mode == EL_NS_JACOBIAN; }
+__host__ __device__ constexpr bool el_pressure(int mode)
+{
+    return mode == EL_STOKES || mode == EL_NS_RESIDUAL || mode == EL_NS_JACOBIAN;
+}
 
 template <int N, int MODE = EL_LINEAR>
 struct ElasShape {
     static constexpr int ND = N * N * N;
     static constexpr int CPB = (256 / ND) > 0 ? 256 / ND : 1;          // cells (slots) per CTA
     static constexpr int THREADS = ((CPB * ND + 31) / 32) * 32;
-    // doubles per slot: vertices, values at the points, work buffer, fluxes (9 per point); the Jacobian
-    // also holds u's values (S_V), Stokes the pressure and its work buffer (S_P, S_Q)
-    static constexpr int SLOT = 24 + 3 * ND + 3 * ND + 9 * ND + (MODE == EL_JACOBIAN ? 3 * ND : 0) +
-                                (MODE == EL_STOKES ? 2 * ND : 0);
+    // doubles per slot: vertices, values at the points, work buffer, fluxes (9 per point); the Jacobians
+    // also hold u's values (S_V), the Taylor-Hood modes the pressure and its work buffer (S_P, S_Q, after S_V)
+    static constexpr int SLOT = 24 + 3 * ND + 3 * ND + 9 * ND + (el_holds_u(MODE) ? 3 * ND : 0) +
+                                (el_pressure(MODE) ? 2 * ND : 0);
     static constexpr size_t SMEM = (size_t)CPB * SLOT * sizeof(double) + (size_t)CPB * ND * sizeof(int);
 };
 
@@ -124,9 +140,9 @@ elasticity_kernel(const __grid_constant__ ElasParams<N> P)
     using S = ElasShape<N, MODE>;
     constexpr int ND = S::ND;
     constexpr int CPB = S::CPB;
-    constexpr bool JAC = MODE == EL_JACOBIAN;
-    constexpr bool STK = MODE == EL_STOKES;
-    constexpr int NP = N - 1;                              // pressure dofs per axis (EL_STOKES)
+    constexpr bool JAC = el_holds_u(MODE);                 // EL_JACOBIAN, EL_NS_JACOBIAN: u in S_V
+    constexpr bool STK = el_pressure(MODE);                // EL_STOKES, EL_NS_*: the pressure space
+    constexpr int NP = N - 1;                              // pressure dofs per axis (EL_STOKES, EL_NS_*)
     extern __shared__ __align__(16) unsigned char smem_raw[];
     const int slot = threadIdx.x / ND;
     const int l = threadIdx.x - slot * ND;                 // this thread's dof / point in the cell
@@ -137,12 +153,12 @@ elasticity_kernel(const __grid_constant__ ElasParams<N> P)
     double *s_u = s_x + 24;                                // [3][ND]
     double *s_t = s_u + 3 * ND;                            // [3][ND]
     double *s_f = s_t + 3 * ND;                            // [3 d][3 m][ND]
-    double *s_v = s_f + 9 * ND;                            // [3][ND], EL_JACOBIAN only
-    double *s_p = s_f + 9 * ND;                            // [ND], EL_STOKES only: pressure
-    double *s_q = s_p + ND;                                // [ND], EL_STOKES only: its work buffer
+    double *s_v = s_f + 9 * ND;                            // [3][ND], EL_JACOBIAN and EL_NS_JACOBIAN only
+    double *s_p = s_f + 9 * ND + (MODE == EL_NS_JACOBIAN ? 3 * ND : 0);   // [ND], pressure modes: pressure
+    double *s_q = s_p + ND;                                // [ND], pressure modes: its work buffer
     int *s_idx = reinterpret_cast<int *>(reinterpret_cast<double *>(smem_raw) + (size_t)CPB * S::SLOT) + sl * ND;
     const int qi = l / (N * N), qj = (l / N) % N, qk = l % N;
-    // EL_STOKES: this thread's pressure dof, if its (i, j, k) is one
+    // pressure modes: this thread's pressure dof, if its (i, j, k) is one
     const bool pdof = STK && qi < NP && qj < NP && qk < NP;
     const int lp = (qi * NP + qj) * NP + qk;
 
@@ -298,7 +314,7 @@ elasticity_kernel(const __grid_constant__ ElasParams<N> P)
                     s_f[(d * 3 + m) * ND + l] = sw * (R[m][0] * sg[0] + R[m][1] * sg[1] + R[m][2] * sg[2]);
                 mres[d] = P.beta * w * fabs(det) * s_u[d * ND + l];
             }
-            } else if (STK) {
+            } else if (MODE == EL_STOKES) {
                 // flux mu G - p I; the pressure's test value -w |det| div u replaces p in S_P
                 const double pv = s_q[l];
                 const double sw = w * fabs(det) * rdet;
@@ -313,6 +329,40 @@ elasticity_kernel(const __grid_constant__ ElasParams<N> P)
                     mres[d] = P.beta * w * fabs(det) * s_u[d * ND + l];
                 }
                 s_p[l] = -w * fabs(det) * (G[0][0] + G[1][1] + G[2][2]);
+            } else if (STK) {
+                // Navier-Stokes: the Stokes flux and pressure test value; the value slot adds the convective
+                // term, (grad u) u (residual: G is grad u) or (grad w) u + (grad u) w (Jacobian: G is grad w,
+                // u and its gradient come from S_V)
+                const double pv = s_q[l];
+                const double wd = w * fabs(det);
+                const double sw = wd * rdet;
+                double uq[3], cv[3];
+#pragma unroll
+                for (int k = 0; k < 3; k++) uq[k] = JAC ? s_v[k * ND + l] : s_u[k * ND + l];
+#pragma unroll
+                for (int d = 0; d < 3; d++) cv[d] = G[d][0] * uq[0] + G[d][1] * uq[1] + G[d][2] * uq[2];
+                if (JAC) {
+#pragma unroll
+                    for (int d = 0; d < 3; d++) {
+                        const double g0 = pass1<N, 0, false>(P.Dt, s_v + d * ND, qi, qj, qk);
+                        const double g1 = pass1<N, 1, false>(P.Dt, s_v + d * ND, qi, qj, qk);
+                        const double g2 = pass1<N, 2, false>(P.Dt, s_v + d * ND, qi, qj, qk);
+#pragma unroll
+                        for (int k = 0; k < 3; k++)
+                            cv[d] = fma((g0 * R[0][k] + g1 * R[1][k] + g2 * R[2][k]) * rdet, s_u[k * ND + l], cv[d]);
+                    }
+                }
+#pragma unroll
+                for (int d = 0; d < 3; d++) {
+                    double sg[3];
+#pragma unroll
+                    for (int k = 0; k < 3; k++) sg[k] = P.mu * G[d][k] - (k == d ? pv : 0.0);
+#pragma unroll
+                    for (int m = 0; m < 3; m++)
+                        s_f[(d * 3 + m) * ND + l] = sw * (R[m][0] * sg[0] + R[m][1] * sg[1] + R[m][2] * sg[2]);
+                    mres[d] = wd * (P.beta * s_u[d * ND + l] + cv[d]);
+                }
+                s_p[l] = -wd * (G[0][0] + G[1][1] + G[2][2]);
             } else {
                 // deformation gradient Fd = I + grad u: u's gradient is G (residual) or comes from S_V
                 double Fd[3][3];
@@ -492,7 +542,8 @@ void fill_tables(const fdb_kernel_s *k, ElasParams<N> &P)
         P.wq[i] = k->desc.wq[i];
         P.xq[i] = k->desc.xq[i];
     }
-    if (k->desc.form == FDB_FORM_STOKES) {
+    if (k->desc.form == FDB_FORM_STOKES || k->desc.form == FDB_FORM_NAVIER_STOKES ||
+        k->desc.form == FDB_FORM_NAVIER_STOKES_JACOBIAN) {
         P.off2 = k->d_off2;
         for (int q = 0; q < N; q++)
             for (int a = 0; a < N; a++) P.Bq[q * N + a] = a < N - 1 ? k->B2[q * (N - 1) + a] : 0.0;
@@ -582,10 +633,10 @@ int action_mode(fdb_kernel_s *k, fdb_int start, fdb_int end, int nlay, const fdb
                 const double *coords, const double *x, const double *u, const fdb_int *map0, const fdb_int *map1,
                 double *yp = nullptr, const double *xp = nullptr, const fdb_int *map2 = nullptr)
 {
-    // Stokes has no degree-1 instantiation (its pressure space would be CG_0)
+    // the Taylor-Hood modes have no degree-1 instantiation (their pressure space would be CG_0)
     switch (k->n1d) {
     case 2:
-        if constexpr (MODE != EL_STOKES)
+        if constexpr (!el_pressure(MODE))
             return action_n<2, MODE>(k, start, end, nlay, subset, y, coords, x, u, map0, map1, yp, xp, map2);
         break;
     case 3: return action_n<3, MODE>(k, start, end, nlay, subset, y, coords, x, u, map0, map1, yp, xp, map2);
@@ -629,9 +680,20 @@ int fdb_launch_elasticity_action(fdb_kernel_s *k, fdb_int start, fdb_int end, in
 
 int fdb_launch_stokes_action(fdb_kernel_s *k, fdb_int start, fdb_int end, int nlay, const fdb_int *subset,
                              double *yu, const double *coords, const double *u, double *yp, const double *p,
-                             const fdb_int *map0, const fdb_int *map1, const fdb_int *map2)
+                             const double *ulin, const fdb_int *map0, const fdb_int *map1, const fdb_int *map2)
 {
-    return action_mode<EL_STOKES>(k, start, end, nlay, subset, yu, coords, u, nullptr, map0, map1, yp, p, map2);
+    switch (k->desc.form) {
+    case FDB_FORM_STOKES:
+        return action_mode<EL_STOKES>(k, start, end, nlay, subset, yu, coords, u, nullptr, map0, map1, yp, p, map2);
+    case FDB_FORM_NAVIER_STOKES:
+        return action_mode<EL_NS_RESIDUAL>(k, start, end, nlay, subset, yu, coords, u, nullptr, map0, map1, yp, p,
+                                           map2);
+    case FDB_FORM_NAVIER_STOKES_JACOBIAN:
+        return action_mode<EL_NS_JACOBIAN>(k, start, end, nlay, subset, yu, coords, u, ulin, map0, map1, yp, p,
+                                           map2);
+    }
+    fdb::set_error("stokes action: form %d is not a Taylor-Hood form", k->desc.form);
+    return 1;
 }
 
 int fdb_launch_elasticity_matrix(fdb_kernel_s *k, fdb_int start, fdb_int end, int nlay, const fdb_int *subset,

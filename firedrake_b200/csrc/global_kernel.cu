@@ -286,7 +286,7 @@ struct fdb_hex_form {
     bool residual;            // a 1-form action only
     int launcher;             // fdb_launch_helmholtz_*, fdb_launch_helmholtz_coef_* (which also run the
                               // nonlinear diffusion and advection-diffusion forms), fdb_launch_elasticity_*
-                              // or fdb_launch_stokes_action
+                              // or fdb_launch_stokes_action (which also runs the Navier-Stokes forms)
     int max_degree[3];        // per mode: action, matrix, diagonal
     int min_degree;
     const char *space2;       // the arguments on a second space (output and input, through a third map), or
@@ -310,6 +310,9 @@ static const fdb_hex_form hex_forms[] = {
      {4, 3, 3}, 1, nullptr},
     // velocity CG_p with pressure CG_{p-1}: p >= 2
     {FDB_FORM_STOKES, "stokes", 3, false, nullptr, 0, false, LAUNCH_STOKES, {4, 0, 0}, 2, "y_p, p"},
+    {FDB_FORM_NAVIER_STOKES, "navier_stokes", 3, false, nullptr, 0, true, LAUNCH_STOKES, {4, 0, 0}, 2, "y_p, p"},
+    {FDB_FORM_NAVIER_STOKES_JACOBIAN, "navier_stokes_jacobian", 3, false, "u", 3, false, LAUNCH_STOKES, {4, 0, 0}, 2,
+     "y_p, p"},
 };
 
 static const char *const mode_name[] = {"action", "matrix", "diagonal"};
@@ -391,14 +394,15 @@ static int kernel_create(const fdb_kernel_desc *d, const fdb_space2_desc *s2, fd
                   "pin the rule with dx(degree=2*p)", f->name, d->nq, d->degree);
         return 1;
     }
-    if (f->residual && mode != MODE_ACTION) {
-        set_error("fdb_kernel_create: %s is the residual, a 1-form action only: its matrix and diagonal are those "
-                  "of %s_jacobian", f->name, f->name);
-        return 1;
-    }
+    // (a mixed residual has no matrix or diagonal, nor has its Jacobian: the mixed-form message comes first)
     if (f->space2 && mode != MODE_ACTION) {
         set_error("fdb_kernel_create: %s is a mixed form, a rank-1 action only: it has no assembled matrix or "
                   "diagonal", f->name);
+        return 1;
+    }
+    if (f->residual && mode != MODE_ACTION) {
+        set_error("fdb_kernel_create: %s is the residual, a 1-form action only: its matrix and diagonal are those "
+                  "of %s_jacobian", f->name, f->name);
         return 1;
     }
     if (d->degree < f->min_degree || d->degree > f->max_degree[mode]) {
@@ -572,7 +576,8 @@ int fdb_kernel_call(fdb_kernel_t k, const fdb_call_args *a)
     // PETSc Mat handle in the same slot, pyop2/types/mat.py:621-623) or [d (INC), coords] (diagonal), then
     // the form's trailing coefficient; maps = [V map, coord map].  A form on two spaces (Stokes) has the
     // output and input of the second space after x and a third map: [y, coords, x, y2, x2], [V map, coord
-    // map, second map]
+    // map, second map]; with a trailing coefficient as well (the Navier-Stokes Jacobian's u) the coefficient
+    // comes last: [y, coords, x, y2, x2, coef]
     const fdb_hex_form *f = k->hex;
     const int mode = hex_mode(&k->desc);
     const int want = (mode == MODE_ACTION ? 3 : 2) + (f->coef ? 1 : 0) + (f->space2 ? 2 : 0);
@@ -581,8 +586,8 @@ int fdb_kernel_call(fdb_kernel_t k, const fdb_call_args *a)
     if (a->nargs != want || a->nmaps != want_maps || (device_only && a->location != FDB_LOC_DEVICE)) {
         static const char *const args[] = {"y, coords, x", "mat, coords", "d, coords"};
         set_error("fdb_kernel_call: %s %s expects %d %sargs (%s%s%s%s%s) and %d maps, got %d/%d", f->name,
-                  mode_name[mode], want, device_only ? "device " : "", args[mode], f->coef ? ", " : "",
-                  f->coef ? f->coef : "", f->space2 ? ", " : "", f->space2 ? f->space2 : "", want_maps, a->nargs,
+                  mode_name[mode], want, device_only ? "device " : "", args[mode], f->space2 ? ", " : "",
+                  f->space2 ? f->space2 : "", f->coef ? ", " : "", f->coef ? f->coef : "", want_maps, a->nargs,
                   a->nmaps);
         return 1;
     }
@@ -626,7 +631,7 @@ int fdb_kernel_call(fdb_kernel_t k, const fdb_call_args *a)
         int rc = pipelined_host_action(k, a, nlay);
         if (rc >= 0) return rc;      // -1: not applicable, fall through to the monolithic path
     }
-    void *dargs[5];
+    void *dargs[6];
     const fdb_int *dmaps[3];
     const fdb_int *dsubset;
     if (device_pointers(a, mat != nullptr, dargs, dmaps, &dsubset)) return 1;
@@ -695,7 +700,7 @@ int fdb_kernel_call(fdb_kernel_t k, const fdb_call_args *a)
         break;
     default:
         rc = fdb_launch_stokes_action(k, a->start, a->end, nlay, dsubset, out, coords, x, (double *)dargs[3],
-                                      (const double *)dargs[4], dmaps[0], dmaps[1], dmaps[2]);
+                                      (const double *)dargs[4], coef, dmaps[0], dmaps[1], dmaps[2]);
     }
     if (rc) return rc;
     if (a->location == FDB_LOC_HOST && a->writeback) {

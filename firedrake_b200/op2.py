@@ -1391,6 +1391,12 @@ class Kernel:
     p*div(v)*dx - q*div(u)*dx`` with the velocity in vector CG_p (``degree`` = p, 2..4; ``cdim`` 3) and the
     pressure in scalar CG_{p-1}, read and written through a second map: a rank-1 action only, (INC, READ,
     READ, INC, READ) = (velocity output, coordinates, u, pressure output, p).
+
+    "navier_stokes" is the residual of steady incompressible Navier-Stokes on the same spaces, the Stokes
+    action with ``mu`` = nu plus ``inner(dot(grad(u), u), v)*dx``, with the arguments of "stokes".
+    "navier_stokes_jacobian" is its Gateaux derivative at the velocity u applied to (w, r), with u as the LAST
+    argument: (INC, READ, READ, INC, READ, READ) = (velocity output, coordinates, w, pressure output, r, u).
+    Neither is symmetric; both are rank-1 actions only.
     """
     form: str = "helmholtz"
     degree: int = 1
@@ -1431,7 +1437,8 @@ class Kernel:
             # refuses)
             if self.cdim == 1:
                 object.__setattr__(self, "cdim", 3)
-            object.__setattr__(self, "accesses", (INC, READ, READ, INC, READ))
+            acc = (INC, READ, READ, INC, READ) + ((READ,) if spec.coefficient else ())
+            object.__setattr__(self, "accesses", acc)
             return
         if spec and spec.residual:
             return          # (INC, READ, READ) whatever rank and diagonal say: the engine refuses them
@@ -1478,7 +1485,9 @@ _FORMS = {"helmholtz": _Form(_lib.FORM_HELMHOLTZ),
           "hyperelasticity": _Form(_lib.FORM_HYPERELASTICITY, residual=True, lame=True),
           "hyperelasticity_jacobian": _Form(_lib.FORM_HYPERELASTICITY_JACOBIAN, coefficient=True, lame=True),
           "advection_diffusion": _Form(_lib.FORM_ADVECTION_DIFFUSION, coefficient=True, coef_cdim=3),
-          "stokes": _Form(_lib.FORM_STOKES, pressure=True)}
+          "stokes": _Form(_lib.FORM_STOKES, pressure=True),
+          "navier_stokes": _Form(_lib.FORM_NAVIER_STOKES, residual=True, pressure=True),
+          "navier_stokes_jacobian": _Form(_lib.FORM_NAVIER_STOKES_JACOBIAN, coefficient=True, pressure=True)}
 _INTEGRALS = {"cell": _lib.INTEGRAL_CELL, "exterior_facet": _lib.INTEGRAL_EXTERIOR_FACET,
               "interior_facet": _lib.INTEGRAL_INTERIOR_FACET, "fused": _lib.INTEGRAL_FUSED}
 

@@ -189,7 +189,7 @@ enum fdb_form {
                                      diagonal  [d INC, coords, b]     (device mode)
                                      rank 2    [Mat, coords, b]  (row = test dof, column = trial dof)
                                    Never the DMMA element-matrix kernels (they assume symmetry).  */
-    FDB_FORM_STOKES = 10
+    FDB_FORM_STOKES = 10,
                                 /* Stokes flow on Taylor-Hood hexahedra: velocity u in vector CG_p
                                    (value size 3, AoS, maps[0]) and pressure p in scalar CG_{p-1}
                                    (one value per node, maps[2]) on the same cells,
@@ -207,6 +207,32 @@ enum fdb_form {
                                    layer offsets).  Rank 1 action only (not rank 2, not diagonal),
                                    device mode only, atomic or coloured scatter:
                                      action  [y_u INC, coords, u, y_p INC, p]
+                                             maps [V map, coord map, Q map]                       */
+    FDB_FORM_NAVIER_STOKES = 11,
+                                /* residual of steady incompressible Navier-Stokes on the Taylor-Hood
+                                   spaces of FDB_FORM_STOKES (NOT symmetric):
+                                     R((u, p); (v, q)) = nu*inner(grad u, grad v)*dx
+                                                         + beta*inner(u, v)*dx
+                                                         + inner(dot(grad u, u), v)*dx
+                                                         - p*div(v)*dx - q*div(u)*dx
+                                   nu = alpha, dot(grad u, u)_d = sum_k du_d/dx_k u_k.  The Stokes sign
+                                   convention: R at u = 0 is the Stokes action.  Same spaces, creation
+                                   (fdb_kernel_create_mixed) and restrictions as FDB_FORM_STOKES; the
+                                   convective term is not integrated exactly by the nq = p+1 rule.
+                                     action  [y_u INC, coords, u, y_p INC, p]
+                                             maps [V map, coord map, Q map]                       */
+    FDB_FORM_NAVIER_STOKES_JACOBIAN = 12
+                                /* its Gateaux derivative at the velocity u (exact Newton Jacobian, NOT
+                                   symmetric), applied to the direction (w, r):
+                                     J(u)[(w, r); (v, q)] = nu*inner(grad w, grad v)*dx
+                                                            + beta*inner(w, v)*dx
+                                                            + inner(dot(grad w, u), v)*dx
+                                                            + inner(dot(grad u, w), v)*dx
+                                                            - r*div(v)*dx - q*div(w)*dx
+                                   J at u = 0 is FDB_FORM_STOKES.  Same restrictions as FDB_FORM_STOKES.
+                                   The second space's arguments come first, then u, always the LAST
+                                   argument, read through maps[0]:
+                                     action  [y_u INC, coords, w, y_p INC, r, u]
                                              maps [V map, coord map, Q map]                       */
 };
 
@@ -275,7 +301,8 @@ typedef struct fdb_kernel_desc {
     double lmbda;
 } fdb_kernel_desc;
 
-/* The second space of a form on two spaces (FDB_FORM_STOKES: the pressure space), passed to
+/* The second space of a form on two spaces (FDB_FORM_STOKES, FDB_FORM_NAVIER_STOKES[_JACOBIAN]: the
+ * pressure space), passed to
  * fdb_kernel_create_mixed next to the descriptor of the first (argument) space, which keeps its
  * layout.  degree: the second space's polynomial degree (Stokes: the velocity degree minus 1);
  * B: its basis at the descriptor's nq Gauss points, row-major (nq, degree+1), 1-D dof numbering;
@@ -293,7 +320,8 @@ typedef struct fdb_kernel_s *fdb_kernel_t;
  * "compile" = validate the descriptor, precompute tables, pick the sm_90a
  * kernel instantiation.  Fails (nonzero) for forms outside the supported set. */
 int fdb_kernel_create(const fdb_kernel_desc *desc, fdb_kernel_t *out);
-/* The same for a form on two spaces (FDB_FORM_STOKES), which fdb_kernel_create refuses; a form on one
+/* The same for a form on two spaces (FDB_FORM_STOKES, FDB_FORM_NAVIER_STOKES[_JACOBIAN]), which
+ * fdb_kernel_create refuses; a form on one
  * space is refused here. */
 int fdb_kernel_create_mixed(const fdb_kernel_desc *desc, const fdb_space2_desc *space2, fdb_kernel_t *out);
 int fdb_kernel_destroy(fdb_kernel_t k);
