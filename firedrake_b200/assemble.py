@@ -1881,7 +1881,7 @@ def solve_nonlinear(F, L: op2.Dat, u: op2.Dat, bcs=(), solver_parameters=None, h
     Navier-Stokes (``F`` a :class:`NavierStokes`): ``L`` and ``u`` are MixedDats (velocity, pressure), the
     Dirichlet conditions are on the velocity, and the residual norm runs over both blocks.  Each step is
     matrix-free GMRES on ``F.jacobian(u)`` with the options of :func:`_solve_stokes`: ``mat_type`` "matfree",
-    ``pc_type`` "none" (default) or "fieldsplit" (schur, diag; ``fieldsplit_0_pc_type`` "jacobi" or "mg" on
+    ``pc_type`` "none" (default) or "fieldsplit" (schur, diag / lower / upper; ``fieldsplit_0_pc_type`` "jacobi" or "mg" on
     ``Form(W, nu, beta)`` per component, ``fieldsplit_1_pc_type`` "jacobi", the pressure mass over nu), built
     once per solve.  ``nullspace`` "constant" removes the pressure mean from the residual, from every
     preconditioned vector and from the final pressure.  A non-finite residual norm ends the solve with a
@@ -2094,7 +2094,9 @@ def _solve_stokes(form: Stokes, L: op2.MixedDat, up: op2.MixedDat, bcs=(), solve
     - ``mat_type`` "matfree" (the only one); ``ksp_type`` "gmres" (default; "cg" is refused, the operator is
       indefinite), ``ksp_gmres_restart`` (30), ``ksp_rtol`` (1e-8), ``ksp_max_it`` (1000).
     - ``pc_type`` "none" (default) or "fieldsplit" with ``pc_fieldsplit_type`` "schur" and
-      ``pc_fieldsplit_schur_fact_type`` "diag": z_u = P_0(r_u), z_p = P_1(r_p).
+      ``pc_fieldsplit_schur_fact_type`` "diag": z_u = P_0(r_u), z_p = P_1(r_p); "lower" or "upper": PETSc's
+      block-triangular factorisations with S^-1 ~ -P_1, one extra Stokes action per application
+      (:func:`_schur_factorisation`).
       ``fieldsplit_0_pc_type`` "jacobi" (default: the inverse diagonal of the velocity block) or "mg" (one
       V-cycle of ``Form(W, mu, beta)`` on the vector spaces of ``hierarchy``, with the velocity conditions'
       sub-domains); ``fieldsplit_1_pc_type`` "jacobi" (default): the inverse diagonal of the Schur complement
@@ -2158,18 +2160,21 @@ def _solve_stokes(form: Stokes, L: op2.MixedDat, up: op2.MixedDat, bcs=(), solve
     return its, hist
 
 
+_SCHUR_FACTORISATIONS = ("diag", "lower", "upper")
+
+
 def _check_fieldsplit(sp, hierarchy):
     """The preconditioner options of the Taylor-Hood solves (:func:`_solve_stokes`, Newton on
-    :class:`NavierStokes`): ``pc_type`` "none" or the diagonal Schur fieldsplit."""
+    :class:`NavierStokes`): ``pc_type`` "none" or the Schur fieldsplit, factorised "diag", "lower" or "upper"."""
     pc = sp["pc_type"]
     if pc not in ("none", "fieldsplit"):
         raise NotImplementedError(f"pc_type {pc!r}: 'none' or 'fieldsplit'")
     if pc == "fieldsplit":
         if sp.get("pc_fieldsplit_type") != "schur":
             raise NotImplementedError(f"pc_fieldsplit_type {sp.get('pc_fieldsplit_type')!r}: 'schur' only")
-        if sp.get("pc_fieldsplit_schur_fact_type") != "diag":
+        if sp.get("pc_fieldsplit_schur_fact_type") not in _SCHUR_FACTORISATIONS:
             raise NotImplementedError(f"pc_fieldsplit_schur_fact_type {sp.get('pc_fieldsplit_schur_fact_type')!r}: "
-                                      f"'diag' only")
+                                      f"not built ('diag' only, or 'lower' / 'upper')")
         for f in ("0", "1"):
             if sp[f"fieldsplit_{f}_ksp_type"] != "preonly":
                 raise NotImplementedError(f"fieldsplit_{f}_ksp_type {sp[f'fieldsplit_{f}_ksp_type']!r}: 'preonly' "
@@ -2194,10 +2199,11 @@ def _pressure_mean_remover(Q):
 
 def _fieldsplit_pc(V, Q, mu, beta, up, bcs, sp, hierarchy, remove_pressure_mean=None):
     """The preconditioner ``M(r, z)`` of the Taylor-Hood GMRES solves (None: none), from the options that
-    :func:`_check_fieldsplit` accepted.  The diagonal Schur fieldsplit preconditions the velocity with Jacobi
-    or one V-cycle per component of ``Form(W, mu, beta)`` and the pressure with the inverse diagonal of
-    (1/mu) M_p.  It does not depend on the velocity, so one is built per solve.  ``remove_pressure_mean``
-    (the constant nullspace) is applied to every preconditioned vector."""
+    :func:`_check_fieldsplit` accepted.  The Schur fieldsplit preconditions the velocity with Jacobi or one
+    V-cycle per component of ``Form(W, mu, beta)`` and the pressure with the inverse diagonal of (1/mu) M_p,
+    combined "diag" or as the "lower" / "upper" factorisation (:func:`_schur_factorisation`).  It does not
+    depend on the velocity, so one is built per solve.  ``remove_pressure_mean`` (the constant nullspace) is
+    applied to every preconditioned vector."""
     from . import _lib
     from . import mg as _mg
     lib = _lib.lib()
@@ -2241,15 +2247,70 @@ def _fieldsplit_pc(V, Q, mu, beta, up, bcs, sp, hierarchy, remove_pressure_mean=
                     _lib.check(lib.fdb_vec_scatter(nn, comp[c].ptr, zs.device_ptr, z.device_ptr))
                 z._device_written()
 
-        def M(r, z):
-            Mu(r[0], z[0])
-            _lib.check(lib.fdb_vec_pointwise_mult(n_p, r[1].device_ptr, dp.device_ptr, z[1].device_ptr))
-            z[1]._device_written()
-            if nullspace:
-                remove_pressure_mean(z)
+        def Mp(r, z):
+            _lib.check(lib.fdb_vec_pointwise_mult(n_p, r.device_ptr, dp.device_ptr, z.device_ptr))
+            z._device_written()
+
+        fact = sp["pc_fieldsplit_schur_fact_type"]
+        if fact == "diag":
+            def M(r, z):
+                Mu(r[0], z[0])
+                Mp(r[1], z[1])
+                if nullspace:
+                    remove_pressure_mean(z)
+        else:
+            # the off-diagonal blocks B and B^T do not depend on u, so the Stokes operator with the velocity
+            # conditions applies them for both solves (cheaper than the Navier-Stokes Jacobian action)
+            S = Stokes(V, Q, mu, beta)
+            M = _schur_factorisation(fact, Mu, Mp, StokesMatrixContext(S, bcs), S.dat, remove_pressure_mean)
     elif nullspace:
         def M(r, z):
             r.copy(z)
+            remove_pressure_mean(z)
+    return M
+
+
+def _schur_factorisation(fact, Mu, Mp, A, new, remove_pressure_mean=None):
+    """``M(r, z)`` of the "lower" or "upper" Schur factorisation (PETSc's ``pc_fieldsplit_schur_fact_type``) of
+    the Taylor-Hood operator A = [[F, B^T], [B, 0]], whose pressure rows are -q div u.  ``Mu(r_u, z_u)`` applies
+    P_0 ~ F^-1 and ``Mp(r_p, z_p)`` applies P_1 ~ (B F^-1 B^T)^-1; the Schur complement is S = -B F^-1 B^T, so
+    S^-1 ~ -P_1 (the "diag" factorisation applies +P_1, PETSc's schur_scale -1):
+
+    - "lower", the inverse of [[F, 0], [B, S]]: z_u = P_0 r_u, then z_p = -P_1 (r_p - B z_u);
+    - "upper", the inverse of [[F, B^T], [0, S]]: z_p = -P_1 r_p, then z_u = P_0 (r_u - B^T z_p).
+
+    ``A.mult`` applies the operator with the velocity conditions: B z_u is the pressure block of A (z_u, 0) and
+    B^T z_p the velocity block of A (0, z_p), zero on the constrained rows.  One extra action of A per
+    application.  ``new()`` makes a MixedDat of the two spaces for the work vectors.  ``remove_pressure_mean``
+    (the constant nullspace) is applied to every preconditioned vector."""
+    from . import _lib
+    lib = _lib.lib()
+    w, y = new(), new()
+
+    def negate(v):
+        _lib.check(lib.fdb_vec_scale(v._data.size, -1.0, v.device_ptr))
+        v._device_written()
+
+    def M(r, z):
+        if fact == "lower":
+            Mu(r[0], z[0])
+            z[0].copy(w[0])
+            w[1].zero()
+            A.mult(w, y)
+            r[1].copy(w[1])
+            w[1].axpy(-1.0, y[1])
+            Mp(w[1], z[1])
+            negate(z[1])
+        else:
+            Mp(r[1], z[1])
+            negate(z[1])
+            w[0].zero()
+            z[1].copy(w[1])
+            A.mult(w, y)
+            r[0].copy(w[0])
+            w[0].axpy(-1.0, y[0])
+            Mu(w[0], z[0])
+        if remove_pressure_mean is not None:
             remove_pressure_mean(z)
     return M
 
