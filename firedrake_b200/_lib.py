@@ -26,6 +26,7 @@ FORM_ADVECTION_DIFFUSION = 9
 FORM_STOKES = 10
 FORM_NAVIER_STOKES = 11
 FORM_NAVIER_STOKES_JACOBIAN = 12
+FORM_BOUNDARY_MASS = 13
 CELL_HEX_EXTRUDED = 1
 CELL_HEX = 2
 CELL_TRIANGLE = 3

@@ -823,6 +823,86 @@ def assemble_advection_diffusion_generic(V: "FunctionSpace", u: op2.Dat, b: op2.
     return tensor
 
 
+def boundary_mass_kernel(degree, gamma=1.0, cdim=1, rank=1, name=None):
+    """C source of the exterior-facet form ``gamma*inner(u, v)*ds`` on Q_p (x) P_p hexes with trilinear
+    geometry, written the way TSFC would (the whole cell's basis at every facet point, the surface measure
+    |dx/dxi_s x dx/dxi_t| of the facet), for the generic wrapper builder: the independent statement of the
+    hand-written FDB_FORM_BOUNDARY_MASS kernel.  ``rank`` 1: the action, arguments y (INC), coords, u,
+    facet; ``rank`` 2: the element matrix (cdim blocks), arguments A, coords, facet.  ``facet`` is the
+    uint32 local facet number 2*direction + side (firedrake_loopy.py:317-381)."""
+    from .codegen import CStringKernel
+    from .fiat_lite import interval_element
+    if cdim not in (1, 3) or rank not in (1, 2):
+        raise ValueError("boundary_mass_kernel: cdim 1 or 3, rank 1 or 2")
+    el = interval_element(degree)
+    n, nd = degree + 1, (degree + 1) ** 3
+    Bend, _ = el.tabulate([0.0, 1.0])
+    tab = lambda a: "{" + ", ".join("{" + ", ".join(repr(float(v)) for v in r) + "}" for r in a) + "}"
+    vec = lambda a: "{" + ", ".join(repr(float(v)) for v in a) + "}"
+    name = name or f"boundary_mass{rank}_c{cdim}"
+    if rank == 1:
+        sig = "double *A, const double *X, const double *u, const unsigned int *facet"
+        body = f"""for (int c = 0; c < {cdim}; ++c) {{
+            double v = 0.0;
+            for (int i = 0; i < {nd}; ++i) v += phi[i] * u[i * {cdim} + c];
+            for (int i = 0; i < {nd}; ++i) A[i * {cdim} + c] += wd * phi[i] * v;
+        }}"""
+    else:
+        sig = "double *A, const double *X, const unsigned int *facet"
+        body = f"""for (int i = 0; i < {nd}; ++i) for (int j = 0; j < {nd}; ++j)
+            for (int c = 0; c < {cdim}; ++c) A[(i * {cdim} + c) * {nd * cdim} + j * {cdim} + c] += wd * phi[i] * phi[j];"""
+    code = f"""
+static const double MB[{n}][{n}] = {tab(el.B)};      /* basis a at Gauss point q: MB[q][a] */
+static const double ME[2][{n}] = {tab(Bend)};        /* basis at the interval's ends */
+static const double MX[{n}] = {vec(el.xq)};
+static const double MW[{n}] = {vec(el.wq)};
+static void {name}({sig})
+{{
+    const int fd = (int)facet[0] / 2, fs = (int)facet[0] % 2;     /* normal direction, side */
+    const int d1 = fd == 0 ? 1 : 0, d2 = fd == 2 ? 1 : 2;           /* tangential directions */
+    for (int q1 = 0; q1 < {n}; ++q1) for (int q2 = 0; q2 < {n}; ++q2) {{
+        double xi[3], J[3][3], phi[{nd}];
+        const double *T[3];
+        xi[fd] = (double)fs; xi[d1] = MX[q1]; xi[d2] = MX[q2];
+        T[fd] = ME[fs]; T[d1] = MB[q1]; T[d2] = MB[q2];
+        for (int c = 0; c < 3; ++c) for (int d = 0; d < 3; ++d) J[c][d] = 0.0;
+        for (int v = 0; v < 8; ++v) {{
+            const int b[3] = {{(v >> 2) & 1, (v >> 1) & 1, v & 1}};
+            for (int d = 0; d < 3; ++d) {{
+                double g = b[d] ? 1.0 : -1.0;
+                for (int e = 0; e < 3; ++e) if (e != d) g *= b[e] ? xi[e] : 1.0 - xi[e];
+                for (int c = 0; c < 3; ++c) J[c][d] += X[v * 3 + c] * g;
+            }}
+        }}
+        const double cx = J[1][d1] * J[2][d2] - J[2][d1] * J[1][d2];
+        const double cy = J[2][d1] * J[0][d2] - J[0][d1] * J[2][d2];
+        const double cz = J[0][d1] * J[1][d2] - J[1][d1] * J[0][d2];
+        const double wd = {float(gamma)!r} * MW[q1] * MW[q2] * sqrt(cx * cx + cy * cy + cz * cz);
+        for (int a = 0; a < {n}; ++a) for (int b = 0; b < {n}; ++b) for (int c = 0; c < {n}; ++c)
+            phi[(a * {n} + b) * {n} + c] = T[0][a] * T[1][b] * T[2][c];
+        {body}
+    }}
+}}
+"""
+    return CStringKernel(code, name)
+
+
+def assemble_boundary_mass_generic(V: "FunctionSpace", u: op2.Dat, gamma=1.0, sub_domain="on_boundary", tensor=None):
+    """``assemble(action(gamma*inner(u, v)*ds(sub_domain), u))`` through the generic wrapper path
+    (:func:`boundary_mass_kernel`) over the same facet sets as :class:`BoundaryMass`: the cross-check and
+    the baseline of the hand-written kernel."""
+    from . import codegen
+    if tensor is None:
+        tensor = V.dat()
+    tensor.zero()
+    tensor.device_ptr
+    k = boundary_mass_kernel(V.degree, gamma, V.cdim)
+    for fset, fmap, cmap, facet in _boundary_groups(V, sub_domain):
+        codegen.par_loop(k, fset, tensor(op2.INC, fmap), V.coordinates(op2.READ, cmap), u(op2.READ, fmap),
+                         facet(op2.READ))
+    return tensor
+
+
 def hyperelasticity_kernel(degree, mu, lmbda, beta=0.0, jacobian=False, name=None):
     """C source of the residual of compressible Neo-Hookean hyperelasticity,
     ``inner(P(F), grad(v))*dx + beta*inner(u, v)*dx`` with ``F = I + grad(u)``, ``J = det(F)`` and
@@ -1060,17 +1140,166 @@ class DirichletBC:
         return lg
 
 
+_BOUNDARY_SUB_DOMAINS = (1, 2, 3, 4, "bottom", "top")
+
+
+def _same_name(a, b):
+    return type(a) is type(b) and a == b
+
+
+def _boundary_sub_domains(sub_domain):
+    """The sub-domain names of ``ds(sub_domain)`` in canonical order: those :class:`DirichletBC` takes (1..4 =
+    x == 0, x == Lx, y == 0, y == Ly; "bottom", "top"; a tuple of them), or "on_boundary" for all six."""
+    if isinstance(sub_domain, str) and sub_domain == "on_boundary":
+        return _BOUNDARY_SUB_DOMAINS
+    subs = sub_domain if isinstance(sub_domain, (list, tuple)) else (sub_domain,)
+    for s in subs:
+        if not any(_same_name(s, t) for t in _BOUNDARY_SUB_DOMAINS):
+            raise ValueError(f"unknown sub_domain {s!r}: 1..4, 'bottom', 'top' or 'on_boundary'")
+    return tuple(t for t in _BOUNDARY_SUB_DOMAINS if any(_same_name(s, t) for s in subs))
+
+
+def _boundary_groups(V: "FunctionSpace", sub_domain):
+    """The exterior facets of ``ds(sub_domain)`` on ``V`` as iteration groups ``(facet set, V map, coordinate
+    map, local facet numbers)``, built once per space and sub-domain and cached on the space.  Vertical facets
+    (sides 1..4) are the base mesh's exterior facets x all layers, as for ``ds_v``; horizontal ones are the base
+    columns with one cell layer and the maps of the bottom cells ("bottom", facet 4) or of the top cells, whose
+    rows are the bottom rows shifted by (nz - 1) * offset ("top", facet 5).  Facet dofs are cell dofs, so the
+    maps are the owning cells' rows and every matrix entry lies in the cell sparsity."""
+    if V.dof_dset.halo is not None or V.cell_set.owner_computes:
+        raise NotImplementedError("boundary terms on a partitioned space are not implemented: the exec-halo columns "
+                                  "would count their facets twice")
+    subs = _boundary_sub_domains(sub_domain)
+    cache = V.__dict__.setdefault("_boundary_facets", {})
+    if subs in cache:
+        return cache[subs]
+    mesh, W = V.mesh, V.V
+    cmap, off = W.cell_node_map.astype(np.int64), np.asarray(W.offset, dtype=np.int64)
+    xmap, xoff = mesh.coord_map.astype(np.int64), np.asarray(mesh.coord_offset, dtype=np.int64)
+    groups = []
+
+    def group(layers, rows, xrows, local):
+        fset = op2.ExtrudedSet(op2.Set(len(local)), layers)
+        groups.append((fset,
+                       op2.Map(fset, V.node_set, W.arity, np.ascontiguousarray(rows, dtype=np.int32), offset=W.offset),
+                       op2.Map(fset, V.vertex_set, 8, np.ascontiguousarray(xrows, dtype=np.int32),
+                               offset=mesh.coord_offset),
+                       op2.Dat(op2.DataSet(fset, 1), np.ascontiguousarray(local, dtype=np.uint32), dtype=np.uint32)))
+
+    sides = [s for s in subs if not isinstance(s, str)]
+    if sides:
+        cells, local = mesh.exterior_vertical_facets()
+        keep = np.isin(local, np.array(sides, dtype=np.uint32) - 1)
+        if keep.any():
+            group(mesh.layers, cmap[cells[keep]], xmap[cells[keep]], local[keep])
+    horiz = [(4, 0) if s == "bottom" else (5, mesh.nz - 1) for s in subs if isinstance(s, str)]
+    if horiz:
+        nb = mesh.num_base_cells
+        group(2, np.concatenate([cmap + off[None, :] * shift for _, shift in horiz]),
+              np.concatenate([xmap + xoff[None, :] * shift for _, shift in horiz]),
+              np.concatenate([np.full(nb, f, dtype=np.uint32) for f, _ in horiz]))
+    cache[subs] = groups
+    return groups
+
+
+def _boundary_kernel(V, gamma, rank, diagonal=False):
+    if V.cdim not in (1, 3):
+        raise NotImplementedError(f"boundary terms take scalar spaces or vector spaces of 3 components, got cdim "
+                                  f"{V.cdim}")
+    return op2.Kernel("boundary_mass", degree=V.degree, alpha=float(gamma), cdim=V.cdim, rank=rank,
+                      diagonal=diagonal, integral="exterior_facet")
+
+
+def _check_ds(form):
+    """Validate a form's ``ds`` terms ((gamma, sub_domain) pairs) and build their facet sets."""
+    for term in form.ds:
+        if not isinstance(term, (tuple, list)) or len(term) != 2:
+            raise ValueError(f"ds holds (gamma, sub_domain) pairs, got {term!r}")
+        _boundary_groups(form.V, term[1])
+
+
+class _BoundaryTerms:
+    """The exterior-facet parloops of sum_k gamma_k*inner(u, v)*ds(sub_domain_k) on ``V``: one hand-written
+    FDB_FORM_BOUNDARY_MASS loop per term and facet group, added into the same output as the cell loop."""
+
+    def __init__(self, V: "FunctionSpace", ds):
+        self.V = V
+        self.terms = [(float(g), _boundary_groups(V, s)) for g, s in ds]
+
+    def action_loops(self, tensor: op2.Dat, u: op2.Dat, scatter="atomic"):
+        V, loops = self.V, []
+        for gamma, groups in self.terms:
+            for fset, fmap, cmap, facet in groups:
+                gk = op2.GlobalKernel(_boundary_kernel(V, gamma, 1), [fmap, cmap], extruded=True, scatter=scatter)
+                loops.append(op2.Parloop(gk, fset, [tensor(op2.INC, fmap), V.coordinates(op2.READ, cmap),
+                                                    u(op2.READ, fmap), facet(op2.READ)], location="device"))
+        return loops
+
+    def diagonal(self, D: op2.Dat):
+        V = self.V
+        for gamma, groups in self.terms:
+            for fset, fmap, cmap, facet in groups:
+                op2.par_loop(_boundary_kernel(V, gamma, 1, diagonal=True), fset, D(op2.INC, fmap),
+                             V.coordinates(op2.READ, cmap), facet(op2.READ))
+
+    def matrix(self, tensor: op2.Mat, lg):
+        V = self.V
+        for gamma, groups in self.terms:
+            for fset, fmap, cmap, facet in groups:
+                op2.par_loop(_boundary_kernel(V, gamma, 2), fset, tensor(op2.INC, (fmap, fmap), lgmaps=lg),
+                             V.coordinates(op2.READ, cmap), facet(op2.READ))
+
+
+@dataclass
+class BoundaryMass:
+    """gamma*inner(u, v)*ds(sub_domain) on ``V`` (scalar, or vector with 3 components): a symmetric bilinear form
+    that lives on exterior facets only.  ``sub_domain`` takes the names :class:`DirichletBC` takes (1..4,
+    "bottom", "top", a tuple of them) and "on_boundary" for the whole boundary.
+
+    Its action gives the boundary loads: ``assemble(BoundaryMass(V, 1.0, 2), u=g)`` is ``inner(g, v)*ds(2)``, a
+    Neumann flux for a scalar g, a traction for a vector g, and ``assemble(BoundaryMass(V, h, 2), u=u_inf)`` the
+    right-hand side of a Robin condition whose operator term is ``ds=((h, 2),)`` on the volume form.
+    ``assemble(F)`` gives an aij Mat (degrees 1..4), ``mat_type="matfree"`` an operator with its diagonal
+    (degrees 1..5).  Partitioned spaces are refused."""
+    V: FunctionSpace
+    gamma: float = 1.0
+    sub_domain: object = "on_boundary"
+    symmetric = True
+    cell_integral = False       # no dx term: only the ds loops run
+
+    def __post_init__(self):
+        _check_ds(self)
+
+    @property
+    def ds(self):
+        return ((self.gamma, self.sub_domain),)
+
+    def coefficient_args(self):
+        return []
+
+    def kernel(self, rank, diagonal=False):
+        return _boundary_kernel(self.V, self.gamma, rank, diagonal)
+
+
 @dataclass
 class Form:
     """alpha*inner(grad(u), grad(v))*dx + beta*inner(u, v)*dx on ``V``.
 
     With ``kappa`` (a scalar Dat on ``V``): alpha*inner(kappa*grad(u), grad(v))*dx +
     beta*inner(u, v)*dx -- a heterogeneous material, or the Jacobian of a nonlinear diffusion
-    problem at the current iterate.  Runs on the hand-written coefficient kernel (scalar spaces)."""
+    problem at the current iterate.  Runs on the hand-written coefficient kernel (scalar spaces).
+
+    ``ds``: boundary terms added to the operator, a tuple of ``(gamma, sub_domain)`` pairs, each
+    ``gamma*inner(u, v)*ds(sub_domain)`` (a Robin condition's operator term; see :class:`BoundaryMass`)."""
     V: FunctionSpace
     alpha: float = 1.0
     beta: float = 0.0
     kappa: op2.Dat | None = None
+    ds: tuple = ()
+
+    def __post_init__(self):
+        if self.ds:
+            _check_ds(self)
 
     def coefficient_args(self):
         """The parloop arguments that follow the coordinates: kappa, read through the argument map."""
@@ -1098,12 +1327,18 @@ class NonlinearDiffusion:
 
     ``assemble(F, u=u)`` is the vector R(u); the problem F(u; v) = inner(f, v)*dx is solved by
     :func:`solve_nonlinear` with ``L = assemble(mass(V), u=f)``.  D(u) is evaluated at each Gauss point
-    from the interpolated u, as TSFC evaluates a coefficient expression."""
+    from the interpolated u, as TSFC evaluates a coefficient expression.  ``ds``: linear boundary terms
+    ``gamma*inner(u, v)*ds(sub_domain)`` (e.g. Robin cooling), in the residual and in its Jacobian."""
     V: FunctionSpace
     alpha: float = 1.0
     beta: float = 0.0
     d: tuple = (1.0, 0.0, 0.0)
+    ds: tuple = ()
     symmetric = False
+
+    def __post_init__(self):
+        if self.ds:
+            _check_ds(self)
 
     def coefficient_args(self):
         return []
@@ -1118,7 +1353,7 @@ class NonlinearDiffusion:
 
     def jacobian(self, u0: op2.Dat):
         """The Gateaux derivative at ``u0`` (the exact Newton Jacobian, a bilinear form)."""
-        return NonlinearDiffusionJacobian(self.V, self.alpha, self.beta, tuple(self.d), u0)
+        return NonlinearDiffusionJacobian(self.V, self.alpha, self.beta, tuple(self.d), u0, self.ds)
 
     def diffusivity(self, u: op2.Dat, target: op2.Dat = None):
         """D(u) at the nodes of ``V`` (a pointwise node loop): the coefficient of the SPD operator
@@ -1142,6 +1377,7 @@ class NonlinearDiffusionJacobian:
     beta: float
     d: tuple
     u0: op2.Dat
+    ds: tuple = ()
     symmetric = False
 
     def coefficient_args(self):
@@ -1165,12 +1401,19 @@ class Elasticity:
     ``assemble(F, u=w)`` (action, degrees 1..4), ``assemble(F)`` (a blocked aij Mat of block size 3,
     degrees 1..3), ``assemble(F, mat_type="matfree")`` and :func:`solve` with ``pc_type`` "none",
     "jacobi" or "mg" (the coarse operators are ``Elasticity(W, mu, lmbda, beta)`` on the coarser
-    levels).  Dirichlet conditions constrain every component of their nodes."""
+    levels).  Dirichlet conditions constrain every component of their nodes.  ``ds``: boundary terms
+    ``gamma*inner(u, v)*ds(sub_domain)`` added to the operator (elastic supports); a traction load is
+    ``assemble(BoundaryMass(V, 1.0, sub_domain), u=t)``."""
     V: FunctionSpace
     mu: float
     lmbda: float
     beta: float = 0.0
+    ds: tuple = ()
     symmetric = True
+
+    def __post_init__(self):
+        if self.ds:
+            _check_ds(self)
 
     def coefficient_args(self):
         return []
@@ -1193,12 +1436,18 @@ class HyperElasticity:
 
     ``assemble(F, u=u)`` is the vector R(u) (degrees 1..4); the problem R(u; v) = inner(f, v)*dx is
     solved by :func:`solve_nonlinear`.  At u = 0 its Jacobian is ``Elasticity(V, mu, lmbda, beta)``.  A
-    point with J <= 0 (an inverted element) makes ln(J) and the residual NaN, as in Firedrake."""
+    point with J <= 0 (an inverted element) makes ln(J) and the residual NaN, as in Firedrake.  ``ds``: linear
+    boundary terms ``gamma*inner(u, v)*ds(sub_domain)``, in the residual and in its Jacobian."""
     V: FunctionSpace
     mu: float
     lmbda: float
     beta: float = 0.0
+    ds: tuple = ()
     symmetric = True
+
+    def __post_init__(self):
+        if self.ds:
+            _check_ds(self)
 
     def coefficient_args(self):
         return []
@@ -1213,7 +1462,7 @@ class HyperElasticity:
 
     def jacobian(self, u0: op2.Dat):
         """The Gateaux derivative at ``u0`` (the exact Newton Jacobian, a symmetric bilinear form)."""
-        return HyperElasticityJacobian(self.V, self.mu, self.lmbda, self.beta, u0)
+        return HyperElasticityJacobian(self.V, self.mu, self.lmbda, self.beta, u0, self.ds)
 
 
 @dataclass
@@ -1227,6 +1476,7 @@ class HyperElasticityJacobian:
     lmbda: float
     beta: float
     u0: op2.Dat
+    ds: tuple = ()
     symmetric = True
 
     def coefficient_args(self):
@@ -1254,11 +1504,14 @@ class AdvectionDiffusion:
     b: op2.Dat
     alpha: float = 1.0
     beta: float = 0.0
+    ds: tuple = ()
     symmetric = False
 
     def __post_init__(self):
         if self.b.cdim != 3:
             raise ValueError(f"the velocity b has 3 values per node (V.vector_dset(3)), got {self.b.cdim}")
+        if self.ds:
+            _check_ds(self)
 
     def coefficient_args(self):
         return [self.b(op2.READ, self.V.cell_node_map)]
@@ -1289,9 +1542,11 @@ class Stokes:
     Q: FunctionSpace
     mu: float = 1.0
     beta: float = 0.0
+    ds: tuple = ()
     symmetric = True
 
     def __post_init__(self):
+        _refuse_taylor_hood_ds(self.ds, "Stokes")
         self.pressure_map = _taylor_hood_pressure_map(self.V, self.Q, "Stokes")
 
     def dat(self, u=None, p=None):
@@ -1306,6 +1561,12 @@ class Stokes:
             raise NotImplementedError("Stokes is an action only: there is no assembled matrix or diagonal "
                                       "(use mat_type='matfree')")
         return op2.Kernel("stokes", degree=self.V.degree, mu=self.mu, beta=self.beta)
+
+
+def _refuse_taylor_hood_ds(ds, what):
+    if ds:
+        raise NotImplementedError(f"boundary terms on the {what} form are not implemented: a velocity Robin or "
+                                  f"slip term needs the fused saddle-point kernel to carry facet integrals")
 
 
 def _taylor_hood_pressure_map(V, Q, what):
@@ -1343,9 +1604,11 @@ class NavierStokes:
     Q: FunctionSpace
     nu: float = 1.0
     beta: float = 0.0
+    ds: tuple = ()
     symmetric = False
 
     def __post_init__(self):
+        _refuse_taylor_hood_ds(self.ds, "Navier-Stokes")
         self.pressure_map = _taylor_hood_pressure_map(self.V, self.Q, "Navier-Stokes")
 
     def dat(self, u=None, p=None):
@@ -1491,23 +1754,33 @@ class OneFormAssembler:
     def __init__(self, form: Form, u: op2.Dat, bcs=(), scatter="atomic"):
         self.form, self.u, self.bcs = form, u, tuple(bcs)
         V = form.V
+        # a BoundaryMass form has no cell integral; the ds terms of a form add facet loops after the cell loop
         self._gk = op2.GlobalKernel(form.kernel(1), [V.cell_node_map, V.coord_map], extruded=True,
-                                    scatter=scatter)
+                                    scatter=scatter) if getattr(form, "cell_integral", True) else None
+        ds = getattr(form, "ds", ())
+        self._ds = _BoundaryTerms(V, ds) if ds else None
+        self._scatter = scatter
         self._loop = None
+        self._tensor = None
 
     def assemble(self, tensor=None):
         V = self.form.V
         if tensor is None:
             tensor = V.dat()
-        if self._loop is None or self._tensor is not tensor:
+        if self._tensor is not tensor:
             self._tensor = tensor
-            self._loop = op2.Parloop(self._gk, V.cell_set,
-                                     [tensor(op2.INC, V.cell_node_map),
-                                      V.coordinates(op2.READ, V.coord_map),
-                                      self.u(op2.READ, V.cell_node_map)] + self.form.coefficient_args(),
-                                     location="device")
+            if self._gk is not None:
+                self._loop = op2.Parloop(self._gk, V.cell_set,
+                                         [tensor(op2.INC, V.cell_node_map),
+                                          V.coordinates(op2.READ, V.coord_map),
+                                          self.u(op2.READ, V.cell_node_map)] + self.form.coefficient_args(),
+                                         location="device")
+            self._ds_loops = self._ds.action_loops(tensor, self.u, self._scatter) if self._ds else []
         tensor.zero()
-        self._loop()
+        if self._loop is not None:
+            self._loop()
+        for loop in self._ds_loops:
+            loop()
         for bc in self.bcs:
             bc.zero(tensor)
         return tensor
@@ -1551,9 +1824,13 @@ def assemble(form: Form, u=None, tensor=None, bcs=(), mat_type="aij"):
             lgm[bc.nodes, :] = -1
         lgm = np.ascontiguousarray(lgm.ravel())
         lg = (lgm, lgm)
-    op2.par_loop(form.kernel(2), V.cell_set,
-                 tensor(op2.INC, (V.cell_node_map, V.cell_node_map), lgmaps=lg),
-                 V.coordinates(op2.READ, V.coord_map), *form.coefficient_args())
+    if getattr(form, "cell_integral", True):
+        op2.par_loop(form.kernel(2), V.cell_set,
+                     tensor(op2.INC, (V.cell_node_map, V.cell_node_map), lgmaps=lg),
+                     V.coordinates(op2.READ, V.coord_map), *form.coefficient_args())
+    if getattr(form, "ds", ()):
+        # facet dofs are cell dofs: the facet element matrices go into the same Mat and pattern
+        _BoundaryTerms(V, form.ds).matrix(tensor, lg)
     owned = V.node_set.size
     for bc in bcs:
         # on a partitioned space a constrained node gets its unit diagonal from its OWNER only:
@@ -1607,7 +1884,9 @@ class ImplicitMatrixContext:
         """``assemble(a, diagonal=True)`` then 1 on the constrained rows
         (matrix_free/operators.py:199-205; firedrake/assemble.py:1226-1241)."""
         V = self.form.V
-        if self.form.coefficient_args() or not isinstance(self.form, Form):
+        if not getattr(self.form, "cell_integral", True):
+            k = None                        # BoundaryMass: the ds loops only
+        elif self.form.coefficient_args() or not isinstance(self.form, Form):
             # coefficient forms (kappa, a Jacobian's linearisation point) and elasticity have their own
             # diagonal kernel
             k = self.form.kernel(1, diagonal=True)
@@ -1615,8 +1894,11 @@ class ImplicitMatrixContext:
             k = op2.Kernel("helmholtz", degree=V.degree, alpha=self.form.alpha, beta=self.form.beta,
                            diagonal=True)
         D.zero()
-        op2.par_loop(k, V.cell_set, D(op2.INC, V.cell_node_map), V.coordinates(op2.READ, V.coord_map),
-                     *self.form.coefficient_args())
+        if k is not None:
+            op2.par_loop(k, V.cell_set, D(op2.INC, V.cell_node_map), V.coordinates(op2.READ, V.coord_map),
+                         *self.form.coefficient_args())
+        if getattr(self.form, "ds", ()):
+            _BoundaryTerms(V, self.form.ds).diagonal(D)
         for bc in self.bcs:
             bc.set(D, 1.0)
         return D
@@ -1961,11 +2243,11 @@ def solve_nonlinear(F, L: op2.Dat, u: op2.Dat, bcs=(), solver_parameters=None, h
             if hyper:
                 # J(0) = Elasticity: the same operator at every Newton step, so one V-cycle per solve
                 if vc is None:
-                    vc = _mg.VCycle(hierarchy, V.degree, lambda W, k=None: Elasticity(W, F.mu, F.lmbda, F.beta),
+                    vc = _mg.VCycle(hierarchy, V.degree, lambda W, k=None: Elasticity(W, F.mu, F.lmbda, F.beta, F.ds),
                                     bc_domains=domains, allreduce=allreduce, cdim=3, omega=0.6)
             else:
                 kap = F.diffusivity(u)
-                vc = _mg.VCycle(hierarchy, V.degree, lambda W, k=None: Form(W, F.alpha, F.beta, k),
+                vc = _mg.VCycle(hierarchy, V.degree, lambda W, k=None: Form(W, F.alpha, F.beta, k, F.ds),
                                 bc_domains=domains, allreduce=allreduce, kappa=kap)
             top = len(hierarchy) - 1
             M = lambda r, z, vc=vc: vc.apply(top, r, z)
@@ -2058,11 +2340,13 @@ def solve(form: Form, L: op2.Dat, u: op2.Dat, bcs=(), solver_parameters=None, hi
             # 97 iterations on 8^3 and 16^3 with 0.8, 8 and 9 with 0.6 (DESIGN.md section 4.8)
             # advection-diffusion: a V-cycle of its symmetric part Form(W, alpha, beta) on every level (the
             # convective term is left to the outer GMRES, DESIGN.md section 4.10)
+            # boundary terms: the same (gamma, sub_domain) pairs on every level (the names are mesh-level)
+            ds = getattr(form, "ds", ())
             if isinstance(form, Elasticity):
-                make = lambda W, k=None: Elasticity(W, form.mu, form.lmbda, form.beta)
+                make = lambda W, k=None: Elasticity(W, form.mu, form.lmbda, form.beta, ds)
                 omega = 0.6
             else:
-                make = lambda W, k=None: Form(W, form.alpha, form.beta, k)
+                make = lambda W, k=None: Form(W, form.alpha, form.beta, k, ds)
                 omega = 0.8
             vc = _mg.VCycle(hierarchy, V.degree, make,
                             bc_domains=tuple(s for bc in bcs for s in bc.sub_domains), allreduce=allreduce,

@@ -150,3 +150,9 @@ int fdb_launch_elasticity_matrix(fdb_kernel_s *k, fdb_int start, fdb_int end, in
 int fdb_launch_stokes_action(fdb_kernel_s *k, fdb_int start, fdb_int end, int nlay, const fdb_int *subset,
                              double *yu, const double *coords, const double *u, double *yp, const double *p,
                              const double *ulin, const fdb_int *map0, const fdb_int *map1, const fdb_int *map2);
+// FDB_FORM_BOUNDARY_MASS (boundary_hex.cu): one exterior facet per iteration entry, facet[col] its local facet
+// number.  mat != NULL: the element matrices into mat; else x != NULL: the action into y; else the diagonal
+// into y (cdim values per node, the same in each component)
+int fdb_launch_boundary_mass(fdb_kernel_s *k, fdb_int start, fdb_int end, int nlay, const fdb_int *subset,
+                             fdb_mat_t mat, double *y, const double *coords, const double *x, const unsigned *facet,
+                             const fdb_int *map0, const fdb_int *map1);

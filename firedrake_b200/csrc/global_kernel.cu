@@ -274,45 +274,52 @@ static int device_pointers(const fdb_call_args *a, bool mat, void **args, const 
 // The forms of the hand-written hex kernels: what fdb_kernel_create accepts for each and how
 // fdb_kernel_call hands its arguments to the launchers.
 enum { MODE_ACTION, MODE_MATRIX, MODE_DIAGONAL };
-enum { LAUNCH_HELMHOLTZ, LAUNCH_HELMHOLTZ_COEF, LAUNCH_ELASTICITY, LAUNCH_STOKES };
+enum { LAUNCH_HELMHOLTZ, LAUNCH_HELMHOLTZ_COEF, LAUNCH_ELASTICITY, LAUNCH_STOKES, LAUNCH_BOUNDARY };
 
 struct fdb_hex_form {
     int form;                 // enum fdb_form
     const char *name;
-    int cdim;                 // value size of the argument space; 0: any of 1..3, the diagonal scalar only
+    int cdim;                 // value size of the argument space; 0: any of 1..3, the diagonal scalar only;
+                              // -1: 1 or 3 in every mode
     bool affine;              // has the affine_cells variant
-    const char *coef;         // the trailing coefficient argument, or NULL
+    const char *coef;         // the trailing coefficient argument (an exterior-facet form: the uint32 local
+                              // facet number of each entry), or NULL
     int coef_cdim;            // its values per node (0 without one): the argument space's, or 3 for b
     bool residual;            // a 1-form action only
     int launcher;             // fdb_launch_helmholtz_*, fdb_launch_helmholtz_coef_* (which also run the
                               // nonlinear diffusion and advection-diffusion forms), fdb_launch_elasticity_*
-                              // or fdb_launch_stokes_action (which also runs the Navier-Stokes forms)
+                              // fdb_launch_stokes_action (which also runs the Navier-Stokes forms) or
+                              // fdb_launch_boundary_mass
     int max_degree[3];        // per mode: action, matrix, diagonal
     int min_degree;
     const char *space2;       // the arguments on a second space (output and input, through a third map), or
                               // NULL: such a form is an action only, in device mode
+    int integral;             // enum fdb_integral: FDB_INTEGRAL_EXTERIOR_FACET forms run in device mode only
 };
 
 static const fdb_hex_form hex_forms[] = {
-    {FDB_FORM_HELMHOLTZ, "helmholtz", 0, true, nullptr, 0, false, LAUNCH_HELMHOLTZ, {5, 4, 3}, 1, nullptr},
+    {FDB_FORM_HELMHOLTZ, "helmholtz", 0, true, nullptr, 0, false, LAUNCH_HELMHOLTZ, {5, 4, 3}, 1, nullptr, FDB_INTEGRAL_CELL},
     {FDB_FORM_HELMHOLTZ_COEF, "helmholtz_coef", 1, false, "kappa", 1, false, LAUNCH_HELMHOLTZ_COEF, {5, 4, 3}, 1,
-     nullptr},
+     nullptr, FDB_INTEGRAL_CELL},
     {FDB_FORM_NONLINEAR_DIFFUSION, "nonlinear_diffusion", 1, false, nullptr, 0, true, LAUNCH_HELMHOLTZ_COEF,
-     {5, 0, 0}, 1, nullptr},
+     {5, 0, 0}, 1, nullptr, FDB_INTEGRAL_CELL},
     {FDB_FORM_NONLINEAR_DIFFUSION_JACOBIAN, "nonlinear_diffusion_jacobian", 1, false, "u", 1, false,
-     LAUNCH_HELMHOLTZ_COEF, {5, 4, 3}, 1, nullptr},
-    {FDB_FORM_ELASTICITY, "elasticity", 3, false, nullptr, 0, false, LAUNCH_ELASTICITY, {4, 3, 3}, 1, nullptr},
+     LAUNCH_HELMHOLTZ_COEF, {5, 4, 3}, 1, nullptr, FDB_INTEGRAL_CELL},
+    {FDB_FORM_ELASTICITY, "elasticity", 3, false, nullptr, 0, false, LAUNCH_ELASTICITY, {4, 3, 3}, 1, nullptr, FDB_INTEGRAL_CELL},
     {FDB_FORM_HYPERELASTICITY, "hyperelasticity", 3, false, nullptr, 0, true, LAUNCH_ELASTICITY, {4, 0, 0}, 1,
-     nullptr},
+     nullptr, FDB_INTEGRAL_CELL},
     {FDB_FORM_HYPERELASTICITY_JACOBIAN, "hyperelasticity_jacobian", 3, false, "u", 3, false, LAUNCH_ELASTICITY,
-     {4, 3, 3}, 1, nullptr},
+     {4, 3, 3}, 1, nullptr, FDB_INTEGRAL_CELL},
     {FDB_FORM_ADVECTION_DIFFUSION, "advection_diffusion", 1, false, "b", 3, false, LAUNCH_HELMHOLTZ_COEF,
-     {4, 3, 3}, 1, nullptr},
+     {4, 3, 3}, 1, nullptr, FDB_INTEGRAL_CELL},
     // velocity CG_p with pressure CG_{p-1}: p >= 2
-    {FDB_FORM_STOKES, "stokes", 3, false, nullptr, 0, false, LAUNCH_STOKES, {4, 0, 0}, 2, "y_p, p"},
-    {FDB_FORM_NAVIER_STOKES, "navier_stokes", 3, false, nullptr, 0, true, LAUNCH_STOKES, {4, 0, 0}, 2, "y_p, p"},
+    {FDB_FORM_STOKES, "stokes", 3, false, nullptr, 0, false, LAUNCH_STOKES, {4, 0, 0}, 2, "y_p, p", FDB_INTEGRAL_CELL},
+    {FDB_FORM_NAVIER_STOKES, "navier_stokes", 3, false, nullptr, 0, true, LAUNCH_STOKES, {4, 0, 0}, 2, "y_p, p", FDB_INTEGRAL_CELL},
     {FDB_FORM_NAVIER_STOKES_JACOBIAN, "navier_stokes_jacobian", 3, false, "u", 3, false, LAUNCH_STOKES, {4, 0, 0}, 2,
-     "y_p, p"},
+     "y_p, p", FDB_INTEGRAL_CELL},
+    // gamma*inner(u, v)*ds: one exterior facet of one cell per entry, its local facet number last
+    {FDB_FORM_BOUNDARY_MASS, "boundary_mass", -1, false, "facet", 1, false, LAUNCH_BOUNDARY, {5, 4, 5}, 1, nullptr,
+     FDB_INTEGRAL_EXTERIOR_FACET},
 };
 
 static const char *const mode_name[] = {"action", "matrix", "diagonal"};
@@ -377,8 +384,13 @@ static int kernel_create(const fdb_kernel_desc *d, const fdb_space2_desc *s2, fd
         set_error("fdb_kernel_create: %s needs hex cells (extruded or native), got cell %d", f->name, d->cell);
         return 1;
     }
+    if (f->cdim < 0 && d->cdim != 1 && d->cdim != 3) {
+        set_error("fdb_kernel_create: %s %s takes a scalar space or a vector space of value size 3 (cdim %d)",
+                  f->name, mode_name[mode], d->cdim);
+        return 1;
+    }
     const int cdim = f->cdim ? f->cdim : (mode == MODE_DIAGONAL ? 1 : 0);
-    if (cdim ? d->cdim != cdim : (d->cdim < 1 || d->cdim > 3)) {
+    if (cdim > 0 ? d->cdim != cdim : (cdim == 0 && (d->cdim < 1 || d->cdim > 3))) {
         set_error("fdb_kernel_create: %s %s takes %s (cdim %d)", f->name, mode_name[mode],
                   cdim == 1 ? "scalar spaces only"
                             : (cdim == 3 ? "a vector space of value size 3 only" : "value sizes 1..3"),
@@ -410,8 +422,18 @@ static int kernel_create(const fdb_kernel_desc *d, const fdb_space2_desc *s2, fd
                   f->min_degree, f->max_degree[mode]);
         return 1;
     }
-    if (d->integral != FDB_INTEGRAL_CELL) {
+    if (f->integral == FDB_INTEGRAL_CELL && d->integral != FDB_INTEGRAL_CELL) {
         set_error("fdb_kernel_create: %s has cell integrals only", f->name);
+        return 1;
+    }
+    if (f->integral == FDB_INTEGRAL_EXTERIOR_FACET && d->integral != FDB_INTEGRAL_EXTERIOR_FACET) {
+        set_error("fdb_kernel_create: %s has exterior-facet integrals only (integral %d: %s)", f->name, d->integral,
+                  d->integral == FDB_INTEGRAL_CELL ? "a cell integral"
+                  : (d->integral == FDB_INTEGRAL_INTERIOR_FACET ? "interior facets are not supported" : "unknown"));
+        return 1;
+    }
+    if (f->integral != FDB_INTEGRAL_CELL && d->cell == FDB_CELL_HEX_EXTRUDED && (!d->offset0 || !d->offset1)) {
+        set_error("fdb_kernel_create: %s on extruded cells needs the layer offsets offset0/offset1", f->name);
         return 1;
     }
     if (d->rank != 1 && d->rank != 2) {
@@ -578,11 +600,18 @@ int fdb_kernel_call(fdb_kernel_t k, const fdb_call_args *a)
     // output and input of the second space after x and a third map: [y, coords, x, y2, x2], [V map, coord
     // map, second map]; with a trailing coefficient as well (the Navier-Stokes Jacobian's u) the coefficient
     // comes last: [y, coords, x, y2, x2, coef]
+    // an exterior-facet form (boundary_mass): the trailing argument is the uint32 local facet number of each
+    // entry, [y, coords, x, facet] / [mat, coords, facet] / [d, coords, facet]
     const fdb_hex_form *f = k->hex;
     const int mode = hex_mode(&k->desc);
+    if (f->integral != FDB_INTEGRAL_CELL && a->location != FDB_LOC_DEVICE) {
+        set_error("fdb_kernel_call: %s takes device-resident Dats only (no host-pointer mode for facet integrals)",
+                  f->name);
+        return 1;
+    }
     const int want = (mode == MODE_ACTION ? 3 : 2) + (f->coef ? 1 : 0) + (f->space2 ? 2 : 0);
     const int want_maps = f->space2 ? 3 : 2;
-    const bool device_only = mode == MODE_DIAGONAL || f->space2;
+    const bool device_only = mode == MODE_DIAGONAL || f->space2 || f->integral != FDB_INTEGRAL_CELL;
     if (a->nargs != want || a->nmaps != want_maps || (device_only && a->location != FDB_LOC_DEVICE)) {
         static const char *const args[] = {"y, coords, x", "mat, coords", "d, coords"};
         set_error("fdb_kernel_call: %s %s expects %d %sargs (%s%s%s%s%s) and %d maps, got %d/%d", f->name,
@@ -657,6 +686,9 @@ int fdb_kernel_call(fdb_kernel_t k, const fdb_call_args *a)
         case LAUNCH_HELMHOLTZ_COEF:
             return fdb_launch_helmholtz_coef_matrix(k, a->start, a->end, nlay, dsubset, mat, coords, coef, dmaps[0],
                                                     dmaps[1], out);
+        case LAUNCH_BOUNDARY:
+            return fdb_launch_boundary_mass(k, a->start, a->end, nlay, dsubset, mat, out, coords, nullptr,
+                                            (const unsigned *)coef, dmaps[0], dmaps[1]);
         default:
             return fdb_launch_elasticity_matrix(k, a->start, a->end, nlay, dsubset, mat, coords, coef, dmaps[0],
                                                 dmaps[1], out);
@@ -697,6 +729,10 @@ int fdb_kernel_call(fdb_kernel_t k, const fdb_call_args *a)
     case LAUNCH_ELASTICITY:
         rc = fdb_launch_elasticity_action(k, a->start, a->end, nlay, dsubset, out, coords, x, coef, dmaps[0],
                                           dmaps[1]);
+        break;
+    case LAUNCH_BOUNDARY:
+        rc = fdb_launch_boundary_mass(k, a->start, a->end, nlay, dsubset, nullptr, out, coords, x,
+                                      (const unsigned *)coef, dmaps[0], dmaps[1]);
         break;
     default:
         rc = fdb_launch_stokes_action(k, a->start, a->end, nlay, dsubset, out, coords, x, (double *)dargs[3],

@@ -1397,6 +1397,13 @@ class Kernel:
     "navier_stokes_jacobian" is its Gateaux derivative at the velocity u applied to (w, r), with u as the LAST
     argument: (INC, READ, READ, INC, READ, READ) = (velocity output, coordinates, w, pressure output, r, u).
     Neither is symmetric; both are rank-1 actions only.
+
+    "boundary_mass" is the exterior-facet integral ``alpha*inner(u, v)*ds`` (gamma = ``alpha``) on a scalar or
+    vector (``cdim=3``) space, with ``integral="exterior_facet"``.  The iteration set has one entry per facet of
+    a cell: its maps are the owning cells' rows, and the LAST argument is a uint32 Dat of the local facet numbers
+    (one per column of an extruded set, 0..5 = 2*direction + side; 4 / 5 are the bottom / top faces), read
+    directly: action (output, coordinates, u, facet), diagonal and rank 2 (output, coordinates, facet).  The
+    action on g is the load ``inner(g, v)*ds`` when ``alpha`` is 1.  Device-resident Dats only.
     """
     form: str = "helmholtz"
     degree: int = 1
@@ -1442,6 +1449,12 @@ class Kernel:
             return
         if spec and spec.residual:
             return          # (INC, READ, READ) whatever rank and diagonal say: the engine refuses them
+        if spec and spec.facet:
+            acc = (INC, READ, READ) if (self.diagonal or self.rank == 2) else (INC, READ, READ, READ)
+            object.__setattr__(self, "accesses", acc)
+            if self.name == "form0_cell_integral":
+                object.__setattr__(self, "name", f"form{'00' if self.rank == 2 else '0'}_{self.integral}_integral")
+            return
         if spec and spec.coefficient:
             acc = (INC, READ, READ) if (self.diagonal or self.rank == 2) else (INC, READ, READ, READ)
             object.__setattr__(self, "accesses", acc)
@@ -1474,6 +1487,7 @@ class _Form(NamedTuple):
     lame: bool = False          # takes mu and lmbda
     coef_cdim: int = 0          # values per node of the trailing coefficient when they differ from the space's
     pressure: bool = False      # also reads and writes a scalar pressure space through a third map (Stokes)
+    facet: bool = False         # an exterior-facet integral: the local facet numbers come last, the integral as given
 
 
 _FORMS = {"helmholtz": _Form(_lib.FORM_HELMHOLTZ),
@@ -1487,7 +1501,8 @@ _FORMS = {"helmholtz": _Form(_lib.FORM_HELMHOLTZ),
           "advection_diffusion": _Form(_lib.FORM_ADVECTION_DIFFUSION, coefficient=True, coef_cdim=3),
           "stokes": _Form(_lib.FORM_STOKES, pressure=True),
           "navier_stokes": _Form(_lib.FORM_NAVIER_STOKES, residual=True, pressure=True),
-          "navier_stokes_jacobian": _Form(_lib.FORM_NAVIER_STOKES_JACOBIAN, coefficient=True, pressure=True)}
+          "navier_stokes_jacobian": _Form(_lib.FORM_NAVIER_STOKES_JACOBIAN, coefficient=True, pressure=True),
+          "boundary_mass": _Form(_lib.FORM_BOUNDARY_MASS, facet=True)}
 _INTEGRALS = {"cell": _lib.INTEGRAL_CELL, "exterior_facet": _lib.INTEGRAL_EXTERIOR_FACET,
               "interior_facet": _lib.INTEGRAL_INTERIOR_FACET, "fused": _lib.INTEGRAL_FUSED}
 
@@ -1564,7 +1579,7 @@ class GlobalKernel:
         d.form = spec.enum
         d.rank = lk.rank
         d.cell = _lib.CELL_HEX_EXTRUDED if self.extruded else _lib.CELL_HEX
-        d.integral = _lib.INTEGRAL_CELL
+        d.integral = _INTEGRALS[lk.integral] if spec.facet else _lib.INTEGRAL_CELL
         d.degree = lk.degree
         d.nq = el.nq
         d.cdim = lk.cdim

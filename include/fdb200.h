@@ -221,7 +221,7 @@ enum fdb_form {
                                    convective term is not integrated exactly by the nq = p+1 rule.
                                      action  [y_u INC, coords, u, y_p INC, p]
                                              maps [V map, coord map, Q map]                       */
-    FDB_FORM_NAVIER_STOKES_JACOBIAN = 12
+    FDB_FORM_NAVIER_STOKES_JACOBIAN = 12,
                                 /* its Gateaux derivative at the velocity u (exact Newton Jacobian, NOT
                                    symmetric), applied to the direction (w, r):
                                      J(u)[(w, r); (v, q)] = nu*inner(grad w, grad v)*dx
@@ -234,6 +234,26 @@ enum fdb_form {
                                    argument, read through maps[0]:
                                      action  [y_u INC, coords, w, y_p INC, r, u]
                                              maps [V map, coord map, Q map]                       */
+    FDB_FORM_BOUNDARY_MASS = 13
+                                /* the boundary mass term, an EXTERIOR-FACET integral (symmetric):
+                                     a(u, v) = gamma*inner(u, v)*ds
+                                   gamma = alpha.  The Robin operator term, and through its action every
+                                   boundary load: inner(g, v)*ds is the action on g with gamma = 1 (a
+                                   Neumann flux for scalar g, a traction for vector g).  integral ==
+                                   FDB_INTEGRAL_EXTERIOR_FACET (cell and interior-facet integrals are
+                                   refused).  Hex cells (extruded or native), cdim 1 or 3, nq ==
+                                   degree+1, affine_cells == 0; degrees 1..5 (action and diagonal), 1..4
+                                   (rank 2).  An iteration entry is one facet of one cell: the maps are
+                                   the owning cell's rows (plus offset * layer on extruded cells), and the
+                                   LAST argument is a uint32 local facet number per entry (per column on
+                                   extruded sets), 2*direction + side: 0 / 1 where the x dof index of the
+                                   local numbering (ax*N + ay)*N + az is 0 / 1, 2 / 3 for y, 4 / 5 for z
+                                   (bottom / top).  Device mode only:
+                                     action    [y INC, coords, u, facet]  (atomic or coloured)
+                                     diagonal  [d INC, coords, facet]     (cdim values per node, the
+                                               same in each component)
+                                     rank 2    [Mat, coords, facet]  (block size cdim; the components
+                                               do not couple: block diagonals only)               */
 };
 
 enum fdb_cell {
