@@ -27,6 +27,8 @@ FORM_STOKES = 10
 FORM_NAVIER_STOKES = 11
 FORM_NAVIER_STOKES_JACOBIAN = 12
 FORM_BOUNDARY_MASS = 13
+FORM_INTERIOR_PENALTY = 14
+FORM_DG_BOUNDARY = 15
 CELL_HEX_EXTRUDED = 1
 CELL_HEX = 2
 CELL_TRIANGLE = 3

@@ -29,11 +29,30 @@ class FunctionSpace:
     """Scalar/vector CG_p space on an extruded hex mesh, bundling the PyOP2
     objects ``assemble`` needs (node set, cell set, maps, coordinates), i.e.
     what ``V.cell_node_map()``, ``mesh.coordinates.dat`` and friends give in
-    Firedrake (firedrake/functionspaceimpl.py:803-812)."""
+    Firedrake (firedrake/functionspaceimpl.py:803-812).
 
-    def __init__(self, mesh, degree, cdim=1, partition=None):
+    ``family="DQ"``: the scalar discontinuous space DQ_p (p = 1..4) with Gauss-Legendre nodes
+    (``mesh.dg_function_space``), for :class:`InteriorPenalty` and the cell forms of :class:`Form`.
+    ``element`` is its 1-D element (the kernels' tables); None for CG, whose kernels use the default GLL
+    element."""
+
+    def __init__(self, mesh, degree, cdim=1, partition=None, family="CG"):
         self.mesh, self.degree, self.cdim = mesh, degree, cdim
-        self.V = V = mesh.function_space(degree)
+        if family not in ("CG", "DQ"):
+            raise ValueError(f"family {family!r}: 'CG' or 'DQ'")
+        self.family = family
+        self.element = None
+        if family == "DQ":
+            from .fiat_lite import interval_element
+            if cdim != 1:
+                raise NotImplementedError("DQ spaces are scalar (vector DQ is not implemented)")
+            if partition is not None:
+                raise NotImplementedError("partitioned DQ spaces are not implemented: the interior facets on a "
+                                          "partition boundary would need both cells")
+            self.element = interval_element(degree, variant="gl")
+            self.V = V = mesh.dg_function_space(degree)
+        else:
+            self.V = V = mesh.function_space(degree)
         if partition is not None:
             cell_sizes, node_sizes = partition.cell_sizes, partition.node_sizes
             halo = Halo(partition.halo_lists(V), max_cdim=cdim) if partition.nranks > 1 else None
@@ -91,6 +110,11 @@ class FunctionSpace:
         return self.V.boundary_nodes(sub_domain)
 
 
+def _refuse_dq(V, what, why="it is stated on CG spaces only"):
+    if getattr(V, "family", "CG") == "DQ":
+        raise NotImplementedError(f"{what} does not take DQ spaces: {why}")
+
+
 def interpolate_q1(V: "FunctionSpace", source: op2.Dat, target: op2.Dat = None):
     """``Function(V).interpolate(w)`` for a Q1 (x) P1 source ``w`` (scalar or
     vector, e.g. the mesh coordinates -> the physical position of every node of
@@ -98,6 +122,7 @@ def interpolate_q1(V: "FunctionSpace", source: op2.Dat, target: op2.Dat = None):
     WRITE access on the target.  Returns the target Dat (device resident)."""
     from . import _lib
     from .fiat_lite import interval_element
+    _refuse_dq(V, "interpolate_q1", "it evaluates at the GLL node positions of CG_p")
     cdim = source.cdim
     if target is None:
         target = op2.Dat(op2.DataSet(V.node_set, cdim))
@@ -152,6 +177,7 @@ def interpolate(V: "FunctionSpace", expressions, target: op2.Dat = None):
     (SURVEY.md section 8f row f2), run as a WRITE parloop through the engine's generic
     wrapper builder.  Nodes shared by several cells are written by each of them with the
     same value, as in the reference's sequential loop."""
+    _refuse_dq(V, "interpolate", "it evaluates at the GLL node positions of CG_p")
     exprs = [expressions] if isinstance(expressions, str) else list(expressions)
     if len(exprs) != V.cdim:
         raise ValueError(f"need {V.cdim} expressions for this space, got {len(exprs)}")
@@ -903,6 +929,167 @@ def assemble_boundary_mass_generic(V: "FunctionSpace", u: op2.Dat, gamma=1.0, su
     return tensor
 
 
+def interior_penalty_kernels(degree, alpha, eta, name=None):
+    """C sources of the facet terms of :class:`InteriorPenalty` on DQ_p hexes (Gauss-Legendre nodes, trilinear
+    geometry), written the way TSFC would (the whole cell's basis and its physical gradient at every facet point,
+    n = J^-T n_ref / |J^-T n_ref| of the '+' cell, the surface measure |det J| |J^-T n_ref|), for the generic wrapper
+    builder: the independent statement of the hand-written FDB_FORM_INTERIOR_PENALTY and FDB_FORM_DG_BOUNDARY
+    kernels.  Returns {"dS_v": action over the vertical interior facets (args y (INC), coords, u, facets uint[2]),
+    "dS_h": the same with the pair (5, 4) baked in, for ON_INTERIOR_FACETS over the cells (args y, coords, u),
+    "ds": the Nitsche operator terms alpha*(-dot(grad u, n)*v - u*dot(grad v, n) + (eta/h)*u*v)*ds (args y, coords,
+    u, facet uint[1])}."""
+    from .codegen import CStringKernel
+    from .fiat_lite import interval_element
+    el = interval_element(degree, variant="gl")
+    n, nd = degree + 1, (degree + 1) ** 3
+    Bend, Dend = el.tabulate([0.0, 1.0])
+    tab = lambda a: "{" + ", ".join("{" + ", ".join(repr(float(v)) for v in r) + "}" for r in a) + "}"
+    vec = lambda a: "{" + ", ".join(repr(float(v)) for v in a) + "}"
+    base = name or f"interior_penalty{degree}"
+    head = f"""
+static const double PB[{n}][{n}] = {tab(el.B)};      /* basis a at Gauss point q */
+static const double PD[{n}][{n}] = {tab(el.D)};      /* its derivative */
+static const double PE[2][{n}] = {tab(Bend)};        /* basis at the interval's ends */
+static const double PF[2][{n}] = {tab(Dend)};        /* derivative at the ends */
+static const double PX[{n}] = {vec(el.xq)};
+static const double PW[{n}] = {vec(el.wq)};
+/* one side of a facet at face point (q1, q2): basis values and physical gradients of the cell's {nd} dofs, the
+   inverse Jacobian K (K[d][c] = dxi_d/dx_c) and |det J| */
+static double side_tables(const double *X, int f, int q1, int q2, double *phi, double (*grad)[3], double K[3][3])
+{{
+    const int fd = f / 2, fs = f % 2, d1 = fd == 0 ? 1 : 0, d2 = fd == 2 ? 1 : 2;
+    double xi[3], J[3][3];
+    const double *T[3], *DT[3];
+    xi[fd] = (double)fs; xi[d1] = PX[q1]; xi[d2] = PX[q2];
+    T[fd] = PE[fs]; T[d1] = PB[q1]; T[d2] = PB[q2];
+    DT[fd] = PF[fs]; DT[d1] = PD[q1]; DT[d2] = PD[q2];
+    for (int c = 0; c < 3; ++c) for (int d = 0; d < 3; ++d) J[c][d] = 0.0;
+    for (int v = 0; v < 8; ++v) {{
+        const int b[3] = {{(v >> 2) & 1, (v >> 1) & 1, v & 1}};
+        for (int d = 0; d < 3; ++d) {{
+            double g = b[d] ? 1.0 : -1.0;
+            for (int e = 0; e < 3; ++e) if (e != d) g *= b[e] ? xi[e] : 1.0 - xi[e];
+            for (int c = 0; c < 3; ++c) J[c][d] += X[v * 3 + c] * g;
+        }}
+    }}
+    const double det = J[0][0] * (J[1][1] * J[2][2] - J[1][2] * J[2][1])
+                     - J[0][1] * (J[1][0] * J[2][2] - J[1][2] * J[2][0])
+                     + J[0][2] * (J[1][0] * J[2][1] - J[1][1] * J[2][0]);
+    for (int d = 0; d < 3; ++d) for (int c = 0; c < 3; ++c) {{
+        const int d1_ = (d + 1) % 3, d2_ = (d + 2) % 3, c1 = (c + 1) % 3, c2 = (c + 2) % 3;
+        K[d][c] = (J[c1][d1_] * J[c2][d2_] - J[c1][d2_] * J[c2][d1_]) / det;   /* cofactor of J[c][d] */
+    }}
+    for (int a = 0; a < {n}; ++a) for (int b = 0; b < {n}; ++b) for (int c = 0; c < {n}; ++c) {{
+        const int i = (a * {n} + b) * {n} + c;
+        const double r[3] = {{DT[0][a] * T[1][b] * T[2][c], T[0][a] * DT[1][b] * T[2][c], T[0][a] * T[1][b] * DT[2][c]}};
+        phi[i] = T[0][a] * T[1][b] * T[2][c];
+        for (int e = 0; e < 3; ++e) grad[i][e] = K[0][e] * r[0] + K[1][e] * r[1] + K[2][e] * r[2];
+    }}
+    return fabs(det);
+}}
+static double diameter(const double *X)
+{{
+    double m = 0.0;
+    for (int i = 0; i < 8; ++i) for (int j = i + 1; j < 8; ++j) {{
+        double s = 0.0;
+        for (int c = 0; c < 3; ++c) s += (X[i * 3 + c] - X[j * 3 + c]) * (X[i * 3 + c] - X[j * 3 + c]);
+        if (s > m) m = s;
+    }}
+    return sqrt(m);
+}}
+/* the unit normal outward from the cell on facet f and the surface measure |det J| |J^-T n_ref| */
+static double normal(int f, double det, double K[3][3], double *nrm)
+{{
+    const int fd = f / 2;
+    const double sg = f % 2 ? 1.0 : -1.0;
+    const double l = sqrt(K[fd][0] * K[fd][0] + K[fd][1] * K[fd][1] + K[fd][2] * K[fd][2]);
+    for (int c = 0; c < 3; ++c) nrm[c] = sg * K[fd][c] / l;
+    return det * l;
+}}
+"""
+    interior = """
+{{
+    const int fac[2] = {{(int)({fp}), (int)({fm})}};
+    const double sig = {eta!r} / (0.5 * (diameter(X) + diameter(X + 24)));
+    for (int q1 = 0; q1 < {n}; ++q1) for (int q2 = 0; q2 < {n}; ++q2) {{
+        double phi[2][{nd}], grad[2][{nd}][3], K[2][3][3], det[2], u[2] = {{0.0, 0.0}}, gu[2][3] = {{{{0.0}}}}, nrm[3];
+        for (int s = 0; s < 2; ++s) {{
+            det[s] = side_tables(X + 24 * s, fac[s], q1, q2, phi[s], grad[s], K[s]);
+            for (int i = 0; i < {nd}; ++i) {{
+                u[s] += phi[s][i] * w[s * {nd} + i];
+                for (int c = 0; c < 3; ++c) gu[s][c] += grad[s][i][c] * w[s * {nd} + i];
+            }}
+        }}
+        const double W = PW[q1] * PW[q2] * normal(fac[0], det[0], K[0], nrm);
+        const double ju = u[0] - u[1];
+        double fu = 0.0;
+        for (int c = 0; c < 3; ++c) fu += 0.5 * nrm[c] * (gu[0][c] + gu[1][c]);
+        for (int s = 0; s < 2; ++s) {{
+            const double sv = s ? -1.0 : 1.0;           /* jump(v, n) = sv v n */
+            for (int i = 0; i < {nd}; ++i) {{
+                double dn = 0.0;
+                for (int c = 0; c < 3; ++c) dn += nrm[c] * grad[s][i][c];
+                A[s * {nd} + i] += {alpha!r} * W * (-fu * sv * phi[s][i] - 0.5 * ju * dn + sig * ju * sv * phi[s][i]);
+            }}
+        }}
+    }}
+}}
+"""
+    dS_v = f"static void {base}_dS(double *A, const double *X, const double *w, const unsigned int *facet)" + \
+        interior.format(fp="facet[0]", fm="facet[1]", eta=float(eta), n=n, nd=nd, alpha=float(alpha))
+    dS_h = f"static void {base}_dSh(double *A, const double *X, const double *w)" + \
+        interior.format(fp="5", fm="4", eta=float(eta), n=n, nd=nd, alpha=float(alpha))
+    ds = f"""static void {base}_ds(double *A, const double *X, const double *w, const unsigned int *facet)
+{{
+    const int f = (int)facet[0];
+    const double pen = {float(eta)!r} / diameter(X);
+    for (int q1 = 0; q1 < {n}; ++q1) for (int q2 = 0; q2 < {n}; ++q2) {{
+        double phi[{nd}], grad[{nd}][3], K[3][3], nrm[3], u = 0.0, dnu = 0.0;
+        const double det = side_tables(X, f, q1, q2, phi, grad, K);
+        const double W = PW[q1] * PW[q2] * normal(f, det, K, nrm);
+        for (int i = 0; i < {nd}; ++i) {{
+            u += phi[i] * w[i];
+            for (int c = 0; c < 3; ++c) dnu += nrm[c] * grad[i][c] * w[i];
+        }}
+        for (int i = 0; i < {nd}; ++i) {{
+            double dn = 0.0;
+            for (int c = 0; c < 3; ++c) dn += nrm[c] * grad[i][c];
+            A[i] += {float(alpha)!r} * W * (-dnu * phi[i] - u * dn + pen * u * phi[i]);
+        }}
+    }}
+}}
+"""
+    return {"dS_v": CStringKernel(head + dS_v, f"{base}_dS"), "dS_h": CStringKernel(head + dS_h, f"{base}_dSh"),
+            "ds": CStringKernel(head + ds, f"{base}_ds")}
+
+
+def assemble_interior_penalty_generic(F: "InteriorPenalty", u: op2.Dat, tensor=None):
+    """The facet terms of ``assemble(action(a, u))`` for an :class:`InteriorPenalty` form through the generic
+    wrapper path (:func:`interior_penalty_kernels`): the vertical interior facets x all layers, the horizontal ones as
+    ON_INTERIOR_FACETS over the cells, and the Nitsche terms on F's weak_bcs facets -- the cross-check and the
+    baseline of the hand-written facet kernels (the cell term is the Helmholtz kernel's and is not included)."""
+    from . import codegen
+    V = F.V
+    if tensor is None:
+        tensor = V.dat()
+    tensor.zero()
+    tensor.device_ptr
+    ks = interior_penalty_kernels(V.degree, F.alpha, F.eta)
+    for fset, fmap, cmap, pairs in _dg_interior_groups(V):
+        if fset.layers == V.mesh.layers:            # the vertical group
+            codegen.par_loop(ks["dS_v"], fset, tensor(op2.INC, fmap), V.coordinates(op2.READ, cmap),
+                             u(op2.READ, fmap), pairs(op2.READ))
+    if V.mesh.nz > 1:
+        codegen.par_loop(ks["dS_h"], V.cell_set, tensor(op2.INC, V.cell_node_map),
+                         V.coordinates(op2.READ, V.coord_map), u(op2.READ, V.cell_node_map),
+                         iteration_region="ON_INTERIOR_FACETS")
+    if F.weak_bcs:
+        for fset, fmap, cmap, facet in _boundary_groups(V, F.weak_bcs):
+            codegen.par_loop(ks["ds"], fset, tensor(op2.INC, fmap), V.coordinates(op2.READ, cmap), u(op2.READ, fmap),
+                             facet(op2.READ))
+    return tensor
+
+
 def hyperelasticity_kernel(degree, mu, lmbda, beta=0.0, jacobian=False, name=None):
     """C source of the residual of compressible Neo-Hookean hyperelasticity,
     ``inner(P(F), grad(v))*dx + beta*inner(u, v)*dx`` with ``F = I + grad(u)``, ``J = det(F)`` and
@@ -1042,6 +1229,7 @@ def assemble_functional(V: "FunctionSpace", f: op2.Dat, measure="dx", integrand=
     bottom / top = iteration regions ON_BOTTOM / ON_TOP over the cells, vertical = the base
     mesh's exterior facets x all layers (firedrake/assemble.py:1810-1850)."""
     from . import codegen
+    _refuse_dq(V, "assemble_functional", "its kernels tabulate the GLL element")
     if V.cdim != 1:
         raise NotImplementedError("functionals of scalar fields only")
     if measure == "ds":
@@ -1106,6 +1294,8 @@ class DirichletBC:
     (firedrake/bcs.py:260-457)."""
 
     def __init__(self, V: FunctionSpace, g, sub_domain):
+        _refuse_dq(V, "DirichletBC", "a DQ space has no boundary nodes; impose the condition weakly with "
+                   "InteriorPenalty(..., weak_bcs=sub_domain) and nitsche_load")
         self.V = V
         subs = sub_domain if isinstance(sub_domain, (list, tuple)) else [sub_domain]
         self.sub_domains = tuple(subs)
@@ -1268,6 +1458,8 @@ class BoundaryMass:
     cell_integral = False       # no dx term: only the ds loops run
 
     def __post_init__(self):
+        _refuse_dq(self.V, "BoundaryMass", "its kernel gathers the face nodes of CG_p; the DQ boundary loads are "
+                   "nitsche_load and dg_flux_load")
         _check_ds(self)
 
     @property
@@ -1279,6 +1471,203 @@ class BoundaryMass:
 
     def kernel(self, rank, diagonal=False):
         return _boundary_kernel(self.V, self.gamma, rank, diagonal)
+
+
+def _face_vertices(f):
+    """The cell-local vertices (bx*2 + by)*2 + bz of local facet f = 2*direction + side, in (s, t) order (s, t: the
+    other two reference axes in increasing order)."""
+    d, side = int(f) // 2, int(f) % 2
+    out = []
+    for sa in (0, 1):
+        for sb in (0, 1):
+            bx, by, bz = {0: (side, sa, sb), 1: (sa, side, sb), 2: (sa, sb, side)}[d]
+            out.append((bx * 2 + by) * 2 + bz)
+    return np.array(out)
+
+
+def _check_facet_orientation(xrows, xoff, pairs):
+    """The interior-facet kernel pairs face point (s, t) of '+' with face point (s, t) of '-': the face's vertices,
+    read through each side's local facet, must be the same vertices in the same order (in the bottom layer and the
+    next, hence in all)."""
+    xrows = np.asarray(xrows, dtype=np.int64)
+    xoff = np.asarray(xoff, dtype=np.int64)
+    for fp, fm in {(int(a), int(b)) for a, b in pairs}:
+        sel = (pairs[:, 0] == fp) & (pairs[:, 1] == fm)
+        vp, vm = _face_vertices(fp), 8 + _face_vertices(fm)
+        for layer in (0, 1):
+            if not np.array_equal(xrows[sel][:, vp] + layer * xoff[vp], xrows[sel][:, vm] + layer * xoff[vm]):
+                raise ValueError(f"interior facets ({fp}, {fm}): the two cells parametrise the face differently")
+
+
+def _dg_interior_groups(V: "FunctionSpace"):
+    """The interior facets of a DQ space as iteration groups ``(facet set, V map, coordinate map, local facet
+    pairs)``, built once and cached on the space.  Vertical facets: the base mesh's interior facets x all layers,
+    maps = the '+' cell's row followed by the '-' cell's (arity 2 (p+1)^3, 16 vertices, offsets tiled), pairs (1, 0)
+    for x-normal and (3, 2) for y-normal facets.  Horizontal facets: the base columns over nz - 1 facet layers,
+    rows [row, row + offset] ('+' the cell below), pair (5, 4)."""
+    if "_dg_interior" in V.__dict__:
+        return V._dg_interior
+    mesh, W = V.mesh, V.V
+    cmap, off = W.cell_node_map.astype(np.int64), np.asarray(W.offset, dtype=np.int64)
+    xmap, xoff = mesh.coord_map.astype(np.int64), np.asarray(mesh.coord_offset, dtype=np.int64)
+    groups = []
+
+    def group(layers, rows, xrows, pairs):
+        _check_facet_orientation(xrows, np.tile(xoff, 2), pairs)
+        fset = op2.ExtrudedSet(op2.Set(len(pairs)), layers)
+        groups.append((fset,
+                       op2.Map(fset, V.node_set, 2 * W.arity, np.ascontiguousarray(rows, dtype=np.int32),
+                               offset=np.tile(W.offset, 2)),
+                       op2.Map(fset, V.vertex_set, 16, np.ascontiguousarray(xrows, dtype=np.int32),
+                               offset=np.tile(mesh.coord_offset, 2)),
+                       op2.Dat(op2.DataSet(fset, 2), np.ascontiguousarray(pairs, dtype=np.uint32), dtype=np.uint32)))
+
+    cp, cm, local = mesh.interior_vertical_facets()
+    if len(cp):
+        group(mesh.layers, np.concatenate([cmap[cp], cmap[cm]], axis=1), np.concatenate([xmap[cp], xmap[cm]], axis=1),
+              local)
+    if mesh.nz > 1:
+        nb = mesh.num_base_cells
+        group(mesh.nz, np.concatenate([cmap, cmap + off[None, :]], axis=1),
+              np.concatenate([xmap, xmap + xoff[None, :]], axis=1), np.tile(np.array([5, 4], dtype=np.uint32), (nb, 1)))
+    V._dg_interior = groups
+    return groups
+
+
+def _dq_diagonal_kernel(V, alpha, beta):
+    """The cell term's diagonal on a DQ space: the Helmholtz diagonal kernel, degrees 1..3."""
+    if V.degree > 3:
+        raise NotImplementedError(f"the diagonal of the DQ{V.degree} cell term is not implemented (the Helmholtz "
+                                  f"diagonal kernel covers degrees 1..3): getDiagonal and pc_type 'jacobi' need "
+                                  f"DQ1..DQ3; use pc_type 'none' on DQ4")
+    return op2.Kernel("helmholtz", degree=V.degree, alpha=alpha, beta=beta, diagonal=True, element=V.element)
+
+
+def _dg_boundary_kernel(V, c_m, c_p, c_s, c_f, diagonal=False):
+    return op2.Kernel("dg_boundary", degree=V.degree, alpha=float(c_f), beta=float(c_p), c_m=float(c_m),
+                      c_s=float(c_s), diagonal=diagonal, integral="exterior_facet", element=V.element)
+
+
+def _dg_boundary_loops(V, coefs, sub_domain, tensor, u, scatter="atomic"):
+    """The FDB_FORM_DG_BOUNDARY parloops of (c_m, c_p, c_s, c_f) on the exterior facets of ``sub_domain``."""
+    loops = []
+    for fset, fmap, cmap, facet in _boundary_groups(V, sub_domain):
+        gk = op2.GlobalKernel(_dg_boundary_kernel(V, *coefs), [fmap, cmap], extruded=True, scatter=scatter)
+        loops.append(op2.Parloop(gk, fset, [tensor(op2.INC, fmap), V.coordinates(op2.READ, cmap), u(op2.READ, fmap),
+                                            facet(op2.READ)], location="device"))
+    return loops
+
+
+class _DGFacetTerms:
+    """The facet parloops of an :class:`InteriorPenalty` form: FDB_FORM_INTERIOR_PENALTY over every interior facet
+    group, FDB_FORM_DG_BOUNDARY with Nitsche's (0, alpha*eta, alpha, alpha) over the weak_bcs facets."""
+
+    def __init__(self, form: "InteriorPenalty"):
+        self.form = form
+        V = form.V
+        self.interior = _dg_interior_groups(V)
+        self.nitsche = (0.0, form.alpha * form.eta, form.alpha, form.alpha)
+
+    def _kernel(self, diagonal=False):
+        F = self.form
+        return op2.Kernel("interior_penalty", degree=F.V.degree, alpha=float(F.alpha), beta=float(F.eta),
+                          diagonal=diagonal, integral="interior_facet", element=F.V.element)
+
+    def action_loops(self, tensor: op2.Dat, u: op2.Dat, scatter="atomic"):
+        V, loops = self.form.V, []
+        for fset, fmap, cmap, pairs in self.interior:
+            gk = op2.GlobalKernel(self._kernel(), [fmap, cmap], extruded=True, scatter=scatter)
+            loops.append(op2.Parloop(gk, fset, [tensor(op2.INC, fmap), V.coordinates(op2.READ, cmap),
+                                                u(op2.READ, fmap), pairs(op2.READ)], location="device"))
+        if self.form.weak_bcs:
+            loops += _dg_boundary_loops(V, self.nitsche, self.form.weak_bcs, tensor, u, scatter)
+        return loops
+
+    def diagonal(self, D: op2.Dat):
+        V = self.form.V
+        for fset, fmap, cmap, pairs in self.interior:
+            op2.par_loop(self._kernel(True), fset, D(op2.INC, fmap), V.coordinates(op2.READ, cmap), pairs(op2.READ))
+        if self.form.weak_bcs:
+            for fset, fmap, cmap, facet in _boundary_groups(V, self.form.weak_bcs):
+                op2.par_loop(_dg_boundary_kernel(V, *self.nitsche, diagonal=True), fset, D(op2.INC, fmap),
+                             V.coordinates(op2.READ, cmap), facet(op2.READ))
+
+
+@dataclass
+class InteriorPenalty:
+    """The symmetric interior penalty (SIPG) discretisation of -div(alpha grad u) + beta u = f on a scalar DQ_p space
+    (``FunctionSpace(mesh, p, family="DQ")``, p = 1..4), with h the cell diameter and n the unit normal:
+
+        a(u, v) = alpha*inner(grad u, grad v)*dx + beta*u*v*dx
+                  + alpha*( -inner(avg(grad u), jump(v, n)) - inner(jump(u, n), avg(grad v))
+                            + (eta/avg(h))*inner(jump(u, n), jump(v, n)) )*dS
+                  + alpha*( -dot(grad u, n)*v - u*dot(grad v, n) + (eta/h)*u*v )*ds(weak_bcs)
+
+    Every integral has p+1 Gauss points per axis.  ``eta`` has no default (the user picks the penalty, as in
+    Firedrake's demos); 3*(p+1)**2 keeps the operator positive definite on the meshes of the tests.  ``weak_bcs``:
+    the sub-domains (the names :class:`DirichletBC` takes, or "on_boundary") where Dirichlet conditions are imposed
+    weakly (Nitsche), ``()`` for natural conditions everywhere; the load of a Dirichlet value g is
+    :func:`nitsche_load`, a flux :func:`dg_flux_load`.  ``assemble(F, u=x)`` is the action, ``mat_type="matfree"``
+    an operator with ``mult`` and ``getDiagonal`` (no assembled matrix; the diagonal for p = 1..3, which is what the
+    cell term's diagonal kernel covers); :func:`solve` runs CG with ``pc_type`` "none" or "jacobi" (p = 1..3).  The cell term runs on the Helmholtz kernels with the DQ element's tables; the facet terms
+    on FDB_FORM_INTERIOR_PENALTY and FDB_FORM_DG_BOUNDARY."""
+    V: FunctionSpace
+    alpha: float = 1.0
+    beta: float = 0.0
+    eta: float = None
+    weak_bcs: object = "on_boundary"
+    symmetric = True
+    ds = ()
+
+    def __post_init__(self):
+        if getattr(self.V, "family", "CG") != "DQ":
+            raise ValueError("InteriorPenalty takes a DQ space: FunctionSpace(mesh, p, family='DQ')")
+        if self.eta is None:
+            raise ValueError("InteriorPenalty needs the penalty eta (no default), e.g. 3*(p+1)**2")
+        self.eta = float(self.eta)
+        if isinstance(self.weak_bcs, list):
+            self.weak_bcs = tuple(self.weak_bcs)
+        if self.weak_bcs:
+            _boundary_groups(self.V, self.weak_bcs)
+        _dg_interior_groups(self.V)
+
+    def coefficient_args(self):
+        return []
+
+    def kernel(self, rank, diagonal=False):
+        """The cell term alpha*inner(grad u, grad v)*dx + beta*u*v*dx on the DQ element."""
+        if diagonal:
+            return _dq_diagonal_kernel(self.V, self.alpha, self.beta)
+        return Form(self.V, self.alpha, self.beta).kernel(rank)
+
+    def facet_terms(self):
+        if "_facet_terms" not in self.__dict__:
+            self._facet_terms = _DGFacetTerms(self)
+        return self._facet_terms
+
+
+def _dg_load(V, coefs, sub_domain, g, tensor):
+    if tensor is None:
+        tensor = V.dat()
+    tensor.zero()
+    for loop in _dg_boundary_loops(V, coefs, sub_domain, tensor, g):
+        loop()
+    return tensor
+
+
+def nitsche_load(F: InteriorPenalty, g: op2.Dat, tensor: op2.Dat = None):
+    """The Dirichlet load of ``g`` (a Dat on F.V) on F's weak_bcs, alpha*(-g*dot(grad v, n) + (eta/h)*g*v)*ds."""
+    if not F.weak_bcs:
+        raise ValueError("the form has no weakly imposed Dirichlet sub-domains (weak_bcs=())")
+    return _dg_load(F.V, (0.0, F.alpha * F.eta, F.alpha, 0.0), F.weak_bcs, g, tensor)
+
+
+def dg_flux_load(V: FunctionSpace, g: op2.Dat, sub_domain="on_boundary", tensor: op2.Dat = None):
+    """The flux (Neumann) load g*v*ds(sub_domain) of a Dat ``g`` on a DQ space ``V``."""
+    if getattr(V, "family", "CG") != "DQ":
+        raise ValueError("dg_flux_load takes a DQ space; on CG spaces the load is assemble(BoundaryMass(V, 1, "
+                         "sub_domain), u=g)")
+    return _dg_load(V, (1.0, 0.0, 0.0, 0.0), sub_domain, g, tensor)
 
 
 @dataclass
@@ -1299,6 +1688,7 @@ class Form:
 
     def __post_init__(self):
         if self.ds:
+            _refuse_dq(self.V, "Form's ds terms", "DQ boundary terms are InteriorPenalty's weak_bcs")
             _check_ds(self)
 
     def coefficient_args(self):
@@ -1306,17 +1696,27 @@ class Form:
         return [] if self.kappa is None else [self.kappa(op2.READ, self.V.cell_node_map)]
 
     def kernel(self, rank, diagonal=False):
+        if getattr(self.V, "family", "CG") == "DQ":
+            if rank == 2:
+                raise NotImplementedError("a DQ space has no assembled matrix here: use the action and the "
+                                          "matrix-free operator (mat_type='matfree')")
+            if self.kappa is not None:
+                _refuse_dq(self.V, "Form with kappa")
+            return op2.Kernel("helmholtz", degree=self.V.degree, alpha=self.alpha, beta=self.beta, rank=rank,
+                              affine=self._affine(rank), element=self.V.element)
         if self.kappa is not None:
             if self.V.cdim != 1:
                 raise NotImplementedError("coefficient forms take scalar spaces only")
             return op2.Kernel("helmholtz_coef", degree=self.V.degree, alpha=self.alpha, beta=self.beta,
                               rank=rank, diagonal=diagonal)
+        return op2.Kernel("helmholtz", degree=self.V.degree, alpha=self.alpha, beta=self.beta,
+                          rank=rank, cdim=self.V.cdim, affine=self._affine(rank))
+
+    def _affine(self, rank):
         import os
         # per-cell metric on meshes whose cells are all parallelepipeds (checked on the device;
         # GPU-validated in round 2, FDB_AFFINE=0 opts out)
-        affine = rank == 1 and os.environ.get("FDB_AFFINE", "1") != "0" and self.V.cells_are_affine()
-        return op2.Kernel("helmholtz", degree=self.V.degree, alpha=self.alpha, beta=self.beta,
-                          rank=rank, cdim=self.V.cdim, affine=affine)
+        return rank == 1 and os.environ.get("FDB_AFFINE", "1") != "0" and self.V.cells_are_affine()
 
 
 @dataclass
@@ -1337,6 +1737,7 @@ class NonlinearDiffusion:
     symmetric = False
 
     def __post_init__(self):
+        _refuse_dq(self.V, "NonlinearDiffusion")
         if self.ds:
             _check_ds(self)
 
@@ -1412,6 +1813,7 @@ class Elasticity:
     symmetric = True
 
     def __post_init__(self):
+        _refuse_dq(self.V, "Elasticity")
         if self.ds:
             _check_ds(self)
 
@@ -1446,6 +1848,7 @@ class HyperElasticity:
     symmetric = True
 
     def __post_init__(self):
+        _refuse_dq(self.V, "HyperElasticity")
         if self.ds:
             _check_ds(self)
 
@@ -1508,6 +1911,7 @@ class AdvectionDiffusion:
     symmetric = False
 
     def __post_init__(self):
+        _refuse_dq(self.V, "AdvectionDiffusion")
         if self.b.cdim != 3:
             raise ValueError(f"the velocity b has 3 values per node (V.vector_dset(3)), got {self.b.cdim}")
         if self.ds:
@@ -1546,6 +1950,8 @@ class Stokes:
     symmetric = True
 
     def __post_init__(self):
+        _refuse_dq(self.V, "Stokes")
+        _refuse_dq(self.Q, "Stokes")
         _refuse_taylor_hood_ds(self.ds, "Stokes")
         self.pressure_map = _taylor_hood_pressure_map(self.V, self.Q, "Stokes")
 
@@ -1608,6 +2014,8 @@ class NavierStokes:
     symmetric = False
 
     def __post_init__(self):
+        _refuse_dq(self.V, "NavierStokes")
+        _refuse_dq(self.Q, "NavierStokes")
         _refuse_taylor_hood_ds(self.ds, "Navier-Stokes")
         self.pressure_map = _taylor_hood_pressure_map(self.V, self.Q, "Navier-Stokes")
 
@@ -1759,6 +2167,8 @@ class OneFormAssembler:
                                     scatter=scatter) if getattr(form, "cell_integral", True) else None
         ds = getattr(form, "ds", ())
         self._ds = _BoundaryTerms(V, ds) if ds else None
+        # an interior penalty form adds its interior- and exterior-facet loops after the cell loop
+        self._facets = form.facet_terms() if hasattr(form, "facet_terms") else None
         self._scatter = scatter
         self._loop = None
         self._tensor = None
@@ -1776,6 +2186,8 @@ class OneFormAssembler:
                                           self.u(op2.READ, V.cell_node_map)] + self.form.coefficient_args(),
                                          location="device")
             self._ds_loops = self._ds.action_loops(tensor, self.u, self._scatter) if self._ds else []
+            if self._facets is not None:
+                self._ds_loops += self._facets.action_loops(tensor, self.u, self._scatter)
         tensor.zero()
         if self._loop is not None:
             self._loop()
@@ -1807,6 +2219,10 @@ def assemble(form: Form, u=None, tensor=None, bcs=(), mat_type="aij"):
         return OneFormAssembler(form, u, bcs).assemble(tensor)
     if mat_type == "matfree":
         return ImplicitMatrixContext(form, bcs)
+    if getattr(V, "family", "CG") == "DQ":
+        raise NotImplementedError(f"mat_type {mat_type!r}: there is no assembled matrix on a DQ space (the facet "
+                                  f"terms couple neighbouring cells outside the cell sparsity); use mat_type "
+                                  f"'matfree'")
     if tensor is None:
         dsets = (V.node_set, V.node_set) if V.cdim == 1 else (V.dof_dset, V.dof_dset)
         tensor = op2.Mat(op2.Sparsity(dsets, [(V.cell_node_map, V.cell_node_map, None)]))
@@ -1891,14 +2307,16 @@ class ImplicitMatrixContext:
             # diagonal kernel
             k = self.form.kernel(1, diagonal=True)
         else:
-            k = op2.Kernel("helmholtz", degree=V.degree, alpha=self.form.alpha, beta=self.form.beta,
-                           diagonal=True)
+            k = _dq_diagonal_kernel(V, self.form.alpha, self.form.beta) if getattr(V, "element", None) is not None else \
+                op2.Kernel("helmholtz", degree=V.degree, alpha=self.form.alpha, beta=self.form.beta, diagonal=True)
         D.zero()
         if k is not None:
             op2.par_loop(k, V.cell_set, D(op2.INC, V.cell_node_map), V.coordinates(op2.READ, V.coord_map),
                          *self.form.coefficient_args())
         if getattr(self.form, "ds", ()):
             _BoundaryTerms(V, self.form.ds).diagonal(D)
+        if hasattr(self.form, "facet_terms"):
+            self.form.facet_terms().diagonal(D)
         for bc in self.bcs:
             bc.set(D, 1.0)
         return D
@@ -2298,6 +2716,15 @@ def solve(form: Form, L: op2.Dat, u: op2.Dat, bcs=(), solver_parameters=None, hi
         raise ValueError(f"ksp_type cg needs a symmetric operator, and {type(form).__name__} is not: use gmres")
     V = form.V
     bcs = tuple(bcs)
+    if getattr(V, "family", "CG") == "DQ":
+        if bcs:
+            raise ValueError("a DQ space takes no DirichletBC: impose the condition weakly "
+                             "(InteriorPenalty(..., weak_bcs=...) and nitsche_load)")
+        if sp["pc_type"] not in ("none", "jacobi"):
+            raise NotImplementedError(f"pc_type {sp['pc_type']!r} on a DQ space: 'none' or 'jacobi' (there is no "
+                                      f"DQ multigrid)")
+        if sp["pc_type"] == "jacobi":
+            _dq_diagonal_kernel(V, 1.0, 0.0)          # refuses DQ4 before anything is assembled
     lib = _lib.lib()
     n = L._data.size
     # lifting (firedrake/assemble.py:1243-1254 + linear solver's rhs): u = g on the constrained nodes,

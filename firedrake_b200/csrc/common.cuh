@@ -64,11 +64,13 @@ struct fdb_kernel_s {
     fdb_int *d_off0 = nullptr;   // device copies of the layer offsets
     fdb_int *d_off1 = nullptr;
     fdb_int h_off0[512];
-    fdb_int h_off1[8];
+    fdb_int h_off1[16];          // 8 vertices per cell, 16 on an interior facet (both cells)
     fdb_int *d_off2 = nullptr;   // a form on two spaces (FDB_FORM_STOKES): the second map's layer offsets
     fdb_int h_off2[512];
     double B2[FDB_MAX_1D * FDB_MAX_1D];   // and the second space's basis at the points, (nq, degree2 + 1)
     double Dt[FDB_MAX_1D * FDB_MAX_1D];   // collocated derivative D * B^{-1}
+    // the DG facet forms: phi_a(0), phi_a(1), phi_a'(0), phi_a'(1), rows of FDB_MAX_1D
+    double Bend[4 * FDB_MAX_1D];
     // colouring plan for FDB_SCATTER_COLOURED, built lazily per map
     const void *colour_map_key = nullptr;   // plan is valid for (map pointer, generation, end)
     uint64_t colour_map_gen = 0;
@@ -156,3 +158,8 @@ int fdb_launch_stokes_action(fdb_kernel_s *k, fdb_int start, fdb_int end, int nl
 int fdb_launch_boundary_mass(fdb_kernel_s *k, fdb_int start, fdb_int end, int nlay, const fdb_int *subset,
                              fdb_mat_t mat, double *y, const double *coords, const double *x, const unsigned *facet,
                              const fdb_int *map0, const fdb_int *map1);
+// FDB_FORM_INTERIOR_PENALTY and FDB_FORM_DG_BOUNDARY (dg_facet_hex.cu): one facet per iteration entry, facet[col *
+// sides + side] its local facet numbers ('+' first).  x != NULL: the action into y; else the diagonal into y
+int fdb_launch_dg_facet(fdb_kernel_s *k, fdb_int start, fdb_int end, int nlay, const fdb_int *subset, double *y,
+                        const double *coords, const double *x, const unsigned *facet, const fdb_int *map0,
+                        const fdb_int *map1);

@@ -52,6 +52,29 @@ int collocated_derivative(int n, const double *B, const double *D, double *Dt)
     return 0;
 }
 
+// The basis and its derivative at the ends of the interval, Bend[e * FDB_MAX_1D + a] = phi_a(0), phi_a(1),
+// phi_a'(0), phi_a'(1) for e = 0..3, from the basis at the n Gauss points: a degree-(n-1) polynomial is its
+// Lagrange interpolant through them, phi_a(x) = sum_q B[q][a] L_q(x), exactly.
+void endpoint_tables(int n, const double *B, const double *xq, double *Bend)
+{
+    for (int e = 0; e < 2; e++) {
+        const double x = (double)e;
+        for (int q = 0; q < n; q++) {
+            double den = 1.0, val = 1.0, der = 0.0;
+            for (int r = 0; r < n; r++) {
+                if (r == q) continue;
+                den *= xq[q] - xq[r];
+                der = der * (x - xq[r]) + val;      // (prod_r (x - x_r))' by the product rule
+                val *= x - xq[r];
+            }
+            for (int a = 0; a < n; a++) {
+                Bend[e * FDB_MAX_1D + a] += B[q * n + a] * val / den;
+                Bend[(2 + e) * FDB_MAX_1D + a] += B[q * n + a] * der / den;
+            }
+        }
+    }
+}
+
 // Greedy colouring of columns (base cells) so that no two columns of one
 // colour share a dof column: the deterministic fallback of the north_star
 // ("warp-aggregated atomic kernel with a colouring fallback").  Host side,
@@ -274,7 +297,7 @@ static int device_pointers(const fdb_call_args *a, bool mat, void **args, const 
 // The forms of the hand-written hex kernels: what fdb_kernel_create accepts for each and how
 // fdb_kernel_call hands its arguments to the launchers.
 enum { MODE_ACTION, MODE_MATRIX, MODE_DIAGONAL };
-enum { LAUNCH_HELMHOLTZ, LAUNCH_HELMHOLTZ_COEF, LAUNCH_ELASTICITY, LAUNCH_STOKES, LAUNCH_BOUNDARY };
+enum { LAUNCH_HELMHOLTZ, LAUNCH_HELMHOLTZ_COEF, LAUNCH_ELASTICITY, LAUNCH_STOKES, LAUNCH_BOUNDARY, LAUNCH_DG_FACET };
 
 struct fdb_hex_form {
     int form;                 // enum fdb_form
@@ -288,13 +311,13 @@ struct fdb_hex_form {
     bool residual;            // a 1-form action only
     int launcher;             // fdb_launch_helmholtz_*, fdb_launch_helmholtz_coef_* (which also run the
                               // nonlinear diffusion and advection-diffusion forms), fdb_launch_elasticity_*
-                              // fdb_launch_stokes_action (which also runs the Navier-Stokes forms) or
-                              // fdb_launch_boundary_mass
+                              // fdb_launch_stokes_action (which also runs the Navier-Stokes forms),
+                              // fdb_launch_boundary_mass or fdb_launch_dg_facet (the DG facet forms)
     int max_degree[3];        // per mode: action, matrix, diagonal
     int min_degree;
     const char *space2;       // the arguments on a second space (output and input, through a third map), or
                               // NULL: such a form is an action only, in device mode
-    int integral;             // enum fdb_integral: FDB_INTEGRAL_EXTERIOR_FACET forms run in device mode only
+    int integral;             // enum fdb_integral: facet forms run in device mode only
 };
 
 static const fdb_hex_form hex_forms[] = {
@@ -319,6 +342,12 @@ static const fdb_hex_form hex_forms[] = {
      "y_p, p", FDB_INTEGRAL_CELL},
     // gamma*inner(u, v)*ds: one exterior facet of one cell per entry, its local facet number last
     {FDB_FORM_BOUNDARY_MASS, "boundary_mass", -1, false, "facet", 1, false, LAUNCH_BOUNDARY, {5, 4, 5}, 1, nullptr,
+     FDB_INTEGRAL_EXTERIOR_FACET},
+    // the SIPG facet terms on DQ_p: one interior facet ('+' row, '-' row) per entry, the two local facet numbers
+    // last; and the Nitsche / load terms on exterior facets.  No rank 2 (no assembled DG matrix)
+    {FDB_FORM_INTERIOR_PENALTY, "interior_penalty", 1, false, "facets", 1, false, LAUNCH_DG_FACET, {4, 0, 4}, 1,
+     nullptr, FDB_INTEGRAL_INTERIOR_FACET},
+    {FDB_FORM_DG_BOUNDARY, "dg_boundary", 1, false, "facet", 1, false, LAUNCH_DG_FACET, {4, 0, 4}, 1, nullptr,
      FDB_INTEGRAL_EXTERIOR_FACET},
 };
 
@@ -417,6 +446,11 @@ static int kernel_create(const fdb_kernel_desc *d, const fdb_space2_desc *s2, fd
                   "of %s_jacobian", f->name, f->name);
         return 1;
     }
+    if (f->launcher == LAUNCH_DG_FACET && mode == MODE_MATRIX) {
+        set_error("fdb_kernel_create: %s has no rank-2 form: there is no assembled DG matrix (the facet terms couple "
+                  "neighbouring cells outside the cell sparsity); use the action and the diagonal", f->name);
+        return 1;
+    }
     if (d->degree < f->min_degree || d->degree > f->max_degree[mode]) {
         set_error("fdb_kernel_create: %s %s: degree %d outside %d..%d", f->name, mode_name[mode], d->degree,
                   f->min_degree, f->max_degree[mode]);
@@ -430,6 +464,10 @@ static int kernel_create(const fdb_kernel_desc *d, const fdb_space2_desc *s2, fd
         set_error("fdb_kernel_create: %s has exterior-facet integrals only (integral %d: %s)", f->name, d->integral,
                   d->integral == FDB_INTEGRAL_CELL ? "a cell integral"
                   : (d->integral == FDB_INTEGRAL_INTERIOR_FACET ? "interior facets are not supported" : "unknown"));
+        return 1;
+    }
+    if (f->integral == FDB_INTEGRAL_INTERIOR_FACET && d->integral != FDB_INTEGRAL_INTERIOR_FACET) {
+        set_error("fdb_kernel_create: %s has interior-facet integrals only (integral %d)", f->name, d->integral);
         return 1;
     }
     if (f->integral != FDB_INTEGRAL_CELL && d->cell == FDB_CELL_HEX_EXTRUDED && (!d->offset0 || !d->offset1)) {
@@ -459,11 +497,14 @@ static int kernel_create(const fdb_kernel_desc *d, const fdb_space2_desc *s2, fd
     k->desc = *d;
     k->hex = f;
     k->n1d = d->degree + 1;
-    k->arity = k->n1d * k->n1d * k->n1d;
+    // an interior-facet entry reads both cells: 2 (p+1)^3 dofs and 16 vertices
+    const int sides = f->integral == FDB_INTEGRAL_INTERIOR_FACET ? 2 : 1;
+    k->arity = sides * k->n1d * k->n1d * k->n1d;
+    const int arity1 = sides * 8;
     memset(k->h_off0, 0, sizeof(k->h_off0));
     memset(k->h_off1, 0, sizeof(k->h_off1));
     if (d->offset0) memcpy(k->h_off0, d->offset0, sizeof(fdb_int) * k->arity);
-    if (d->offset1) memcpy(k->h_off1, d->offset1, sizeof(fdb_int) * 8);
+    if (d->offset1) memcpy(k->h_off1, d->offset1, sizeof(fdb_int) * arity1);
     k->desc.offset0 = k->h_off0;
     k->desc.offset1 = k->h_off1;
     // the second space's map: CG_{p-1}, p^3 dofs per cell
@@ -479,11 +520,13 @@ static int kernel_create(const fdb_kernel_desc *d, const fdb_space2_desc *s2, fd
         delete k;
         return 1;
     }
+    memset(k->Bend, 0, sizeof(k->Bend));
+    if (f->launcher == LAUNCH_DG_FACET) endpoint_tables(k->n1d, d->B, d->xq, k->Bend);
     FDB_CUDA(cudaMalloc(&k->d_off0, sizeof(fdb_int) * k->arity));
-    FDB_CUDA(cudaMalloc(&k->d_off1, sizeof(fdb_int) * 8));
+    FDB_CUDA(cudaMalloc(&k->d_off1, sizeof(fdb_int) * arity1));
     FDB_CUDA(cudaMemcpyAsync(k->d_off0, k->h_off0, sizeof(fdb_int) * k->arity,
                              cudaMemcpyHostToDevice, ctx().stream));
-    FDB_CUDA(cudaMemcpyAsync(k->d_off1, k->h_off1, sizeof(fdb_int) * 8, cudaMemcpyHostToDevice,
+    FDB_CUDA(cudaMemcpyAsync(k->d_off1, k->h_off1, sizeof(fdb_int) * arity1, cudaMemcpyHostToDevice,
                              ctx().stream));
     if (f->space2) {
         FDB_CUDA(cudaMalloc(&k->d_off2, sizeof(fdb_int) * arity2));
@@ -601,7 +644,8 @@ int fdb_kernel_call(fdb_kernel_t k, const fdb_call_args *a)
     // map, second map]; with a trailing coefficient as well (the Navier-Stokes Jacobian's u) the coefficient
     // comes last: [y, coords, x, y2, x2, coef]
     // an exterior-facet form (boundary_mass): the trailing argument is the uint32 local facet number of each
-    // entry, [y, coords, x, facet] / [mat, coords, facet] / [d, coords, facet]
+    // entry, [y, coords, x, facet] / [mat, coords, facet] / [d, coords, facet]; an interior-facet form
+    // (interior_penalty): the two local facet numbers ('+', '-') of each entry, [y, coords, x, facets]
     const fdb_hex_form *f = k->hex;
     const int mode = hex_mode(&k->desc);
     if (f->integral != FDB_INTEGRAL_CELL && a->location != FDB_LOC_DEVICE) {
@@ -689,6 +733,9 @@ int fdb_kernel_call(fdb_kernel_t k, const fdb_call_args *a)
         case LAUNCH_BOUNDARY:
             return fdb_launch_boundary_mass(k, a->start, a->end, nlay, dsubset, mat, out, coords, nullptr,
                                             (const unsigned *)coef, dmaps[0], dmaps[1]);
+        case LAUNCH_DG_FACET:
+            return fdb_launch_dg_facet(k, a->start, a->end, nlay, dsubset, out, coords, nullptr,
+                                       (const unsigned *)coef, dmaps[0], dmaps[1]);
         default:
             return fdb_launch_elasticity_matrix(k, a->start, a->end, nlay, dsubset, mat, coords, coef, dmaps[0],
                                                 dmaps[1], out);
@@ -733,6 +780,10 @@ int fdb_kernel_call(fdb_kernel_t k, const fdb_call_args *a)
     case LAUNCH_BOUNDARY:
         rc = fdb_launch_boundary_mass(k, a->start, a->end, nlay, dsubset, nullptr, out, coords, x,
                                       (const unsigned *)coef, dmaps[0], dmaps[1]);
+        break;
+    case LAUNCH_DG_FACET:
+        rc = fdb_launch_dg_facet(k, a->start, a->end, nlay, dsubset, out, coords, x, (const unsigned *)coef,
+                                 dmaps[0], dmaps[1]);
         break;
     default:
         rc = fdb_launch_stokes_action(k, a->start, a->end, nlay, dsubset, out, coords, x, (double *)dargs[3],

@@ -322,6 +322,10 @@ class VCycle:
         else:
             self.kappas = self._coarsen_coefficient(kappa)
             forms = [make_form(V, k) for V, k in zip(self.spaces, self.kappas)]
+        for f in forms:
+            if getattr(f.V, "family", "CG") == "DQ":
+                raise NotImplementedError("VCycle does not take DQ spaces: its transfers and smoothers are those of "
+                                          "nested CG spaces; DQ solves take pc_type 'none' or 'jacobi'")
         self.ops = [assemble(f, bcs=b, mat_type="matfree") for f, b in zip(forms, self.bcs)]
         self.nu, self.omega = nu, omega
         self.coarse_rtol, self.coarse_maxit = coarse_rtol, coarse_maxit

@@ -1404,6 +1404,16 @@ class Kernel:
     (one per column of an extruded set, 0..5 = 2*direction + side; 4 / 5 are the bottom / top faces), read
     directly: action (output, coordinates, u, facet), diagonal and rank 2 (output, coordinates, facet).  The
     action on g is the load ``inner(g, v)*ds`` when ``alpha`` is 1.  Device-resident Dats only.
+
+    "interior_penalty" is the interior-facet part of the symmetric interior penalty discretisation on a scalar DQ_p
+    space (``element`` = its Gauss-Legendre ``Interval1D``), ``alpha*(-inner(avg(grad u), jump(v, n)) -
+    inner(jump(u, n), avg(grad v)) + (eta/avg(h))*inner(jump(u, n), jump(v, n)))*dS`` with eta = ``beta``, with
+    ``integral="interior_facet"``: one entry per facet, maps holding the '+' cell's row then the '-' cell's, and
+    the LAST argument a uint32 Dat of the two local facet numbers ('+', '-') of each entry.  "dg_boundary" is its
+    exterior-facet counterpart ``(c_m*u*v + (c_p/h)*u*v - c_s*u*dot(grad v, n) - c_f*dot(grad u, n)*v)*ds`` with
+    c_f = ``alpha``, c_p = ``beta``, and ``c_m``, ``c_s``, with ``integral="exterior_facet"`` and the arguments
+    of "boundary_mass".  Both: action (output, coordinates, u, facets) and diagonal (output, coordinates,
+    facets), no rank 2; device-resident Dats only.
     """
     form: str = "helmholtz"
     degree: int = 1
@@ -1423,6 +1433,8 @@ class Kernel:
     d: tuple = (1.0, 0.0, 0.0)      # nonlinear diffusion: D(s) = d[0] + d[1] s + d[2] s^2
     mu: float = 1.0                 # (hyper)elasticity: Lame parameters
     lmbda: float = 0.0
+    c_m: float = 0.0                # dg_boundary: the u*v and u*dot(grad v, n) coefficients
+    c_s: float = 0.0
 
     def __new__(cls, *args, **kwargs):
         # ``op2.Kernel(code, name)`` with C source (pyop2/local_kernel.py:33-43) builds the
@@ -1502,7 +1514,9 @@ _FORMS = {"helmholtz": _Form(_lib.FORM_HELMHOLTZ),
           "stokes": _Form(_lib.FORM_STOKES, pressure=True),
           "navier_stokes": _Form(_lib.FORM_NAVIER_STOKES, residual=True, pressure=True),
           "navier_stokes_jacobian": _Form(_lib.FORM_NAVIER_STOKES_JACOBIAN, coefficient=True, pressure=True),
-          "boundary_mass": _Form(_lib.FORM_BOUNDARY_MASS, facet=True)}
+          "boundary_mass": _Form(_lib.FORM_BOUNDARY_MASS, facet=True),
+          "interior_penalty": _Form(_lib.FORM_INTERIOR_PENALTY, facet=True),
+          "dg_boundary": _Form(_lib.FORM_DG_BOUNDARY, facet=True)}
 _INTEGRALS = {"cell": _lib.INTEGRAL_CELL, "exterior_facet": _lib.INTEGRAL_EXTERIOR_FACET,
               "interior_facet": _lib.INTEGRAL_INTERIOR_FACET, "fused": _lib.INTEGRAL_FUSED}
 
@@ -1589,6 +1603,8 @@ class GlobalKernel:
         d.affine_cells = int(lk.affine and lk.rank == 1 and not lk.diagonal)
         for i in range(3):
             d.dcoef[i] = lk.d[i]
+        if lk.form == "dg_boundary":
+            d.dcoef[0], d.dcoef[1], d.dcoef[2] = lk.c_m, lk.c_s, 0.0
         if spec.lame:
             d.alpha, d.lmbda = lk.mu, lk.lmbda
         s2 = None

@@ -22,12 +22,12 @@ from __future__ import annotations
 
 import numpy as np
 
-from .fiat_lite import gll_points
+from .fiat_lite import gauss_legendre, gll_points
 
 IntType = np.int32
 ScalarType = np.float64
 
-__all__ = ["ExtrudedHexMesh", "ExtrudedFunctionSpace", "UnitSquareTriMesh",
+__all__ = ["ExtrudedHexMesh", "ExtrudedFunctionSpace", "ExtrudedDGFunctionSpace", "UnitSquareTriMesh",
            "QuadMesh"]
 
 
@@ -194,6 +194,13 @@ class ExtrudedHexMesh:
         if degree not in self._fs_cache:
             self._fs_cache[degree] = ExtrudedFunctionSpace(self, degree)
         return self._fs_cache[degree]
+
+    def dg_function_space(self, degree: int) -> "ExtrudedDGFunctionSpace":
+        """Scalar DQ_p (p = 1..4) with Firedrake's default "spectral" variant: Gauss-Legendre nodes."""
+        cache = self.__dict__.setdefault("_dg_fs_cache", {})
+        if degree not in cache:
+            cache[degree] = ExtrudedDGFunctionSpace(self, degree)
+        return cache[degree]
 
     def _apply_warp(self, X):
         if self.warp == 0.0:
@@ -371,6 +378,62 @@ class ExtrudedFunctionSpace:
         size = nb[ents] * (p * nz + 1)
         idx = np.concatenate([np.arange(s, s + k) for s, k in zip(st[ents], size)])
         return np.sort(idx).astype(IntType)
+
+
+class ExtrudedDGFunctionSpace:
+    """Scalar DQ_p = dQ_p (x) dP_p space on an :class:`ExtrudedHexMesh` with Gauss-Legendre nodes (the default
+    "spectral" variant of a DG element, SURVEY.md section 7).  Every dof belongs to one cell: the numbering is
+    cell-major, base column c (in the mesh's cell order) holds the ``nz * (p+1)^3`` dofs ``c * nz * (p+1)^3 ..``
+    layer by layer, so the layer offset of every local dof is ``(p+1)^3``.  The local index is ``(ax*n + ay)*n +
+    az`` with the 1-D indices in ascending node position."""
+
+    def __init__(self, mesh: ExtrudedHexMesh, degree: int):
+        p = int(degree)
+        if not 1 <= p <= 4:
+            raise ValueError(f"DQ degree {p} outside 1..4")
+        self.mesh = mesh
+        self.degree = p
+        self.n = n = p + 1
+        self.arity = n ** 3
+        nz = mesh.nz
+        self.node_count = mesh.num_base_cells * nz * self.arity
+        self.owned_node_count = self.node_count
+        self.ghost_node_count = 0
+        if self.node_count >= 2 ** 31:
+            raise ValueError("node count exceeds int32 IntType")
+        self.cell_node_map = (np.arange(mesh.num_base_cells, dtype=np.int64)[:, None] * (nz * self.arity)
+                              + np.arange(self.arity)[None, :]).astype(IntType)
+        self.offset = np.full(self.arity, self.arity, dtype=IntType)
+
+    def full_cell_node_list(self):
+        """(num_cells, arity) map with the layer loop expanded: row ``c*nz + l`` is column c, layer l."""
+        nz = self.mesh.nz
+        lay = np.arange(nz, dtype=np.int64)
+        full = (self.cell_node_map[:, None, :].astype(np.int64)
+                + lay[None, :, None] * self.offset[None, None, :])
+        return full.reshape(-1, self.arity).astype(IntType)
+
+    def dof_coordinates(self):
+        """Physical positions of all dofs, (node_count, 3): the trilinear image of the Gauss-Legendre points."""
+        mesh, n = self.mesh, self.n
+        xi, _ = gauss_legendre(n)
+        full = self.full_cell_node_list().astype(np.int64)
+        XV = mesh.coordinates[mesh.coord_space.full_cell_node_list().astype(np.int64)]     # (ncell, 8, 3)
+        out = np.empty((self.node_count, 3), dtype=ScalarType)
+        for ax in range(n):
+            for ay in range(n):
+                for az in range(n):
+                    pt = np.zeros((full.shape[0], 3))
+                    for v in range(8):
+                        bx, by, bz = (v >> 2) & 1, (v >> 1) & 1, v & 1
+                        pt += ((xi[ax] if bx else 1 - xi[ax]) * (xi[ay] if by else 1 - xi[ay])
+                               * (xi[az] if bz else 1 - xi[az])) * XV[:, v, :]
+                    out[full[:, (ax * n + ay) * n + az]] = pt
+        return out
+
+    def boundary_nodes(self, sub_domain):
+        raise ValueError("a DQ space has no boundary nodes: every dof is interior to its cell.  Impose Dirichlet "
+                         "conditions weakly (InteriorPenalty's weak_bcs and nitsche_load)")
 
 
 class UnitSquareTriMesh:

@@ -234,7 +234,7 @@ enum fdb_form {
                                    argument, read through maps[0]:
                                      action  [y_u INC, coords, w, y_p INC, r, u]
                                              maps [V map, coord map, Q map]                       */
-    FDB_FORM_BOUNDARY_MASS = 13
+    FDB_FORM_BOUNDARY_MASS = 13,
                                 /* the boundary mass term, an EXTERIOR-FACET integral (symmetric):
                                      a(u, v) = gamma*inner(u, v)*ds
                                    gamma = alpha.  The Robin operator term, and through its action every
@@ -254,6 +254,42 @@ enum fdb_form {
                                                same in each component)
                                      rank 2    [Mat, coords, facet]  (block size cdim; the components
                                                do not couple: block diagonals only)               */
+    FDB_FORM_INTERIOR_PENALTY = 14,
+                                /* the interior-facet terms of the symmetric interior penalty (SIPG)
+                                   discretisation on scalar DQ_p (Gauss-Legendre nodes), an
+                                   INTERIOR-FACET integral (symmetric):
+                                     a(u, v) = alpha*( -inner(avg(grad u), jump(v, n))
+                                                       - inner(jump(u, n), avg(grad v))
+                                                       + (eta/avg(h))*inner(jump(u, n), jump(v, n)) )*dS
+                                   alpha = alpha, eta = beta; h = the cell diameter (largest distance
+                                   between two of the cell's 8 vertices), n the unit normal outward from
+                                   '+'.  integral == FDB_INTEGRAL_INTERIOR_FACET.  Hex cells (extruded or
+                                   native), cdim 1, nq == degree+1, affine_cells == 0, degrees 1..4,
+                                   action and diagonal (there is no assembled DG matrix: rank 2 is
+                                   refused).  An iteration entry is one facet: maps[0] is the '+' cell's
+                                   row followed by the '-' cell's (arity 2*(degree+1)^3, offsets tiled),
+                                   maps[1] their 8 + 8 vertices; the LAST argument holds the two uint32
+                                   local facet numbers ('+', '-') of each entry (per column on extruded
+                                   sets, numbered as for FDB_FORM_BOUNDARY_MASS).  Both sides must
+                                   parametrise the face alike: face point (s, t) of '+' is face point
+                                   (s, t) of '-'.  Device mode only:
+                                     action    [y INC, coords, u, facets]  (atomic or coloured)
+                                     diagonal  [d INC, coords, facets]                            */
+    FDB_FORM_DG_BOUNDARY = 15
+                                /* the exterior-facet terms of the same discretisation, an
+                                   EXTERIOR-FACET integral:
+                                     a(u, v) = ( c_m*u*v + (c_p/h)*u*v - c_s*u*dot(grad v, n)
+                                                 - c_f*dot(grad u, n)*v )*ds
+                                   c_f = alpha, c_p = beta, c_m = dcoef[0], c_s = dcoef[1].  Nitsche's
+                                   weak Dirichlet operator is (c_m, c_p, c_s, c_f) = (0, alpha*eta,
+                                   alpha, alpha); its action on g with (0, alpha*eta, alpha, 0) is the
+                                   Dirichlet load of g, with (1, 0, 0, 0) the flux load g*v*ds.  Hex
+                                   cells, cdim 1, nq == degree+1, affine_cells == 0, degrees 1..4,
+                                   action and diagonal (rank 2 is refused).  An iteration entry is one
+                                   facet of one cell: the cell's rows (full (degree+1)^3 and 8), the LAST
+                                   argument its uint32 local facet number.  Device mode only:
+                                     action    [y INC, coords, u, facet]  (atomic or coloured)
+                                     diagonal  [d INC, coords, facet]                             */
 };
 
 enum fdb_cell {
@@ -314,6 +350,7 @@ typedef struct fdb_kernel_desc {
      * tsfc/fem.py:793-797 unrolls only simplices); fdb_cells_are_affine() checks the promise. */
     int32_t affine_cells;
     /* FDB_FORM_NONLINEAR_DIFFUSION[_JACOBIAN]: D(s) = dcoef[0] + dcoef[1] s + dcoef[2] s^2.
+     * FDB_FORM_DG_BOUNDARY: c_m = dcoef[0], c_s = dcoef[1].
      * Ignored by every other form (a zeroed descriptor stays valid for them). */
     double dcoef[3];
     /* FDB_FORM_ELASTICITY, FDB_FORM_HYPERELASTICITY[_JACOBIAN]: the Lame parameter lambda (mu is
