@@ -29,6 +29,7 @@ FORM_NAVIER_STOKES_JACOBIAN = 12
 FORM_BOUNDARY_MASS = 13
 FORM_INTERIOR_PENALTY = 14
 FORM_DG_BOUNDARY = 15
+FORM_DG_TRANSPORT = 16
 CELL_HEX_EXTRUDED = 1
 CELL_HEX = 2
 CELL_TRIANGLE = 3

@@ -1090,6 +1090,163 @@ def assemble_interior_penalty_generic(F: "InteriorPenalty", u: op2.Dat, tensor=N
     return tensor
 
 
+def dg_transport_kernels(degree, name=None):
+    """C sources of the transport terms of :class:`DGTransport` on DQ_p hexes (Gauss-Legendre nodes, trilinear
+    geometry, b trilinear from the 8 vertex values), written the way TSFC would (the whole cell's basis and its
+    physical gradient at every point, n and the surface measure of the '+' cell), for the generic wrapper builder:
+    the independent statement of the hand-written FDB_FORM_DG_TRANSPORT kernels.  Returns {"cell": -u*dot(b, grad
+    v)*dx (args y (INC), coords, u, b), "dS_v": the upwind flux over the vertical interior facets (args y, coords, u,
+    b, facets uint[2]), "dS_h": the same with the pair (5, 4) baked in, for ON_INTERIOR_FACETS over the cells (args y,
+    coords, u, b), "ds": the outflow term max(dot(b, n), 0)*u*v*ds (args y, coords, u, b, facet uint[1])}."""
+    from .codegen import CStringKernel
+    from .fiat_lite import interval_element
+    el = interval_element(degree, variant="gl")
+    n, nd = degree + 1, (degree + 1) ** 3
+    Bend, Dend = el.tabulate([0.0, 1.0])
+    tab = lambda a: "{" + ", ".join("{" + ", ".join(repr(float(v)) for v in r) + "}" for r in a) + "}"
+    vec = lambda a: "{" + ", ".join(repr(float(v)) for v in a) + "}"
+    base = name or f"dg_transport{degree}"
+    head = f"""
+static const double TB[{n}][{n}] = {tab(el.B)};      /* basis a at Gauss point q */
+static const double TD[{n}][{n}] = {tab(el.D)};      /* its derivative */
+static const double TE[2][{n}] = {tab(Bend)};        /* basis at the interval's ends */
+static const double TF[2][{n}] = {tab(Dend)};        /* derivative at the ends */
+static const double TX[{n}] = {vec(el.xq)};
+static const double TW[{n}] = {vec(el.wq)};
+/* at reference point xi, with the 1-D tables T, DT of each axis there: the values and physical gradients of the
+   cell's {nd} basis functions, the inverse Jacobian K (K[d][c] = dxi_d/dx_c), b (trilinear) and |det J| */
+static double tables(const double *X, const double *bv, const double xi[3], const double *T[3], const double *DT[3],
+                     double *phi, double (*grad)[3], double K[3][3], double *b)
+{{
+    double J[3][3];
+    for (int c = 0; c < 3; ++c) {{ b[c] = 0.0; for (int d = 0; d < 3; ++d) J[c][d] = 0.0; }}
+    for (int v = 0; v < 8; ++v) {{
+        const int bb[3] = {{(v >> 2) & 1, (v >> 1) & 1, v & 1}};
+        double w = 1.0;
+        for (int e = 0; e < 3; ++e) w *= bb[e] ? xi[e] : 1.0 - xi[e];
+        for (int c = 0; c < 3; ++c) b[c] += w * bv[v * 3 + c];
+        for (int d = 0; d < 3; ++d) {{
+            double g = bb[d] ? 1.0 : -1.0;
+            for (int e = 0; e < 3; ++e) if (e != d) g *= bb[e] ? xi[e] : 1.0 - xi[e];
+            for (int c = 0; c < 3; ++c) J[c][d] += X[v * 3 + c] * g;
+        }}
+    }}
+    const double det = J[0][0] * (J[1][1] * J[2][2] - J[1][2] * J[2][1])
+                     - J[0][1] * (J[1][0] * J[2][2] - J[1][2] * J[2][0])
+                     + J[0][2] * (J[1][0] * J[2][1] - J[1][1] * J[2][0]);
+    for (int d = 0; d < 3; ++d) for (int c = 0; c < 3; ++c) {{
+        const int d1_ = (d + 1) % 3, d2_ = (d + 2) % 3, c1 = (c + 1) % 3, c2 = (c + 2) % 3;
+        K[d][c] = (J[c1][d1_] * J[c2][d2_] - J[c1][d2_] * J[c2][d1_]) / det;   /* cofactor of J[c][d] */
+    }}
+    for (int a = 0; a < {n}; ++a) for (int b1 = 0; b1 < {n}; ++b1) for (int c = 0; c < {n}; ++c) {{
+        const int i = (a * {n} + b1) * {n} + c;
+        const double r[3] = {{DT[0][a] * T[1][b1] * T[2][c], T[0][a] * DT[1][b1] * T[2][c], T[0][a] * T[1][b1] * DT[2][c]}};
+        phi[i] = T[0][a] * T[1][b1] * T[2][c];
+        for (int e = 0; e < 3; ++e) grad[i][e] = K[0][e] * r[0] + K[1][e] * r[1] + K[2][e] * r[2];
+    }}
+    return fabs(det);
+}}
+/* the tables of facet f at face point (q1, q2) */
+static double face_tables(const double *X, const double *bv, int f, int q1, int q2, double *phi, double (*grad)[3],
+                          double K[3][3], double *b)
+{{
+    const int fd = f / 2, fs = f % 2, d1 = fd == 0 ? 1 : 0, d2 = fd == 2 ? 1 : 2;
+    double xi[3];
+    const double *T[3], *DT[3];
+    xi[fd] = (double)fs; xi[d1] = TX[q1]; xi[d2] = TX[q2];
+    T[fd] = TE[fs]; T[d1] = TB[q1]; T[d2] = TB[q2];
+    DT[fd] = TF[fs]; DT[d1] = TD[q1]; DT[d2] = TD[q2];
+    return tables(X, bv, xi, T, DT, phi, grad, K, b);
+}}
+/* the unit normal outward from the cell on facet f and the surface measure |det J| |J^-T n_ref| */
+static double normal(int f, double det, double K[3][3], double *nrm)
+{{
+    const int fd = f / 2;
+    const double sg = f % 2 ? 1.0 : -1.0;
+    const double l = sqrt(K[fd][0] * K[fd][0] + K[fd][1] * K[fd][1] + K[fd][2] * K[fd][2]);
+    for (int c = 0; c < 3; ++c) nrm[c] = sg * K[fd][c] / l;
+    return det * l;
+}}
+"""
+    cell = f"""static void {base}_cell(double *A, const double *X, const double *w, const double *bv)
+{{
+    for (int qx = 0; qx < {n}; ++qx) for (int qy = 0; qy < {n}; ++qy) for (int qz = 0; qz < {n}; ++qz) {{
+        double phi[{nd}], grad[{nd}][3], K[3][3], b[3], u = 0.0;
+        const double xi[3] = {{TX[qx], TX[qy], TX[qz]}};
+        const double *T[3] = {{TB[qx], TB[qy], TB[qz]}}, *DT[3] = {{TD[qx], TD[qy], TD[qz]}};
+        const double W = TW[qx] * TW[qy] * TW[qz] * tables(X, bv, xi, T, DT, phi, grad, K, b);
+        for (int i = 0; i < {nd}; ++i) u += phi[i] * w[i];
+        for (int i = 0; i < {nd}; ++i) A[i] -= W * u * (b[0] * grad[i][0] + b[1] * grad[i][1] + b[2] * grad[i][2]);
+    }}
+}}
+"""
+    interior = """
+{{
+    const int fac[2] = {{(int)({fp}), (int)({fm})}};
+    for (int q1 = 0; q1 < {n}; ++q1) for (int q2 = 0; q2 < {n}; ++q2) {{
+        double phi[2][{nd}], grad[{nd}][3], K[3][3], b[3], bm[3], nrm[3], u[2] = {{0.0, 0.0}};
+        const double det = face_tables(X, bv, fac[0], q1, q2, phi[0], grad, K, b);
+        const double W = TW[q1] * TW[q2] * normal(fac[0], det, K, nrm);
+        face_tables(X + 24, bv + 24, fac[1], q1, q2, phi[1], grad, K, bm);
+        for (int s = 0; s < 2; ++s) for (int i = 0; i < {nd}; ++i) u[s] += phi[s][i] * w[s * {nd} + i];
+        const double bn = b[0] * nrm[0] + b[1] * nrm[1] + b[2] * nrm[2];
+        const double flux = W * bn * (bn >= 0.0 ? u[0] : u[1]);
+        for (int i = 0; i < {nd}; ++i) {{
+            A[i] += flux * phi[0][i];
+            A[{nd} + i] -= flux * phi[1][i];
+        }}
+    }}
+}}
+"""
+    dS_v = f"static void {base}_dS(double *A, const double *X, const double *w, const double *bv, " \
+           f"const unsigned int *facet)" + interior.format(fp="facet[0]", fm="facet[1]", n=n, nd=nd)
+    dS_h = f"static void {base}_dSh(double *A, const double *X, const double *w, const double *bv)" + \
+        interior.format(fp="5", fm="4", n=n, nd=nd)
+    ds = f"""static void {base}_ds(double *A, const double *X, const double *w, const double *bv,
+                                  const unsigned int *facet)
+{{
+    const int f = (int)facet[0];
+    for (int q1 = 0; q1 < {n}; ++q1) for (int q2 = 0; q2 < {n}; ++q2) {{
+        double phi[{nd}], grad[{nd}][3], K[3][3], b[3], nrm[3], u = 0.0;
+        const double det = face_tables(X, bv, f, q1, q2, phi, grad, K, b);
+        const double W = TW[q1] * TW[q2] * normal(f, det, K, nrm);
+        const double bn = b[0] * nrm[0] + b[1] * nrm[1] + b[2] * nrm[2];
+        for (int i = 0; i < {nd}; ++i) u += phi[i] * w[i];
+        for (int i = 0; i < {nd}; ++i) A[i] += W * (bn > 0.0 ? bn : 0.0) * u * phi[i];
+    }}
+}}
+"""
+    return {"cell": CStringKernel(head + cell, f"{base}_cell"), "dS_v": CStringKernel(head + dS_v, f"{base}_dS"),
+            "dS_h": CStringKernel(head + dS_h, f"{base}_dSh"), "ds": CStringKernel(head + ds, f"{base}_ds")}
+
+
+def assemble_dg_transport_generic(F: "DGTransport", u: op2.Dat, tensor=None):
+    """The transport terms of ``assemble(action(a, u))`` for a :class:`DGTransport` form (cell, upwind dS and outflow
+    ds; not the Helmholtz or interior penalty parts) through the generic wrapper path (:func:`dg_transport_kernels`),
+    over the same facet sets as the hand-written path: the cross-check and the baseline of FDB_FORM_DG_TRANSPORT."""
+    from . import codegen
+    V, b = F.V, F.b
+    if tensor is None:
+        tensor = V.dat()
+    tensor.zero()
+    tensor.device_ptr
+    ks = dg_transport_kernels(V.degree)
+    codegen.par_loop(ks["cell"], V.cell_set, tensor(op2.INC, V.cell_node_map), V.coordinates(op2.READ, V.coord_map),
+                     u(op2.READ, V.cell_node_map), b(op2.READ, V.coord_map))
+    for fset, fmap, cmap, pairs in _dg_interior_groups(V):
+        if fset.layers == V.mesh.layers:            # the vertical group
+            codegen.par_loop(ks["dS_v"], fset, tensor(op2.INC, fmap), V.coordinates(op2.READ, cmap),
+                             u(op2.READ, fmap), b(op2.READ, cmap), pairs(op2.READ))
+    if V.mesh.nz > 1:
+        codegen.par_loop(ks["dS_h"], V.cell_set, tensor(op2.INC, V.cell_node_map),
+                         V.coordinates(op2.READ, V.coord_map), u(op2.READ, V.cell_node_map),
+                         b(op2.READ, V.coord_map), iteration_region="ON_INTERIOR_FACETS")
+    for fset, fmap, cmap, facet in _boundary_groups(V, "on_boundary"):
+        codegen.par_loop(ks["ds"], fset, tensor(op2.INC, fmap), V.coordinates(op2.READ, cmap), u(op2.READ, fmap),
+                         b(op2.READ, cmap), facet(op2.READ))
+    return tensor
+
+
 def hyperelasticity_kernel(degree, mu, lmbda, beta=0.0, jacobian=False, name=None):
     """C source of the residual of compressible Neo-Hookean hyperelasticity,
     ``inner(P(F), grad(v))*dx + beta*inner(u, v)*dx`` with ``F = I + grad(u)``, ``J = det(F)`` and
@@ -1656,7 +1813,8 @@ def _dg_load(V, coefs, sub_domain, g, tensor):
 
 
 def nitsche_load(F: InteriorPenalty, g: op2.Dat, tensor: op2.Dat = None):
-    """The Dirichlet load of ``g`` (a Dat on F.V) on F's weak_bcs, alpha*(-g*dot(grad v, n) + (eta/h)*g*v)*ds."""
+    """The Dirichlet load of ``g`` (a Dat on F.V) on F's weak_bcs, alpha*(-g*dot(grad v, n) + (eta/h)*g*v)*ds, for an
+    :class:`InteriorPenalty` form or the diffusion part of a :class:`DGTransport` form."""
     if not F.weak_bcs:
         raise ValueError("the form has no weakly imposed Dirichlet sub-domains (weak_bcs=())")
     return _dg_load(F.V, (0.0, F.alpha * F.eta, F.alpha, 0.0), F.weak_bcs, g, tensor)
@@ -1668,6 +1826,192 @@ def dg_flux_load(V: FunctionSpace, g: op2.Dat, sub_domain="on_boundary", tensor:
         raise ValueError("dg_flux_load takes a DQ space; on CG spaces the load is assemble(BoundaryMass(V, 1, "
                          "sub_domain), u=g)")
     return _dg_load(V, (1.0, 0.0, 0.0, 0.0), sub_domain, g, tensor)
+
+
+def _dg_transport_kernel(V, integral, diagonal=False, c_out=1.0, c_in=0.0):
+    return op2.Kernel("dg_transport", degree=V.degree, integral=integral, diagonal=diagonal, element=V.element,
+                      c_out=float(c_out), c_in=float(c_in))
+
+
+def _dg_transport_boundary_loops(F, tensor, u, c_out, c_in, scatter="atomic"):
+    """The FDB_FORM_DG_TRANSPORT exterior-facet parloops of (c_out, c_in) over every boundary facet of F.V."""
+    V, loops = F.V, []
+    for fset, fmap, cmap, facet in _boundary_groups(V, "on_boundary"):
+        gk = op2.GlobalKernel(_dg_transport_kernel(V, "exterior_facet", False, c_out, c_in), [fmap, cmap],
+                              extruded=True, scatter=scatter)
+        loops.append(op2.Parloop(gk, fset, [tensor(op2.INC, fmap), V.coordinates(op2.READ, cmap), u(op2.READ, fmap),
+                                            F.b(op2.READ, cmap), facet(op2.READ)], location="device"))
+    return loops
+
+
+class _DGTransportTerms:
+    """The loops of a :class:`DGTransport` form after its transport cell loop: the Helmholtz cell loop (alpha or
+    beta nonzero), :class:`InteriorPenalty`'s own facet loops (alpha > 0), the upwind FDB_FORM_DG_TRANSPORT loops over
+    every interior facet group and the outflow loops (c_out, c_in) = (1, 0) over every boundary facet."""
+
+    def __init__(self, form: "DGTransport"):
+        self.form = form
+        V = form.V
+        self.interior = _dg_interior_groups(V)
+        self.helmholtz = Form(V, form.alpha, form.beta) if (form.alpha or form.beta) else None
+        self.sipg = _DGFacetTerms(form) if form.alpha > 0 else None
+
+    def action_loops(self, tensor: op2.Dat, u: op2.Dat, scatter="atomic"):
+        F = self.form
+        V, loops = F.V, []
+        if self.helmholtz is not None:
+            gk = op2.GlobalKernel(self.helmholtz.kernel(1), [V.cell_node_map, V.coord_map], extruded=True,
+                                  scatter=scatter)
+            loops.append(op2.Parloop(gk, V.cell_set, [tensor(op2.INC, V.cell_node_map),
+                                                      V.coordinates(op2.READ, V.coord_map),
+                                                      u(op2.READ, V.cell_node_map)], location="device"))
+        if self.sipg is not None:
+            loops += self.sipg.action_loops(tensor, u, scatter)
+        for fset, fmap, cmap, pairs in self.interior:
+            gk = op2.GlobalKernel(_dg_transport_kernel(V, "interior_facet"), [fmap, cmap], extruded=True,
+                                  scatter=scatter)
+            loops.append(op2.Parloop(gk, fset, [tensor(op2.INC, fmap), V.coordinates(op2.READ, cmap),
+                                                u(op2.READ, fmap), F.b(op2.READ, cmap), pairs(op2.READ)],
+                                     location="device"))
+        return loops + _dg_transport_boundary_loops(F, tensor, u, 1.0, 0.0, scatter)
+
+    def diagonal(self, D: op2.Dat):
+        F = self.form
+        V = F.V
+        if self.helmholtz is not None:
+            op2.par_loop(_dq_diagonal_kernel(V, F.alpha, F.beta), V.cell_set, D(op2.INC, V.cell_node_map),
+                         V.coordinates(op2.READ, V.coord_map))
+        if self.sipg is not None:
+            self.sipg.diagonal(D)
+        for fset, fmap, cmap, pairs in self.interior:
+            op2.par_loop(_dg_transport_kernel(V, "interior_facet", True), fset, D(op2.INC, fmap),
+                         V.coordinates(op2.READ, cmap), F.b(op2.READ, cmap), pairs(op2.READ))
+        for fset, fmap, cmap, facet in _boundary_groups(V, "on_boundary"):
+            op2.par_loop(_dg_transport_kernel(V, "exterior_facet", True), fset, D(op2.INC, fmap),
+                         V.coordinates(op2.READ, cmap), F.b(op2.READ, cmap), facet(op2.READ))
+
+
+@dataclass
+class DGTransport:
+    """Upwind DG transport of a scalar DQ_p field (``FunctionSpace(mesh, p, family="DQ")``, p = 1..4) by a velocity
+    ``b`` given at the mesh vertices (a Dat on ``op2.DataSet(V.vertex_set, 3)``, interpolated trilinearly), in the
+    conservative form of Firedrake's DG_advection demo, with optional reaction and diffusion:
+
+        a(u, v) = - u*dot(b, grad v)*dx + beta*u*v*dx + alpha*inner(grad u, grad v)*dx
+                  + dot(b, n('+'))*u_up*(v('+') - v('-'))*dS       (u_up: u on the side b.n points away from)
+                  + max(dot(b, n), 0)*u*v*ds                        (outflow)
+                  + [alpha > 0] the dS terms and the ds(weak_bcs) Nitsche terms of InteriorPenalty(V, alpha, 0, eta,
+                    weak_bcs)
+
+    Every integral has p+1 Gauss points per axis.  b is single-valued on every face, so the flux is exactly
+    conservative: ``1^T A q`` is the outflow flux.  The inflow condition u = g enters through the load
+    :func:`inflow_load`; Dirichlet values of the diffusion part through :func:`nitsche_load`.  ``assemble(F, u=x)`` is
+    the action, ``mat_type="matfree"`` an operator with ``mult`` and ``getDiagonal`` (no assembled matrix; the
+    diagonal for p = 1..4 without alpha and beta, p = 1..3 with them); :func:`solve` runs GMRES with ``pc_type``
+    "none" or "jacobi", and :func:`ssprk3` steps ``M dq/dt = load - A q`` in time.  The transport terms run on
+    FDB_FORM_DG_TRANSPORT, the rest on the kernels of :class:`InteriorPenalty`."""
+    V: FunctionSpace
+    b: op2.Dat
+    beta: float = 0.0
+    alpha: float = 0.0
+    eta: float = None
+    weak_bcs: object = ()
+    symmetric = False
+    ds = ()
+
+    def __post_init__(self):
+        if getattr(self.V, "family", "CG") != "DQ":
+            raise ValueError("DGTransport takes a DQ space: FunctionSpace(mesh, p, family='DQ')")
+        ds = getattr(self.b, "dataset", None)
+        if ds is None or ds.set is not self.V.vertex_set or self.b.cdim != 3:
+            raise ValueError("DGTransport's b has 3 values per mesh vertex: a Dat on op2.DataSet(V.vertex_set, 3)")
+        self.alpha, self.beta = float(self.alpha), float(self.beta)
+        if self.alpha < 0:
+            raise ValueError(f"DGTransport: the diffusivity alpha must be >= 0, got {self.alpha}")
+        if self.alpha > 0 and self.eta is None:
+            raise ValueError("DGTransport with alpha > 0 needs the interior penalty eta (no default), e.g. 3*(p+1)**2")
+        if self.eta is not None:
+            self.eta = float(self.eta)
+        if isinstance(self.weak_bcs, list):
+            self.weak_bcs = tuple(self.weak_bcs)
+        if self.weak_bcs and not self.alpha > 0:
+            raise ValueError("DGTransport's weak_bcs are the Nitsche terms of the diffusion part and need alpha > 0; "
+                             "the inflow condition is inflow_load")
+        if self.weak_bcs:
+            _boundary_groups(self.V, self.weak_bcs)
+        _boundary_groups(self.V, "on_boundary")
+        _dg_interior_groups(self.V)
+
+    def coefficient_args(self):
+        return [self.b(op2.READ, self.V.coord_map)]
+
+    def kernel(self, rank, diagonal=False):
+        """The transport cell term - u*dot(b, grad v)*dx (its diagonal with ``diagonal``)."""
+        if rank == 2:
+            raise NotImplementedError("DGTransport has no assembled matrix: use the action and mat_type 'matfree'")
+        return _dg_transport_kernel(self.V, "cell", diagonal)
+
+    def facet_terms(self):
+        if "_facet_terms" not in self.__dict__:
+            self._facet_terms = _DGTransportTerms(self)
+        return self._facet_terms
+
+
+def inflow_load(F: DGTransport, g: op2.Dat, tensor: op2.Dat = None):
+    """The inflow load -min(dot(b, n), 0)*g*v*ds of a boundary value ``g`` (a Dat on F.V) for a
+    :class:`DGTransport` form: the right-hand side that imposes u = g where the flow enters."""
+    if not isinstance(F, DGTransport):
+        raise TypeError("inflow_load takes a DGTransport form")
+    if tensor is None:
+        tensor = F.V.dat()
+    tensor.zero()
+    for loop in _dg_transport_boundary_loops(F, tensor, g, 0.0, -1.0):
+        loop()
+    return tensor
+
+
+def ssprk3(F: DGTransport, q: op2.Dat, dt, steps, load: op2.Dat = None):
+    """Advance ``M dq/dt = load - A q`` by ``steps`` steps of the three-stage strong-stability-preserving Runge-Kutta
+    method of Firedrake's DG_advection demo, in place on the device; A is F's operator, M the mass matrix of F.V and
+    ``load`` (e.g. :func:`inflow_load`) is constant in time.  With Gauss-Legendre collocation M is exactly diagonal on
+    any hex mesh, and M^-1 is the reciprocal of ``assemble(mass(V), u=1)``.  Stability is the caller's: the scheme is
+    explicit and dt must satisfy the CFL condition of the mesh, the degree and b (roughly dt <= h / ((2p + 1) |b|)).
+    Returns q."""
+    from . import _lib
+    from . import mg as _mg
+    V = F.V
+    lib = _lib.lib()
+    n = q._data.size
+    minv = assemble(mass(V), u=V.dat(np.ones(V.node_count)))
+    op2.par_loop(_mg.reciprocal_kernel(1), V.node_set, minv(op2.RW))
+    A = ImplicitMatrixContext(F)
+    r, s1, s2 = V.dat(), V.dat(), V.dat()
+    dt = float(dt)
+
+    def stage(src, dst):
+        """dst = src + dt M^-1 (load - A src)"""
+        A.mult(src, r)
+        if load is not None:
+            _lib.check(lib.fdb_vec_aypx(n, -1.0, load.device_ptr, r.device_ptr))
+        else:
+            _lib.check(lib.fdb_vec_scale(n, -1.0, r.device_ptr))
+        _lib.check(lib.fdb_vec_pointwise_mult(n, r.device_ptr, minv.device_ptr, r.device_ptr))
+        r._device_written()
+        if dst is not src:
+            src.copy(dst)
+        dst.axpy(dt, r)
+
+    for _ in range(int(steps)):
+        stage(q, s1)                                    # q1 = q + dt L(q)
+        stage(s1, s1)
+        _lib.check(lib.fdb_vec_scale(n, 0.25, s1.device_ptr))
+        s1._device_written()
+        s1.axpy(0.75, q)                                # q2 = 3/4 q + 1/4 (q1 + dt L(q1))
+        stage(s1, s2)
+        _lib.check(lib.fdb_vec_scale(n, 1.0 / 3.0, q.device_ptr))
+        q._device_written()
+        q.axpy(2.0 / 3.0, s2)                           # q = 1/3 q + 2/3 (q2 + dt L(q2))
+    return q
 
 
 @dataclass
@@ -2349,7 +2693,7 @@ class ImplicitMatrixContext:
         is not implemented."""
         if not getattr(self.form, "symmetric", True):
             which = "advection-diffusion" if isinstance(self.form, AdvectionDiffusion) else \
-                "the nonlinear diffusion Jacobian"
+                "DG transport" if isinstance(self.form, DGTransport) else "the nonlinear diffusion Jacobian"
             raise NotImplementedError(f"multTranspose of a nonsymmetric form ({which})")
         return self.mult(X, Y)
 
@@ -2723,7 +3067,7 @@ def solve(form: Form, L: op2.Dat, u: op2.Dat, bcs=(), solver_parameters=None, hi
         if sp["pc_type"] not in ("none", "jacobi"):
             raise NotImplementedError(f"pc_type {sp['pc_type']!r} on a DQ space: 'none' or 'jacobi' (there is no "
                                       f"DQ multigrid)")
-        if sp["pc_type"] == "jacobi":
+        if sp["pc_type"] == "jacobi" and not (isinstance(form, DGTransport) and not (form.alpha or form.beta)):
             _dq_diagonal_kernel(V, 1.0, 0.0)          # refuses DQ4 before anything is assembled
     lib = _lib.lib()
     n = L._data.size

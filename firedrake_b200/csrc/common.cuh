@@ -163,3 +163,11 @@ int fdb_launch_boundary_mass(fdb_kernel_s *k, fdb_int start, fdb_int end, int nl
 int fdb_launch_dg_facet(fdb_kernel_s *k, fdb_int start, fdb_int end, int nlay, const fdb_int *subset, double *y,
                         const double *coords, const double *x, const unsigned *facet, const fdb_int *map0,
                         const fdb_int *map1);
+// FDB_FORM_DG_TRANSPORT: the cell term (dg_transport_hex.cu, facet == NULL) or the upwind facet terms
+// (dg_facet_hex.cu); b holds 3 values per vertex, read through map1.  x != NULL: the action; else the diagonal
+int fdb_launch_dg_transport(fdb_kernel_s *k, fdb_int start, fdb_int end, int nlay, const fdb_int *subset, double *y,
+                            const double *coords, const double *x, const double *b, const unsigned *facet,
+                            const fdb_int *map0, const fdb_int *map1);
+int fdb_launch_dg_upwind(fdb_kernel_s *k, fdb_int start, fdb_int end, int nlay, const fdb_int *subset, double *y,
+                         const double *coords, const double *x, const double *b, const unsigned *facet,
+                         const fdb_int *map0, const fdb_int *map1);

@@ -28,6 +28,7 @@
 //             coloured)
 //   DIAGONAL  the self-terms of each side: point stage, t^T pass and s^T pass on squared tables (atomic)
 #include "common.cuh"
+#include "dg_hex.cuh"
 
 namespace {
 
@@ -99,41 +100,7 @@ __device__ __forceinline__ double face_inverse_jacobian(const double *X, int dir
 {
     double xi[3];
     from_face_axes(dir, s, t, (double)side, xi);
-    double J[3][3];
-#pragma unroll
-    for (int c = 0; c < 3; c++)
-#pragma unroll
-        for (int d = 0; d < 3; d++) J[c][d] = 0.0;
-#pragma unroll
-    for (int v = 0; v < 8; v++) {
-        const int b0 = (v >> 2) & 1, b1 = (v >> 1) & 1, b2 = v & 1;
-        const double f0 = b0 ? xi[0] : 1.0 - xi[0], f1 = b1 ? xi[1] : 1.0 - xi[1], f2 = b2 ? xi[2] : 1.0 - xi[2];
-        const double g0 = (b0 ? 1.0 : -1.0) * f1 * f2;
-        const double g1 = (b1 ? 1.0 : -1.0) * f0 * f2;
-        const double g2 = (b2 ? 1.0 : -1.0) * f0 * f1;
-#pragma unroll
-        for (int c = 0; c < 3; c++) {
-            const double xc = X[v * 3 + c];
-            J[c][0] = fma(xc, g0, J[c][0]);
-            J[c][1] = fma(xc, g1, J[c][1]);
-            J[c][2] = fma(xc, g2, J[c][2]);
-        }
-    }
-    const double A00 = J[1][1] * J[2][2] - J[1][2] * J[2][1];
-    const double A01 = J[0][2] * J[2][1] - J[0][1] * J[2][2];
-    const double A02 = J[0][1] * J[1][2] - J[0][2] * J[1][1];
-    const double det = J[0][0] * A00 + J[1][0] * A01 + J[2][0] * A02;
-    const double r = 1.0 / det;
-    K[0][0] = A00 * r;
-    K[0][1] = A01 * r;
-    K[0][2] = A02 * r;
-    K[1][0] = (J[1][2] * J[2][0] - J[1][0] * J[2][2]) * r;
-    K[1][1] = (J[0][0] * J[2][2] - J[0][2] * J[2][0]) * r;
-    K[1][2] = (J[0][2] * J[1][0] - J[0][0] * J[1][2]) * r;
-    K[2][0] = (J[1][0] * J[2][1] - J[1][1] * J[2][0]) * r;
-    K[2][1] = (J[0][1] * J[2][0] - J[0][0] * J[2][1]) * r;
-    K[2][2] = (J[0][0] * J[1][1] - J[0][1] * J[1][0]) * r;
-    return fabs(det);
+    return trilinear_inverse_jacobian(X, xi, K);
 }
 
 template <int N, bool INTERIOR, int MODE, bool ATOMIC>
@@ -427,20 +394,188 @@ dg_facet_kernel(const __grid_constant__ DGFacetParams<N> P)
     }
 }
 
+// The upwind facet terms of FDB_FORM_DG_TRANSPORT on the collocated GL element (B = I): the trace of side sd at face
+// point (a, b) is the phi(side) contraction of its normal line (a, b), b.n comes from b interpolated trilinearly
+// from the '+' cell's vertices and n from the '+' Jacobian, and the flux times the weight goes back along the
+// normal line of each side with opposite signs.  Only values are read: no tangential contractions, no '-' geometry.
+//   ACTION    gather ('+' vertices and b, both cells' values), point stage + scatter (atomic or coloured)
+//   DIAGONAL  the self-terms: max(+-b.n, 0) phi_k(side)^2 W per side, or (c_out max + c_in min)(b.n) phi_k^2 W (atomic)
+template <int N>
+struct DGUpwindParams {
+    double *y;                   // action / diagonal output
+    const double *x;             // action input
+    const double *coords, *b;    // AoS, 3 per vertex
+    const fdb_int *map0, *map1;  // dof map (NS * N^3 per column), vertex map (NS * 8; the '+' 8 are read)
+    const fdb_int *off0, *off1;  // layer offsets (zeros for native hexes)
+    const unsigned *facet;       // NS local facet numbers per column of the iteration set
+    const fdb_int *collist;      // columns to visit (subset / colour) or NULL = col0 + i
+    int col0, ncols;
+    int nlay_items, lay_first, lay_step;   // layers lay_first + lay_step * k, k < nlay_items
+    double c_out, c_in;          // exterior: the max(b.n, 0) and min(b.n, 0) coefficients
+    double wq[N], xq[N];
+    double E[2][N];              // phi_k(0), phi_k(1)
+};
+
 template <int N, bool INTERIOR, int MODE, bool ATOMIC>
-int launch(cudaStream_t st, const DGFacetParams<N> &P, int sm_count)
+__global__ void __launch_bounds__(DGFacetShape<N>::THREADS)
+dg_upwind_kernel(const __grid_constant__ DGUpwindParams<N> P)
 {
     using S = DGFacetShape<N>;
-    auto kern = dg_facet_kernel<N, INTERIOR, MODE, ATOMIC>;
-    int per_sm = 0;
-    FDB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, S::THREADS, 0));
+    constexpr int NF = S::NF;
+    constexpr int FPB = S::FPB;
+    constexpr int ND = N * N * N;
+    constexpr int NS = INTERIOR ? 2 : 1;                          // sides
+    __shared__ double s_x[FPB][24];                               // the '+' cell's vertices
+    __shared__ double s_b[FPB][24];                               // and b at them
+    __shared__ double s_u[FPB][MODE == DG_ACTION ? NS * ND : 1];  // both cells' values
+    const int slot = threadIdx.x / NF;
+    const int l = threadIdx.x - slot * NF;
+    const bool in_cta = slot < FPB;
+    const int sl = in_cta ? slot : 0;
+    const int a = l / N, b = l - (l / N) * N;                    // point (a along s, b along t) = face node
+
     const long long nunits = (long long)P.ncols * P.nlay_items;
-    long long grid = (nunits + S::FPB - 1) / S::FPB;
+    for (long long base = (long long)blockIdx.x * FPB; base < nunits; base += (long long)gridDim.x * FPB) {
+        const long long unit = base + slot;
+        const bool valid = in_cta && unit < nunits;
+        int col = 0, layer = 0;
+        unsigned f[NS];
+#pragma unroll
+        for (int sd = 0; sd < NS; sd++) f[sd] = sd == 0 ? 5u : 4u;   // idle slot: any valid facet pair
+        if (valid) {
+            const int ci = (int)(unit / P.nlay_items);
+            layer = P.lay_first + P.lay_step * (int)(unit - (long long)ci * P.nlay_items);
+            col = P.collist ? __ldg(P.collist + ci) : P.col0 + ci;
+#pragma unroll
+            for (int sd = 0; sd < NS; sd++) f[sd] = __ldg(P.facet + (long long)col * NS + sd);
+        }
+        if (valid) {
+            if (MODE == DG_ACTION) {
+                for (int i = l; i < NS * ND; i += NF) {
+                    const int g = __ldg(P.map0 + (long long)col * NS * ND + i) + __ldg(P.off0 + i) * layer;
+                    s_u[sl][i] = __ldg(P.x + g);
+                }
+            }
+            for (int i = l; i < 24; i += NF) {
+                const int v = i / 3, c = i - 3 * v;
+                const long long gv = (long long)(__ldg(P.map1 + (long long)col * NS * 8 + v) + __ldg(P.off1 + v) * layer);
+                s_x[sl][i] = __ldg(P.coords + gv * 3 + c);
+                s_b[sl][i] = __ldg(P.b + gv * 3 + c);
+            }
+        } else if (in_cta) {
+            // idle slot: the unit cube at rest with zero values, nothing scattered
+            if (MODE == DG_ACTION)
+                for (int i = l; i < NS * ND; i += NF) s_u[sl][i] = 0.0;
+            for (int i = l; i < 24; i += NF) {
+                const int v = i / 3, c = i % 3;
+                s_x[sl][i] = (double)((v >> (2 - c)) & 1);
+                s_b[sl][i] = 0.0;
+            }
+        }
+        __syncthreads();
+        if (valid) {
+            // unit normal, surface weight and b.n from '+' (as in dg_facet_kernel)
+            const int dir0 = (int)(f[0] >> 1), side0 = (int)(f[0] & 1u);
+            double xi[3], K[3][3], bq[3];
+            from_face_axes(dir0, P.xq[a], P.xq[b], (double)side0, xi);
+            const double detJ0 = trilinear_inverse_jacobian(&s_x[sl][0], xi, K);
+            trilinear_interpolate(&s_b[sl][0], xi, bq);
+            const double n0 = dir0 == 0 ? K[0][0] : (dir0 == 1 ? K[1][0] : K[2][0]);
+            const double n1 = dir0 == 0 ? K[0][1] : (dir0 == 1 ? K[1][1] : K[2][1]);
+            const double n2 = dir0 == 0 ? K[0][2] : (dir0 == 1 ? K[1][2] : K[2][2]);
+            const double gn = sqrt(n0 * n0 + n1 * n1 + n2 * n2);
+            const double W = P.wq[a] * P.wq[b] * detJ0 * gn;
+            const double bn = (side0 ? 1.0 : -1.0) * (n0 * bq[0] + n1 * bq[1] + n2 * bq[2]) / gn;
+            double cv[NS];                                     // the coefficient of phi_k(side) on each side
+            if (MODE == DG_ACTION) {
+                double tr[NS];
+#pragma unroll
+                for (int sd = 0; sd < NS; sd++) {
+                    const int dir = (int)(f[sd] >> 1), side = (int)(f[sd] & 1u);
+                    double t0 = 0.0;
+#pragma unroll
+                    for (int k = 0; k < N; k++) t0 = fma(P.E[side][k], s_u[sl][sd * ND + cell_dof<N>(dir, a, b, k)], t0);
+                    tr[sd] = t0;
+                }
+                if (INTERIOR) {
+                    cv[0] = W * bn * (bn >= 0.0 ? tr[0] : tr[NS - 1]);
+                    cv[NS - 1] = -cv[0];
+                } else {
+                    cv[0] = W * (P.c_out * fmax(bn, 0.0) + P.c_in * fmin(bn, 0.0)) * tr[0];
+                }
+            } else {
+                if (INTERIOR) {
+                    cv[0] = W * fmax(bn, 0.0);
+                    cv[NS - 1] = W * fmax(-bn, 0.0);
+                } else {
+                    cv[0] = W * (P.c_out * fmax(bn, 0.0) + P.c_in * fmin(bn, 0.0));
+                }
+            }
+#pragma unroll
+            for (int sd = 0; sd < NS; sd++) {
+                const int dir = (int)(f[sd] >> 1), side = (int)(f[sd] & 1u);
+#pragma unroll
+                for (int k = 0; k < N; k++) {
+                    const int i = sd * ND + cell_dof<N>(dir, a, b, k);
+                    const int g = __ldg(P.map0 + (long long)col * NS * ND + i) + __ldg(P.off0 + i) * layer;
+                    const double pk = P.E[side][k];
+                    const double val = MODE == DG_ACTION ? pk * cv[sd] : pk * pk * cv[sd];
+                    if (ATOMIC) atomicAdd(P.y + g, val);
+                    else P.y[g] += val;
+                }
+            }
+        }
+        __syncthreads();          // the slot's buffers are refilled by the next facet
+    }
+}
+
+template <class Kern, class Params>
+int launch_facets(Kern kern, int threads, int fpb, cudaStream_t st, const Params &P, int sm_count)
+{
+    int per_sm = 0;
+    FDB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, threads, 0));
+    const long long nunits = (long long)P.ncols * P.nlay_items;
+    long long grid = (nunits + fpb - 1) / fpb;
     const long long cap = (long long)sm_count * (per_sm > 0 ? per_sm : 1);
     if (grid > cap) grid = cap;
     if (grid < 1) return 0;
-    kern<<<(int)grid, S::THREADS, 0, st>>>(P);
+    kern<<<(int)grid, threads, 0, st>>>(P);
     FDB_LAUNCH_CHECK();
+    return 0;
+}
+
+// The launches of one facet call: one atomic launch (the diagonal, or FDB_SCATTER_ATOMIC), or one launch per
+// (colour, layer parity), in which no two facets share a dof.  run(P, diagonal, atomic) launches the kernel.
+template <class Params, class Run>
+int schedule_facets(const fdb_kernel_s *k, fdb_int start, fdb_int end, int nlay, const fdb_int *subset, bool diagonal,
+                    Params &P, Run run)
+{
+    if (diagonal || k->desc.scatter == FDB_SCATTER_ATOMIC) {
+        P.collist = subset;
+        P.col0 = start;
+        P.ncols = end - start;
+        P.nlay_items = nlay;
+        P.lay_first = 0;
+        P.lay_step = 1;
+        if (P.ncols <= 0 || nlay <= 0) return 0;
+        return run(P, diagonal, true);
+    }
+    if (subset) {
+        fdb::set_error("coloured scatter does not support subsets yet");
+        return 1;
+    }
+    for (int col = 0; col < k->ncolours; col++) {
+        P.collist = k->d_colour_cols + k->colour_start[col];
+        P.col0 = 0;
+        P.ncols = k->colour_start[col + 1] - k->colour_start[col];
+        for (int par = 0; par < (nlay > 1 ? 2 : 1); par++) {
+            P.lay_first = par;
+            P.lay_step = 2;
+            P.nlay_items = (nlay - par + 1) / 2;
+            if (P.ncols <= 0 || P.nlay_items <= 0) continue;
+            if (run(P, false, false)) return 1;
+        }
+    }
     return 0;
 }
 
@@ -472,35 +607,44 @@ int run_n(fdb_kernel_s *k, fdb_int start, fdb_int end, int nlay, const fdb_int *
     P.facet = facet;
     P.map0 = map0;
     P.map1 = map1;
-    if (!x || k->desc.scatter == FDB_SCATTER_ATOMIC) {
-        P.collist = subset;
-        P.col0 = start;
-        P.ncols = end - start;
-        P.nlay_items = nlay;
-        P.lay_first = 0;
-        P.lay_step = 1;
-        if (P.ncols <= 0 || nlay <= 0) return 0;
-        if (!x) return launch<N, INTERIOR, DG_DIAGONAL, true>(c.stream, P, c.sm_count);
-        return launch<N, INTERIOR, DG_ACTION, true>(c.stream, P, c.sm_count);
+    using S = DGFacetShape<N>;
+    return schedule_facets(k, start, end, nlay, subset, !x, P, [&](const DGFacetParams<N> &Q, bool diag, bool atomic) {
+        if (diag) return launch_facets(dg_facet_kernel<N, INTERIOR, DG_DIAGONAL, true>, S::THREADS, S::FPB, c.stream, Q, c.sm_count);
+        if (atomic) return launch_facets(dg_facet_kernel<N, INTERIOR, DG_ACTION, true>, S::THREADS, S::FPB, c.stream, Q, c.sm_count);
+        return launch_facets(dg_facet_kernel<N, INTERIOR, DG_ACTION, false>, S::THREADS, S::FPB, c.stream, Q, c.sm_count);
+    });
+}
+
+template <int N, bool INTERIOR>
+int run_upwind_n(fdb_kernel_s *k, fdb_int start, fdb_int end, int nlay, const fdb_int *subset, double *y,
+                 const double *coords, const double *x, const double *b, const unsigned *facet, const fdb_int *map0,
+                 const fdb_int *map1)
+{
+    fdb::Context &c = fdb::ctx();
+    DGUpwindParams<N> P;
+    memset(&P, 0, sizeof(P));
+    P.off0 = k->d_off0;
+    P.off1 = k->d_off1;
+    P.c_out = k->desc.dcoef[0];
+    P.c_in = k->desc.dcoef[1];
+    for (int i = 0; i < N; i++) {
+        P.wq[i] = k->desc.wq[i];
+        P.xq[i] = k->desc.xq[i];
+        for (int e = 0; e < 2; e++) P.E[e][i] = k->Bend[e * FDB_MAX_1D + i];
     }
-    // deterministic: one launch per (colour, layer parity), no two facets of a launch share a dof
-    if (subset) {
-        fdb::set_error("coloured scatter does not support subsets yet");
-        return 1;
-    }
-    for (int col = 0; col < k->ncolours; col++) {
-        P.collist = k->d_colour_cols + k->colour_start[col];
-        P.col0 = 0;
-        P.ncols = k->colour_start[col + 1] - k->colour_start[col];
-        for (int par = 0; par < (nlay > 1 ? 2 : 1); par++) {
-            P.lay_first = par;
-            P.lay_step = 2;
-            P.nlay_items = (nlay - par + 1) / 2;
-            if (P.ncols <= 0 || P.nlay_items <= 0) continue;
-            if (launch<N, INTERIOR, DG_ACTION, false>(c.stream, P, c.sm_count)) return 1;
-        }
-    }
-    return 0;
+    P.y = y;
+    P.x = x;
+    P.coords = coords;
+    P.b = b;
+    P.facet = facet;
+    P.map0 = map0;
+    P.map1 = map1;
+    using S = DGFacetShape<N>;
+    return schedule_facets(k, start, end, nlay, subset, !x, P, [&](const DGUpwindParams<N> &Q, bool diag, bool atomic) {
+        if (diag) return launch_facets(dg_upwind_kernel<N, INTERIOR, DG_DIAGONAL, true>, S::THREADS, S::FPB, c.stream, Q, c.sm_count);
+        if (atomic) return launch_facets(dg_upwind_kernel<N, INTERIOR, DG_ACTION, true>, S::THREADS, S::FPB, c.stream, Q, c.sm_count);
+        return launch_facets(dg_upwind_kernel<N, INTERIOR, DG_ACTION, false>, S::THREADS, S::FPB, c.stream, Q, c.sm_count);
+    });
 }
 
 template <bool INTERIOR>
@@ -518,6 +662,21 @@ int run_interior(fdb_kernel_s *k, fdb_int start, fdb_int end, int nlay, const fd
     return 1;
 }
 
+template <bool INTERIOR>
+int run_upwind(fdb_kernel_s *k, fdb_int start, fdb_int end, int nlay, const fdb_int *subset, double *y,
+               const double *coords, const double *x, const double *b, const unsigned *facet, const fdb_int *map0,
+               const fdb_int *map1)
+{
+    switch (k->n1d) {
+    case 2: return run_upwind_n<2, INTERIOR>(k, start, end, nlay, subset, y, coords, x, b, facet, map0, map1);
+    case 3: return run_upwind_n<3, INTERIOR>(k, start, end, nlay, subset, y, coords, x, b, facet, map0, map1);
+    case 4: return run_upwind_n<4, INTERIOR>(k, start, end, nlay, subset, y, coords, x, b, facet, map0, map1);
+    case 5: return run_upwind_n<5, INTERIOR>(k, start, end, nlay, subset, y, coords, x, b, facet, map0, map1);
+    }
+    fdb::set_error("dg upwind kernel: degree %d not instantiated (1..4)", k->n1d - 1);
+    return 1;
+}
+
 }  // namespace
 
 int fdb_launch_dg_facet(fdb_kernel_s *k, fdb_int start, fdb_int end, int nlay, const fdb_int *subset, double *y,
@@ -527,4 +686,13 @@ int fdb_launch_dg_facet(fdb_kernel_s *k, fdb_int start, fdb_int end, int nlay, c
     if (k->desc.integral == FDB_INTEGRAL_INTERIOR_FACET)
         return run_interior<true>(k, start, end, nlay, subset, y, coords, x, facet, map0, map1);
     return run_interior<false>(k, start, end, nlay, subset, y, coords, x, facet, map0, map1);
+}
+
+int fdb_launch_dg_upwind(fdb_kernel_s *k, fdb_int start, fdb_int end, int nlay, const fdb_int *subset, double *y,
+                         const double *coords, const double *x, const double *b, const unsigned *facet,
+                         const fdb_int *map0, const fdb_int *map1)
+{
+    if (k->desc.integral == FDB_INTEGRAL_INTERIOR_FACET)
+        return run_upwind<true>(k, start, end, nlay, subset, y, coords, x, b, facet, map0, map1);
+    return run_upwind<false>(k, start, end, nlay, subset, y, coords, x, b, facet, map0, map1);
 }

@@ -297,7 +297,8 @@ static int device_pointers(const fdb_call_args *a, bool mat, void **args, const 
 // The forms of the hand-written hex kernels: what fdb_kernel_create accepts for each and how
 // fdb_kernel_call hands its arguments to the launchers.
 enum { MODE_ACTION, MODE_MATRIX, MODE_DIAGONAL };
-enum { LAUNCH_HELMHOLTZ, LAUNCH_HELMHOLTZ_COEF, LAUNCH_ELASTICITY, LAUNCH_STOKES, LAUNCH_BOUNDARY, LAUNCH_DG_FACET };
+enum { LAUNCH_HELMHOLTZ, LAUNCH_HELMHOLTZ_COEF, LAUNCH_ELASTICITY, LAUNCH_STOKES, LAUNCH_BOUNDARY, LAUNCH_DG_FACET,
+       LAUNCH_DG_TRANSPORT };
 
 struct fdb_hex_form {
     int form;                 // enum fdb_form
@@ -312,12 +313,14 @@ struct fdb_hex_form {
     int launcher;             // fdb_launch_helmholtz_*, fdb_launch_helmholtz_coef_* (which also run the
                               // nonlinear diffusion and advection-diffusion forms), fdb_launch_elasticity_*
                               // fdb_launch_stokes_action (which also runs the Navier-Stokes forms),
-                              // fdb_launch_boundary_mass or fdb_launch_dg_facet (the DG facet forms)
+                              // fdb_launch_boundary_mass, fdb_launch_dg_facet (the DG facet forms) or
+                              // fdb_launch_dg_transport
     int max_degree[3];        // per mode: action, matrix, diagonal
     int min_degree;
     const char *space2;       // the arguments on a second space (output and input, through a third map), or
                               // NULL: such a form is an action only, in device mode
-    int integral;             // enum fdb_integral: facet forms run in device mode only
+    int integral;             // enum fdb_integral: facet forms run in device mode only; -1: the descriptor's
+                              // integral (cell, exterior or interior facet) selects the term
 };
 
 static const fdb_hex_form hex_forms[] = {
@@ -349,6 +352,9 @@ static const fdb_hex_form hex_forms[] = {
      nullptr, FDB_INTEGRAL_INTERIOR_FACET},
     {FDB_FORM_DG_BOUNDARY, "dg_boundary", 1, false, "facet", 1, false, LAUNCH_DG_FACET, {4, 0, 4}, 1, nullptr,
      FDB_INTEGRAL_EXTERIOR_FACET},
+    // upwind DG transport on DQ_p: b (3 values per vertex, through the vertex map), then on facets the local
+    // facet numbers.  Device mode only, no rank 2
+    {FDB_FORM_DG_TRANSPORT, "dg_transport", 1, false, "b", 3, false, LAUNCH_DG_TRANSPORT, {4, 0, 4}, 1, nullptr, -1},
 };
 
 static const char *const mode_name[] = {"action", "matrix", "diagonal"};
@@ -446,7 +452,7 @@ static int kernel_create(const fdb_kernel_desc *d, const fdb_space2_desc *s2, fd
                   "of %s_jacobian", f->name, f->name);
         return 1;
     }
-    if (f->launcher == LAUNCH_DG_FACET && mode == MODE_MATRIX) {
+    if ((f->launcher == LAUNCH_DG_FACET || f->launcher == LAUNCH_DG_TRANSPORT) && mode == MODE_MATRIX) {
         set_error("fdb_kernel_create: %s has no rank-2 form: there is no assembled DG matrix (the facet terms couple "
                   "neighbouring cells outside the cell sparsity); use the action and the diagonal", f->name);
         return 1;
@@ -469,6 +475,21 @@ static int kernel_create(const fdb_kernel_desc *d, const fdb_space2_desc *s2, fd
     if (f->integral == FDB_INTEGRAL_INTERIOR_FACET && d->integral != FDB_INTEGRAL_INTERIOR_FACET) {
         set_error("fdb_kernel_create: %s has interior-facet integrals only (integral %d)", f->name, d->integral);
         return 1;
+    }
+    if (f->integral < 0 && (d->integral < FDB_INTEGRAL_CELL || d->integral > FDB_INTEGRAL_INTERIOR_FACET)) {
+        set_error("fdb_kernel_create: %s takes a cell, exterior-facet or interior-facet integral (integral %d)",
+                  f->name, d->integral);
+        return 1;
+    }
+    if (f->launcher == LAUNCH_DG_TRANSPORT) {
+        // the form is stated on the collocated GL element: u at Gauss point q is the dof u[q]
+        for (int q = 0; q < d->nq; q++)
+            for (int a = 0; a <= d->degree; a++)
+                if (d->B[q * (d->degree + 1) + a] != (q == a ? 1.0 : 0.0)) {
+                    set_error("fdb_kernel_create: %s needs the collocated Gauss-Legendre element (B must be the "
+                              "identity: B[%d][%d] = %g)", f->name, q, a, d->B[q * (d->degree + 1) + a]);
+                    return 1;
+                }
     }
     if (f->integral != FDB_INTEGRAL_CELL && d->cell == FDB_CELL_HEX_EXTRUDED && (!d->offset0 || !d->offset1)) {
         set_error("fdb_kernel_create: %s on extruded cells needs the layer offsets offset0/offset1", f->name);
@@ -498,7 +519,7 @@ static int kernel_create(const fdb_kernel_desc *d, const fdb_space2_desc *s2, fd
     k->hex = f;
     k->n1d = d->degree + 1;
     // an interior-facet entry reads both cells: 2 (p+1)^3 dofs and 16 vertices
-    const int sides = f->integral == FDB_INTEGRAL_INTERIOR_FACET ? 2 : 1;
+    const int sides = d->integral == FDB_INTEGRAL_INTERIOR_FACET ? 2 : 1;
     k->arity = sides * k->n1d * k->n1d * k->n1d;
     const int arity1 = sides * 8;
     memset(k->h_off0, 0, sizeof(k->h_off0));
@@ -521,7 +542,7 @@ static int kernel_create(const fdb_kernel_desc *d, const fdb_space2_desc *s2, fd
         return 1;
     }
     memset(k->Bend, 0, sizeof(k->Bend));
-    if (f->launcher == LAUNCH_DG_FACET) endpoint_tables(k->n1d, d->B, d->xq, k->Bend);
+    if (f->launcher == LAUNCH_DG_FACET || f->launcher == LAUNCH_DG_TRANSPORT) endpoint_tables(k->n1d, d->B, d->xq, k->Bend);
     FDB_CUDA(cudaMalloc(&k->d_off0, sizeof(fdb_int) * k->arity));
     FDB_CUDA(cudaMalloc(&k->d_off1, sizeof(fdb_int) * arity1));
     FDB_CUDA(cudaMemcpyAsync(k->d_off0, k->h_off0, sizeof(fdb_int) * k->arity,
@@ -645,22 +666,26 @@ int fdb_kernel_call(fdb_kernel_t k, const fdb_call_args *a)
     // comes last: [y, coords, x, y2, x2, coef]
     // an exterior-facet form (boundary_mass): the trailing argument is the uint32 local facet number of each
     // entry, [y, coords, x, facet] / [mat, coords, facet] / [d, coords, facet]; an interior-facet form
-    // (interior_penalty): the two local facet numbers ('+', '-') of each entry, [y, coords, x, facets]
+    // (interior_penalty): the two local facet numbers ('+', '-') of each entry, [y, coords, x, facets]; dg_transport
+    // reads b before them: [y, coords, x, b], [d, coords, b] on cells, [y, coords, x, b, facets], [d, coords, b,
+    // facets] on facets
     const fdb_hex_form *f = k->hex;
     const int mode = hex_mode(&k->desc);
+    const bool transport_facets = f->launcher == LAUNCH_DG_TRANSPORT && k->desc.integral != FDB_INTEGRAL_CELL;
     if (f->integral != FDB_INTEGRAL_CELL && a->location != FDB_LOC_DEVICE) {
         set_error("fdb_kernel_call: %s takes device-resident Dats only (no host-pointer mode for facet integrals)",
                   f->name);
         return 1;
     }
-    const int want = (mode == MODE_ACTION ? 3 : 2) + (f->coef ? 1 : 0) + (f->space2 ? 2 : 0);
+    const int want = (mode == MODE_ACTION ? 3 : 2) + (f->coef ? 1 : 0) + (f->space2 ? 2 : 0) + (transport_facets ? 1 : 0);
     const int want_maps = f->space2 ? 3 : 2;
     const bool device_only = mode == MODE_DIAGONAL || f->space2 || f->integral != FDB_INTEGRAL_CELL;
     if (a->nargs != want || a->nmaps != want_maps || (device_only && a->location != FDB_LOC_DEVICE)) {
         static const char *const args[] = {"y, coords, x", "mat, coords", "d, coords"};
         set_error("fdb_kernel_call: %s %s expects %d %sargs (%s%s%s%s%s) and %d maps, got %d/%d", f->name,
                   mode_name[mode], want, device_only ? "device " : "", args[mode], f->space2 ? ", " : "",
-                  f->space2 ? f->space2 : "", f->coef ? ", " : "", f->coef ? f->coef : "", want_maps, a->nargs,
+                  f->space2 ? f->space2 : "", f->coef ? ", " : "",
+                  transport_facets ? "b, facets" : (f->coef ? f->coef : ""), want_maps, a->nargs,
                   a->nmaps);
         return 1;
     }
@@ -710,6 +735,9 @@ int fdb_kernel_call(fdb_kernel_t k, const fdb_call_args *a)
     if (device_pointers(a, mat != nullptr, dargs, dmaps, &dsubset)) return 1;
     const double *coords = (const double *)dargs[1];
     const double *coef = f->coef ? (const double *)dargs[want - 1] : nullptr;
+    // dg_transport: b, and on facets the local facet numbers after it
+    const double *vel = f->launcher == LAUNCH_DG_TRANSPORT ? (const double *)dargs[mode == MODE_ACTION ? 3 : 2] : nullptr;
+    const unsigned *tfacets = transport_facets ? (const unsigned *)dargs[want - 1] : nullptr;
     double *out = mat ? nullptr : (double *)dargs[0];     // the action's y or the diagonal
     if (mode != MODE_ACTION) {
         switch (f->launcher) {
@@ -736,12 +764,16 @@ int fdb_kernel_call(fdb_kernel_t k, const fdb_call_args *a)
         case LAUNCH_DG_FACET:
             return fdb_launch_dg_facet(k, a->start, a->end, nlay, dsubset, out, coords, nullptr,
                                        (const unsigned *)coef, dmaps[0], dmaps[1]);
+        case LAUNCH_DG_TRANSPORT:
+            return fdb_launch_dg_transport(k, a->start, a->end, nlay, dsubset, out, coords, nullptr, vel, tfacets,
+                                           dmaps[0], dmaps[1]);
         default:
             return fdb_launch_elasticity_matrix(k, a->start, a->end, nlay, dsubset, mat, coords, coef, dmaps[0],
                                                 dmaps[1], out);
         }
     }
-    if (k->desc.scatter == FDB_SCATTER_COLOURED &&
+    // (the dg_transport cell term needs no colours: a DQ cell owns its dofs)
+    if (k->desc.scatter == FDB_SCATTER_COLOURED && !(f->launcher == LAUNCH_DG_TRANSPORT && !transport_facets) &&
         (k->colour_map_key != (const void *)a->maps[0] || k->colour_map_gen != map_ver(a, 0) ||
          k->colour_end != a->end)) {
         // colouring covers columns [0, end): copy the map to the host if needed
@@ -784,6 +816,10 @@ int fdb_kernel_call(fdb_kernel_t k, const fdb_call_args *a)
     case LAUNCH_DG_FACET:
         rc = fdb_launch_dg_facet(k, a->start, a->end, nlay, dsubset, out, coords, x, (const unsigned *)coef,
                                  dmaps[0], dmaps[1]);
+        break;
+    case LAUNCH_DG_TRANSPORT:
+        rc = fdb_launch_dg_transport(k, a->start, a->end, nlay, dsubset, out, coords, x, vel, tfacets, dmaps[0],
+                                     dmaps[1]);
         break;
     default:
         rc = fdb_launch_stokes_action(k, a->start, a->end, nlay, dsubset, out, coords, x, (double *)dargs[3],

@@ -1414,6 +1414,13 @@ class Kernel:
     c_f = ``alpha``, c_p = ``beta``, and ``c_m``, ``c_s``, with ``integral="exterior_facet"`` and the arguments
     of "boundary_mass".  Both: action (output, coordinates, u, facets) and diagonal (output, coordinates,
     facets), no rank 2; device-resident Dats only.
+
+    "dg_transport" is upwind DG transport of a scalar DQ_p field by a velocity b given at the mesh vertices (a Dat
+    on ``DataSet(vertex set, 3)``, read through the coordinate map), on the collocated Gauss-Legendre ``element``.
+    The integral selects the term: "cell" ``-u*dot(b, grad v)*dx``, "interior_facet" the upwind flux
+    ``dot(b, n('+'))*u_up*(v('+') - v('-'))*dS``, "exterior_facet" ``(c_out*max(b.n, 0) + c_in*min(b.n, 0))*u*v*ds``.
+    Arguments: action (output, coordinates, u, b[, facets]), diagonal (output, coordinates, b[, facets]), with the
+    facet numbers on facet integrals only; no rank 2; device-resident Dats only.
     """
     form: str = "helmholtz"
     degree: int = 1
@@ -1435,6 +1442,8 @@ class Kernel:
     lmbda: float = 0.0
     c_m: float = 0.0                # dg_boundary: the u*v and u*dot(grad v, n) coefficients
     c_s: float = 0.0
+    c_out: float = 1.0              # dg_transport (exterior facets): the max(b.n, 0) and min(b.n, 0) coefficients
+    c_in: float = 0.0
 
     def __new__(cls, *args, **kwargs):
         # ``op2.Kernel(code, name)`` with C source (pyop2/local_kernel.py:33-43) builds the
@@ -1461,6 +1470,13 @@ class Kernel:
             return
         if spec and spec.residual:
             return          # (INC, READ, READ) whatever rank and diagonal say: the engine refuses them
+        if spec and spec.velocity:
+            # (output, coordinates[, u], b[, facets])
+            acc = (INC, READ) + (() if self.diagonal else (READ,)) + (READ,) + \
+                (() if self.integral == "cell" else (READ,))
+            object.__setattr__(self, "accesses", acc)
+            object.__setattr__(self, "name", f"form0_{self.integral}_integral")
+            return
         if spec and spec.facet:
             acc = (INC, READ, READ) if (self.diagonal or self.rank == 2) else (INC, READ, READ, READ)
             object.__setattr__(self, "accesses", acc)
@@ -1500,6 +1516,7 @@ class _Form(NamedTuple):
     coef_cdim: int = 0          # values per node of the trailing coefficient when they differ from the space's
     pressure: bool = False      # also reads and writes a scalar pressure space through a third map (Stokes)
     facet: bool = False         # an exterior-facet integral: the local facet numbers come last, the integral as given
+    velocity: bool = False      # reads b (3 values per vertex) through the coordinate map after u
 
 
 _FORMS = {"helmholtz": _Form(_lib.FORM_HELMHOLTZ),
@@ -1516,7 +1533,8 @@ _FORMS = {"helmholtz": _Form(_lib.FORM_HELMHOLTZ),
           "navier_stokes_jacobian": _Form(_lib.FORM_NAVIER_STOKES_JACOBIAN, coefficient=True, pressure=True),
           "boundary_mass": _Form(_lib.FORM_BOUNDARY_MASS, facet=True),
           "interior_penalty": _Form(_lib.FORM_INTERIOR_PENALTY, facet=True),
-          "dg_boundary": _Form(_lib.FORM_DG_BOUNDARY, facet=True)}
+          "dg_boundary": _Form(_lib.FORM_DG_BOUNDARY, facet=True),
+          "dg_transport": _Form(_lib.FORM_DG_TRANSPORT, facet=True, velocity=True)}
 _INTEGRALS = {"cell": _lib.INTEGRAL_CELL, "exterior_facet": _lib.INTEGRAL_EXTERIOR_FACET,
               "interior_facet": _lib.INTEGRAL_INTERIOR_FACET, "fused": _lib.INTEGRAL_FUSED}
 
@@ -1605,6 +1623,8 @@ class GlobalKernel:
             d.dcoef[i] = lk.d[i]
         if lk.form == "dg_boundary":
             d.dcoef[0], d.dcoef[1], d.dcoef[2] = lk.c_m, lk.c_s, 0.0
+        if lk.form == "dg_transport":
+            d.dcoef[0], d.dcoef[1], d.dcoef[2] = lk.c_out, lk.c_in, 0.0
         if spec.lame:
             d.alpha, d.lmbda = lk.mu, lk.lmbda
         s2 = None
@@ -1751,6 +1771,12 @@ class Parloop:
             # fewer would be read past its end
             raise ValueError(f"{lk.form}: the trailing coefficient has {spec.coef_cdim} values per node, "
                              f"{self.args[-1].data.name} has {self.args[-1].data.cdim}")
+        if spec and spec.velocity:
+            # b is read at the 8 vertices of a cell, 3 values each, through the coordinate map
+            b = self.args[2 if lk.diagonal else 3]
+            if b.data.cdim != 3 or b.map is not self.args[1].map:
+                raise ValueError(f"{lk.form}: b has 3 values per vertex and is read through the coordinate map, "
+                                 f"{b.data.name} has {b.data.cdim} through {getattr(b.map, 'name', None)}")
         if spec and spec.pressure:
             # the kernel reads and writes one pressure value per node of the third map: a Dat with more
             # values per node would be misread, one with fewer nodes read past its end

@@ -275,7 +275,7 @@ enum fdb_form {
                                    (s, t) of '-'.  Device mode only:
                                      action    [y INC, coords, u, facets]  (atomic or coloured)
                                      diagonal  [d INC, coords, facets]                            */
-    FDB_FORM_DG_BOUNDARY = 15
+    FDB_FORM_DG_BOUNDARY = 15,
                                 /* the exterior-facet terms of the same discretisation, an
                                    EXTERIOR-FACET integral:
                                      a(u, v) = ( c_m*u*v + (c_p/h)*u*v - c_s*u*dot(grad v, n)
@@ -290,6 +290,31 @@ enum fdb_form {
                                    argument its uint32 local facet number.  Device mode only:
                                      action    [y INC, coords, u, facet]  (atomic or coloured)
                                      diagonal  [d INC, coords, facet]                             */
+    FDB_FORM_DG_TRANSPORT = 16
+                                /* upwind DG transport of a scalar DQ_p field (Gauss-Legendre nodes) by
+                                   a velocity b given at the mesh VERTICES (3 values per vertex, read
+                                   through maps[1], the vertex map), in conservative form (NOT
+                                   symmetric).  The integral selects the term:
+                                     cell            - u*dot(b, grad v)*dx
+                                     interior facet  dot(b, n('+'))*u_up*(v('+') - v('-'))*dS,
+                                                     u_up = u('+') if b.n >= 0 else u('-')
+                                     exterior facet  (c_out*max(b.n, 0) + c_in*min(b.n, 0))*u*v*ds
+                                   c_out = dcoef[0], c_in = dcoef[1] (the outflow operator is (1, 0),
+                                   the inflow load of g the action on g with (0, -1)).  b is the
+                                   trilinear interpolant of the vertex values; n and the face weight
+                                   are the '+' side's, applied with opposite signs to the two sides, so
+                                   1^T A q is exactly the outflow flux.  Hex cells, cdim 1, degrees
+                                   1..4, action and diagonal (rank 2 is refused: there is no assembled
+                                   DG matrix).  The collocated GL element only: B must be the identity
+                                   and nq == degree+1.  Facet entries and maps as for
+                                   FDB_FORM_INTERIOR_PENALTY / FDB_FORM_DG_BOUNDARY; a cell entry's
+                                   dofs must belong to that cell alone (a DQ map), since the cell
+                                   kernel adds into y without atomics.  Device mode only:
+                                     cell      action    [y INC, coords, u, b]
+                                               diagonal  [d INC, coords, b]
+                                     facets    action    [y INC, coords, u, b, facets]  (atomic or
+                                                                                         coloured)
+                                               diagonal  [d INC, coords, b, facets]               */
 };
 
 enum fdb_cell {
@@ -351,6 +376,7 @@ typedef struct fdb_kernel_desc {
     int32_t affine_cells;
     /* FDB_FORM_NONLINEAR_DIFFUSION[_JACOBIAN]: D(s) = dcoef[0] + dcoef[1] s + dcoef[2] s^2.
      * FDB_FORM_DG_BOUNDARY: c_m = dcoef[0], c_s = dcoef[1].
+     * FDB_FORM_DG_TRANSPORT (exterior facets): c_out = dcoef[0], c_in = dcoef[1].
      * Ignored by every other form (a zeroed descriptor stays valid for them). */
     double dcoef[3];
     /* FDB_FORM_ELASTICITY, FDB_FORM_HYPERELASTICITY[_JACOBIAN]: the Lame parameter lambda (mu is
