@@ -30,6 +30,9 @@ FORM_BOUNDARY_MASS = 13
 FORM_INTERIOR_PENALTY = 14
 FORM_DG_BOUNDARY = 15
 FORM_DG_TRANSPORT = 16
+FORM_P_PROLONG = 17
+FORM_P_RESTRICT = 18
+FORM_P_INJECT = 19
 CELL_HEX_EXTRUDED = 1
 CELL_HEX = 2
 CELL_TRIANGLE = 3
@@ -182,6 +185,8 @@ SIGNATURES = {
     "fdb_asm_get_blocks": (C.c_int, [C.c_void_p, C.c_void_p]),
     "fdb_vec_dot": (C.c_int, [C.c_size_t, C.c_void_p, C.c_void_p, C.POINTER(C.c_double)]),
     "fdb_vec_pointwise_mult": (C.c_int, [C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "fdb_vec_chebyshev": (C.c_int, [C.c_size_t, C.c_double, C.c_double, C.c_void_p, C.c_void_p, C.c_void_p,
+                                    C.c_void_p, C.c_void_p]),
     "fdb_interpolate_q1": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                      C.c_int32, C.c_int, C.c_int, C.c_int, C.c_void_p]),
     "fdb_comm_get_unique_id": (C.c_int, [C.c_char_p]),

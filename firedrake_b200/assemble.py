@@ -2900,6 +2900,52 @@ def gmres(A, b: op2.Dat, x: op2.Dat, M=None, rtol=1e-5, atol=0.0, restart=30, ma
     return it, hist
 
 
+_PMG_KEYS = {"pmg_mg_coarse_degree": 1,
+             "pmg_mg_levels_ksp_type": "chebyshev", "pmg_mg_levels_ksp_max_it": 2, "pmg_mg_levels_pc_type": "jacobi",
+             "pmg_mg_levels_ksp_chebyshev_esteig": "0,0.1,0,1.1",
+             "pmg_mg_coarse_ksp_type": "cg", "pmg_mg_coarse_pc_type": "jacobi", "pmg_mg_coarse_ksp_rtol": 1e-3,
+             "pmg_mg_coarse_ksp_max_it": 500}
+
+
+def pmg_options(sp):
+    """The p-multigrid settings of ``solver_parameters`` with ``pc_type "python"``: ``pc_python_type``
+    "firedrake.PMGPC" (halve the degree) or "firedrake.P1PC" (straight to the coarse degree), and the ``pmg_*`` keys of
+    ``_PMG_KEYS`` with their defaults.  Nested dicts (``"pmg_mg_levels": {...}``, ``"pmg_mg_coarse": {...}``) are
+    flattened as Firedrake does; any other ``pmg_*`` key is refused by name."""
+    kind = sp.get("pc_python_type")
+    if kind not in ("firedrake.PMGPC", "firedrake.P1PC"):
+        raise NotImplementedError(f"pc_python_type {kind!r}: 'firedrake.PMGPC' or 'firedrake.P1PC'")
+    flat = {}
+    for k, v in sp.items():
+        if isinstance(v, dict) and k.startswith("pmg_"):
+            flat.update({f"{k}_{kk}": vv for kk, vv in v.items()})
+        elif k.startswith("pmg_"):
+            flat[k] = v
+    bad = sorted(k for k in flat if k not in _PMG_KEYS)
+    if bad:
+        raise NotImplementedError(f"unknown p-multigrid option(s) {', '.join(bad)}: the supported ones are "
+                                  f"{', '.join(_PMG_KEYS)}")
+    o = dict(_PMG_KEYS, **flat)
+    if o["pmg_mg_levels_pc_type"] != "jacobi":
+        raise NotImplementedError(f"pmg_mg_levels_pc_type {o['pmg_mg_levels_pc_type']!r}: the level smoothers are "
+                                  f"Jacobi-preconditioned ('jacobi')")
+    o["halve"] = kind == "firedrake.PMGPC"
+    return o
+
+
+def _pmg(V, make, sp, bcs, hierarchy, allreduce, kappa=None, omega=0.8):
+    """The :class:`mg.PMG` of the ``pc_type "python"`` options (:func:`pmg_options`) for the level forms ``make``."""
+    from . import mg as _mg
+    o = pmg_options(sp)
+    est = tuple(float(v) for v in str(o["pmg_mg_levels_ksp_chebyshev_esteig"]).split(","))
+    return _mg.PMG(V, make, bc_domains=tuple(s for bc in bcs for s in bc.sub_domains),
+                   coarse_degree=int(o["pmg_mg_coarse_degree"]), halve=o["halve"], kappa=kappa,
+                   smoother=o["pmg_mg_levels_ksp_type"], nu=int(o["pmg_mg_levels_ksp_max_it"]), omega=omega,
+                   esteig=est, coarse_ksp=o["pmg_mg_coarse_ksp_type"], coarse_pc=o["pmg_mg_coarse_pc_type"],
+                   coarse_rtol=float(o["pmg_mg_coarse_ksp_rtol"]), coarse_maxit=int(o["pmg_mg_coarse_ksp_max_it"]),
+                   hierarchy=hierarchy, allreduce=allreduce)
+
+
 def solve_nonlinear(F, L: op2.Dat, u: op2.Dat, bcs=(), solver_parameters=None, hierarchy=None, allreduce=None,
                     nullspace=None):
     """``solve(F == 0, u, bcs=bcs, solver_parameters=...)`` for nonlinear diffusion (``F`` a
@@ -2916,7 +2962,8 @@ def solve_nonlinear(F, L: op2.Dat, u: op2.Dat, bcs=(), solver_parameters=None, h
     (default) | "jacobi" (the Jacobian's exact diagonal) | "mg" (needs ``hierarchy``; nonlinear
     diffusion: a V-cycle of the SPD operator ``Form(V, alpha, beta, kappa=D(u))``, rebuilt at every
     Newton step; hyperelasticity: a V-cycle of ``Elasticity(V, mu, lmbda, beta)``, the Jacobian at u = 0,
-    built once per solve, with Jacobi smoothing damped by 0.6 as in :func:`solve`).
+    built once per solve, with Jacobi smoothing damped by 0.6 as in :func:`solve`) | "python" (p-multigrid,
+    :func:`pmg_options`, of the same operators).
     Converged when ||R(u)|| <= max(snes_rtol * ||R(u_0)||, snes_atol).  For hyperelasticity a
     non-finite residual norm (an inverted element: ln J of J <= 0) ends the solve with a
     :class:`ConvergenceError` whose reason is "DIVERGED_FNORM_NAN".  Returns (Newton residual norms,
@@ -3013,6 +3060,17 @@ def solve_nonlinear(F, L: op2.Dat, u: op2.Dat, bcs=(), solver_parameters=None, h
                                 bc_domains=domains, allreduce=allreduce, kappa=kap)
             top = len(hierarchy) - 1
             M = lambda r, z, vc=vc: vc.apply(top, r, z)
+        elif pc == "python":
+            # p-multigrid with the level forms of the "mg" branch: J(0) = Elasticity once per solve for
+            # hyperelasticity, Form(V, alpha, beta, kappa=D(u)) at every Newton step for nonlinear diffusion
+            if hyper:
+                if vc is None:
+                    vc = _pmg(V, lambda W, k=None: Elasticity(W, F.mu, F.lmbda, F.beta, F.ds), sp, bcs, hierarchy,
+                              allreduce, omega=0.6)
+            else:
+                vc = _pmg(V, lambda W, k=None: Form(W, F.alpha, F.beta, k, F.ds), sp, bcs, hierarchy, allreduce,
+                          kappa=F.diffusivity(u))
+            M = lambda r, z, vc=vc: vc.apply(vc.top, r, z)
         else:
             raise NotImplementedError(f"pc_type {pc!r}")
         du.zero()
@@ -3042,7 +3100,9 @@ def solve(form: Form, L: op2.Dat, u: op2.Dat, bcs=(), solver_parameters=None, hi
     "gmres" (:func:`gmres`, right-preconditioned and flexible; the default for nonsymmetric forms, which
     cg refuses), ``ksp_gmres_restart`` (30); ``pc_type`` "none" (default) | "jacobi" | "mg" (needs
     ``hierarchy``, a mg.MeshHierarchy whose finest mesh is ``form.V.mesh``; for advection-diffusion a
-    V-cycle of its symmetric part ``Form(W, alpha, beta)``); ``ksp_rtol`` (1e-8), ``ksp_max_it`` (1000).
+    V-cycle of its symmetric part ``Form(W, alpha, beta)``) | "python" with ``pc_python_type``
+    "firedrake.PMGPC" or "firedrake.P1PC" (p-multigrid on ``V.mesh``, :class:`mg.PMG`, with the level forms of
+    "mg" and the ``pmg_*`` options of :func:`pmg_options`; CG2 and CG3); ``ksp_rtol`` (1e-8), ``ksp_max_it`` (1000).
     A :class:`Stokes` form takes MixedDats and its own options (:func:`_solve_stokes`), and the only form
     that takes ``nullspace``.  Returns (iterations, residual history)."""
     from . import _lib
@@ -3124,6 +3184,15 @@ def solve(form: Form, L: op2.Dat, u: op2.Dat, bcs=(), solver_parameters=None, hi
                             kappa=getattr(form, "kappa", None), cdim=V.cdim, omega=omega)
             top = len(hierarchy) - 1
             M = lambda r, z: vc.apply(top, r, z)
+        elif pc == "python":
+            # p-multigrid (firedrake.PMGPC / P1PC) with the level forms and Jacobi damping of the "mg" branch
+            ds = getattr(form, "ds", ())
+            if isinstance(form, Elasticity):
+                make, omega = (lambda W, k=None: Elasticity(W, form.mu, form.lmbda, form.beta, ds)), 0.6
+            else:
+                make, omega = (lambda W, k=None: Form(W, form.alpha, form.beta, k, ds)), 0.8
+            pm = _pmg(V, make, sp, bcs, hierarchy, allreduce, kappa=getattr(form, "kappa", None), omega=omega)
+            M = lambda r, z: pm.apply(pm.top, r, z)
         else:
             raise NotImplementedError(f"pc_type {pc!r}")
     if sp["ksp_type"] == "gmres":

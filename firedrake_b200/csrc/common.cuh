@@ -171,3 +171,7 @@ int fdb_launch_dg_transport(fdb_kernel_s *k, fdb_int start, fdb_int end, int nla
 int fdb_launch_dg_upwind(fdb_kernel_s *k, fdb_int start, fdb_int end, int nlay, const fdb_int *subset, double *y,
                          const double *coords, const double *x, const double *b, const unsigned *facet,
                          const fdb_int *map0, const fdb_int *map1);
+// FDB_FORM_P_PROLONG / P_RESTRICT / P_INJECT (p_transfer_hex.cu): mapf the fine rows ((degree+1)^3), mapc the coarse
+// rows ((nq)^3); w the restriction's fine-node weights (NULL for the other two)
+int fdb_launch_p_transfer(fdb_kernel_s *k, fdb_int start, fdb_int end, int nlay, const fdb_int *subset, double *out,
+                          const double *in, const double *w, const fdb_int *mapf, const fdb_int *mapc);

@@ -298,7 +298,11 @@ static int device_pointers(const fdb_call_args *a, bool mat, void **args, const 
 // fdb_kernel_call hands its arguments to the launchers.
 enum { MODE_ACTION, MODE_MATRIX, MODE_DIAGONAL };
 enum { LAUNCH_HELMHOLTZ, LAUNCH_HELMHOLTZ_COEF, LAUNCH_ELASTICITY, LAUNCH_STOKES, LAUNCH_BOUNDARY, LAUNCH_DG_FACET,
-       LAUNCH_DG_TRANSPORT };
+       LAUNCH_DG_TRANSPORT, LAUNCH_P_TRANSFER };
+// the degree of the second space of a form on two spaces: the descriptor's degree - 1 (Stokes' pressure, the
+// default of a row that does not name one), or any lower degree of an instantiated (fine, coarse) pair (the
+// p-multigrid transfers)
+enum { SPACE2_PRESSURE = 0, SPACE2_COARSER };
 
 struct fdb_hex_form {
     int form;                 // enum fdb_form
@@ -321,6 +325,7 @@ struct fdb_hex_form {
                               // NULL: such a form is an action only, in device mode
     int integral;             // enum fdb_integral: facet forms run in device mode only; -1: the descriptor's
                               // integral (cell, exterior or interior facet) selects the term
+    int space2_degree;        // SPACE2_*: the degree the second space must have (read when space2 is set)
 };
 
 static const fdb_hex_form hex_forms[] = {
@@ -355,7 +360,21 @@ static const fdb_hex_form hex_forms[] = {
     // upwind DG transport on DQ_p: b (3 values per vertex, through the vertex map), then on facets the local
     // facet numbers.  Device mode only, no rank 2
     {FDB_FORM_DG_TRANSPORT, "dg_transport", 1, false, "b", 3, false, LAUNCH_DG_TRANSPORT, {4, 0, 4}, 1, nullptr, -1},
+    // the p-multigrid degree transfers: the descriptor is the fine space CG_p, the second space the coarse CG_q, and
+    // R (desc.B, nq = q+1) and P (space2.B) their 1-D tables.  Device mode only, rank 1, no diagonal
+    {FDB_FORM_P_PROLONG, "p_prolong", -1, false, nullptr, 0, false, LAUNCH_P_TRANSFER, {3, 0, 0}, 2, "coarse",
+     FDB_INTEGRAL_CELL, SPACE2_COARSER},
+    {FDB_FORM_P_RESTRICT, "p_restrict", -1, false, nullptr, 0, false, LAUNCH_P_TRANSFER, {3, 0, 0}, 2, "fine, w",
+     FDB_INTEGRAL_CELL, SPACE2_COARSER},
+    {FDB_FORM_P_INJECT, "p_inject", -1, false, nullptr, 0, false, LAUNCH_P_TRANSFER, {3, 0, 0}, 2, "fine",
+     FDB_INTEGRAL_CELL, SPACE2_COARSER},
 };
+
+// the (fine, coarse) degree pairs the transfer kernels instantiate (p_transfer_hex.cu)
+static bool p_transfer_pair(int p, int q)
+{
+    return (p == 2 && q == 1) || (p == 3 && q == 1) || (p == 3 && q == 2);
+}
 
 static const char *const mode_name[] = {"action", "matrix", "diagonal"};
 
@@ -436,7 +455,13 @@ static int kernel_create(const fdb_kernel_desc *d, const fdb_space2_desc *s2, fd
         set_error("fdb_kernel_create: %s has no affine-cell variant (affine_cells must be 0)", f->name);
         return 1;
     }
-    if (d->nq != d->degree + 1) {
+    const bool transfer = f->launcher == LAUNCH_P_TRANSFER;
+    if (transfer && s2->degree + 1 != d->nq) {
+        set_error("fdb_kernel_create_mixed: %s: R (desc.B) has nq = q+1 rows, got nq=%d for the coarse degree %d",
+                  f->name, d->nq, s2->degree);
+        return 1;
+    }
+    if (!transfer && d->nq != d->degree + 1) {
         set_error("fdb_kernel_create: %s needs nq == degree+1 Gauss points per axis (got nq=%d for degree %d); "
                   "pin the rule with dx(degree=2*p)", f->name, d->nq, d->degree);
         return 1;
@@ -499,15 +524,41 @@ static int kernel_create(const fdb_kernel_desc *d, const fdb_space2_desc *s2, fd
         set_error("fdb_kernel_create: rank must be 1 or 2");
         return 1;
     }
-    if (d->cell == FDB_CELL_HEX_EXTRUDED && (!d->offset0 || !d->offset1)) {
+    // (a transfer reads no coordinates: offset1 is not used)
+    if (d->cell == FDB_CELL_HEX_EXTRUDED && (!d->offset0 || (!d->offset1 && !transfer))) {
         set_error("fdb_kernel_create: extruded cells need offset0/offset1");
         return 1;
     }
     // the second space: CG_{p-1} with p^3 dofs per cell (Stokes' pressure)
-    if (f->space2 && s2->degree != d->degree - 1) {
+    if (f->space2 && f->space2_degree == SPACE2_PRESSURE && s2->degree != d->degree - 1) {
         set_error("fdb_kernel_create_mixed: %s of degree %d needs a second space of degree %d, got %d", f->name,
                   d->degree, d->degree - 1, s2->degree);
         return 1;
+    }
+    // or a coarser CG_q of an instantiated pair, with exact unit endpoint rows in P and R (GLL nodes at both ends)
+    if (f->space2_degree == SPACE2_COARSER) {
+        if (!p_transfer_pair(d->degree, s2->degree)) {
+            set_error("fdb_kernel_create_mixed: %s: degree pair (fine %d, coarse %d) not instantiated: (2, 1), "
+                      "(3, 1), (3, 2)", f->name, d->degree, s2->degree);
+            return 1;
+        }
+        const int nf = d->degree + 1, nc = s2->degree + 1;
+        for (int e = 0; e < 2; e++) {
+            for (int a = 0; a < nc; a++)
+                if (s2->B[e * nc + a] != (a == e ? 1.0 : 0.0)) {
+                    set_error("fdb_kernel_create_mixed: %s needs GLL elements: row %d of P (space2.B) must be the "
+                              "exact unit vector e_%d (P[%d][%d] = %.17g); a Gauss-Legendre (DQ) element has no "
+                              "nodes at the ends", f->name, e, e, e, a, s2->B[e * nc + a]);
+                    return 1;
+                }
+            for (int i = 0; i < nf; i++)
+                if (d->B[e * nf + i] != (i == e ? 1.0 : 0.0)) {
+                    set_error("fdb_kernel_create_mixed: %s needs GLL elements: row %d of R (desc.B) must be the "
+                              "exact unit vector e_%d (R[%d][%d] = %.17g); a Gauss-Legendre (DQ) element has no "
+                              "nodes at the ends", f->name, e, e, e, i, d->B[e * nf + i]);
+                    return 1;
+                }
+        }
     }
     if (f->space2 && d->cell == FDB_CELL_HEX_EXTRUDED && !s2->offset) {
         set_error("fdb_kernel_create_mixed: %s on extruded cells needs the layer offsets of the second map "
@@ -528,15 +579,15 @@ static int kernel_create(const fdb_kernel_desc *d, const fdb_space2_desc *s2, fd
     if (d->offset1) memcpy(k->h_off1, d->offset1, sizeof(fdb_int) * arity1);
     k->desc.offset0 = k->h_off0;
     k->desc.offset1 = k->h_off1;
-    // the second space's map: CG_{p-1}, p^3 dofs per cell
-    const int arity2 = d->degree * d->degree * d->degree;
+    // the second space's map: (degree2 + 1)^3 dofs per cell
+    const int arity2 = f->space2 ? (s2->degree + 1) * (s2->degree + 1) * (s2->degree + 1) : 0;
     memset(k->h_off2, 0, sizeof(k->h_off2));
     memset(k->B2, 0, sizeof(k->B2));
     if (f->space2) {
         if (s2->offset) memcpy(k->h_off2, s2->offset, sizeof(fdb_int) * arity2);
         memcpy(k->B2, s2->B, sizeof(k->B2));
     }
-    if (collocated_derivative(k->n1d, d->B, d->D, k->Dt)) {
+    if (!transfer && collocated_derivative(k->n1d, d->B, d->D, k->Dt)) {
         set_error("fdb_kernel_create: basis table B is singular");
         delete k;
         return 1;
@@ -557,6 +608,54 @@ static int kernel_create(const fdb_kernel_desc *d, const fdb_space2_desc *s2, fd
     FDB_CUDA(cudaStreamSynchronize(ctx().stream));
     *out = k;
     return 0;
+}
+
+// the colouring plan of the call's map m (arity k->arity), rebuilt when the map, its generation or the range
+// changes.  It covers columns [0, end): the map is copied to the host if needed
+static int colouring_for(fdb_kernel_s *k, const fdb_call_args *a, int m)
+{
+    if (k->colour_map_key == (const void *)a->maps[m] && k->colour_map_gen == map_ver(a, m) &&
+        k->colour_end == a->end)
+        return 0;
+    std::vector<fdb_int> hmap;
+    const fdb_int *src = a->maps[m];
+    if (a->location == FDB_LOC_DEVICE) {
+        hmap.resize((size_t)a->end * k->arity);
+        FDB_CUDA(cudaMemcpy(hmap.data(), a->maps[m], sizeof(fdb_int) * hmap.size(), cudaMemcpyDeviceToHost));
+        src = hmap.data();
+    }
+    if (build_colouring(k, src, a->end)) return 1;
+    k->colour_map_key = (const void *)a->maps[m];
+    k->colour_map_gen = map_ver(a, m);
+    k->colour_end = a->end;
+    return 0;
+}
+
+// the p-multigrid transfers: args and maps in first-use order (include/fdb200.h), device mode only.  A coloured
+// restriction is coloured on the fine map: two cells that share a coarse node share a fine node too
+static int p_transfer_call(fdb_kernel_s *k, const fdb_call_args *a, int nlay)
+{
+    const int form = k->desc.form;
+    const fdb_hex_form *f = k->hex;
+    const int want = form == FDB_FORM_P_RESTRICT ? 3 : 2;
+    if (a->nargs != want || a->nmaps != 2 || a->location != FDB_LOC_DEVICE) {
+        set_error("fdb_kernel_call: %s expects %d device args (%s, %s) and 2 maps (%s), got %d/%d", f->name, want,
+                  form == FDB_FORM_P_PROLONG ? "fine" : "coarse", f->space2,
+                  form == FDB_FORM_P_PROLONG ? "fine map, coarse map" : "coarse map, fine map", a->nargs, a->nmaps);
+        return 1;
+    }
+    const int fm = form == FDB_FORM_P_PROLONG ? 0 : 1;      // the fine map's slot
+    if (form == FDB_FORM_P_RESTRICT && k->desc.scatter == FDB_SCATTER_COLOURED) {
+        if (a->start != 0) {
+            set_error("fdb_kernel_call: coloured scatter needs start == 0");
+            return 1;
+        }
+        if (colouring_for(k, a, fm)) return 1;
+    }
+    return fdb_launch_p_transfer(k, a->start, a->end, nlay, a->subset, (double *)a->args[0],
+                                 (const double *)a->args[1],
+                                 form == FDB_FORM_P_RESTRICT ? (const double *)a->args[2] : nullptr,
+                                 a->maps[fm], a->maps[1 - fm]);
 }
 
 extern "C" {
@@ -670,6 +769,7 @@ int fdb_kernel_call(fdb_kernel_t k, const fdb_call_args *a)
     // reads b before them: [y, coords, x, b], [d, coords, b] on cells, [y, coords, x, b, facets], [d, coords, b,
     // facets] on facets
     const fdb_hex_form *f = k->hex;
+    if (f->launcher == LAUNCH_P_TRANSFER) return p_transfer_call(k, a, nlay);
     const int mode = hex_mode(&k->desc);
     const bool transport_facets = f->launcher == LAUNCH_DG_TRANSPORT && k->desc.integral != FDB_INTEGRAL_CELL;
     if (f->integral != FDB_INTEGRAL_CELL && a->location != FDB_LOC_DEVICE) {
@@ -774,22 +874,8 @@ int fdb_kernel_call(fdb_kernel_t k, const fdb_call_args *a)
     }
     // (the dg_transport cell term needs no colours: a DQ cell owns its dofs)
     if (k->desc.scatter == FDB_SCATTER_COLOURED && !(f->launcher == LAUNCH_DG_TRANSPORT && !transport_facets) &&
-        (k->colour_map_key != (const void *)a->maps[0] || k->colour_map_gen != map_ver(a, 0) ||
-         k->colour_end != a->end)) {
-        // colouring covers columns [0, end): copy the map to the host if needed
-        std::vector<fdb_int> hmap;
-        const fdb_int *src = a->maps[0];
-        if (a->location == FDB_LOC_DEVICE) {
-            hmap.resize((size_t)a->end * k->arity);
-            FDB_CUDA(cudaMemcpy(hmap.data(), a->maps[0], sizeof(fdb_int) * hmap.size(),
-                                cudaMemcpyDeviceToHost));
-            src = hmap.data();
-        }
-        if (build_colouring(k, src, a->end)) return 1;
-        k->colour_map_key = (const void *)a->maps[0];
-        k->colour_map_gen = map_ver(a, 0);
-        k->colour_end = a->end;
-    }
+        colouring_for(k, a, 0))
+        return 1;
     if (k->desc.scatter == FDB_SCATTER_COLOURED && a->start != 0) {
         set_error("fdb_kernel_call: coloured scatter needs start == 0");
         return 1;

@@ -96,6 +96,21 @@ __global__ void k_scatter(size_t n, const fdb_int *__restrict__ idx, const doubl
     for (size_t j = (size_t)blockIdx.x * blockDim.x + threadIdx.x; j < n; j += stride) dst[idx[j]] = src[j];
 }
 
+// one Chebyshev iteration's vector work, d = c_d d + c_z dinv o (b - ax), x += d, in a single pass (c_d == 0: the
+// first iteration, d is not read)
+__global__ void k_chebyshev(size_t n, double cd, double cz, const double *__restrict__ b, const double *__restrict__ ax,
+                            const double *__restrict__ dinv, double *__restrict__ d, double *__restrict__ x)
+{
+    size_t stride = (size_t)gridDim.x * blockDim.x;
+    const bool first = cd == 0.0;
+    for (size_t j = (size_t)blockIdx.x * blockDim.x + threadIdx.x; j < n; j += stride) {
+        const double z = cz * (dinv[j] * (b[j] - ax[j]));
+        const double dj = first ? z : fma(cd, d[j], z);
+        d[j] = dj;
+        x[j] += dj;
+    }
+}
+
 constexpr int DOT_BLOCKS_MAX = 1056;   // 132 SMs x 8 (H100 SXM)
 
 __global__ void __launch_bounds__(256)
@@ -251,6 +266,16 @@ int fdb_vec_pointwise_mult(size_t n, const double *x, const double *y, double *w
 {
     if (require_init()) return 1;
     k_stream<3><<<stream_grid(n), 256, 0, ctx().stream>>>(n, 0.0, x, const_cast<double *>(y), w);
+    FDB_LAUNCH_CHECK();
+    return 0;
+}
+
+int fdb_vec_chebyshev(size_t n, double c_d, double c_z, const double *b, const double *ax, const double *dinv,
+                      double *d, double *x)
+{
+    if (require_init()) return 1;
+    if (n == 0) return 0;
+    k_chebyshev<<<stream_grid(2 * n), 256, 0, ctx().stream>>>(n, c_d, c_z, b, ax, dinv, d, x);
     FDB_LAUNCH_CHECK();
     return 0;
 }

@@ -294,7 +294,60 @@ class MeshHierarchy:
         return self.meshes[i]
 
 
-class VCycle:
+class _LevelCycle:
+    """The multigrid cycle shared by :class:`VCycle` (levels = meshes) and :class:`PMG` (levels = degrees on one
+    mesh): pre-smooth, residual, restrict, coarse correction, prolong, post-smooth, one level at a time.  A subclass
+    sets ``ops``, ``bcs``, ``transfers``, ``invdiag``, ``_work`` (per level: r, e, t, b, x) and ``nu`` / ``omega``, and
+    provides ``_coarse_solve``; ``_smooth`` defaults to damped Jacobi."""
+
+    def _smooth(self, l, b, x):
+        """x += omega D^-1 (b - A x), nu times."""
+        from . import _lib
+        L = _lib.lib()
+        A, w = self.ops[l], self._work[l]
+        n = b._data.size
+        for _ in range(self.nu):
+            A.mult(x, w["t"])
+            _lib.check(L.fdb_vec_aypx(n, -1.0, b.device_ptr, w["t"].device_ptr))        # t = b - A x
+            _lib.check(L.fdb_vec_pointwise_mult(n, w["t"].device_ptr, self.invdiag[l].device_ptr,
+                                                w["t"].device_ptr))
+            _touched(w["t"])
+            _lib.check(L.fdb_vec_axpy(n, self.omega, w["t"].device_ptr, x.device_ptr))
+            _touched(x)
+
+    def apply(self, l, b, x):
+        """One cycle on level l for A x = b, starting from the x passed in."""
+        from . import _lib
+        L = _lib.lib()
+        A, w = self.ops[l], self._work[l]
+        n = b._data.size
+        if l == 0:
+            self._coarse_solve(b, x)
+            return x
+        self._smooth(l, b, x)
+        A.mult(x, w["r"])
+        _lib.check(L.fdb_vec_aypx(n, -1.0, b.device_ptr, w["r"].device_ptr))             # r = b - A x
+        _touched(w["r"])
+        for bc in self.bcs[l]:
+            bc.zero(w["r"])
+        wc = self._work[l - 1]
+        T = self.transfers[l - 1]
+        T.restrict(w["r"], wc["b"])
+        for bc in self.bcs[l - 1]:
+            bc.zero(wc["b"])
+        wc["x"].zero()
+        wc["x"].device_ptr
+        self.apply(l - 1, wc["b"], wc["x"])
+        T.prolong(wc["x"], w["e"])
+        for bc in self.bcs[l]:
+            bc.zero(w["e"])
+        _lib.check(L.fdb_vec_axpy(n, 1.0, w["e"].device_ptr, x.device_ptr))
+        _touched(x)
+        self._smooth(l, b, x)
+        return x
+
+
+class VCycle(_LevelCycle):
     """Matrix-free geometric multigrid V-cycle for the Helmholtz family with rediscretised
     coarse operators (the ``pc_type mg`` + ``mat_type matfree`` setup of
     demos/multigrid/geometric_multigrid.py.rst): damped-Jacobi smoothing with the
@@ -354,53 +407,11 @@ class VCycle:
             out.insert(0, self.transfers[l].inject(out[0], self.spaces[l].dat()))
         return out
 
-    def _smooth(self, l, b, x):
-        """x += omega D^-1 (b - A x), nu times."""
-        from . import _lib
-        L = _lib.lib()
-        A, w = self.ops[l], self._work[l]
-        n = b._data.size
-        for _ in range(self.nu):
-            A.mult(x, w["t"])
-            _lib.check(L.fdb_vec_aypx(n, -1.0, b.device_ptr, w["t"].device_ptr))        # t = b - A x
-            _lib.check(L.fdb_vec_pointwise_mult(n, w["t"].device_ptr, self.invdiag[l].device_ptr,
-                                                w["t"].device_ptr))
-            _touched(w["t"])
-            _lib.check(L.fdb_vec_axpy(n, self.omega, w["t"].device_ptr, x.device_ptr))
-            _touched(x)
-
-    def apply(self, l, b, x):
-        """One V-cycle on level l for A x = b, starting from the x passed in."""
-        from . import _lib
+    def _coarse_solve(self, b, x):
+        """The coarsest level: CG to ``coarse_rtol``."""
         from .assemble import cg
-        L = _lib.lib()
-        A, w = self.ops[l], self._work[l]
-        n = b._data.size
-        if l == 0:
-            cg(A, b, x, rtol=self.coarse_rtol, maxit=self.coarse_maxit, allreduce=self.allreduce)
-            _touched(x)
-            return x
-        self._smooth(l, b, x)
-        A.mult(x, w["r"])
-        _lib.check(L.fdb_vec_aypx(n, -1.0, b.device_ptr, w["r"].device_ptr))             # r = b - A x
-        _touched(w["r"])
-        for bc in self.bcs[l]:
-            bc.zero(w["r"])
-        wc = self._work[l - 1]
-        T = self.transfers[l - 1]
-        T.restrict(w["r"], wc["b"])
-        for bc in self.bcs[l - 1]:
-            bc.zero(wc["b"])
-        wc["x"].zero()
-        wc["x"].device_ptr
-        self.apply(l - 1, wc["b"], wc["x"])
-        T.prolong(wc["x"], w["e"])
-        for bc in self.bcs[l]:
-            bc.zero(w["e"])
-        _lib.check(L.fdb_vec_axpy(n, 1.0, w["e"].device_ptr, x.device_ptr))
+        cg(self.ops[0], b, x, rtol=self.coarse_rtol, maxit=self.coarse_maxit, allreduce=self.allreduce)
         _touched(x)
-        self._smooth(l, b, x)
-        return x
 
 
 def pcg(A, b, x, M, rtol=1e-8, maxit=200, allreduce=None):
@@ -447,3 +458,267 @@ def pcg(A, b, x, M, rtol=1e-8, maxit=200, allreduce=None):
         rz = rz_new
         it += 1
     return it, hist
+
+
+# ------------------------------------------------------------------ p-multigrid
+class PTransfer:
+    """prolong / restrict / inject between two degrees on ONE mesh, CG_q (``Vc``) and CG_p (``Vf``), q < p, with
+    :class:`TransferManager`'s interface, on the hand-written kernels of csrc/p_transfer_hex.cu (forms "p_prolong",
+    "p_restrict", "p_inject").  The pairs (p, q) are (2, 1), (3, 1) and (3, 2); the engine refuses the others.
+    ``scatter``: "atomic" or "coloured" (bit-reproducible) for the restriction."""
+
+    def __init__(self, Vc, Vf, scatter="atomic"):
+        for W in (Vc, Vf):
+            if getattr(W, "family", "CG") != "CG":
+                raise NotImplementedError("PTransfer: CG spaces only (there is no DQ p-multigrid)")
+        if Vc.mesh is not Vf.mesh or Vc.cdim != Vf.cdim or not Vc.degree < Vf.degree:
+            raise ValueError("PTransfer: Vc and Vf must be spaces of one value size on the same mesh, Vc of the "
+                             "lower degree")
+        if Vf.dof_dset.halo is not None or Vc.dof_dset.halo is not None:
+            raise NotImplementedError("PTransfer: partitioned spaces are not supported")
+        self.Vc, self.Vf, self.scatter = Vc, Vf, scatter
+        # the coarse rows on the fine space's cell set: every loop iterates Vf.cell_set
+        self.cmap = op2.Map(Vf.cell_set, Vc.node_set, Vc.V.arity, Vc.V.cell_node_map, offset=Vc.V.offset,
+                            name="p_coarse")
+        kw = dict(degree=Vf.degree, coarse_degree=Vc.degree, cdim=Vf.cdim)
+        self._k = {f: op2.Kernel(f, **kw) for f in ("p_prolong", "p_restrict", "p_inject")}
+        self._gk = {}
+        self._weight = None
+
+    @property
+    def weight(self):
+        """1 / (number of cells containing the fine node), a scalar Dat on the fine nodes: set-up only, so it runs
+        on the generic wrapper path."""
+        if self._weight is None:
+            w = op2.Dat(op2.DataSet(self.Vf.node_set, 1))
+            nd = self.Vf.V.arity
+            count = CStringKernel(f"static void count(double *w) {{ for (int i = 0; i < {nd}; ++i) w[i] += 1.0; }}",
+                                  "count")
+            op2.par_loop(count, self.Vf.cell_set, w(op2.INC, self.Vf.cell_node_map))
+            op2.par_loop(reciprocal_kernel(1), self.Vf.node_set, w(op2.RW))
+            self._weight = w
+        return self._weight
+
+    def _loop(self, form, *args):
+        gk = self._gk.get(form)
+        if gk is None:
+            maps = []
+            for a in args:
+                if a.map not in maps:
+                    maps.append(a.map)
+            gk = self._gk[form] = op2.GlobalKernel(self._k[form], maps, extruded=True,
+                                                   scatter=self.scatter if form == "p_restrict" else "atomic")
+        op2.Parloop(gk, self.Vf.cell_set, args)()
+
+    def prolong(self, coarse: op2.Dat, fine: op2.Dat):
+        self._loop("p_prolong", fine(op2.WRITE, self.Vf.cell_node_map), coarse(op2.READ, self.cmap))
+        return fine
+
+    def restrict(self, fine_dual: op2.Dat, coarse_dual: op2.Dat):
+        w = self.weight
+        coarse_dual.zero()
+        coarse_dual.device_ptr                      # materialise the zero on the device
+        self._loop("p_restrict", coarse_dual(op2.INC, self.cmap), fine_dual(op2.READ, self.Vf.cell_node_map),
+                   w(op2.READ, self.Vf.cell_node_map))
+        return coarse_dual
+
+    def inject(self, fine: op2.Dat, coarse: op2.Dat):
+        self._loop("p_inject", coarse(op2.WRITE, self.cmap), fine(op2.READ, self.Vf.cell_node_map))
+        return coarse
+
+
+def pmg_degrees(p, coarse_degree=1, halve=True):
+    """The level degrees of p-multigrid, coarsest first: PMGPC halves the degree (p -> max(p // 2, coarse)), P1PC
+    (``halve=False``) goes straight to the coarse degree."""
+    degs = [p]
+    while degs[-1] > coarse_degree:
+        degs.append(max(degs[-1] // 2, coarse_degree) if halve else coarse_degree)
+    return degs[::-1]
+
+
+def jacobi_lanczos_bounds(A, invdiag, b, steps=10):
+    """The extreme eigenvalues (lmin, lmax) of D^-1 A estimated by ``steps`` Jacobi-preconditioned CG steps from the right-hand
+    side ``b`` (PETSc's KSPChebyshev estimate): the CG coefficients give the Lanczos tridiagonal, whose extreme
+    eigenvalues are computed on the host."""
+    import ctypes as C
+    from . import _lib
+    if steps < 1:
+        raise ValueError(f"jacobi_lanczos_bounds: steps must be at least 1, got {steps}")
+    L = _lib.lib()
+    V = b.dataset
+    r, z, p, Ap = (op2.Dat(V) for _ in range(4))
+    n = b._data.size
+
+    def dot(u, v):
+        out = C.c_double()
+        _lib.check(L.fdb_vec_dot(n, u.device_ptr, v.device_ptr, C.byref(out)))
+        return out.value
+    _lib.check(L.fdb_memcpy_d2d(r.device_ptr, b.device_ptr, b.nbytes))
+    _touched(r)
+    _lib.check(L.fdb_vec_pointwise_mult(n, r.device_ptr, invdiag.device_ptr, z.device_ptr))
+    _touched(z)
+    _lib.check(L.fdb_memcpy_d2d(p.device_ptr, z.device_ptr, z.nbytes))
+    _touched(p)
+    rz = dot(r, z)
+    alphas, betas = [], []
+    for _ in range(steps):
+        A.mult(p, Ap)
+        pAp = dot(p, Ap)
+        if not pAp > 0.0:
+            break
+        alpha = rz / pAp
+        _lib.check(L.fdb_vec_axpy(n, -alpha, Ap.device_ptr, r.device_ptr))
+        _lib.check(L.fdb_vec_pointwise_mult(n, r.device_ptr, invdiag.device_ptr, z.device_ptr))
+        _touched(r, z)
+        rz_new = dot(r, z)
+        alphas.append(alpha)
+        betas.append(rz_new / rz)
+        if not rz_new > 0.0:
+            break
+        _lib.check(L.fdb_vec_aypx(n, rz_new / rz, z.device_ptr, p.device_ptr))           # p = z + beta p
+        _touched(p)
+        rz = rz_new
+    k = len(alphas)
+    if k == 0:
+        raise ArithmeticError(f"Chebyshev eigenvalue estimate: p.A p = {pAp} at the first step (D^-1 A is not "
+                              f"positive definite, or the right-hand side is zero)")
+    T = np.zeros((k, k))
+    for j in range(k):
+        T[j, j] = 1.0 / alphas[j] + (betas[j - 1] / alphas[j - 1] if j else 0.0)
+        if j + 1 < k:
+            T[j, j + 1] = T[j + 1, j] = np.sqrt(betas[j]) / alphas[j]
+    ev = np.linalg.eigvalsh(T)
+    return float(ev[0]), float(ev[-1])
+
+
+def chebyshev_coefficients(emin, emax, k):
+    """(c_d, c_z) of the k iterations d = c_d d + c_z D^-1 (b - A x), x += d of the Chebyshev iteration for D^-1 A
+    with spectrum bounds [emin, emax] (Saad, Iterative Methods for Sparse Linear Systems, Algorithm 12.1); the first
+    has c_d = 0."""
+    theta, delta = 0.5 * (emax + emin), 0.5 * (emax - emin)
+    sigma = theta / delta
+    rho = 1.0 / sigma
+    out = [(0.0, 1.0 / theta)]
+    for _ in range(k - 1):
+        rho_new = 1.0 / (2.0 * sigma - rho)
+        out.append((rho_new * rho, 2.0 * rho_new / delta))
+        rho = rho_new
+    return out
+
+
+class PMG(_LevelCycle):
+    """p-multigrid on one mesh (Firedrake's ``firedrake.PMGPC`` / ``firedrake.P1PC``): the levels are CG spaces of
+    falling degree on ``V.mesh`` (:func:`pmg_degrees`), the operators rediscretised on every level, the transfers
+    :class:`PTransfer`.  The cycle is :class:`VCycle`'s (``_LevelCycle.apply``); the top level is ``len(ops) - 1``.
+
+    ``make_form(W[, kappa])``: the form on a level space (with the level's coefficient when ``kappa``, a Dat on
+    ``V``, is given; each coarser level gets the injection of the next finer one's).  ``bc_domains``: the
+    Dirichlet sub-domains, whose rows are zeroed on every level.
+
+    Smoother on the levels above the coarsest: ``smoother`` "chebyshev" (Chebyshev-Jacobi, ``nu`` iterations with
+    the bounds ``esteig`` = (a, b, c, d): [a lmin + b lmax, c lmin + d lmax] with lmin, lmax of D^-1 A estimated
+    by :func:`jacobi_lanczos_bounds` in ``esteig_steps`` steps from a right-hand side seeded by ``seed``) or "richardson" (damped Jacobi with ``omega``, ``nu`` sweeps).
+
+    Coarse solve: ``coarse_ksp`` "cg" with ``coarse_pc`` "jacobi" or "none" to ``coarse_rtol`` /
+    ``coarse_maxit``, or "preonly" with "mg": one :class:`VCycle` at the coarse degree on ``hierarchy``, whose
+    finest mesh must be ``V.mesh`` and whose top space then is this hierarchy's coarse space."""
+
+    def __init__(self, V, make_form, bc_domains=(), coarse_degree=1, halve=True, kappa=None, smoother="chebyshev",
+                 nu=2, omega=0.8, esteig=(0.0, 0.1, 0.0, 1.1), esteig_steps=10, coarse_ksp="cg", coarse_pc="jacobi",
+                 coarse_rtol=1e-3, coarse_maxit=500, hierarchy=None, allreduce=None, scatter="atomic", seed=0):
+        from .assemble import DirichletBC, FunctionSpace, assemble
+        if getattr(V, "family", "CG") != "CG":
+            raise NotImplementedError("PMG takes CG spaces (there is no DQ p-multigrid)")
+        if allreduce is not None or V.dof_dset.halo is not None:
+            raise NotImplementedError("PMG on a partitioned space is not implemented (multi-GPU p-multigrid)")
+        if V.degree <= coarse_degree or coarse_degree < 1:
+            raise ValueError(f"PMG: fine degree {V.degree} has nothing to coarsen to degree {coarse_degree}")
+        if V.degree > 3:
+            raise NotImplementedError(f"PMG: fine degree {V.degree}: the Jacobi smoother needs the diagonal, which "
+                                      f"the hand-written kernels give up to degree 3")
+        if smoother not in ("chebyshev", "richardson"):
+            raise NotImplementedError(f"PMG level smoother {smoother!r}: 'chebyshev' or 'richardson'")
+        if (coarse_ksp, coarse_pc) not in (("cg", "jacobi"), ("cg", "none"), ("preonly", "mg")):
+            raise NotImplementedError(f"PMG coarse solve ksp_type {coarse_ksp!r} with pc_type {coarse_pc!r}: cg with "
+                                      f"jacobi or none, or preonly with mg")
+        self.nu, self.omega, self.smoother = nu, omega, smoother
+        self.coarse_ksp, self.coarse_pc = coarse_ksp, coarse_pc
+        self.coarse_rtol, self.coarse_maxit = coarse_rtol, coarse_maxit
+        self.degrees = pmg_degrees(V.degree, coarse_degree, halve)
+        self.coarse_mg = None
+        spaces = [FunctionSpace(V.mesh, q, V.cdim) for q in self.degrees[:-1]] + [V]
+        self.transfers = [PTransfer(spaces[l], spaces[l + 1], scatter) for l in range(len(spaces) - 1)]
+        if kappa is not None:
+            kappas = [kappa]
+            for T in self.transfers[::-1]:
+                kappas.insert(0, T.inject(kappas[0], T.Vc.dat()))
+            self.kappas = kappas
+        if coarse_pc == "mg":
+            # the same mesh object: the coarse space becomes the V-cycle's top space, which PTransfer pairs with the
+            # finer PMG levels on V.mesh
+            if hierarchy is None or hierarchy[len(hierarchy) - 1] is not V.mesh:
+                raise ValueError("PMG coarse pc_type mg needs a mesh hierarchy whose finest mesh is V's mesh")
+            self.coarse_mg = VCycle(hierarchy, coarse_degree, make_form, bc_domains, omega=omega,
+                                    kappa=None if kappa is None else self.kappas[0], cdim=V.cdim)
+            self._coarse_top = len(hierarchy) - 1
+            spaces[0] = self.coarse_mg.spaces[-1]     # the same numbering as FunctionSpace(V.mesh, coarse_degree)
+            self.transfers[0] = PTransfer(spaces[0], spaces[1], scatter)
+        self.spaces = spaces
+        self.bcs = [[DirichletBC(W, 0.0, s) for s in bc_domains] for W in spaces]
+        self.ops, self.invdiag = [], []
+        for l, W in enumerate(spaces):
+            if l == 0 and self.coarse_mg is not None:
+                self.ops.append(self.coarse_mg.ops[-1])
+                self.invdiag.append(self.coarse_mg.invdiag[-1])
+                continue
+            f = make_form(W) if kappa is None else make_form(W, self.kappas[l])
+            A = assemble(f, bcs=self.bcs[l], mat_type="matfree")
+            d = A.getDiagonal(W.dat())
+            op2.par_loop(reciprocal_kernel(V.cdim), W.node_set, d(op2.RW))
+            self.ops.append(A)
+            self.invdiag.append(d)
+        self._work = [dict(r=W.dat(), e=W.dat(), t=W.dat(), b=W.dat(), x=W.dat(), d=W.dat()) for W in spaces]
+        self.top = len(spaces) - 1
+        # Chebyshev bounds of D^-1 A on every smoothed level
+        self.bounds = [None] * len(spaces)
+        if smoother == "chebyshev":
+            a, b_, c, d_ = esteig
+            rng = np.random.default_rng(seed)
+            for l in range(1, len(spaces)):
+                W = spaces[l]
+                shape = (W.node_count, W.cdim) if W.cdim > 1 else (W.node_count,)
+                rhs = W.dat(rng.standard_normal(shape))
+                for bc in self.bcs[l]:
+                    bc.zero(rhs)
+                lmin, lmax = jacobi_lanczos_bounds(self.ops[l], self.invdiag[l], rhs, esteig_steps)
+                self.bounds[l] = (a * lmin + b_ * lmax, c * lmin + d_ * lmax)
+
+    def _smooth(self, l, b, x):
+        if self.smoother == "richardson":
+            return super()._smooth(l, b, x)
+        # one action and one fused vector pass per iteration
+        from . import _lib
+        L = _lib.lib()
+        A, w = self.ops[l], self._work[l]
+        n = b._data.size
+        for cd, cz in chebyshev_coefficients(*self.bounds[l], self.nu):
+            A.mult(x, w["t"])
+            _lib.check(L.fdb_vec_chebyshev(n, cd, cz, b.device_ptr, w["t"].device_ptr, self.invdiag[l].device_ptr,
+                                           w["d"].device_ptr, x.device_ptr))
+            _touched(w["d"], x)
+
+    def _coarse_solve(self, b, x):
+        from . import _lib
+        from .assemble import cg
+        if self.coarse_mg is not None:
+            self.coarse_mg.apply(self._coarse_top, b, x)
+        elif self.coarse_pc == "none":
+            cg(self.ops[0], b, x, rtol=self.coarse_rtol, maxit=self.coarse_maxit)
+        else:
+            L, d, n = _lib.lib(), self.invdiag[0], b._data.size
+
+            def M(r, z):
+                _lib.check(L.fdb_vec_pointwise_mult(n, r.device_ptr, d.device_ptr, z.device_ptr))
+                _touched(z)
+            pcg(self.ops[0], b, x, M, rtol=self.coarse_rtol, maxit=self.coarse_maxit)
+        _touched(x)

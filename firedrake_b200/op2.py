@@ -1421,6 +1421,12 @@ class Kernel:
     ``dot(b, n('+'))*u_up*(v('+') - v('-'))*dS``, "exterior_facet" ``(c_out*max(b.n, 0) + c_in*min(b.n, 0))*u*v*ds``.
     Arguments: action (output, coordinates, u, b[, facets]), diagonal (output, coordinates, b[, facets]), with the
     facet numbers on facet integrals only; no rank 2; device-resident Dats only.
+
+    "p_prolong", "p_restrict" and "p_inject" are the degree transfers of p-multigrid between the fine space CG_p
+    (``degree``) and a coarse space CG_q (``coarse_degree``) on the same cells, value size ``cdim`` 1 or 3: prolong
+    (fine WRITE, coarse READ), restrict (coarse INC, fine READ, w READ: ``coarse += P^T (w * fine)``, w one value per
+    fine node) and inject (coarse WRITE, fine READ).  The fine Dats go through the fine space's map, the coarse ones
+    through the coarse space's; no coordinates.  Device-resident Dats only.
     """
     form: str = "helmholtz"
     degree: int = 1
@@ -1444,6 +1450,7 @@ class Kernel:
     c_s: float = 0.0
     c_out: float = 1.0              # dg_transport (exterior facets): the max(b.n, 0) and min(b.n, 0) coefficients
     c_in: float = 0.0
+    coarse_degree: int = 0          # p_prolong / p_restrict / p_inject: the coarse space's degree q
 
     def __new__(cls, *args, **kwargs):
         # ``op2.Kernel(code, name)`` with C source (pyop2/local_kernel.py:33-43) builds the
@@ -1460,6 +1467,11 @@ class Kernel:
             if len(self.d) != 3:
                 raise ValueError("d holds the three coefficients of D(s) = d0 + d1 s + d2 s^2")
         spec = _FORMS.get(self.form)
+        if spec and spec.transfer:
+            acc = (INC, READ, READ) if self.form == "p_restrict" else (WRITE, READ)
+            object.__setattr__(self, "accesses", acc)
+            object.__setattr__(self, "name", self.form)
+            return
         if spec and spec.pressure:
             # the velocity space is always a vector space: cdim is 3 unless given otherwise (which the engine
             # refuses)
@@ -1517,6 +1529,7 @@ class _Form(NamedTuple):
     pressure: bool = False      # also reads and writes a scalar pressure space through a third map (Stokes)
     facet: bool = False         # an exterior-facet integral: the local facet numbers come last, the integral as given
     velocity: bool = False      # reads b (3 values per vertex) through the coordinate map after u
+    transfer: bool = False      # a p-multigrid degree transfer: fine and coarse maps, no coordinates
 
 
 _FORMS = {"helmholtz": _Form(_lib.FORM_HELMHOLTZ),
@@ -1534,9 +1547,28 @@ _FORMS = {"helmholtz": _Form(_lib.FORM_HELMHOLTZ),
           "boundary_mass": _Form(_lib.FORM_BOUNDARY_MASS, facet=True),
           "interior_penalty": _Form(_lib.FORM_INTERIOR_PENALTY, facet=True),
           "dg_boundary": _Form(_lib.FORM_DG_BOUNDARY, facet=True),
-          "dg_transport": _Form(_lib.FORM_DG_TRANSPORT, facet=True, velocity=True)}
+          "dg_transport": _Form(_lib.FORM_DG_TRANSPORT, facet=True, velocity=True),
+          "p_prolong": _Form(_lib.FORM_P_PROLONG, transfer=True),
+          "p_restrict": _Form(_lib.FORM_P_RESTRICT, transfer=True),
+          "p_inject": _Form(_lib.FORM_P_INJECT, transfer=True)}
 _INTEGRALS = {"cell": _lib.INTEGRAL_CELL, "exterior_facet": _lib.INTEGRAL_EXTERIOR_FACET,
               "interior_facet": _lib.INTEGRAL_INTERIOR_FACET, "fused": _lib.INTEGRAL_FUSED}
+
+
+def p_transfer_tables(p, q):
+    """The 1-D tables of the degree transfers between CG_p and CG_q on GLL nodes, in dof numbering: P (p+1, q+1), the
+    coarse basis at the fine nodes, and R (q+1, p+1), the fine basis at the coarse nodes.  Both spaces have nodes at
+    the ends of the interval (dofs 0 and 1), so the endpoint rows are unit vectors: they are set exactly, which is
+    what makes every cell sharing a node write bitwise the same value."""
+    from .fiat_lite import interval_element
+    fine, coarse = interval_element(p), interval_element(q)
+    P, _ = coarse.tabulate(fine.nodes)
+    R, _ = fine.tabulate(coarse.nodes)
+    P, R = np.array(P, dtype=float), np.array(R, dtype=float)
+    for T in (P, R):
+        T[:2] = 0.0
+        T[0, 0] = T[1, 1] = 1.0
+    return P, R
 
 
 class GlobalKernel:
@@ -1602,6 +1634,8 @@ class GlobalKernel:
             _lib.check(_lib.lib().fdb_kernel_create(C.byref(d), C.byref(h)), "fdb_kernel_create")
             self._handle = h
             return h
+        if _FORMS[lk.form].transfer:
+            return self._compile_transfer()
         el = lk.element or interval_element(lk.degree)
         n = lk.degree + 1
         if el.ndof != n:
@@ -1664,6 +1698,47 @@ class GlobalKernel:
                        "fdb_kernel_create_mixed")
         else:
             _lib.check(_lib.lib().fdb_kernel_create(C.byref(d), C.byref(h)), "fdb_kernel_create")
+        del keep
+        self._handle = h
+        return h
+
+    def _compile_transfer(self):
+        """fdb_kernel_create_mixed of a p-multigrid transfer: R in the descriptor's B (nq = q+1), P in the second
+        space's (include/fdb200.h).  The maps come in first-use order: prolong (fine, coarse), restrict and inject
+        (coarse, fine)."""
+        from .fiat_lite import interval_element
+        lk = self.local_kernel
+        d = _lib.KernelDesc()
+        d.form, d.rank, d.integral = _FORMS[lk.form].enum, 1, _lib.INTEGRAL_CELL
+        d.cell = _lib.CELL_HEX_EXTRUDED if self.extruded else _lib.CELL_HEX
+        d.degree, d.nq, d.cdim = lk.degree, lk.coarse_degree + 1, lk.cdim
+        d.scatter = {"atomic": _lib.SCATTER_ATOMIC, "coloured": _lib.SCATTER_COLOURED}[self.scatter]
+        s2 = _lib.Space2Desc()
+        s2.degree = lk.coarse_degree
+        if lk.element is None and lk.coarse_degree >= 1:
+            P, R = p_transfer_tables(lk.degree, lk.coarse_degree)
+        else:                               # another fine element (the engine refuses one without end nodes)
+            fine = lk.element or interval_element(lk.degree)
+            coarse = interval_element(lk.coarse_degree, variant=getattr(fine, "variant", "gll"))
+            P, _ = coarse.tabulate(fine.nodes)
+            R, _ = fine.tabulate(coarse.nodes)
+        nf, nc = P.shape
+        for i in range(nf):
+            for a in range(nc):
+                s2.B[i * nc + a] = P[i, a]
+                d.B[a * nf + i] = R[a, i]
+        fm, cm = self.arguments[:2] if lk.form == "p_prolong" else self.arguments[1::-1]
+        keep = []
+        if self.extruded:
+            if fm.offset is None or cm.offset is None:
+                raise MapValueError("extruded parloop needs maps with offsets")
+            of = np.ascontiguousarray(fm.offset, dtype=IntType)
+            oc = np.ascontiguousarray(cm.offset, dtype=IntType)
+            keep = [of, oc]
+            d.offset0 = of.ctypes.data_as(C.POINTER(C.c_int32))
+            s2.offset = oc.ctypes.data_as(C.POINTER(C.c_int32))
+        h = C.c_void_p()
+        _lib.check(_lib.lib().fdb_kernel_create_mixed(C.byref(d), C.byref(s2), C.byref(h)), "fdb_kernel_create_mixed")
         del keep
         self._handle = h
         return h

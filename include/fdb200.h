@@ -290,7 +290,7 @@ enum fdb_form {
                                    argument its uint32 local facet number.  Device mode only:
                                      action    [y INC, coords, u, facet]  (atomic or coloured)
                                      diagonal  [d INC, coords, facet]                             */
-    FDB_FORM_DG_TRANSPORT = 16
+    FDB_FORM_DG_TRANSPORT = 16,
                                 /* upwind DG transport of a scalar DQ_p field (Gauss-Legendre nodes) by
                                    a velocity b given at the mesh VERTICES (3 values per vertex, read
                                    through maps[1], the vertex map), in conservative form (NOT
@@ -315,6 +315,35 @@ enum fdb_form {
                                      facets    action    [y INC, coords, u, b, facets]  (atomic or
                                                                                          coloured)
                                                diagonal  [d INC, coords, b, facets]               */
+    FDB_FORM_P_PROLONG = 17,
+    FDB_FORM_P_RESTRICT = 18,
+    FDB_FORM_P_INJECT = 19
+                                /* the degree transfers of p-multigrid between a fine space CG_p and a
+                                   coarse space CG_q on the SAME hex cells, both on GLL nodes (value size
+                                   cdim 1 or 3, AoS), cell-local and sum-factorised:
+                                     P_PROLONG   fine    = (P (x) P (x) P) coarse           WRITE
+                                     P_RESTRICT  coarse += (P (x) P (x) P)^T (w o fine)     INC
+                                     P_INJECT    coarse  = (R (x) R (x) R) fine             WRITE
+                                   Tables, row-major in 1-D dof numbering (dof 0 at x = 0, dof 1 at x = 1,
+                                   then the interior nodes):
+                                     P (p+1, q+1), the coarse basis at the fine nodes: fdb_space2_desc.B
+                                     R (q+1, p+1), the fine basis at the coarse nodes: fdb_kernel_desc.B,
+                                                   with nq = q+1
+                                   The descriptor describes the fine space (degree = p, cdim, offset0 = the
+                                   fine map's layer offsets; offset1, D, wq, xq unused), fdb_space2_desc the
+                                   coarse space (degree = q, offset = the coarse map's layer offsets).
+                                   Created by fdb_kernel_create_mixed, rank 1, cell integral.  (p, q) in
+                                   {(2, 1), (3, 1), (3, 2)}.  The endpoint rows (dofs 0 and 1) of P and R
+                                   must be exact unit vectors, as they are for GLL elements (a Gauss-Legendre,
+                                   DQ, element is refused): every cell that writes a shared node then
+                                   writes bitwise the same value.  w is one value per fine node, 1 / (number
+                                   of cells containing it), so that the restriction is exactly P^T.  The
+                                   maps are in first-use order of the arguments.  Device mode only:
+                                     P_PROLONG   [fine WRITE, coarse]       maps [fine map, coarse map]
+                                     P_RESTRICT  [coarse INC, fine, w]      maps [coarse map, fine map]
+                                                                            (atomic or coloured scatter;
+                                                                            coloured is bit-reproducible)
+                                     P_INJECT    [coarse WRITE, fine]       maps [coarse map, fine map]  */
 };
 
 enum fdb_cell {
@@ -390,7 +419,8 @@ typedef struct fdb_kernel_desc {
  * layout.  degree: the second space's polynomial degree (Stokes: the velocity degree minus 1);
  * B: its basis at the descriptor's nq Gauss points, row-major (nq, degree+1), 1-D dof numbering;
  * offset: the extruded layer offsets of the second space's map, (degree+1)^3 entries, NULL for
- * native hexes, copied at creation. */
+ * native hexes, copied at creation.  The p-multigrid transfers (FDB_FORM_P_PROLONG, _RESTRICT, _INJECT)
+ * describe their coarse space CG_q here: degree = q and B = P, (fine degree + 1, q + 1). */
 typedef struct fdb_space2_desc {
     int32_t degree;
     double B[FDB_MAX_1D * FDB_MAX_1D];
@@ -403,7 +433,8 @@ typedef struct fdb_kernel_s *fdb_kernel_t;
  * "compile" = validate the descriptor, precompute tables, pick the sm_90a
  * kernel instantiation.  Fails (nonzero) for forms outside the supported set. */
 int fdb_kernel_create(const fdb_kernel_desc *desc, fdb_kernel_t *out);
-/* The same for a form on two spaces (FDB_FORM_STOKES, FDB_FORM_NAVIER_STOKES[_JACOBIAN]), which
+/* The same for a form on two spaces (FDB_FORM_STOKES, FDB_FORM_NAVIER_STOKES[_JACOBIAN], the
+ * p-multigrid transfers FDB_FORM_P_*), which
  * fdb_kernel_create refuses; a form on one
  * space is refused here. */
 int fdb_kernel_create_mixed(const fdb_kernel_desc *desc, const fdb_space2_desc *space2, fdb_kernel_t *out);
@@ -629,6 +660,11 @@ int fdb_vec_fill(size_t n, double a, double *x);                              /*
                                                                                  pyop2/types/dat.py:633-636 */
 int fdb_vec_dot(size_t n, const double *x, const double *y, double *out);
 int fdb_vec_pointwise_mult(size_t n, const double *x, const double *y, double *w);
+/* the vector part of one Chebyshev iteration with a diagonal preconditioner, in one pass, given ax = A x:
+ *   d = c_d d + c_z dinv o (b - ax);  x += d
+ * (c_d == 0: d is not read, the first iteration) */
+int fdb_vec_chebyshev(size_t n, double c_d, double c_z, const double *b, const double *ax, const double *dinv,
+                      double *d, double *x);
 /* compact gather / scatter through a device index list: the VecScatter of a virtual sub-matrix
  * (MatCreateSubMatrixVirtual, the fallback of firedrake/matrix_free/operators.py:380-405) */
 int fdb_vec_gather(size_t n, const fdb_int *idx, const double *src, double *dst);   /* dst[j] = src[idx[j]] */
