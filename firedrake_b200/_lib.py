@@ -33,6 +33,8 @@ FORM_DG_TRANSPORT = 16
 FORM_P_PROLONG = 17
 FORM_P_RESTRICT = 18
 FORM_P_INJECT = 19
+FORM_SPECTRAL_HELMHOLTZ = 20           # alpha*inner(grad u, grad v)*dx(GLL) + beta*inner(u, v)*dx(GLL)
+FORM_SPECTRAL_HELMHOLTZ_COEF = 21      # the same with a trailing nodal kappa in the stiffness term
 CELL_HEX_EXTRUDED = 1
 CELL_HEX = 2
 CELL_TRIANGLE = 3
@@ -176,6 +178,9 @@ SIGNATURES = {
     "fdb_vec_aypx": (C.c_int, [C.c_size_t, C.c_double, C.c_void_p, C.c_void_p]),
     "fdb_vec_scale": (C.c_int, [C.c_size_t, C.c_double, C.c_void_p]),
     "fdb_vec_fill": (C.c_int, [C.c_size_t, C.c_double, C.c_void_p]),
+    "fdb_vec_leapfrog": (C.c_int, [C.c_size_t, C.c_double, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "fdb_point_eval": (C.c_int, [C.c_int32, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "fdb_point_load": (C.c_int, [C.c_int32, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_double, C.c_void_p]),
     "fdb_vec_gather": (C.c_int, [C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p]),
     "fdb_vec_scatter": (C.c_int, [C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p]),
     "fdb_asm_create": (C.c_int, [C.c_int, C.c_void_p, C.c_void_p, C.POINTER(C.c_void_p)]),

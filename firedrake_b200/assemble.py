@@ -2014,6 +2014,370 @@ def ssprk3(F: DGTransport, q: op2.Dat, dt, steps, load: op2.Dat = None):
     return q
 
 
+def spectral_helmholtz_kernel(degree, alpha=1.0, beta=0.0, coef=False, name=None):
+    """C source of the spectral-element Helmholtz action ``alpha*inner(kappa*grad u, grad v)*dx(GLL) +
+    beta*inner(u, v)*dx(GLL)`` on CG_p hexes (p = 1..3), written the way TSFC writes a collocated kernel (the whole
+    cell's basis gradient at every GLL point, the full Jacobian there), for the generic wrapper builder: the
+    independent statement of FDB_FORM_SPECTRAL_HELMHOLTZ[_COEF].  Arguments: y (INC), coordinates, u[, kappa]."""
+    from .codegen import CStringKernel
+    from .fiat_lite import interval_element
+    if not 1 <= degree <= 3:
+        raise NotImplementedError(f"spectral_helmholtz_kernel: degree {degree} (1..3 on the generic path)")
+    el = interval_element(degree, quadrature="gll")
+    n, nd = degree + 1, (degree + 1) ** 3
+    tab = lambda a: "{" + ", ".join("{" + ", ".join(repr(float(v)) for v in r) + "}" for r in a) + "}"
+    vec = lambda a: "{" + ", ".join(repr(float(v)) for v in a) + "}"
+    base = name or f"spectral_helmholtz{degree}{'_coef' if coef else ''}"
+    kap = ", const double *kap" if coef else ""
+    src = f"""
+static const double TD[{n}][{n}] = {tab(el.D)};      /* d l_a / dx at GLL point q (B is the identity) */
+static const double TX[{n}] = {vec(el.xq)};
+static const double TW[{n}] = {vec(el.wq)};
+static void {base}(double *A, const double *X, const double *w{kap})
+{{
+    for (int qx = 0; qx < {n}; ++qx) for (int qy = 0; qy < {n}; ++qy) for (int qz = 0; qz < {n}; ++qz) {{
+        const int q = (qx * {n} + qy) * {n} + qz;
+        const double xi[3] = {{TX[qx], TX[qy], TX[qz]}};
+        double J[3][3], K[3][3], grad[{nd}][3], gu[3] = {{0.0, 0.0, 0.0}};
+        for (int c = 0; c < 3; ++c) for (int d = 0; d < 3; ++d) J[c][d] = 0.0;
+        for (int v = 0; v < 8; ++v) {{
+            const int bb[3] = {{(v >> 2) & 1, (v >> 1) & 1, v & 1}};
+            for (int d = 0; d < 3; ++d) {{
+                double g = bb[d] ? 1.0 : -1.0;
+                for (int e = 0; e < 3; ++e) if (e != d) g *= bb[e] ? xi[e] : 1.0 - xi[e];
+                for (int c = 0; c < 3; ++c) J[c][d] += X[v * 3 + c] * g;
+            }}
+        }}
+        const double det = J[0][0] * (J[1][1] * J[2][2] - J[1][2] * J[2][1])
+                         - J[0][1] * (J[1][0] * J[2][2] - J[1][2] * J[2][0])
+                         + J[0][2] * (J[1][0] * J[2][1] - J[1][1] * J[2][0]);
+        for (int d = 0; d < 3; ++d) for (int c = 0; c < 3; ++c) {{
+            const int d1 = (d + 1) % 3, d2 = (d + 2) % 3, c1 = (c + 1) % 3, c2 = (c + 2) % 3;
+            K[d][c] = (J[c1][d1] * J[c2][d2] - J[c1][d2] * J[c2][d1]) / det;
+        }}
+        for (int a = 0; a < {n}; ++a) for (int b = 0; b < {n}; ++b) for (int c = 0; c < {n}; ++c) {{
+            const int i = (a * {n} + b) * {n} + c;
+            const double r[3] = {{TD[qx][a] * (b == qy) * (c == qz), (a == qx) * TD[qy][b] * (c == qz),
+                                 (a == qx) * (b == qy) * TD[qz][c]}};
+            for (int e = 0; e < 3; ++e) {{
+                grad[i][e] = K[0][e] * r[0] + K[1][e] * r[1] + K[2][e] * r[2];
+                gu[e] += grad[i][e] * w[i];
+            }}
+        }}
+        const double W = TW[qx] * TW[qy] * TW[qz] * fabs(det);
+        const double s = {repr(float(alpha))} * W{" * kap[q]" if coef else ""};
+        for (int i = 0; i < {nd}; ++i)
+            A[i] += s * (gu[0] * grad[i][0] + gu[1] * grad[i][1] + gu[2] * grad[i][2]);
+        A[q] += {repr(float(beta))} * W * w[q];
+    }}
+}}
+"""
+    return CStringKernel(src, base)
+
+
+@dataclass
+class SpectralForm:
+    """The spectral-element (SEM) Helmholtz operator on a scalar CG_p space (p = 1..5), integrated with the GLL rule
+    at the nodes themselves (Firedrake's ``dx(scheme=gauss_lobatto_legendre_cube_rule(...))``):
+
+        a(u, v) = alpha*inner(kappa*grad(u), grad(v))*dx(GLL) + beta*inner(u, v)*dx(GLL)
+
+    ``kappa``: a nodal scalar Dat on ``V`` (c**2 of the wave equation), or None for 1.  The mass term is diagonal (mass
+    lumping): ``lumped_mass(V)`` is ``SpectralForm(V, 0, 1)``'s diagonal.  ``assemble(F, u=x)`` is the action,
+    ``assemble(F, mat_type="matfree")`` an :class:`ImplicitMatrixContext` with ``getDiagonal`` at every degree, and
+    :func:`solve` runs CG with ``pc_type`` "none" or "jacobi".  There is no assembled matrix (aij), no geometric or
+    p-multigrid, and no ds terms; DQ, vector and partitioned spaces are refused.  Runs on
+    FDB_FORM_SPECTRAL_HELMHOLTZ[_COEF] (csrc/sem_hex.cu); :func:`leapfrog` steps the wave equation with it."""
+    V: FunctionSpace
+    alpha: float = 1.0
+    beta: float = 0.0
+    kappa: op2.Dat | None = None
+    ds: tuple = ()
+    symmetric = True
+
+    def __post_init__(self):
+        V = self.V
+        _refuse_dq(V, "SpectralForm", "it is stated on the GLL nodes of CG spaces")
+        if V.cdim != 1:
+            raise NotImplementedError("SpectralForm takes scalar spaces only (vector spaces are not implemented)")
+        if V.dof_dset.halo is not None:
+            raise NotImplementedError("SpectralForm on a partitioned space is not implemented")
+        if self.ds:
+            raise NotImplementedError("SpectralForm has no ds terms (boundary integrals on the GLL rule are not "
+                                      "implemented)")
+        if not 1 <= V.degree <= 5:
+            raise NotImplementedError(f"SpectralForm: degree {V.degree} outside 1..5")
+        self.alpha, self.beta = float(self.alpha), float(self.beta)
+
+    def coefficient_args(self):
+        """The parloop arguments that follow the coordinates: kappa, read through the argument map."""
+        return [] if self.kappa is None else [self.kappa(op2.READ, self.V.cell_node_map)]
+
+    def kernel(self, rank, diagonal=False):
+        if rank == 2:
+            raise NotImplementedError("SpectralForm has no assembled matrix (aij): there is no assembled SEM "
+                                      "matrix; use the action and mat_type 'matfree'")
+        return op2.Kernel("spectral_helmholtz" if self.kappa is None else "spectral_helmholtz_coef",
+                          degree=self.V.degree, alpha=self.alpha, beta=self.beta, diagonal=diagonal)
+
+
+def lumped_mass(V: FunctionSpace, rho: op2.Dat = None, tensor: op2.Dat = None):
+    """The GLL (lumped) mass diagonal of ``V``, the diagonal of ``SpectralForm(V, 0, 1)``, times the nodal ``rho`` if
+    given: under collocation that is exactly the GLL mass of rho*u*v.  A Dat on V."""
+    from . import _lib
+    m = ImplicitMatrixContext(SpectralForm(V, 0.0, 1.0)).getDiagonal(tensor if tensor is not None else V.dat())
+    if rho is not None:
+        _lib.check(_lib.lib().fdb_vec_pointwise_mult(m._data.size, m.device_ptr, rho.device_ptr, m.device_ptr))
+        m._device_written()
+    return m
+
+
+def wave_dt_bound(F: SpectralForm, m: op2.Dat, steps=30):
+    """A stable leapfrog step for ``M u'' + K u = f`` with the lumped M = diag(``m``) and K the operator of ``F``:
+    ``2 / sqrt(1.1 * lambda_max(M^-1 K))``, lambda_max from ``steps`` Jacobi-Lanczos steps
+    (:func:`mg.jacobi_lanczos_bounds` with ``invdiag = 1/m``) on the SEM action, from a seeded random start.  The
+    factor 1.1 covers the Lanczos estimate's approach from below."""
+    from . import mg as _mg
+    V = F.V
+    minv = V.dat()
+    m.copy(minv)
+    op2.par_loop(_mg.reciprocal_kernel(1), V.node_set, minv(op2.RW))
+    b = V.dat(np.random.default_rng(0).standard_normal(V.node_count))
+    _, lmax = _mg.jacobi_lanczos_bounds(ImplicitMatrixContext(F), minv, b, steps=steps)
+    return 2.0 / np.sqrt(1.1 * lmax)
+
+
+def ricker(t, f_peak, t0):
+    """The Ricker wavelet (1 - 2 (pi f (t - t0))^2) exp(-(pi f (t - t0))^2) of peak frequency ``f_peak`` centred at
+    ``t0`` (the source of Firedrake's full-waveform-inversion demo)."""
+    a = (np.pi * f_peak * (np.asarray(t, dtype=float) - t0)) ** 2
+    return (1.0 - 2.0 * a) * np.exp(-a)
+
+
+class PointEvaluator:
+    """Evaluation of fields of the CG_p space ``V`` at fixed physical ``points`` (m, 3), and its adjoint, the point
+    load (Firedrake's ``PointEvaluator`` / ``VertexOnlyMesh`` interpolation and its adjoint).
+
+    The points are located once, on the host: a uniform bin grid narrows each point to the cells whose vertex
+    bounding boxes contain it, and Newton's method on the trilinear map gives its reference coordinates, accepted
+    within ``[-tol, 1 + tol]^3`` (``tolerance``, default 1e-8).  A point on a shared face, edge or vertex goes to the
+    lowest cell number (row ``c*nz + l`` of ``full_cell_node_list``).  ``missing_points_behaviour``: "error" (a point
+    in no cell raises, naming its index) or "ignore" (its value is NaN and it loads nothing).  Each point keeps its
+    cell's (p+1)^3 node ids and basis weights on the device: ``evaluate`` is ``fdb_point_eval``, ``adjoint``
+    ``fdb_point_load``, both bit-reproducible."""
+
+    def __init__(self, V: FunctionSpace, points, tolerance=None, missing_points_behaviour="error"):
+        if missing_points_behaviour not in ("error", "ignore"):
+            raise ValueError(f"missing_points_behaviour {missing_points_behaviour!r}: 'error' or 'ignore'")
+        _refuse_dq(V, "PointEvaluator")
+        if V.cdim != 1:
+            raise NotImplementedError("PointEvaluator takes scalar spaces only")
+        self.V = V
+        self.points = np.ascontiguousarray(np.asarray(points, dtype=float).reshape(-1, 3))
+        self.tolerance = 1e-8 if tolerance is None else float(tolerance)
+        self.cells, self.xi = locate_points(V, self.points, self.tolerance)
+        missing = np.flatnonzero(self.cells < 0)
+        if len(missing) and missing_points_behaviour == "error":
+            raise ValueError(f"PointEvaluator: point {int(missing[0])} ({self.points[missing[0]]}) is not in the mesh "
+                             f"({len(missing)} missing); missing_points_behaviour='ignore' gives NaN there")
+        self.idx, self.w = point_weights(V, self.cells, self.xi)
+        self.npts, self.nper = len(self.points), (V.degree + 1) ** 3
+        self._didx = op2.DeviceArray.from_host(self.idx) if self.npts else None
+        self._dw = op2.DeviceArray.from_host(self.w) if self.npts else None
+
+    def _eval_into(self, u: op2.Dat, out_ptr):
+        from . import _lib
+        _lib.check(_lib.lib().fdb_point_eval(self.npts, self.nper, self._didx.ptr, self._dw.ptr, u.device_ptr,
+                                             out_ptr), "fdb_point_eval")
+
+    def _load_into(self, a_ptr, scale, y: op2.Dat):
+        from . import _lib
+        _lib.check(_lib.lib().fdb_point_load(self.npts, self.nper, self._didx.ptr, self._dw.ptr, a_ptr,
+                                             float(scale), y.device_ptr), "fdb_point_load")
+        y._device_written()
+
+    def evaluate(self, u: op2.Dat, out=None):
+        """The values of ``u`` at the points, (m,) on the host (NaN at missing points)."""
+        out = np.empty(self.npts) if out is None else out
+        if self.npts:
+            buf = op2.DeviceArray(8 * self.npts)
+            self._eval_into(u, buf.ptr)
+            buf.to_host(out)
+        return out
+
+    def adjoint(self, values, tensor: op2.Dat = None):
+        """The point load ``sum_k values[k] phi_i(x_k)`` (E^T values), a Dat on V (added into ``tensor`` if given)."""
+        tensor = self.V.dat() if tensor is None else tensor
+        a = np.ascontiguousarray(np.asarray(values, dtype=float).reshape(self.npts))
+        if self.npts:
+            da = op2.DeviceArray.from_host(a)
+            self._load_into(da.ptr, 1.0, tensor)
+        return tensor
+
+
+def _cell_vertices(V):
+    """The vertex coordinates (nc, 8, 3) of every cell, row c*nz + l."""
+    mesh = V.mesh
+    return mesh.coordinates[mesh.coord_space.full_cell_node_list().astype(np.int64)]
+
+
+_VERTS = np.array([[(v >> 2) & 1, (v >> 1) & 1, v & 1] for v in range(8)], dtype=float)
+
+
+def _trilinear(Xc, xi):
+    """The trilinear maps of cells Xc (k, 8, 3) at reference points xi (k, 3): x (k, 3) and J (k, 3, 3), J[:, i, d] =
+    dx_i/dxi_d."""
+    f = np.where(_VERTS[None] > 0, xi[:, None, :], 1.0 - xi[:, None, :])              # (k, 8, 3)
+    s = np.where(_VERTS > 0, 1.0, -1.0)
+    N = f.prod(axis=2)
+    dN = np.stack([s[None, :, d] * np.prod(np.delete(f, d, axis=2), axis=2) for d in range(3)], axis=2)
+    return np.einsum("kv,kvi->ki", N, Xc), np.einsum("kvd,kvi->kid", dN, Xc)
+
+
+def _newton(Xc, x, iters=30):
+    """Reference coordinates of physical points x (k, 3) under the trilinear maps of cells Xc (k, 8, 3)."""
+    xi = np.full(x.shape, 0.5)
+    for _ in range(iters):
+        X, J = _trilinear(Xc, xi)
+        xi = xi - np.linalg.solve(J, (X - x)[..., None])[..., 0]
+        xi = np.clip(xi, -1.0, 2.0)              # keep far-away candidates finite
+    return xi
+
+
+def locate_points(V, points, tol):
+    """(cell, xi) of every point: the lowest-numbered cell (row c*nz + l) whose trilinear map takes a reference point
+    within [-tol, 1 + tol]^3 to it, found through a uniform bin grid over the cells' vertex bounding boxes; cell -1
+    for a point in no cell."""
+    Xc = _cell_vertices(V)
+    nc, m = len(Xc), len(points)
+    lo, hi = Xc.min(axis=1), Xc.max(axis=1)
+    pad = tol * (hi - lo).max(axis=1, keepdims=True) + 1e-12 * np.abs(hi).max()
+    lo, hi = lo - pad, hi + pad
+    g0, g1 = lo.min(axis=0), hi.max(axis=0)
+    nb = max(1, int(np.ceil(nc ** (1.0 / 3.0))))
+    h = np.maximum((g1 - g0) / nb, 1e-300)
+    b_lo = np.clip(((lo - g0) / h).astype(np.int64), 0, nb - 1)
+    b_hi = np.clip(((hi - g0) / h).astype(np.int64), 0, nb - 1)
+    span = (b_hi - b_lo + 1).max(axis=0)
+    keys, owners = [], []
+    for di in range(span[0]):
+        for dj in range(span[1]):
+            for dk in range(span[2]):
+                b = b_lo + np.array([di, dj, dk])
+                ok = (b <= b_hi).all(axis=1)
+                keys.append(((b[ok, 0] * nb + b[ok, 1]) * nb + b[ok, 2]))
+                owners.append(np.flatnonzero(ok))
+    keys, owners = np.concatenate(keys), np.concatenate(owners)
+    order = np.lexsort((owners, keys))                    # by bin, then by cell number
+    keys, owners = keys[order], owners[order]
+    starts = np.searchsorted(keys, np.arange(nb ** 3 + 1))
+    pb = np.floor((points - g0) / h).astype(np.int64)
+    inside_grid = ((pb >= 0) & (pb < nb)).all(axis=1)
+    pkey = np.where(inside_grid, (np.clip(pb[:, 0], 0, nb - 1) * nb + np.clip(pb[:, 1], 0, nb - 1)) * nb
+                    + np.clip(pb[:, 2], 0, nb - 1), 0)
+    counts = np.where(inside_grid, starts[pkey + 1] - starts[pkey], 0)
+    pid = np.repeat(np.arange(m), counts)
+    first = np.repeat(starts[pkey] - np.concatenate([[0], np.cumsum(counts)[:-1]]), counts)
+    cand = owners[first + np.arange(len(pid))] if len(pid) else np.zeros(0, dtype=np.int64)
+    # the candidates' bounding boxes, then Newton
+    box = ((points[pid] >= lo[cand]) & (points[pid] <= hi[cand])).all(axis=1)
+    pid, cand = pid[box], cand[box]
+    cells, xis = np.full(m, -1, dtype=np.int64), np.zeros((m, 3))
+    if len(pid):
+        xi = _newton(Xc[cand], points[pid])
+        ok = ((xi >= -tol) & (xi <= 1.0 + tol)).all(axis=1)
+        pid, cand, xi = pid[ok], cand[ok], xi[ok]
+        order = np.lexsort((cand, pid))                   # per point, the lowest cell number first
+        pid, cand, xi = pid[order], cand[order], xi[order]
+        first = np.ones(len(pid), dtype=bool)
+        first[1:] = pid[1:] != pid[:-1]
+        cells[pid[first]] = cand[first]
+        xis[pid[first]] = np.clip(xi[first], 0.0, 1.0)
+    return cells, xis
+
+
+def point_weights(V, cells, xi):
+    """(idx, w), each (m, (p+1)^3): the global nodes of each point's cell and the basis weights phi_j(x_k) there;
+    idx -1 and w 0 for a missing point (cell -1)."""
+    from .fiat_lite import interval_element
+    W, nz = V.V, V.mesh.nz
+    el = interval_element(V.degree)
+    n, m = V.degree + 1, len(cells)
+    found = cells >= 0
+    idx = np.full((m, n ** 3), -1, dtype=np.int32)
+    w = np.zeros((m, n ** 3))
+    if found.any():
+        B = [el.tabulate(xi[found, d])[0] for d in range(3)]
+        w[found] = np.einsum("ka,kb,kc->kabc", B[0], B[1], B[2]).reshape(-1, n ** 3)
+        c = cells[found]
+        idx[found] = W.cell_node_map[c // nz].astype(np.int64) + (c % nz)[:, None] * W.offset[None, :].astype(np.int64)
+    return np.ascontiguousarray(idx), np.ascontiguousarray(w)
+
+
+def leapfrog(F: SpectralForm, u: op2.Dat, u_prev: op2.Dat, dt, steps, m: op2.Dat, bcs=(), sources=None,
+             receivers=None, scatter="coloured"):
+    """Step ``M u'' + K u = sum_k r_k(t) delta(x - x_k)`` with the explicit central difference (leapfrog) scheme
+
+        u^{n+1} = 2 u^n - u^{n-1} - dt^2 M^-1 (K u^n - f^n),     M = diag(m) (the lumped mass, :func:`lumped_mass`)
+
+    on the device, ``steps`` times from ``u`` = u^0 and ``u_prev`` = u^{-1}; K is the operator of ``F``.  ``sources``:
+    ``(PointEvaluator, amplitudes)`` with amplitudes (steps, nsrc), r_k(t_n) = amplitudes[n, k], uploaded once.
+    ``receivers``: a PointEvaluator sampling u^{n+1} after every step into a device trace.  ``bcs``: rigid walls (u =
+    0), held by zeroing M^-1 and u, u_prev on their nodes.  Each step is one SEM action, one ``fdb_point_load`` into its
+    output, one ``fdb_vec_leapfrog`` pass and one ``fdb_point_eval``; nothing is copied to the host in the loop.  dt
+    is the caller's (:func:`wave_dt_bound`).  ``scatter``: "coloured" (the default: the traces are bitwise repeatable
+    from run to run) or "atomic".  Returns the traces (steps, nrec) (None without receivers) and leaves ``u`` and
+    ``u_prev`` at u^steps and u^{steps-1}."""
+    from . import _lib
+    if not isinstance(F, SpectralForm):
+        raise TypeError("leapfrog takes a SpectralForm")
+    V, L = F.V, _lib.lib()
+    steps, dt = int(steps), float(dt)
+    n = V.node_count
+    minv = V.dat()
+    m.copy(minv)
+    from . import mg as _mg
+    op2.par_loop(_mg.reciprocal_kernel(1), V.node_set, minv(op2.RW))
+    for bc in bcs:
+        bc.zero(minv)
+        bc.zero(u)
+        bc.zero(u_prev)
+    src_amp = None
+    if sources is not None:
+        src, amp = sources
+        amp = np.ascontiguousarray(np.asarray(amp, dtype=float))
+        if amp.shape != (steps, src.npts):
+            raise ValueError(f"leapfrog: source amplitudes have shape {amp.shape}, need (steps, nsrc) = "
+                             f"{(steps, src.npts)}")
+        src_amp = op2.DeviceArray.from_host(amp) if amp.size else None
+    nrec = receivers.npts if receivers is not None else 0
+    traces = op2.DeviceArray(8 * steps * nrec) if nrec and steps else None
+    r = V.dat()
+    asm = (OneFormAssembler(F, u, scatter=scatter), OneFormAssembler(F, u_prev, scatter=scatter))
+    cur, prev = u, u_prev
+    minv_ptr = minv.device_ptr
+    for s in range(steps):
+        asm[s % 2].assemble(tensor=r)                             # r = K u^n
+        if src_amp is not None:
+            src._load_into(src_amp.ptr + 8 * s * src.npts, -1.0, r)    # r -= f^n
+        _lib.check(L.fdb_vec_leapfrog(n, dt * dt, minv_ptr, r.device_ptr, cur.device_ptr, prev.device_ptr),
+                   "fdb_vec_leapfrog")
+        prev._device_written()
+        cur, prev = prev, cur                                    # u^{n+1} is in the old u^{n-1}'s buffer
+        if traces is not None:
+            receivers._eval_into(cur, traces.ptr + 8 * s * nrec)
+    out = None
+    if traces is not None:
+        out = traces.to_host(np.empty((steps, nrec)))
+    if cur is not u:
+        # an odd number of steps: u^steps sits in u_prev's buffer; swap the values back
+        tmp = V.dat()
+        cur.copy(tmp)
+        prev.copy(u_prev)
+        tmp.copy(u)
+    return out
+
+
 @dataclass
 class Form:
     """alpha*inner(grad(u), grad(v))*dx + beta*inner(u, v)*dx on ``V``.
@@ -2563,6 +2927,9 @@ def assemble(form: Form, u=None, tensor=None, bcs=(), mat_type="aij"):
         return OneFormAssembler(form, u, bcs).assemble(tensor)
     if mat_type == "matfree":
         return ImplicitMatrixContext(form, bcs)
+    if isinstance(form, SpectralForm):
+        raise NotImplementedError(f"mat_type {mat_type!r}: SpectralForm has no assembled matrix (there is no "
+                                  f"assembled SEM matrix); use mat_type 'matfree'")
     if getattr(V, "family", "CG") == "DQ":
         raise NotImplementedError(f"mat_type {mat_type!r}: there is no assembled matrix on a DQ space (the facet "
                                   f"terms couple neighbouring cells outside the cell sparsity); use mat_type "
@@ -3118,6 +3485,14 @@ def solve(form: Form, L: op2.Dat, u: op2.Dat, bcs=(), solver_parameters=None, hi
         raise NotImplementedError(f"ksp_type {sp['ksp_type']!r}: cg or gmres")
     if sp["ksp_type"] == "cg" and not symmetric:
         raise ValueError(f"ksp_type cg needs a symmetric operator, and {type(form).__name__} is not: use gmres")
+    if isinstance(form, SpectralForm):
+        if sp["mat_type"] != "matfree":
+            raise NotImplementedError(f"mat_type {sp['mat_type']!r}: SpectralForm has no assembled matrix (there is "
+                                      f"no assembled SEM matrix); use mat_type 'matfree'")
+        if sp["pc_type"] not in ("none", "jacobi"):
+            what = {"mg": "geometric multigrid", "python": "p-multigrid (PMGPC / P1PC)"}.get(sp["pc_type"], "it")
+            raise NotImplementedError(f"pc_type {sp['pc_type']!r} on a SpectralForm: 'none' or 'jacobi' ({what} is "
+                                      f"not implemented for the SEM operator)")
     V = form.V
     bcs = tuple(bcs)
     if getattr(V, "family", "CG") == "DQ":

@@ -175,3 +175,8 @@ int fdb_launch_dg_upwind(fdb_kernel_s *k, fdb_int start, fdb_int end, int nlay, 
 // rows ((nq)^3); w the restriction's fine-node weights (NULL for the other two)
 int fdb_launch_p_transfer(fdb_kernel_s *k, fdb_int start, fdb_int end, int nlay, const fdb_int *subset, double *out,
                           const double *in, const double *w, const fdb_int *mapf, const fdb_int *mapc);
+// FDB_FORM_SPECTRAL_HELMHOLTZ[_COEF] (sem_hex.cu): the collocated GLL kernel; kappa (nodal, through map0) or NULL.
+// x != NULL: the action into y; else the diagonal into y.  Atomic or coloured scatter (the colouring of map0)
+int fdb_launch_spectral_helmholtz(fdb_kernel_s *k, fdb_int start, fdb_int end, int nlay, const fdb_int *subset,
+                                  double *y, const double *coords, const double *x, const double *kappa,
+                                  const fdb_int *map0, const fdb_int *map1);

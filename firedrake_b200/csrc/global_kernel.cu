@@ -298,7 +298,7 @@ static int device_pointers(const fdb_call_args *a, bool mat, void **args, const 
 // fdb_kernel_call hands its arguments to the launchers.
 enum { MODE_ACTION, MODE_MATRIX, MODE_DIAGONAL };
 enum { LAUNCH_HELMHOLTZ, LAUNCH_HELMHOLTZ_COEF, LAUNCH_ELASTICITY, LAUNCH_STOKES, LAUNCH_BOUNDARY, LAUNCH_DG_FACET,
-       LAUNCH_DG_TRANSPORT, LAUNCH_P_TRANSFER };
+       LAUNCH_DG_TRANSPORT, LAUNCH_P_TRANSFER, LAUNCH_SPECTRAL };
 // the degree of the second space of a form on two spaces: the descriptor's degree - 1 (Stokes' pressure, the
 // default of a row that does not name one), or any lower degree of an instantiated (fine, coarse) pair (the
 // p-multigrid transfers)
@@ -317,8 +317,8 @@ struct fdb_hex_form {
     int launcher;             // fdb_launch_helmholtz_*, fdb_launch_helmholtz_coef_* (which also run the
                               // nonlinear diffusion and advection-diffusion forms), fdb_launch_elasticity_*
                               // fdb_launch_stokes_action (which also runs the Navier-Stokes forms),
-                              // fdb_launch_boundary_mass, fdb_launch_dg_facet (the DG facet forms) or
-                              // fdb_launch_dg_transport
+                              // fdb_launch_boundary_mass, fdb_launch_dg_facet (the DG facet forms),
+                              // fdb_launch_dg_transport or fdb_launch_spectral_helmholtz
     int max_degree[3];        // per mode: action, matrix, diagonal
     int min_degree;
     const char *space2;       // the arguments on a second space (output and input, through a third map), or
@@ -368,6 +368,12 @@ static const fdb_hex_form hex_forms[] = {
      FDB_INTEGRAL_CELL, SPACE2_COARSER},
     {FDB_FORM_P_INJECT, "p_inject", -1, false, nullptr, 0, false, LAUNCH_P_TRANSFER, {3, 0, 0}, 2, "fine",
      FDB_INTEGRAL_CELL, SPACE2_COARSER},
+    // the spectral-element Helmholtz operator on the collocated GLL rule, without and with a nodal kappa (one kernel
+    // template).  Device mode only, action and diagonal, no rank 2; no second space (space2_degree is the default)
+    {FDB_FORM_SPECTRAL_HELMHOLTZ, "spectral_helmholtz", 1, false, nullptr, 0, false, LAUNCH_SPECTRAL, {5, 0, 5}, 1,
+     nullptr, FDB_INTEGRAL_CELL, SPACE2_PRESSURE},
+    {FDB_FORM_SPECTRAL_HELMHOLTZ_COEF, "spectral_helmholtz_coef", 1, false, "kappa", 1, false, LAUNCH_SPECTRAL,
+     {5, 0, 5}, 1, nullptr, FDB_INTEGRAL_CELL, SPACE2_PRESSURE},
 };
 
 // the (fine, coarse) degree pairs the transfer kernels instantiate (p_transfer_hex.cu)
@@ -456,6 +462,33 @@ static int kernel_create(const fdb_kernel_desc *d, const fdb_space2_desc *s2, fd
         return 1;
     }
     const bool transfer = f->launcher == LAUNCH_P_TRANSFER;
+    if (f->launcher == LAUNCH_SPECTRAL) {
+        // the GLL rule in dof order: the points are the nodes (dof 0 at 0, dof 1 at 1), so B is the identity
+        if (d->rank == 2) {
+            set_error("fdb_kernel_create: %s has no rank-2 form: there is no assembled SEM matrix; use the action "
+                      "and the diagonal", f->name);
+            return 1;
+        }
+        if (d->nq != d->degree + 1) {
+            set_error("fdb_kernel_create: %s needs the GLL rule at the nodes: nq == degree+1 (got nq=%d for degree "
+                      "%d)", f->name, d->nq, d->degree);
+            return 1;
+        }
+        if (d->nq >= 2 && (d->xq[0] != 0.0 || d->xq[1] != 1.0)) {
+            set_error("fdb_kernel_create: %s needs the GLL rule in dof order: xq[0] == 0 and xq[1] == 1 exactly "
+                      "(got %.17g, %.17g)", f->name, d->xq[0], d->xq[1]);
+            return 1;
+        }
+        const int n = d->degree + 1;
+        if (n <= FDB_MAX_1D)
+            for (int q = 0; q < n; q++)
+                for (int a = 0; a < n; a++)
+                    if (d->B[q * n + a] != (q == a ? 1.0 : 0.0)) {
+                        set_error("fdb_kernel_create: %s needs the collocated GLL element: B must be exactly the "
+                                  "identity (B[%d][%d] = %.17g)", f->name, q, a, d->B[q * n + a]);
+                        return 1;
+                    }
+    }
     if (transfer && s2->degree + 1 != d->nq) {
         set_error("fdb_kernel_create_mixed: %s: R (desc.B) has nq = q+1 rows, got nq=%d for the coarse degree %d",
                   f->name, d->nq, s2->degree);
@@ -780,6 +813,10 @@ int fdb_kernel_call(fdb_kernel_t k, const fdb_call_args *a)
     const int want = (mode == MODE_ACTION ? 3 : 2) + (f->coef ? 1 : 0) + (f->space2 ? 2 : 0) + (transport_facets ? 1 : 0);
     const int want_maps = f->space2 ? 3 : 2;
     const bool device_only = mode == MODE_DIAGONAL || f->space2 || f->integral != FDB_INTEGRAL_CELL;
+    if (f->launcher == LAUNCH_SPECTRAL && a->location != FDB_LOC_DEVICE) {
+        set_error("fdb_kernel_call: %s takes device-resident Dats only (no host-pointer mode)", f->name);
+        return 1;
+    }
     if (a->nargs != want || a->nmaps != want_maps || (device_only && a->location != FDB_LOC_DEVICE)) {
         static const char *const args[] = {"y, coords, x", "mat, coords", "d, coords"};
         set_error("fdb_kernel_call: %s %s expects %d %sargs (%s%s%s%s%s) and %d maps, got %d/%d", f->name,
@@ -867,6 +904,17 @@ int fdb_kernel_call(fdb_kernel_t k, const fdb_call_args *a)
         case LAUNCH_DG_TRANSPORT:
             return fdb_launch_dg_transport(k, a->start, a->end, nlay, dsubset, out, coords, nullptr, vel, tfacets,
                                            dmaps[0], dmaps[1]);
+        case LAUNCH_SPECTRAL:
+            // the diagonal's scatter is coloured like the action's
+            if (k->desc.scatter == FDB_SCATTER_COLOURED) {
+                if (a->start != 0) {
+                    set_error("fdb_kernel_call: coloured scatter needs start == 0");
+                    return 1;
+                }
+                if (colouring_for(k, a, 0)) return 1;
+            }
+            return fdb_launch_spectral_helmholtz(k, a->start, a->end, nlay, dsubset, out, coords, nullptr, coef,
+                                                 dmaps[0], dmaps[1]);
         default:
             return fdb_launch_elasticity_matrix(k, a->start, a->end, nlay, dsubset, mat, coords, coef, dmaps[0],
                                                 dmaps[1], out);
@@ -906,6 +954,10 @@ int fdb_kernel_call(fdb_kernel_t k, const fdb_call_args *a)
     case LAUNCH_DG_TRANSPORT:
         rc = fdb_launch_dg_transport(k, a->start, a->end, nlay, dsubset, out, coords, x, vel, tfacets, dmaps[0],
                                      dmaps[1]);
+        break;
+    case LAUNCH_SPECTRAL:
+        rc = fdb_launch_spectral_helmholtz(k, a->start, a->end, nlay, dsubset, out, coords, x, coef, dmaps[0],
+                                           dmaps[1]);
         break;
     default:
         rc = fdb_launch_stokes_action(k, a->start, a->end, nlay, dsubset, out, coords, x, (double *)dargs[3],

@@ -111,6 +111,15 @@ __global__ void k_chebyshev(size_t n, double cd, double cz, const double *__rest
     }
 }
 
+// uprev = 2 u - uprev - dt2 minv o r: one leapfrog step, four reads and one write per entry
+__global__ void k_leapfrog(size_t n, double dt2, const double *__restrict__ minv, const double *__restrict__ r,
+                           const double *__restrict__ u, double *__restrict__ uprev)
+{
+    size_t stride = (size_t)gridDim.x * blockDim.x;
+    for (size_t j = (size_t)blockIdx.x * blockDim.x + threadIdx.x; j < n; j += stride)
+        uprev[j] = fma(-dt2 * minv[j], r[j], 2.0 * u[j] - uprev[j]);
+}
+
 constexpr int DOT_BLOCKS_MAX = 1056;   // 132 SMs x 8 (H100 SXM)
 
 __global__ void __launch_bounds__(256)
@@ -276,6 +285,15 @@ int fdb_vec_chebyshev(size_t n, double c_d, double c_z, const double *b, const d
     if (require_init()) return 1;
     if (n == 0) return 0;
     k_chebyshev<<<stream_grid(2 * n), 256, 0, ctx().stream>>>(n, c_d, c_z, b, ax, dinv, d, x);
+    FDB_LAUNCH_CHECK();
+    return 0;
+}
+
+int fdb_vec_leapfrog(size_t n, double dt2, const double *minv, const double *r, const double *u, double *uprev)
+{
+    if (require_init()) return 1;
+    if (n == 0) return 0;
+    k_leapfrog<<<stream_grid(2 * n), 256, 0, ctx().stream>>>(n, dt2, minv, r, u, uprev);
     FDB_LAUNCH_CHECK();
     return 0;
 }

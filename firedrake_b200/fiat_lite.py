@@ -17,7 +17,7 @@ from __future__ import annotations
 import numpy as np
 from numpy.polynomial import legendre as _leg
 
-__all__ = ["gll_points", "gauss_legendre", "Interval1D", "interval_element"]
+__all__ = ["gll_points", "gll_weights", "gauss_legendre", "Interval1D", "interval_element"]
 
 
 def gauss_legendre(m: int):
@@ -43,6 +43,15 @@ def gll_points(p: int) -> np.ndarray:
     x = np.concatenate([[-1.0], r, [1.0]])
     x = 0.5 * (x - x[::-1])          # enforce symmetry
     return 0.5 * (x + 1.0)
+
+
+def gll_weights(p: int) -> np.ndarray:
+    """The weights of the (p+1)-point Gauss-Lobatto-Legendre rule on [0, 1] at :func:`gll_points` (ascending),
+    exact to degree 2p-1: w_i = 1 / (p (p+1) P_p(x_i)^2) with x_i on [-1, 1]."""
+    x = 2.0 * gll_points(p) - 1.0
+    c = np.zeros(p + 1)
+    c[p] = 1.0
+    return 1.0 / (p * (p + 1) * _leg.legval(x, c) ** 2)
 
 
 def _lagrange_tab(nodes: np.ndarray, pts: np.ndarray):
@@ -74,9 +83,14 @@ class Interval1D:
     B, D  : (nq, p+1) basis values / derivatives at the quadrature points,
             columns in dof numbering
     xq, wq : quadrature points and weights on [0, 1]
+
+    ``quadrature="gauss"`` (the default) tabulates at the nq-point Gauss-Legendre rule.  ``quadrature="gll"``
+    tabulates at the p+1 Gauss-Lobatto-Legendre points of a "gll" element, in DOF order (xq = nodes): the rule is
+    collocated with the nodes, so B is exactly the identity, D is the GLL differentiation matrix in dof numbering
+    and the mass matrix integrated with the rule is diagonal (spectral-element mass lumping).
     """
 
-    def __init__(self, degree: int, nq: int, variant: str = "gll"):
+    def __init__(self, degree: int, nq: int, variant: str = "gll", quadrature: str = "gauss"):
         self.degree = degree
         n = degree + 1
         if variant == "gll":
@@ -96,8 +110,19 @@ class Interval1D:
             order = np.array([0, n - 1] + list(range(1, n - 1)))
         self.dof_to_pos = order                    # dof a sits at ascending position order[a]
         self.nodes = pos[order]
-        self.xq, self.wq = gauss_legendre(nq)
-        self.B, self.D = _lagrange_tab(self.nodes, self.xq)
+        self.quadrature = quadrature
+        if quadrature == "gauss":
+            self.xq, self.wq = gauss_legendre(nq)
+            self.B, self.D = _lagrange_tab(self.nodes, self.xq)
+        elif quadrature == "gll":
+            if variant != "gll" or nq != n:
+                raise ValueError(f"quadrature 'gll' is collocated with the nodes of a 'gll' element: nq = degree+1 "
+                                 f"= {n} (got variant {variant!r}, nq {nq})")
+            self.xq, self.wq = self.nodes.copy(), gll_weights(degree)[order]
+            _, self.D = _lagrange_tab(self.nodes, self.xq)
+            self.B = np.eye(n)                     # exactly: l_a(x_b) = delta_ab
+        else:
+            raise ValueError(f"unknown quadrature {quadrature!r}: 'gauss' or 'gll'")
         self.nq = nq
         self.ndof = n
 
@@ -108,13 +133,15 @@ class Interval1D:
 _cache = {}
 
 
-def interval_element(degree: int, nq: int | None = None, variant: str = "gll") -> Interval1D:
+def interval_element(degree: int, nq: int | None = None, variant: str = "gll",
+                     quadrature: str = "gauss") -> Interval1D:
     """Cached constructor.  ``nq`` defaults to degree+1 Gauss points, the rule
     SURVEY.md section 8(d) pins for Poisson/Helmholtz CGp (Firedrake side:
-    ``dx(degree=2*p)``)."""
+    ``dx(degree=2*p)``).  ``quadrature="gll"``: the GLL rule at the nodes, in dof order (Firedrake's
+    ``dx(scheme=gauss_lobatto_legendre_cube_rule(...))``)."""
     if nq is None:
         nq = degree + 1
-    key = (degree, nq, variant)
+    key = (degree, nq, variant, quadrature)
     if key not in _cache:
-        _cache[key] = Interval1D(degree, nq, variant)
+        _cache[key] = Interval1D(degree, nq, variant, quadrature)
     return _cache[key]

@@ -1427,6 +1427,13 @@ class Kernel:
     (fine WRITE, coarse READ), restrict (coarse INC, fine READ, w READ: ``coarse += P^T (w * fine)``, w one value per
     fine node) and inject (coarse WRITE, fine READ).  The fine Dats go through the fine space's map, the coarse ones
     through the coarse space's; no coordinates.  Device-resident Dats only.
+
+    "spectral_helmholtz" is the spectral-element operator ``alpha*inner(grad u, grad v)*dx(GLL) +
+    beta*inner(u, v)*dx(GLL)`` on scalar CG_p (p = 1..5), integrated with the GLL rule at the nodes (``element`` =
+    ``interval_element(p, quadrature="gll")``, the default for these forms), so that its mass term is diagonal:
+    action (output, coordinates, u), diagonal (output, coordinates) at every degree.  "spectral_helmholtz_coef" adds a
+    nodal kappa to the stiffness term, ``alpha*inner(kappa*grad u, grad v)*dx(GLL)``, as the LAST argument (READ,
+    through the argument map) like "helmholtz_coef".  No rank 2; device-resident Dats only.
     """
     form: str = "helmholtz"
     degree: int = 1
@@ -1530,6 +1537,7 @@ class _Form(NamedTuple):
     facet: bool = False         # an exterior-facet integral: the local facet numbers come last, the integral as given
     velocity: bool = False      # reads b (3 values per vertex) through the coordinate map after u
     transfer: bool = False      # a p-multigrid degree transfer: fine and coarse maps, no coordinates
+    gll: bool = False           # stated on the GLL rule at the nodes: the default element is the collocated GLL one
 
 
 _FORMS = {"helmholtz": _Form(_lib.FORM_HELMHOLTZ),
@@ -1550,7 +1558,9 @@ _FORMS = {"helmholtz": _Form(_lib.FORM_HELMHOLTZ),
           "dg_transport": _Form(_lib.FORM_DG_TRANSPORT, facet=True, velocity=True),
           "p_prolong": _Form(_lib.FORM_P_PROLONG, transfer=True),
           "p_restrict": _Form(_lib.FORM_P_RESTRICT, transfer=True),
-          "p_inject": _Form(_lib.FORM_P_INJECT, transfer=True)}
+          "p_inject": _Form(_lib.FORM_P_INJECT, transfer=True),
+          "spectral_helmholtz": _Form(_lib.FORM_SPECTRAL_HELMHOLTZ, gll=True),
+          "spectral_helmholtz_coef": _Form(_lib.FORM_SPECTRAL_HELMHOLTZ_COEF, coefficient=True, gll=True)}
 _INTEGRALS = {"cell": _lib.INTEGRAL_CELL, "exterior_facet": _lib.INTEGRAL_EXTERIOR_FACET,
               "interior_facet": _lib.INTEGRAL_INTERIOR_FACET, "fused": _lib.INTEGRAL_FUSED}
 
@@ -1636,7 +1646,8 @@ class GlobalKernel:
             return h
         if _FORMS[lk.form].transfer:
             return self._compile_transfer()
-        el = lk.element or interval_element(lk.degree)
+        el = lk.element or (interval_element(lk.degree, quadrature="gll") if _FORMS[lk.form].gll
+                             else interval_element(lk.degree))
         n = lk.degree + 1
         if el.ndof != n:
             raise ValueError("element degree does not match the kernel")

@@ -317,7 +317,7 @@ enum fdb_form {
                                                diagonal  [d INC, coords, b, facets]               */
     FDB_FORM_P_PROLONG = 17,
     FDB_FORM_P_RESTRICT = 18,
-    FDB_FORM_P_INJECT = 19
+    FDB_FORM_P_INJECT = 19,
                                 /* the degree transfers of p-multigrid between a fine space CG_p and a
                                    coarse space CG_q on the SAME hex cells, both on GLL nodes (value size
                                    cdim 1 or 3, AoS), cell-local and sum-factorised:
@@ -344,6 +344,25 @@ enum fdb_form {
                                                                             (atomic or coloured scatter;
                                                                             coloured is bit-reproducible)
                                      P_INJECT    [coarse WRITE, fine]       maps [coarse map, fine map]  */
+    FDB_FORM_SPECTRAL_HELMHOLTZ = 20,
+    FDB_FORM_SPECTRAL_HELMHOLTZ_COEF = 21
+                                /* the spectral-element (SEM) Helmholtz operator on scalar CG_p, integrated
+                                   with the GLL rule at the nodes themselves (mass lumping):
+                                     alpha*inner(kappa*grad u, grad v)*dx(GLL) + beta*inner(u, v)*dx(GLL)
+                                   kappa = 1 for SPECTRAL_HELMHOLTZ; SPECTRAL_HELMHOLTZ_COEF reads a
+                                   nodal kappa (c^2 of the wave equation) through maps[0].  The tables
+                                   are the GLL rule in dof order: nq == degree+1, xq = the nodes (xq[0]
+                                   == 0, xq[1] == 1 exactly), B exactly the identity, D the GLL
+                                   differentiation matrix D[q][a] = l_a'(x_q).  The mass term is then
+                                   diagonal, beta*w_i*|det J_i| at node i.  Trilinear geometry.  Hex cells
+                                   (extruded or native), cdim 1, affine_cells 0, degrees 1..5, action
+                                   and diagonal at every degree; rank 2 is refused (there is no
+                                   assembled SEM matrix).  Device mode only, atomic or coloured scatter
+                                   (coloured is bit-reproducible):
+                                     action    [y INC, coords, u]            SPECTRAL_HELMHOLTZ
+                                               [y INC, coords, u, kappa]     SPECTRAL_HELMHOLTZ_COEF
+                                     diagonal  [d INC, coords]               SPECTRAL_HELMHOLTZ
+                                               [d INC, coords, kappa]        SPECTRAL_HELMHOLTZ_COEF      */
 };
 
 enum fdb_cell {
@@ -665,10 +684,27 @@ int fdb_vec_pointwise_mult(size_t n, const double *x, const double *y, double *w
  * (c_d == 0: d is not read, the first iteration) */
 int fdb_vec_chebyshev(size_t n, double c_d, double c_z, const double *b, const double *ax, const double *dinv,
                       double *d, double *x);
+/* one explicit central-difference (leapfrog) step of M u'' = -r with a lumped (diagonal) M, in one pass:
+ *   uprev = 2 u - uprev - dt2 minv o r
+ * (four reads, one write per entry); the caller then swaps the roles of u and uprev.  A row with minv == 0 and u, uprev
+ * zero (a rigid wall) stays zero. */
+int fdb_vec_leapfrog(size_t n, double dt2, const double *minv, const double *r, const double *u, double *uprev);
 /* compact gather / scatter through a device index list: the VecScatter of a virtual sub-matrix
  * (MatCreateSubMatrixVirtual, the fallback of firedrake/matrix_free/operators.py:380-405) */
 int fdb_vec_gather(size_t n, const fdb_int *idx, const double *src, double *dst);   /* dst[j] = src[idx[j]] */
 int fdb_vec_scatter(size_t n, const fdb_int *idx, const double *src, double *dst);  /* dst[idx[j]] = src[j] */
+
+/* ------------------------------------------------------- point evaluation
+ * A point x_k inside a cell is given by the nper = (p+1)^3 global node ids idx[k*nper + j] of its cell and the
+ * basis weights w[k*nper + j] = phi_j(x_k) (located on the host).  Device pointers; both are bit-reproducible:
+ *   fdb_point_eval   out[k] = sum_j w_kj u[idx_kj], summed in j order                  (point evaluation E u)
+ *   fdb_point_load   y[idx_kj] += scale * a_k * w_kj                                  (its adjoint E^T a: the load
+ *                    sum_k a_k phi_i(x_k) of point sources), every node's sum in k order, even when points share
+ *                    nodes.
+ * A point with idx[k*nper] < 0 (one not found in the mesh) evaluates to NaN and adds nothing. */
+int fdb_point_eval(fdb_int npts, int nper, const fdb_int *idx, const double *w, const double *u, double *out);
+int fdb_point_load(fdb_int npts, int nper, const fdb_int *idx, const double *w, const double *a, double scale,
+                   double *y);
 
 /* ----------------------------------------------------------- interpolation
  * Dual-evaluation parloop with WRITE access (firedrake/interpolation.py:977-1171):
