@@ -13,6 +13,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("FDB200_LIB", os.path.join(HERE, "lib", "libfdb200.so"))
 
 MAX_1D = 8
+BV_MAX_COLUMNS = 64                    # FDB_BV_MAX_COLUMNS: columns of one fdb_bv_dot / fdb_bv_mult operand
 
 FORM_HELMHOLTZ = 1
 FORM_DG_ADVECTION = 2
@@ -189,6 +190,10 @@ SIGNATURES = {
     "fdb_asm_apply": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p]),
     "fdb_asm_get_blocks": (C.c_int, [C.c_void_p, C.c_void_p]),
     "fdb_vec_dot": (C.c_int, [C.c_size_t, C.c_void_p, C.c_void_p, C.POINTER(C.c_double)]),
+    "fdb_bv_dot": (C.c_int, [C.c_size_t, C.c_int, C.POINTER(C.c_void_p), C.c_int, C.POINTER(C.c_void_p),
+                             C.POINTER(C.c_double)]),
+    "fdb_bv_mult": (C.c_int, [C.c_size_t, C.c_int, C.POINTER(C.c_void_p), C.c_double, C.c_double, C.c_int,
+                              C.POINTER(C.c_void_p), C.POINTER(C.c_double)]),
     "fdb_vec_pointwise_mult": (C.c_int, [C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p]),
     "fdb_vec_chebyshev": (C.c_int, [C.c_size_t, C.c_double, C.c_double, C.c_void_p, C.c_void_p, C.c_void_p,
                                     C.c_void_p, C.c_void_p]),

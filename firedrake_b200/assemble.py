@@ -3453,6 +3453,66 @@ def solve_nonlinear(F, L: op2.Dat, u: op2.Dat, bcs=(), solver_parameters=None, h
     return hist, kits
 
 
+def _preconditioner(form, A, bcs, sp, hierarchy=None, allreduce=None):
+    """The preconditioner of ``sp["pc_type"]`` on the operator of ``form`` with the conditions ``bcs``, as a function
+    ``M(r, z)`` that writes z = P^-1 r, or None for "none": the diagonal of the matrix-free operator ("jacobi"; ``A``
+    is that operator when it is one, else one is made), a geometric V-cycle on ``hierarchy`` ("mg") or p-multigrid
+    ("python", :func:`pmg_options`), with the level forms and Jacobi damping of each form.  :func:`solve` and
+    :class:`eigensolver.LinearEigensolver` build their preconditioners here."""
+    from . import _lib
+    from . import mg as _mg
+    V = form.V
+    lib = _lib.lib()
+    pc = sp["pc_type"]
+    if pc == "none":
+        return None
+    if pc == "jacobi":
+        ctx = A if isinstance(A, ImplicitMatrixContext) else ImplicitMatrixContext(form, bcs)
+        d = ctx.getDiagonal(V.dat())
+        op2.par_loop(_mg.reciprocal_kernel(V.cdim), V.node_set, d(op2.RW))
+        n = d._data.size
+
+        def M(r, z):
+            _lib.check(lib.fdb_vec_pointwise_mult(n, r.device_ptr, d.device_ptr, z.device_ptr))
+            z._device_written()
+    elif pc == "mg":
+        if hierarchy is None:
+            raise ValueError("pc_type mg needs the mesh hierarchy")
+        # with a coefficient field, every coarser level gets the injection of the next finer
+        # level's kappa (VCycle's ``kappa``), as Firedrake coarsens coefficients for rediscretised
+        # multigrid
+        # elasticity: the Jacobi smoother's damping is 0.6, not 0.8.  The spectrum of D^-1 A of the coupled
+        # operator reaches past 2 / 0.8, so 0.8 amplifies its highest modes: CG1 at nu = 0.3 took 16 and
+        # 97 iterations on 8^3 and 16^3 with 0.8, 8 and 9 with 0.6 (DESIGN.md section 4.8)
+        # advection-diffusion: a V-cycle of its symmetric part Form(W, alpha, beta) on every level (the
+        # convective term is left to the outer GMRES, DESIGN.md section 4.10)
+        # boundary terms: the same (gamma, sub_domain) pairs on every level (the names are mesh-level)
+        ds = getattr(form, "ds", ())
+        if isinstance(form, Elasticity):
+            make = lambda W, k=None: Elasticity(W, form.mu, form.lmbda, form.beta, ds)
+            omega = 0.6
+        else:
+            make = lambda W, k=None: Form(W, form.alpha, form.beta, k, ds)
+            omega = 0.8
+        vc = _mg.VCycle(hierarchy, V.degree, make,
+                        bc_domains=tuple(s for bc in bcs for s in bc.sub_domains), allreduce=allreduce,
+                        kappa=getattr(form, "kappa", None), cdim=V.cdim, omega=omega)
+        top = len(hierarchy) - 1
+        M = lambda r, z: vc.apply(top, r, z)
+    elif pc == "python":
+        # p-multigrid (firedrake.PMGPC / P1PC) with the level forms and Jacobi damping of the "mg" branch
+        ds = getattr(form, "ds", ())
+        if isinstance(form, Elasticity):
+            make, omega = (lambda W, k=None: Elasticity(W, form.mu, form.lmbda, form.beta, ds)), 0.6
+        else:
+            make, omega = (lambda W, k=None: Form(W, form.alpha, form.beta, k, ds)), 0.8
+        pm = _pmg(V, make, sp, bcs, hierarchy, allreduce, kappa=getattr(form, "kappa", None), omega=omega)
+        M = lambda r, z: pm.apply(pm.top, r, z)
+    else:
+        raise NotImplementedError(f"pc_type {pc!r}")
+    return M
+
+
 def solve(form: Form, L: op2.Dat, u: op2.Dat, bcs=(), solver_parameters=None, hierarchy=None, allreduce=None,
           nullspace=None):
     """``solve(a == L, u, bcs=bcs, solver_parameters=...)`` for the supported forms
@@ -3472,7 +3532,6 @@ def solve(form: Form, L: op2.Dat, u: op2.Dat, bcs=(), solver_parameters=None, hi
     "mg" and the ``pmg_*`` options of :func:`pmg_options`; CG2 and CG3); ``ksp_rtol`` (1e-8), ``ksp_max_it`` (1000).
     A :class:`Stokes` form takes MixedDats and its own options (:func:`_solve_stokes`), and the only form
     that takes ``nullspace``.  Returns (iterations, residual history)."""
-    from . import _lib
     if isinstance(form, Stokes):
         return _solve_stokes(form, L, u, bcs, solver_parameters, hierarchy, nullspace)
     if nullspace is not None:
@@ -3504,8 +3563,6 @@ def solve(form: Form, L: op2.Dat, u: op2.Dat, bcs=(), solver_parameters=None, hi
                                       f"DQ multigrid)")
         if sp["pc_type"] == "jacobi" and not (isinstance(form, DGTransport) and not (form.alpha or form.beta)):
             _dq_diagonal_kernel(V, 1.0, 0.0)          # refuses DQ4 before anything is assembled
-    lib = _lib.lib()
-    n = L._data.size
     # lifting (firedrake/assemble.py:1243-1254 + linear solver's rhs): u = g on the constrained nodes,
     # solve A (u - g) = L - K g on the free rows with homogeneous conditions
     g = V.dat()
@@ -3523,59 +3580,14 @@ def solve(form: Form, L: op2.Dat, u: op2.Dat, bcs=(), solver_parameters=None, hi
     A = assemble(form, bcs=bcs, mat_type=sp["mat_type"])
     u.zero()
     u.device_ptr
-    pc = sp["pc_type"]
-    M = None
-    if pc != "none":
-        from . import mg as _mg
-        if pc == "jacobi":
-            ctx = A if isinstance(A, ImplicitMatrixContext) else ImplicitMatrixContext(form, bcs)
-            d = ctx.getDiagonal(V.dat())
-            op2.par_loop(_mg.reciprocal_kernel(V.cdim), V.node_set, d(op2.RW))
-
-            def M(r, z):
-                _lib.check(lib.fdb_vec_pointwise_mult(n, r.device_ptr, d.device_ptr, z.device_ptr))
-                z._device_written()
-        elif pc == "mg":
-            if hierarchy is None:
-                raise ValueError("pc_type mg needs the mesh hierarchy")
-            # with a coefficient field, every coarser level gets the injection of the next finer
-            # level's kappa (VCycle's ``kappa``), as Firedrake coarsens coefficients for rediscretised
-            # multigrid
-            # elasticity: the Jacobi smoother's damping is 0.6, not 0.8.  The spectrum of D^-1 A of the coupled
-            # operator reaches past 2 / 0.8, so 0.8 amplifies its highest modes: CG1 at nu = 0.3 took 16 and
-            # 97 iterations on 8^3 and 16^3 with 0.8, 8 and 9 with 0.6 (DESIGN.md section 4.8)
-            # advection-diffusion: a V-cycle of its symmetric part Form(W, alpha, beta) on every level (the
-            # convective term is left to the outer GMRES, DESIGN.md section 4.10)
-            # boundary terms: the same (gamma, sub_domain) pairs on every level (the names are mesh-level)
-            ds = getattr(form, "ds", ())
-            if isinstance(form, Elasticity):
-                make = lambda W, k=None: Elasticity(W, form.mu, form.lmbda, form.beta, ds)
-                omega = 0.6
-            else:
-                make = lambda W, k=None: Form(W, form.alpha, form.beta, k, ds)
-                omega = 0.8
-            vc = _mg.VCycle(hierarchy, V.degree, make,
-                            bc_domains=tuple(s for bc in bcs for s in bc.sub_domains), allreduce=allreduce,
-                            kappa=getattr(form, "kappa", None), cdim=V.cdim, omega=omega)
-            top = len(hierarchy) - 1
-            M = lambda r, z: vc.apply(top, r, z)
-        elif pc == "python":
-            # p-multigrid (firedrake.PMGPC / P1PC) with the level forms and Jacobi damping of the "mg" branch
-            ds = getattr(form, "ds", ())
-            if isinstance(form, Elasticity):
-                make, omega = (lambda W, k=None: Elasticity(W, form.mu, form.lmbda, form.beta, ds)), 0.6
-            else:
-                make, omega = (lambda W, k=None: Form(W, form.alpha, form.beta, k, ds)), 0.8
-            pm = _pmg(V, make, sp, bcs, hierarchy, allreduce, kappa=getattr(form, "kappa", None), omega=omega)
-            M = lambda r, z: pm.apply(pm.top, r, z)
-        else:
-            raise NotImplementedError(f"pc_type {pc!r}")
+    M = _preconditioner(form, A, bcs, sp, hierarchy, allreduce)
     if sp["ksp_type"] == "gmres":
         its, hist = gmres(A, b, u, M, rtol=sp["ksp_rtol"], restart=sp["ksp_gmres_restart"], maxit=sp["ksp_max_it"],
                           allreduce=allreduce)
     elif M is None:
         its, hist = cg(A, b, u, rtol=sp["ksp_rtol"], maxit=sp["ksp_max_it"], allreduce=allreduce)
     else:
+        from . import mg as _mg
         its, hist = _mg.pcg(A, b, u, M, rtol=sp["ksp_rtol"], maxit=sp["ksp_max_it"], allreduce=allreduce)
     if lift:
         u.axpy(1.0, g)

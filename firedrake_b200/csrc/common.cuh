@@ -27,6 +27,7 @@ struct Context {
 Context &ctx();
 void set_error(const char *fmt, ...);
 int require_init();
+void fdb_bv_release();   // frees the buffers of fdb_bv_dot / fdb_bv_mult (bv.cu); called by fdb_finalize
 
 #define FDB_CUDA(call)                                                              \
     do {                                                                            \

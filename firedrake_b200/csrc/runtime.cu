@@ -125,6 +125,7 @@ int fdb_finalize(void)
         g_side = nullptr;
         g_side_pending = false;
     }
+    fdb_bv_release();
     cudaFree(c.reduce_scratch);
     cudaFree(c.work_counter);
     cudaFreeHost(c.reduce_host);

@@ -694,6 +694,20 @@ int fdb_vec_leapfrog(size_t n, double dt2, const double *minv, const double *r, 
 int fdb_vec_gather(size_t n, const fdb_int *idx, const double *src, double *dst);   /* dst[j] = src[idx[j]] */
 int fdb_vec_scatter(size_t n, const fdb_int *idx, const double *src, double *dst);  /* dst[idx[j]] = src[j] */
 
+/* ------------------------------------------------- block vectors (BV)
+ * SLEPc's BVDot and BVMult over columns that are ordinary device Dats: x and y are HOST arrays of device
+ * pointers, one per column, over rows [0, n) (the owned rows).  m and k are each in 1..FDB_BV_MAX_COLUMNS; a NULL
+ * array, column or host matrix is refused, and fdb_bv_mult refuses any y_j equal to any x_i (no in-place update).
+ *   fdb_bv_dot   G[i*k + j] = x_i . y_j               G on the host, m x k row-major; bitwise repeatable for the
+ *                                                     same inputs (fixed-order reduction on a grid fixed by n);
+ *                                                     n = 0 gives G = 0
+ *   fdb_bv_mult  y_j = beta y_j + alpha sum_i x_i Q[i*k + j]   Q on the host, m x k row-major; beta == 0 does not
+ *                                                     read y; n = 0 leaves y unchanged */
+#define FDB_BV_MAX_COLUMNS 64
+int fdb_bv_dot(size_t n, int m, const double *const *x, int k, const double *const *y, double *g_host);
+int fdb_bv_mult(size_t n, int k, double *const *y, double beta, double alpha,
+                int m, const double *const *x, const double *q_host);
+
 /* ------------------------------------------------------- point evaluation
  * A point x_k inside a cell is given by the nper = (p+1)^3 global node ids idx[k*nper + j] of its cell and the
  * basis weights w[k*nper + j] = phi_j(x_k) (located on the host).  Device pointers; both are bit-reproducible:
