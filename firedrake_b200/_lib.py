@@ -189,6 +189,12 @@ SIGNATURES = {
     "fdb_asm_update": (C.c_int, [C.c_void_p, C.c_void_p, C.POINTER(C.c_int)]),
     "fdb_asm_apply": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p]),
     "fdb_asm_get_blocks": (C.c_int, [C.c_void_p, C.c_void_p]),
+    "fdb_fdm_star_create": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int32, C.c_int,
+                                      C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int,
+                                      C.c_void_p, C.POINTER(C.c_void_p)]),
+    "fdb_fdm_star_update": (C.c_int, [C.c_void_p, C.c_double, C.c_double, C.c_void_p]),
+    "fdb_fdm_star_apply": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p]),
+    "fdb_fdm_star_destroy": (C.c_int, [C.c_void_p]),
     "fdb_vec_dot": (C.c_int, [C.c_size_t, C.c_void_p, C.c_void_p, C.POINTER(C.c_double)]),
     "fdb_bv_dot": (C.c_int, [C.c_size_t, C.c_int, C.POINTER(C.c_void_p), C.c_int, C.POINTER(C.c_void_p),
                              C.POINTER(C.c_double)]),

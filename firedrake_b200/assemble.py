@@ -3313,6 +3313,117 @@ def _pmg(V, make, sp, bcs, hierarchy, allreduce, kappa=None, omega=0.8):
                    hierarchy=hierarchy, allreduce=allreduce)
 
 
+_STAR_TYPES = ("firedrake.ASMExtrudedStarPC", "firedrake.ASMStarPC")
+_STAR_KEYS = {"pc_star_construct_dim": 0, "pc_star_sub_sub_pc_type": "lu", "pc_star_use_coloring": True}
+_DIRECT = ("lu", "cholesky", "ilu", "icc", "redundant", "mumps")
+
+
+def _flatten(prefix, d):
+    out = {}
+    for k, v in d.items():
+        key = f"{prefix}_{k}" if prefix else k
+        out.update(_flatten(key, v) if isinstance(v, dict) else {key: v})
+    return out
+
+
+def _star_options(o, where):
+    """Check the ``pc_star_*`` options of a vertex-star relaxation (``o`` without the prefix ``where``)."""
+    bad = sorted(k for k in o if k.startswith("pc_star_") and k not in _STAR_KEYS)
+    if bad:
+        raise NotImplementedError(f"unknown vertex-star option(s) {', '.join(where + k for k in bad)}: the supported "
+                                  f"ones are {', '.join(where + k for k in _STAR_KEYS)}")
+    o = dict(_STAR_KEYS, **{k: v for k, v in o.items() if k in _STAR_KEYS})
+    if int(o["pc_star_construct_dim"]) != 0:
+        raise NotImplementedError(f"{where}pc_star_construct_dim {o['pc_star_construct_dim']!r}: vertex stars (0) "
+                                  f"only; edge and face stars are not implemented")
+    if o["pc_star_sub_sub_pc_type"] != "lu":
+        raise NotImplementedError(f"{where}pc_star_sub_sub_pc_type {o['pc_star_sub_sub_pc_type']!r}: 'lu' (the "
+                                  f"fast-diagonalisation solve is exact for the separable patch operator)")
+
+
+def fdm_options(sp):
+    """The inner relaxation of ``pc_python_type "firedrake.FDMPC"``, from the nested ``"fdm": {...}`` dict or the
+    flattened ``fdm_*`` keys.  Returns ``("star", None)`` for the one-level ``fdm_pc_python_type``
+    "firedrake.ASMExtrudedStarPC" / "firedrake.ASMStarPC" (the same vertex-star patches on these meshes), or
+    ``("pmg", o)`` for ``fdm_pc_python_type`` "firedrake.P1PC" / "firedrake.PMGPC" with the star smoother in
+    ``fdm_pmg_mg_levels`` (``o``: :func:`pmg_options` with ``level_pc`` "star")."""
+    flat = _flatten("", {k: v for k, v in sp.items() if k == "fdm" or k.startswith("fdm_")})
+    inner = {k[len("fdm_"):]: v for k, v in flat.items()}
+    pc, kind = inner.get("pc_type"), inner.get("pc_python_type")
+    if pc in _DIRECT:
+        raise NotImplementedError(f"fdm_pc_type {pc!r}: there is no direct solver; FDMPC takes the vertex-star "
+                                  f"relaxation (ASMExtrudedStarPC) or P1PC / PMGPC with it")
+    if pc != "python":
+        raise NotImplementedError(f"fdm_pc_type {pc!r}: 'python' with fdm_pc_python_type "
+                                  f"{' / '.join(_STAR_TYPES + ('firedrake.P1PC', 'firedrake.PMGPC'))}")
+    def refuse_unknown(keys, known):
+        other = sorted(k for k in keys if not known(k))
+        if other:
+            raise NotImplementedError(f"unknown FDMPC option(s) {', '.join('fdm_' + k for k in other)}")
+    top = ("pc_type", "pc_python_type")
+    if kind in _STAR_TYPES:
+        refuse_unknown(inner, lambda k: k in top or k.startswith("pc_star_"))
+        _star_options(inner, "fdm_")
+        return "star", None
+    if kind not in ("firedrake.P1PC", "firedrake.PMGPC"):
+        raise NotImplementedError(f"fdm_pc_python_type {kind!r}: "
+                                  f"{', '.join(_STAR_TYPES + ('firedrake.P1PC', 'firedrake.PMGPC'))}")
+    lev = "pmg_mg_levels_"
+    # the p-multigrid keys are checked by pmg_options; a level pc_* key other than the star's is refused here
+    refuse_unknown(inner, lambda k: k in top or (k.startswith("pmg_") and not (
+        k.startswith(lev + "pc_") and k[len(lev):] not in top and not k[len(lev):].startswith("pc_star_"))))
+    levels = {k[len(lev):]: v for k, v in inner.items() if k.startswith(lev)}
+    if levels.get("pc_type") != "python" or levels.get("pc_python_type") not in _STAR_TYPES:
+        raise NotImplementedError(f"FDMPC with {kind}: fdm_pmg_mg_levels_pc_type 'python' with "
+                                  f"fdm_pmg_mg_levels_pc_python_type 'firedrake.ASMExtrudedStarPC' (got "
+                                  f"{levels.get('pc_type')!r}, {levels.get('pc_python_type')!r})")
+    if levels.get("ksp_type", "chebyshev") != "chebyshev":
+        raise NotImplementedError(f"fdm_pmg_mg_levels_ksp_type {levels['ksp_type']!r}: the star smoother runs "
+                                  f"under 'chebyshev'")
+    _star_options(levels, "fdm_" + lev)
+    rest = {k: v for k, v in inner.items() if not (k.startswith(lev) and (k[len(lev):].startswith("pc_")))}
+    o = pmg_options(rest)
+    o["level_pc"] = "star"
+    return "pmg", o
+
+
+def _fdm(form, bcs, sp, hierarchy=None):
+    """``M(r, z)`` of ``pc_python_type "firedrake.FDMPC"`` (:func:`fdm_options`) on a scalar :class:`Form`: the
+    vertex-star relaxation of ``form`` (:class:`patch.FDMStar`), or p-multigrid smoothed by it.  The one-level ``M``
+    has ``M.update()``, which refreshes the star coefficients after ``form.kappa`` changed."""
+    from . import mg as _mg
+    from .patch import FDMStar
+    kind, o = fdm_options(sp)
+    V = form.V
+    if type(form) is not Form:
+        raise NotImplementedError(f"FDMPC on {type(form).__name__}: it takes scalar Form (alpha, beta, kappa) "
+                                  f"operators only")
+    if getattr(V, "family", "CG") != "CG" or V.cdim != 1:
+        raise NotImplementedError("FDMPC takes scalar CG spaces only (no vector or DQ spaces)")
+    if form.ds:
+        raise NotImplementedError("FDMPC on a Form with ds terms: the star operators have no boundary terms")
+    if V.dof_dset.halo is not None:
+        raise NotImplementedError("FDMPC on a partitioned space is not implemented")
+    if kind == "star":
+        star = FDMStar(form, bcs)
+
+        def M(r, z):
+            star.apply(r, z)
+        M.update = star.update           # after form.kappa changed: the tables stay, the coefficients are refreshed
+        return M
+    if not 2 <= V.degree <= 3:
+        raise NotImplementedError(f"FDMPC with P1PC / PMGPC at fine degree {V.degree}: 2 or 3 (the degree "
+                                  f"transfers stop at 3); the one-level FDMPC with ASMExtrudedStarPC takes 1..5")
+    est = tuple(float(v) for v in str(o["pmg_mg_levels_ksp_chebyshev_esteig"]).split(","))
+    pm = _mg.PMG(V, lambda W, k=None: Form(W, form.alpha, form.beta, k), bc_domains=tuple(s for bc in bcs
+                                                                                            for s in bc.sub_domains),
+                 coarse_degree=int(o["pmg_mg_coarse_degree"]), halve=o["halve"], kappa=form.kappa,
+                 nu=int(o["pmg_mg_levels_ksp_max_it"]), esteig=est, coarse_ksp=o["pmg_mg_coarse_ksp_type"],
+                 coarse_pc=o["pmg_mg_coarse_pc_type"], coarse_rtol=float(o["pmg_mg_coarse_ksp_rtol"]),
+                 coarse_maxit=int(o["pmg_mg_coarse_ksp_max_it"]), hierarchy=hierarchy, level_pc="star")
+    return lambda r, z: pm.apply(pm.top, r, z)
+
+
 def solve_nonlinear(F, L: op2.Dat, u: op2.Dat, bcs=(), solver_parameters=None, hierarchy=None, allreduce=None,
                     nullspace=None):
     """``solve(F == 0, u, bcs=bcs, solver_parameters=...)`` for nonlinear diffusion (``F`` a
@@ -3397,7 +3508,7 @@ def solve_nonlinear(F, L: op2.Dat, u: op2.Dat, bcs=(), solver_parameters=None, h
     pc = sp["pc_type"]
     A = ctx = None
     d = V.dat() if pc == "jacobi" else None
-    vc = None
+    vc = kap = fdm = None
     while hist[-1] > tol and len(kits) < sp["snes_max_it"]:
         if A is None or sp["mat_type"] != "matfree":
             A = assemble(J, bcs=bcs, mat_type=sp["mat_type"])
@@ -3427,6 +3538,21 @@ def solve_nonlinear(F, L: op2.Dat, u: op2.Dat, bcs=(), solver_parameters=None, h
                                 bc_domains=domains, allreduce=allreduce, kappa=kap)
             top = len(hierarchy) - 1
             M = lambda r, z, vc=vc: vc.apply(top, r, z)
+        elif pc == "python" and sp.get("pc_python_type") == "firedrake.FDMPC":
+            # FDMPC of Form(V, alpha, beta, kappa=D(u)).  The one-level star tables depend on the mesh and the
+            # conditions only: they are built once per solve, and the coefficient alpha * mean D(u) of every star
+            # is refreshed on the device at each Newton step.  P1PC / PMGPC is rebuilt at every step, as p-multigrid
+            # is in the branch below.
+            if hyper:
+                raise NotImplementedError("FDMPC on HyperElasticity: it takes scalar Form operators only")
+            if kap is None:
+                kap = V.dat()
+            F.diffusivity(u, kap)
+            if getattr(fdm, "update", None) is not None:
+                fdm.update()
+            else:
+                fdm = _fdm(Form(V, F.alpha, F.beta, kap, F.ds), bcs, sp, hierarchy)
+            M = fdm
         elif pc == "python":
             # p-multigrid with the level forms of the "mg" branch: J(0) = Elasticity once per solve for
             # hyperelasticity, Form(V, alpha, beta, kappa=D(u)) at every Newton step for nonlinear diffusion
@@ -3499,7 +3625,13 @@ def _preconditioner(form, A, bcs, sp, hierarchy=None, allreduce=None):
                         kappa=getattr(form, "kappa", None), cdim=V.cdim, omega=omega)
         top = len(hierarchy) - 1
         M = lambda r, z: vc.apply(top, r, z)
+    elif pc == "python" and sp.get("pc_python_type") == "firedrake.FDMPC":
+        M = _fdm(form, bcs, sp, hierarchy)
     elif pc == "python":
+        if sp.get("pc_python_type") in _STAR_TYPES:
+            raise NotImplementedError(f"pc_python_type {sp['pc_python_type']!r} outside firedrake.FDMPC: exact patch "
+                                      f"solves of the true operator are not implemented; use it as FDMPC's "
+                                      f"fdm_pc_python_type")
         # p-multigrid (firedrake.PMGPC / P1PC) with the level forms and Jacobi damping of the "mg" branch
         ds = getattr(form, "ds", ())
         if isinstance(form, Elasticity):
@@ -3529,7 +3661,9 @@ def solve(form: Form, L: op2.Dat, u: op2.Dat, bcs=(), solver_parameters=None, hi
     ``hierarchy``, a mg.MeshHierarchy whose finest mesh is ``form.V.mesh``; for advection-diffusion a
     V-cycle of its symmetric part ``Form(W, alpha, beta)``) | "python" with ``pc_python_type``
     "firedrake.PMGPC" or "firedrake.P1PC" (p-multigrid on ``V.mesh``, :class:`mg.PMG`, with the level forms of
-    "mg" and the ``pmg_*`` options of :func:`pmg_options`; CG2 and CG3); ``ksp_rtol`` (1e-8), ``ksp_max_it`` (1000).
+    "mg" and the ``pmg_*`` options of :func:`pmg_options`; CG2 and CG3) or "firedrake.FDMPC" (scalar :class:`Form`
+    without ds: the fast-diagonalisation vertex-star relaxation, or P1PC / PMGPC smoothed by it, :func:`fdm_options`);
+    ``ksp_rtol`` (1e-8), ``ksp_max_it`` (1000).
     A :class:`Stokes` form takes MixedDats and its own options (:func:`_solve_stokes`), and the only form
     that takes ``nullspace``.  Returns (iterations, residual history)."""
     if isinstance(form, Stokes):

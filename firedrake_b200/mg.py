@@ -536,10 +536,11 @@ def pmg_degrees(p, coarse_degree=1, halve=True):
     return degs[::-1]
 
 
-def jacobi_lanczos_bounds(A, invdiag, b, steps=10):
+def jacobi_lanczos_bounds(A, invdiag, b, steps=10, M=None):
     """The extreme eigenvalues (lmin, lmax) of D^-1 A estimated by ``steps`` Jacobi-preconditioned CG steps from the right-hand
     side ``b`` (PETSc's KSPChebyshev estimate): the CG coefficients give the Lanczos tridiagonal, whose extreme
-    eigenvalues are computed on the host."""
+    eigenvalues are computed on the host.  ``M(r, z)``: another preconditioner, writing z = P^-1 r (``invdiag`` is
+    then not used); the estimate is then of P^-1 A."""
     import ctypes as C
     from . import _lib
     if steps < 1:
@@ -553,9 +554,12 @@ def jacobi_lanczos_bounds(A, invdiag, b, steps=10):
         out = C.c_double()
         _lib.check(L.fdb_vec_dot(n, u.device_ptr, v.device_ptr, C.byref(out)))
         return out.value
+    if M is None:
+        def M(r, z):
+            _lib.check(L.fdb_vec_pointwise_mult(n, r.device_ptr, invdiag.device_ptr, z.device_ptr))
     _lib.check(L.fdb_memcpy_d2d(r.device_ptr, b.device_ptr, b.nbytes))
     _touched(r)
-    _lib.check(L.fdb_vec_pointwise_mult(n, r.device_ptr, invdiag.device_ptr, z.device_ptr))
+    M(r, z)
     _touched(z)
     _lib.check(L.fdb_memcpy_d2d(p.device_ptr, z.device_ptr, z.nbytes))
     _touched(p)
@@ -568,7 +572,7 @@ def jacobi_lanczos_bounds(A, invdiag, b, steps=10):
             break
         alpha = rz / pAp
         _lib.check(L.fdb_vec_axpy(n, -alpha, Ap.device_ptr, r.device_ptr))
-        _lib.check(L.fdb_vec_pointwise_mult(n, r.device_ptr, invdiag.device_ptr, z.device_ptr))
+        M(r, z)
         _touched(r, z)
         rz_new = dot(r, z)
         alphas.append(alpha)
@@ -580,7 +584,7 @@ def jacobi_lanczos_bounds(A, invdiag, b, steps=10):
         rz = rz_new
     k = len(alphas)
     if k == 0:
-        raise ArithmeticError(f"Chebyshev eigenvalue estimate: p.A p = {pAp} at the first step (D^-1 A is not "
+        raise ArithmeticError(f"Chebyshev eigenvalue estimate: p.A p = {pAp} at the first step (P^-1 A is not "
                               f"positive definite, or the right-hand side is zero)")
     T = np.zeros((k, k))
     for j in range(k):
@@ -618,6 +622,9 @@ class PMG(_LevelCycle):
     Smoother on the levels above the coarsest: ``smoother`` "chebyshev" (Chebyshev-Jacobi, ``nu`` iterations with
     the bounds ``esteig`` = (a, b, c, d): [a lmin + b lmax, c lmin + d lmax] with lmin, lmax of D^-1 A estimated
     by :func:`jacobi_lanczos_bounds` in ``esteig_steps`` steps from a right-hand side seeded by ``seed``) or "richardson" (damped Jacobi with ``omega``, ``nu`` sweeps).
+    ``level_pc`` "jacobi" (the above) or "star": Chebyshev preconditioned by the fast-diagonalisation vertex-star
+    relaxation of the level form (:class:`patch.FDMStar`, ``ASMExtrudedStarPC`` under FDMPC), with the bounds of
+    P^-1 A; "star" takes scalar :class:`assemble.Form` levels without ``ds`` terms and the "chebyshev" smoother.
 
     Coarse solve: ``coarse_ksp`` "cg" with ``coarse_pc`` "jacobi" or "none" to ``coarse_rtol`` /
     ``coarse_maxit``, or "preonly" with "mg": one :class:`VCycle` at the coarse degree on ``hierarchy``, whose
@@ -625,7 +632,8 @@ class PMG(_LevelCycle):
 
     def __init__(self, V, make_form, bc_domains=(), coarse_degree=1, halve=True, kappa=None, smoother="chebyshev",
                  nu=2, omega=0.8, esteig=(0.0, 0.1, 0.0, 1.1), esteig_steps=10, coarse_ksp="cg", coarse_pc="jacobi",
-                 coarse_rtol=1e-3, coarse_maxit=500, hierarchy=None, allreduce=None, scatter="atomic", seed=0):
+                 coarse_rtol=1e-3, coarse_maxit=500, hierarchy=None, allreduce=None, scatter="atomic", seed=0,
+                 level_pc="jacobi"):
         from .assemble import DirichletBC, FunctionSpace, assemble
         if getattr(V, "family", "CG") != "CG":
             raise NotImplementedError("PMG takes CG spaces (there is no DQ p-multigrid)")
@@ -638,6 +646,10 @@ class PMG(_LevelCycle):
                                       f"the hand-written kernels give up to degree 3")
         if smoother not in ("chebyshev", "richardson"):
             raise NotImplementedError(f"PMG level smoother {smoother!r}: 'chebyshev' or 'richardson'")
+        if level_pc not in ("jacobi", "star") or (level_pc == "star" and smoother != "chebyshev"):
+            raise NotImplementedError(f"PMG level pc {level_pc!r} with smoother {smoother!r}: 'jacobi', or 'star' "
+                                      f"under 'chebyshev'")
+        self.level_pc = level_pc
         if (coarse_ksp, coarse_pc) not in (("cg", "jacobi"), ("cg", "none"), ("preonly", "mg")):
             raise NotImplementedError(f"PMG coarse solve ksp_type {coarse_ksp!r} with pc_type {coarse_pc!r}: cg with "
                                       f"jacobi or none, or preonly with mg")
@@ -665,7 +677,7 @@ class PMG(_LevelCycle):
             self.transfers[0] = PTransfer(spaces[0], spaces[1], scatter)
         self.spaces = spaces
         self.bcs = [[DirichletBC(W, 0.0, s) for s in bc_domains] for W in spaces]
-        self.ops, self.invdiag = [], []
+        self.ops, self.invdiag, self.stars = [], [], [None] * len(spaces)
         for l, W in enumerate(spaces):
             if l == 0 and self.coarse_mg is not None:
                 self.ops.append(self.coarse_mg.ops[-1])
@@ -673,11 +685,21 @@ class PMG(_LevelCycle):
                 continue
             f = make_form(W) if kappa is None else make_form(W, self.kappas[l])
             A = assemble(f, bcs=self.bcs[l], mat_type="matfree")
+            self.ops.append(A)
+            if l > 0 and level_pc == "star":
+                from .patch import FDMStar
+                self.stars[l] = FDMStar(f, self.bcs[l])
+                self.invdiag.append(None)
+                continue
             d = A.getDiagonal(W.dat())
             op2.par_loop(reciprocal_kernel(V.cdim), W.node_set, d(op2.RW))
-            self.ops.append(A)
             self.invdiag.append(d)
         self._work = [dict(r=W.dat(), e=W.dat(), t=W.dat(), b=W.dat(), x=W.dat(), d=W.dat()) for W in spaces]
+        if level_pc == "star":
+            # the fused Chebyshev pass takes the preconditioned residual as its b, with ax = 0 and dinv = 1
+            for l in range(1, len(spaces)):
+                w = self._work[l]
+                w["s"], w["zero"], w["one"] = (spaces[l].dat(np.full(spaces[l].node_count, v)) for v in (0.0, 0.0, 1.0))
         self.top = len(spaces) - 1
         # Chebyshev bounds of D^-1 A on every smoothed level
         self.bounds = [None] * len(spaces)
@@ -690,7 +712,9 @@ class PMG(_LevelCycle):
                 rhs = W.dat(rng.standard_normal(shape))
                 for bc in self.bcs[l]:
                     bc.zero(rhs)
-                lmin, lmax = jacobi_lanczos_bounds(self.ops[l], self.invdiag[l], rhs, esteig_steps)
+                star = self.stars[l]
+                lmin, lmax = jacobi_lanczos_bounds(self.ops[l], self.invdiag[l], rhs, esteig_steps,
+                                                   M=None if star is None else star.apply)
                 self.bounds[l] = (a * lmin + b_ * lmax, c * lmin + d_ * lmax)
 
     def _smooth(self, l, b, x):
@@ -701,6 +725,17 @@ class PMG(_LevelCycle):
         L = _lib.lib()
         A, w = self.ops[l], self._work[l]
         n = b._data.size
+        if self.stars[l] is not None:
+            # z = P^-1 (b - A x); d = c_d d + c_z z; x += d
+            for cd, cz in chebyshev_coefficients(*self.bounds[l], self.nu):
+                A.mult(x, w["t"])
+                _lib.check(L.fdb_vec_aypx(n, -1.0, b.device_ptr, w["t"].device_ptr))
+                _touched(w["t"])
+                self.stars[l].apply(w["t"], w["s"])
+                _lib.check(L.fdb_vec_chebyshev(n, cd, cz, w["s"].device_ptr, w["zero"].device_ptr,
+                                               w["one"].device_ptr, w["d"].device_ptr, x.device_ptr))
+                _touched(w["d"], x)
+            return
         for cd, cz in chebyshev_coefficients(*self.bounds[l], self.nu):
             A.mult(x, w["t"])
             _lib.check(L.fdb_vec_chebyshev(n, cd, cz, b.device_ptr, w["t"].device_ptr, self.invdiag[l].device_ptr,

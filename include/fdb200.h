@@ -661,6 +661,28 @@ int fdb_asm_update(fdb_asm_t a, fdb_mat_t mat, int *nsingular);
 int fdb_asm_apply(fdb_asm_t a, const double *b, double *x);
 int fdb_asm_get_blocks(fdb_asm_t a, double *out_host);
 
+/* ------------------------------------------- fast-diagonalisation vertex-star relaxation (DESIGN.md 4.20)
+ * z = sum_v R_v^T A_v^-1 R_v r over the vertex stars of an extruded CG_p space (p = 1..5), A_v the separable
+ * patch operator alpha*kbar_v*(K(x)M(x)M + M(x)K(x)M + M(x)M(x)K) + beta*M(x)M(x)M applied through its 1-D
+ * eigenbases (csrc/fdm_star_hex.cu).
+ *   cell_node_map [ncols][(p+1)^3], offset [(p+1)^3]: the extruded cell-node map, DEVICE arrays that the handle
+ *   reads but does not copy or own (they must outlive it).  The other arrays are host arrays, copied at create:
+ *   vert_cols [nvert][4]: base column of each quadrant sx*2 + sy around a base vertex, -1 where there is none;
+ *   star_vert, star_layer [nstar]: a star's base vertex and node layer; stars sorted by colour (parities of the
+ *   vertex lattice), colour c holding stars colour_ptr[c] .. colour_ptr[c+1]-1;
+ *   star_table [nstar][3]: pool entries of the x, y, z tables; pool [npool][m*m + 3m], m = 2p-1: S (row = star
+ *   node, column = mode), eigenvalues, active mask, existence mask.
+ * fdb_fdm_star_update sets alpha, beta and kbar_v = mean of kappa (device, NULL: 1) over the star's nodes;
+ * fdb_fdm_star_apply overwrites z (device pointers, r != z). */
+typedef struct fdb_fdm_star_s *fdb_fdm_star_t;
+int fdb_fdm_star_create(int degree, int nz, int ncols, const fdb_int *cell_node_map, const fdb_int *offset,
+                        fdb_int node_count, int nvert, const fdb_int *vert_cols, int nstar, const fdb_int *star_vert,
+                        const fdb_int *star_layer, const fdb_int *star_table, const long long *colour_ptr, int npool,
+                        const double *pool, fdb_fdm_star_t *out);
+int fdb_fdm_star_update(fdb_fdm_star_t h, double alpha, double beta, const double *kappa);
+int fdb_fdm_star_apply(fdb_fdm_star_t h, const double *r, double *z);
+int fdb_fdm_star_destroy(fdb_fdm_star_t h);
+
 /* --------------------------------------------------------- Dat subset ops (K5)
  * DirichletBC.zero / DirichletBC.set on a node subset (firedrake/bcs.py:192-221,
  * pyop2/types/dat.py:297-311).  Device pointers. */
