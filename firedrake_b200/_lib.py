@@ -36,6 +36,8 @@ FORM_P_RESTRICT = 18
 FORM_P_INJECT = 19
 FORM_SPECTRAL_HELMHOLTZ = 20           # alpha*inner(grad u, grad v)*dx(GLL) + beta*inner(u, v)*dx(GLL)
 FORM_SPECTRAL_HELMHOLTZ_COEF = 21      # the same with a trailing nodal kappa in the stiffness term
+FORM_MIXED_POISSON = 22                # alpha*dot(sigma, tau)*dx + div(tau)*u*dx + div(sigma)*v*dx on NCF_k x DQ_{k-1}
+FORM_MIXED_POISSON_SCHUR = 23          # its selfp Schur complement B W B^T (metric-free)
 CELL_HEX_EXTRUDED = 1
 CELL_HEX = 2
 CELL_TRIANGLE = 3

@@ -34,15 +34,26 @@ class FunctionSpace:
     ``family="DQ"``: the scalar discontinuous space DQ_p (p = 1..4) with Gauss-Legendre nodes
     (``mesh.dg_function_space``), for :class:`InteriorPenalty` and the cell forms of :class:`Form`.
     ``element`` is its 1-D element (the kernels' tables); None for CG, whose kernels use the default GLL
-    element."""
+    element.
+
+    ``family="NCF"``: the H(div) space NCF_k (k = 2..4, ``mesh.hdiv_function_space``), the flux space of
+    :class:`MixedPoisson`; no other form takes it."""
 
     def __init__(self, mesh, degree, cdim=1, partition=None, family="CG"):
         self.mesh, self.degree, self.cdim = mesh, degree, cdim
-        if family not in ("CG", "DQ"):
-            raise ValueError(f"family {family!r}: 'CG' or 'DQ'")
+        if family not in ("CG", "DQ", "NCF"):
+            raise ValueError(f"family {family!r}: 'CG', 'DQ' or 'NCF'")
         self.family = family
         self.element = None
-        if family == "DQ":
+        if family == "NCF":
+            if cdim != 1:
+                raise NotImplementedError("an NCF space has one value per dof (cdim 1): its dofs are the "
+                                          "components of the Piola-mapped field")
+            if partition is not None:
+                raise NotImplementedError("partitioned NCF spaces are not implemented: a face shared by two ranks "
+                                          "would need its own halo design")
+            self.V = V = mesh.hdiv_function_space(degree)
+        elif family == "DQ":
             from .fiat_lite import interval_element
             if cdim != 1:
                 raise NotImplementedError("DQ spaces are scalar (vector DQ is not implemented)")
@@ -111,8 +122,14 @@ class FunctionSpace:
 
 
 def _refuse_dq(V, what, why="it is stated on CG spaces only"):
+    _refuse_ncf(V, what)
     if getattr(V, "family", "CG") == "DQ":
         raise NotImplementedError(f"{what} does not take DQ spaces: {why}")
+
+
+def _refuse_ncf(V, what):
+    if getattr(V, "family", "CG") == "NCF":
+        raise NotImplementedError(f"{what} does not take NCF (H(div)) spaces: the only form on NCF is MixedPoisson")
 
 
 def interpolate_q1(V: "FunctionSpace", source: op2.Dat, target: op2.Dat = None):
@@ -1451,8 +1468,12 @@ class DirichletBC:
     (firedrake/bcs.py:260-457)."""
 
     def __init__(self, V: FunctionSpace, g, sub_domain):
-        _refuse_dq(V, "DirichletBC", "a DQ space has no boundary nodes; impose the condition weakly with "
-                   "InteriorPenalty(..., weak_bcs=sub_domain) and nitsche_load")
+        if getattr(V, "family", "CG") == "NCF" and not (np.isscalar(g) and g == 0.0):
+            raise NotImplementedError("DirichletBC on an NCF space imposes sigma.n = 0 only: a nonzero flux value "
+                                      "needs the face metric, which is not implemented")
+        if getattr(V, "family", "CG") != "NCF":
+            _refuse_dq(V, "DirichletBC", "a DQ space has no boundary nodes; impose the condition weakly with "
+                       "InteriorPenalty(..., weak_bcs=sub_domain) and nitsche_load")
         self.V = V
         subs = sub_domain if isinstance(sub_domain, (list, tuple)) else [sub_domain]
         self.sub_domains = tuple(subs)
@@ -1777,6 +1798,7 @@ class InteriorPenalty:
     ds = ()
 
     def __post_init__(self):
+        _refuse_ncf(self.V, "InteriorPenalty")
         if getattr(self.V, "family", "CG") != "DQ":
             raise ValueError("InteriorPenalty takes a DQ space: FunctionSpace(mesh, p, family='DQ')")
         if self.eta is None:
@@ -1822,6 +1844,7 @@ def nitsche_load(F: InteriorPenalty, g: op2.Dat, tensor: op2.Dat = None):
 
 def dg_flux_load(V: FunctionSpace, g: op2.Dat, sub_domain="on_boundary", tensor: op2.Dat = None):
     """The flux (Neumann) load g*v*ds(sub_domain) of a Dat ``g`` on a DQ space ``V``."""
+    _refuse_ncf(V, "dg_flux_load")
     if getattr(V, "family", "CG") != "DQ":
         raise ValueError("dg_flux_load takes a DQ space; on CG spaces the load is assemble(BoundaryMass(V, 1, "
                          "sub_domain), u=g)")
@@ -1920,6 +1943,7 @@ class DGTransport:
     ds = ()
 
     def __post_init__(self):
+        _refuse_ncf(self.V, "DGTransport")
         if getattr(self.V, "family", "CG") != "DQ":
             raise ValueError("DGTransport takes a DQ space: FunctionSpace(mesh, p, family='DQ')")
         ds = getattr(self.b, "dataset", None)
@@ -2395,6 +2419,7 @@ class Form:
     ds: tuple = ()
 
     def __post_init__(self):
+        _refuse_ncf(self.V, "Form")
         if self.ds:
             _refuse_dq(self.V, "Form's ds terms", "DQ boundary terms are InteriorPenalty's weak_bcs")
             _check_ds(self)
@@ -2842,6 +2867,273 @@ class StokesMatrixContext:
         return self.mult(X, Y)
 
 
+@dataclass
+class MixedPoisson:
+    """Mixed Poisson / Darcy flow on the H(div) pair NCF_k x DQ_{k-1} (``Sigma = FunctionSpace(mesh, k,
+    family="NCF")``, k = 2..4; ``Q = FunctionSpace(mesh, k - 1, family="DQ")``), the form of Firedrake's
+    saddle_point_pc demo:
+
+        a((sigma, u), (tau, v)) = alpha*dot(sigma, tau)*dx + div(tau)*u*dx + div(sigma)*v*dx
+
+    alpha is a constant (the inverse permeability).  The form is symmetric and indefinite.  Vectors are
+    :class:`op2.MixedDat` (sigma, u), e.g. ``F.dat()``; ``assemble(F, u=up)`` is the action and ``assemble(F,
+    mat_type="matfree")`` the matrix-free operator (:class:`MixedPoissonMatrixContext`); :func:`solve` runs GMRES with
+    the selfp Schur fieldsplit.  The source term of -div(grad u) = f is ``L[1] = -assemble(mass(Q), u=f)``; the
+    natural condition u = g is :func:`mixed_dirichlet_load`, the essential one sigma.n = 0 ``DirichletBC(Sigma, 0.0,
+    sub_domain)``."""
+    Sigma: FunctionSpace
+    Q: FunctionSpace
+    alpha: float = 1.0
+    symmetric = True
+
+    def __post_init__(self):
+        S, Q = self.Sigma, self.Q
+        if getattr(S, "family", "CG") != "NCF":
+            raise ValueError("MixedPoisson's flux space is NCF_k: FunctionSpace(mesh, k, family='NCF')")
+        if getattr(Q, "family", "CG") != "DQ" or Q.degree != S.degree - 1:
+            raise ValueError(f"MixedPoisson pairs NCF_k with DQ_(k-1): got {getattr(Q, 'family', 'CG')} degree "
+                             f"{Q.degree} for NCF degree {S.degree}")
+        if S.mesh is not Q.mesh:
+            raise ValueError("the MixedPoisson flux and scalar spaces must be on the same mesh")
+        self.V = S
+        self.pressure_map = op2.Map(S.cell_set, Q.node_set, Q.V.arity, Q.V.cell_node_map, offset=Q.V.offset)
+
+    def dat(self, sigma=None, u=None):
+        """A (flux, scalar) vector: ``op2.MixedDat([Sigma.dat(sigma), Q.dat(u)])``."""
+        return op2.MixedDat([self.Sigma.dat(sigma), self.Q.dat(u)])
+
+    def coefficient_args(self):
+        return []
+
+    def kernel(self, rank=1, diagonal=False):
+        if rank != 1:
+            raise NotImplementedError("MixedPoisson has no assembled matrix: use the action, the diagonal of the "
+                                      "flux block and mat_type='matfree'")
+        return op2.Kernel("mixed_poisson", degree=self.Sigma.degree, alpha=self.alpha, diagonal=diagonal)
+
+
+class MixedPoissonMatrixContext(StokesMatrixContext):
+    """The matrix-free operator of :class:`MixedPoisson` (:class:`StokesMatrixContext`: identity on the flux rows
+    of the DirichletBCs) with ``getDiagonal``, the diagonal of the flux block alpha*M (1 on the constrained rows)."""
+
+    def getDiagonal(self, d: op2.Dat = None, scatter="atomic"):
+        F = self.form
+        S = F.Sigma
+        if d is None:
+            d = S.dat()
+        d.zero()
+        gk = op2.GlobalKernel(F.kernel(1, diagonal=True), [S.cell_node_map, S.coord_map, F.pressure_map],
+                              extruded=True, scatter=scatter)
+        op2.Parloop(gk, S.cell_set, [d(op2.INC, S.cell_node_map), S.coordinates(op2.READ, S.coord_map)],
+                    location="device")()
+        for bc in self.bcs:
+            bc.set(d, 1.0)
+        return d
+
+
+class MixedPoissonSchur:
+    """The selfp Schur complement S_p = B W B^T of :class:`MixedPoisson` on the DQ space, W one value per flux dof
+    (``w``, a Dat of ``Sigma``; PETSc's ``selfp`` takes diag(A00)^-1 with zeros on the flux-condition rows, whose
+    A01 rows vanish).  Metric-free kernels (form "mixed_poisson_schur"): ``mult`` is two passes over the cells with
+    the NCF scratch vector zeroed in between, ``getDiagonal`` one."""
+
+    def __init__(self, F: MixedPoisson, w: op2.Dat, scatter="atomic"):
+        self.form, self.w = F, w
+        S = F.Sigma
+        maps = [F.pressure_map, S.cell_node_map]
+        self._gk = op2.GlobalKernel(op2.Kernel("mixed_poisson_schur", degree=S.degree), maps, extruded=True,
+                                    scatter=scatter)
+        self._gkd = op2.GlobalKernel(op2.Kernel("mixed_poisson_schur", degree=S.degree, diagonal=True), maps,
+                                     extruded=True, scatter=scatter)
+        self._t = S.dat()
+        self._loops = {}
+
+    def mult(self, x: op2.Dat, y: op2.Dat):
+        F, S = self.form, self.form.Sigma
+        key = (id(x), id(y))
+        if key not in self._loops:
+            self._loops = {key: op2.Parloop(self._gk, S.cell_set,
+                                            [y(op2.INC, F.pressure_map), x(op2.READ, F.pressure_map),
+                                             self.w(op2.READ, S.cell_node_map), self._t(op2.INC, S.cell_node_map)],
+                                            location="device")}
+        y.zero()
+        self._t.zero()
+        self._loops[key]()
+        return y
+
+    def getDiagonal(self, d: op2.Dat = None):
+        F, S = self.form, self.form.Sigma
+        if d is None:
+            d = F.Q.dat()
+        d.zero()
+        op2.Parloop(self._gkd, S.cell_set, [d(op2.INC, F.pressure_map), self.w(op2.READ, S.cell_node_map)],
+                    location="device")()
+        return d
+
+
+def mixed_poisson_load_kernel(degree, name=None):
+    """C source of the natural-condition load ``inner(dot(tau, n), g)*ds`` on one exterior facet of an NCF_k cell
+    (arguments: y INC (flux dofs), coordinates, g READ at the 8 vertices (trilinear), the uint32 local facet
+    number).  Under the contravariant Piola map tau.n ds = tau^.n^ ds^, so only the reference face enters; the
+    (k+1)^2-point Gauss rule on the face."""
+    from .codegen import CStringKernel
+    from .fiat_lite import interval_element
+    k = degree
+    name = name or f"mixed_poisson_load{k}"
+    el = interval_element(k - 1, k + 1, "gl")
+    vec = lambda a: "{" + ", ".join(repr(float(v)) for v in a) + "}"
+    tab = "{" + ", ".join(vec(r) for r in el.B) + "}"
+    code = f"""
+static void {name}(double *y, const double *X, const double *g, const unsigned *facet)
+{{
+    const double xq[{k + 1}] = {vec(el.xq)}, wq[{k + 1}] = {vec(el.wq)};
+    const double G[{k + 1}][{k}] = {tab};            /* DG_{{k-1}} (Gauss-Legendre) at the face points */
+    const int d = (int)(facet[0] / 2), s = (int)(facet[0] % 2);
+    const int e0 = d == 0 ? 1 : 0, e1 = d == 2 ? 1 : 2;
+    const int n1 = d == 1 ? {k + 1} : {k}, n2 = d == 2 ? {k + 1} : {k};
+    for (int p = 0; p < {k + 1}; ++p)
+    for (int r = 0; r < {k + 1}; ++r) {{
+        double xi[3];
+        xi[d] = (double)s; xi[e0] = xq[p]; xi[e1] = xq[r];
+        double gv = 0.0;
+        for (int v = 0; v < 8; ++v)
+            gv += ((v & 4) ? xi[0] : 1.0 - xi[0]) * ((v & 2) ? xi[1] : 1.0 - xi[1]) * ((v & 1) ? xi[2] : 1.0 - xi[2])
+                  * g[v];
+        const double c = (s ? 1.0 : -1.0) * wq[p] * wq[r] * gv;
+        for (int t0 = 0; t0 < {k}; ++t0)
+        for (int t1 = 0; t1 < {k}; ++t1) {{
+            int idx[3];
+            idx[d] = s; idx[e0] = t0; idx[e1] = t1;
+            y[d * {k * k * (k + 1)} + (idx[0] * n1 + idx[1]) * n2 + idx[2]] += c * G[p][t0] * G[r][t1];
+        }}
+    }}
+}}
+"""
+    return CStringKernel(code, name)
+
+
+def mixed_dirichlet_load(F: MixedPoisson, g: op2.Dat, sub_domain="on_boundary", tensor: op2.Dat = None):
+    """The natural condition u = g of :class:`MixedPoisson` on ``sub_domain`` (1..4, "bottom", "top", a tuple of
+    them or "on_boundary"): the flux load ``inner(dot(tau, n), g)*ds`` with g a Dat of vertex values
+    (``DataSet(vertex set, 1)``, trilinear), added into ``tensor`` (a flux Dat; new and zeroed if None).  Set-up
+    work: the generic wrapper path over the exterior facets."""
+    from . import codegen
+    S = F.Sigma
+    if tensor is None:
+        tensor = S.dat()
+        tensor.zero()
+    if g.dataset.set is not S.vertex_set or g.cdim != 1:
+        raise ValueError("mixed_dirichlet_load: g is one value per mesh vertex, a Dat on DataSet(Sigma.vertex_set, 1)")
+    tensor.device_ptr
+    k = mixed_poisson_load_kernel(S.degree)
+    for fset, fmap, cmap, facet in _boundary_groups(S, sub_domain):
+        codegen.par_loop(k, fset, tensor(op2.INC, fmap), S.coordinates(op2.READ, cmap), g(op2.READ, cmap),
+                         facet(op2.READ))
+    return tensor
+
+
+def mixed_poisson_kernel(degree, alpha=1.0, name=None):
+    """C source of the :class:`MixedPoisson` action on the generic wrapper path, with MixedDat arguments: y (INC) and
+    up, each the 3 k^2 (k+1) flux dofs followed by the k^3 DQ dofs, and the coordinates.  Every basis function is
+    evaluated at every Gauss point (no sum factorisation), the metric J^T J / det J formed there: the independent
+    statement of the hand-written FDB_FORM_MIXED_POISSON kernel."""
+    from .codegen import CStringKernel
+    from .fiat_lite import interval_element
+    k = degree
+    if not 2 <= k <= 4:
+        raise NotImplementedError(f"the generic-path mixed Poisson statement covers degrees 2..4, got {k}")
+    name = name or f"mixed_poisson_action{k}"
+    cg, dg = interval_element(k), interval_element(k - 1, k + 1, "gl")
+    vec = lambda a: "{" + ", ".join(repr(float(v)) for v in a) + "}"
+    tab = lambda a: "{" + ", ".join(vec(r) for r in a) + "}"
+    ns = 3 * k * k * (k + 1)
+    code = f"""
+#define MQ {k + 1}
+#define MK {k}
+#define MS {ns}
+static const double MX[MQ] = {vec(cg.xq)}, MW[MQ] = {vec(cg.wq)};
+static const double MC[MQ][MK + 1] = {tab(cg.B)}, MD[MQ][MK + 1] = {tab(cg.D)}, MG[MQ][MK] = {tab(dg.B)};
+/* the value (der = 0) or the axis-d derivative (der = 1) of the d-component of flux basis function (d, i) at point q */
+static double mp_basis(int d, const int *i, const int *q, int der)
+{{
+    double f = 1.0;
+    for (int e = 0; e < 3; ++e)
+        f *= e == d ? (der ? MD[q[e]][i[e]] : MC[q[e]][i[e]]) : MG[q[e]][i[e]];
+    return f;
+}}
+static void {name}(double *y, const double *X, const double *up)
+{{
+    const double *u = up + MS;
+    for (int qx = 0; qx < MQ; ++qx) for (int qy = 0; qy < MQ; ++qy) for (int qz = 0; qz < MQ; ++qz) {{
+        const int q[3] = {{qx, qy, qz}};
+        const double xi[3] = {{MX[qx], MX[qy], MX[qz]}};
+        double J[3][3] = {{{{0}}}};
+        for (int v = 0; v < 8; ++v) {{
+            const int b[3] = {{(v >> 2) & 1, (v >> 1) & 1, v & 1}};
+            for (int r = 0; r < 3; ++r) {{
+                double gr = b[r] ? 1.0 : -1.0;
+                for (int e = 0; e < 3; ++e) if (e != r) gr *= b[e] ? xi[e] : 1.0 - xi[e];
+                for (int c = 0; c < 3; ++c) J[c][r] += X[v * 3 + c] * gr;
+            }}
+        }}
+        const double det = J[0][0] * (J[1][1] * J[2][2] - J[1][2] * J[2][1])
+                         - J[0][1] * (J[1][0] * J[2][2] - J[1][2] * J[2][0])
+                         + J[0][2] * (J[1][0] * J[2][1] - J[1][1] * J[2][0]);
+        const double w = MW[qx] * MW[qy] * MW[qz];
+        double sh[3] = {{0.0, 0.0, 0.0}}, dv = 0.0, uq = 0.0;
+        int j = 0;
+        for (int d = 0; d < 3; ++d)
+            for (int i0 = 0; i0 < (d == 0 ? MK + 1 : MK); ++i0)
+            for (int i1 = 0; i1 < (d == 1 ? MK + 1 : MK); ++i1)
+            for (int i2 = 0; i2 < (d == 2 ? MK + 1 : MK); ++i2, ++j) {{
+                const int i[3] = {{i0, i1, i2}};
+                sh[d] += up[j] * mp_basis(d, i, q, 0);
+                dv += up[j] * mp_basis(d, i, q, 1);
+            }}
+        for (int a = 0; a < MK; ++a) for (int b = 0; b < MK; ++b) for (int c = 0; c < MK; ++c)
+            uq += u[(a * MK + b) * MK + c] * MG[qx][a] * MG[qy][b] * MG[qz][c];
+        double f[3];
+        for (int a = 0; a < 3; ++a) {{
+            f[a] = 0.0;
+            for (int b = 0; b < 3; ++b)
+                f[a] += (J[0][a] * J[0][b] + J[1][a] * J[1][b] + J[2][a] * J[2][b]) * sh[b];
+            f[a] *= {float(alpha)!r} * w / det;
+        }}
+        j = 0;
+        for (int d = 0; d < 3; ++d)
+            for (int i0 = 0; i0 < (d == 0 ? MK + 1 : MK); ++i0)
+            for (int i1 = 0; i1 < (d == 1 ? MK + 1 : MK); ++i1)
+            for (int i2 = 0; i2 < (d == 2 ? MK + 1 : MK); ++i2, ++j) {{
+                const int i[3] = {{i0, i1, i2}};
+                y[j] += f[d] * mp_basis(d, i, q, 0) + w * uq * mp_basis(d, i, q, 1);
+            }}
+        for (int a = 0; a < MK; ++a) for (int b = 0; b < MK; ++b) for (int c = 0; c < MK; ++c)
+            y[MS + (a * MK + b) * MK + c] += w * dv * MG[qx][a] * MG[qy][b] * MG[qz][c];
+    }}
+}}
+#undef MQ
+#undef MK
+#undef MS
+"""
+    return CStringKernel(code, name)
+
+
+def assemble_mixed_poisson_generic(F: MixedPoisson, up: op2.MixedDat, tensor=None):
+    """``assemble(action(a, up))`` of :class:`MixedPoisson` through the generic wrapper path
+    (:func:`mixed_poisson_kernel`, MixedDat arguments over the NCF and DQ maps): the cross-check and the baseline of
+    the hand-written kernel."""
+    S = F.Sigma
+    if tensor is None:
+        tensor = F.dat()
+    tensor.zero()
+    for d in tensor:
+        d.device_ptr
+    mm = op2.MixedMap([S.cell_node_map, F.pressure_map])
+    op2.par_loop(mixed_poisson_kernel(S.degree, F.alpha), S.cell_set, tensor(op2.INC, mm),
+                 S.coordinates(op2.READ, S.coord_map), up(op2.READ, mm))
+    return tensor
+
+
 class ConvergenceError(RuntimeError):
     """A nonlinear solve that cannot go on (firedrake.exceptions.ConvergenceError); ``reason`` is the
     SNES converged reason, e.g. "DIVERGED_FNORM_NAN"."""
@@ -2912,6 +3204,13 @@ def assemble(form: Form, u=None, tensor=None, bcs=(), mat_type="aij"):
     unassembled), ``"matfree"`` -> :class:`ImplicitMatrixContext`."""
     V = form.V
     bcs = tuple(bcs)
+    if isinstance(form, MixedPoisson):
+        if u is not None:
+            return StokesAssembler(form, u, bcs).assemble(tensor)
+        if mat_type != "matfree":
+            raise NotImplementedError(f"mat_type {mat_type!r}: MixedPoisson has no assembled matrix, use mat_type "
+                                      f"'matfree'")
+        return MixedPoissonMatrixContext(form, bcs)
     if isinstance(form, _TAYLOR_HOOD_FORMS):
         if u is not None:
             return StokesAssembler(form, u, bcs).assemble(tensor)
@@ -3398,6 +3697,7 @@ def _fdm(form, bcs, sp, hierarchy=None):
     if type(form) is not Form:
         raise NotImplementedError(f"FDMPC on {type(form).__name__}: it takes scalar Form (alpha, beta, kappa) "
                                   f"operators only")
+    _refuse_ncf(V, "FDMPC")
     if getattr(V, "family", "CG") != "CG" or V.cdim != 1:
         raise NotImplementedError("FDMPC takes scalar CG spaces only (no vector or DQ spaces)")
     if form.ds:
@@ -3664,12 +3964,15 @@ def solve(form: Form, L: op2.Dat, u: op2.Dat, bcs=(), solver_parameters=None, hi
     "mg" and the ``pmg_*`` options of :func:`pmg_options`; CG2 and CG3) or "firedrake.FDMPC" (scalar :class:`Form`
     without ds: the fast-diagonalisation vertex-star relaxation, or P1PC / PMGPC smoothed by it, :func:`fdm_options`);
     ``ksp_rtol`` (1e-8), ``ksp_max_it`` (1000).
-    A :class:`Stokes` form takes MixedDats and its own options (:func:`_solve_stokes`), and the only form
-    that takes ``nullspace``.  Returns (iterations, residual history)."""
+    A :class:`Stokes` form takes MixedDats and its own options (:func:`_solve_stokes`), and so does a
+    :class:`MixedPoisson` form (:func:`_solve_mixed_poisson`); they are the only forms that take ``nullspace``.
+    Returns (iterations, residual history)."""
     if isinstance(form, Stokes):
         return _solve_stokes(form, L, u, bcs, solver_parameters, hierarchy, nullspace)
+    if isinstance(form, MixedPoisson):
+        return _solve_mixed_poisson(form, L, u, bcs, solver_parameters, nullspace)
     if nullspace is not None:
-        raise NotImplementedError("nullspace is implemented for Stokes forms only")
+        raise NotImplementedError("nullspace is implemented for MixedPoisson and Stokes forms only")
     symmetric = getattr(form, "symmetric", True)
     sp = {"mat_type": "matfree", "ksp_type": "cg" if symmetric else "gmres", "pc_type": "none", "ksp_rtol": 1e-8,
           "ksp_max_it": 1000, "ksp_gmres_restart": 30}
@@ -3839,6 +4142,7 @@ def _pressure_mean_remover(Q):
 
     def remove_pressure_mean(v):
         v[1].axpy(-v[1].inner(ones) / Q.node_count, ones)
+    remove_pressure_mean.ones = ones
     return remove_pressure_mean
 
 
@@ -3958,6 +4262,170 @@ def _schur_factorisation(fact, Mu, Mp, A, new, remove_pressure_mean=None):
         if remove_pressure_mean is not None:
             remove_pressure_mean(z)
     return M
+
+
+_MIXED_POISSON_OPTIONS = {"mat_type": "matfree", "ksp_type": "gmres", "ksp_rtol": 1e-8, "ksp_max_it": 1000,
+                          "ksp_gmres_restart": 30, "pc_type": "none", "pc_fieldsplit_type": "schur",
+                          "pc_fieldsplit_schur_fact_type": "full", "pc_fieldsplit_schur_precondition": "selfp",
+                          "fieldsplit_0_ksp_type": "preonly", "fieldsplit_0_pc_type": "jacobi",
+                          "fieldsplit_1_ksp_type": "cg", "fieldsplit_1_pc_type": "jacobi", "fieldsplit_1_ksp_rtol": 1e-5,
+                          "fieldsplit_1_ksp_max_it": 1000}
+
+
+def _check_mixed_poisson_options(sp):
+    """The options of :func:`_solve_mixed_poisson`: the demo's "Schur complement with S_p" and its variants."""
+    for key in sp:
+        if key not in _MIXED_POISSON_OPTIONS:
+            raise NotImplementedError(f"option {key!r} is not implemented for MixedPoisson")
+    if sp["ksp_type"] == "cg":
+        raise ValueError("ksp_type cg needs a positive definite operator, and the mixed Poisson operator is "
+                         "indefinite: use gmres")
+    if sp["ksp_type"] != "gmres":
+        raise NotImplementedError(f"ksp_type {sp['ksp_type']!r}: MixedPoisson solves with gmres")
+    if sp["mat_type"] != "matfree":
+        raise NotImplementedError(f"mat_type {sp['mat_type']!r}: MixedPoisson has no assembled matrix, use 'matfree'")
+    if sp["pc_type"] not in ("none", "fieldsplit"):
+        raise NotImplementedError(f"pc_type {sp['pc_type']!r}: 'none' or 'fieldsplit'")
+    if sp["pc_type"] == "none":
+        return
+    want = {"pc_fieldsplit_type": ("schur",), "pc_fieldsplit_schur_fact_type": ("diag", "lower", "upper", "full"),
+            "pc_fieldsplit_schur_precondition": ("selfp",), "fieldsplit_0_ksp_type": ("preonly",),
+            "fieldsplit_0_pc_type": ("jacobi",), "fieldsplit_1_ksp_type": ("cg", "preonly"),
+            "fieldsplit_1_pc_type": ("jacobi",)}
+    for key, ok in want.items():
+        if sp[key] not in ok:
+            raise NotImplementedError(f"{key} {sp[key]!r}: {' or '.join(repr(v) for v in ok)}")
+
+
+def _solve_mixed_poisson(F: MixedPoisson, L: op2.MixedDat, up: op2.MixedDat, bcs=(), solver_parameters=None,
+                         nullspace=None):
+    """``solve(a == L, up, bcs=bcs, solver_parameters=..., nullspace=...)`` for :class:`MixedPoisson`, with the
+    options of Firedrake's saddle_point_pc demo, "Schur complement with S_p":
+
+    - ``ksp_type`` "gmres" (flexible, right-preconditioned; "cg" is refused, the operator is indefinite),
+      ``ksp_rtol``, ``ksp_max_it``, ``ksp_gmres_restart``.
+    - ``pc_type`` "none" or "fieldsplit" with ``pc_fieldsplit_type`` "schur", ``pc_fieldsplit_schur_precondition``
+      "selfp" and ``pc_fieldsplit_schur_fact_type`` "diag", "lower", "upper" or "full" (PETSc's upper . diag .
+      lower: two extra operator actions per application).  fieldsplit_0 is "preonly" / "jacobi": one application
+      of diag(alpha M)^-1 (1 on the flux-condition rows).  fieldsplit_1 preconditions S_p = B W B^T, W =
+      diag(alpha M)^-1 with zeros on the flux-condition rows (:class:`MixedPoissonSchur`): "cg" / "jacobi" runs
+      Jacobi-preconditioned CG on S_p to ``fieldsplit_1_ksp_rtol`` (``fieldsplit_1_ksp_max_it``), "preonly" /
+      "jacobi" is one application of diag(S_p)^-1.
+    - ``nullspace`` "constant": when flux conditions cover the whole boundary, u is determined up to a constant;
+      its dof-mean is removed from the right-hand side, every preconditioned vector (inside the inner CG too)
+      and the solution.
+
+    Every other option is refused by name.  DirichletBCs are on ``Sigma`` with value 0 (sigma.n = 0).  Returns
+    (iterations, residual history)."""
+    from . import _lib
+    from . import mg as _mg
+    sp = dict(_MIXED_POISSON_OPTIONS)
+    sp.update(solver_parameters or {})
+    _check_mixed_poisson_options(sp)
+    if nullspace not in (None, "constant"):
+        raise NotImplementedError(f"nullspace {nullspace!r}: None or 'constant' (constant u)")
+    bcs = tuple(bcs)
+    for bc in bcs:
+        if bc.V is not F.Sigma:
+            raise ValueError("MixedPoisson's DirichletBCs are flux conditions on its NCF space")
+    lib = _lib.lib()
+    S, Q = F.Sigma, F.Q
+    remove_mean = _pressure_mean_remover(Q) if nullspace else None
+    b = F.dat()
+    L.copy(b)
+    for bc in bcs:
+        bc.zero(b[0])
+    if nullspace:
+        remove_mean(b)
+    A = MixedPoissonMatrixContext(F, bcs)
+    up.zero()
+    for d in up:
+        d.device_ptr
+    M = None
+    if sp["pc_type"] == "fieldsplit":
+        n_s, n_u = up[0]._data.size, up[1]._data.size
+        dinv = A.getDiagonal()
+        op2.par_loop(_mg.reciprocal_kernel(1), S.node_set, dinv(op2.RW))
+        w = S.dat()
+        dinv.copy(w)
+        for bc in bcs:
+            bc.set(w, 0.0)
+        Sp = MixedPoissonSchur(F, w)
+
+        def Mu(r, z):
+            _lib.check(lib.fdb_vec_pointwise_mult(n_s, r.device_ptr, dinv.device_ptr, z.device_ptr))
+            z._device_written()
+
+        sdinv = Sp.getDiagonal()
+        op2.par_loop(_mg.reciprocal_kernel(1), Q.node_set, sdinv(op2.RW))
+
+        def jacobi_Sp(r, z):
+            _lib.check(lib.fdb_vec_pointwise_mult(n_u, r.device_ptr, sdinv.device_ptr, z.device_ptr))
+            z._device_written()
+            if nullspace:
+                z.axpy(-z.inner(remove_mean.ones) / Q.node_count, remove_mean.ones)
+
+        if sp["fieldsplit_1_ksp_type"] == "preonly":
+            Mp = jacobi_Sp
+        else:
+            class _Projected:
+                def mult(self, x, y):
+                    Sp.mult(x, y)
+                    if nullspace:
+                        y.axpy(-y.inner(remove_mean.ones) / Q.node_count, remove_mean.ones)
+
+            Sop = _Projected() if nullspace else Sp
+            rtol1, maxit1 = sp["fieldsplit_1_ksp_rtol"], sp["fieldsplit_1_ksp_max_it"]
+
+            def Mp(r, z):
+                z.zero()
+                z.device_ptr
+                _mg.pcg(Sop, r, z, jacobi_Sp, rtol=rtol1, maxit=maxit1)
+                if nullspace:
+                    z.axpy(-z.inner(remove_mean.ones) / Q.node_count, remove_mean.ones)
+
+        fact = sp["pc_fieldsplit_schur_fact_type"]
+        if fact in ("lower", "upper"):
+            M = _schur_factorisation(fact, Mu, Mp, A, F.dat, remove_mean)
+        else:
+            wv, yv, tu = F.dat(), F.dat(), F.dat()
+
+            def negate(v):
+                _lib.check(lib.fdb_vec_scale(v._data.size, -1.0, v.device_ptr))
+                v._device_written()
+
+            def M(r, z):
+                if fact == "diag":
+                    Mu(r[0], z[0])
+                    Mp(r[1], z[1])
+                else:
+                    # full: t = P0 r_u;  z_p = -P1 (r_p - B t);  z_u = t - P0 B^T z_p
+                    Mu(r[0], tu[0])
+                    tu[0].copy(wv[0])
+                    wv[1].zero()
+                    A.mult(wv, yv)
+                    r[1].copy(wv[1])
+                    wv[1].axpy(-1.0, yv[1])
+                    Mp(wv[1], z[1])
+                    negate(z[1])
+                    wv[0].zero()
+                    z[1].copy(wv[1])
+                    A.mult(wv, yv)
+                    Mu(yv[0], z[0])
+                    negate(z[0])
+                    z[0].axpy(1.0, tu[0])
+                if nullspace:
+                    remove_mean(z)
+    elif nullspace:
+        def M(r, z):
+            r.copy(z)
+            remove_mean(z)
+    its, hist = gmres(A, b, up, M, rtol=sp["ksp_rtol"], restart=sp["ksp_gmres_restart"], maxit=sp["ksp_max_it"])
+    if nullspace:
+        remove_mean(up)
+    for bc in bcs:
+        bc.apply(up[0])
+    return its, hist
 
 
 def _solve_navier_stokes(F: NavierStokes, L: op2.MixedDat, up: op2.MixedDat, bcs=(), solver_parameters=None,

@@ -181,3 +181,6 @@ int fdb_launch_p_transfer(fdb_kernel_s *k, fdb_int start, fdb_int end, int nlay,
 int fdb_launch_spectral_helmholtz(fdb_kernel_s *k, fdb_int start, fdb_int end, int nlay, const fdb_int *subset,
                                   double *y, const double *coords, const double *x, const double *kappa,
                                   const fdb_int *map0, const fdb_int *map1);
+// FDB_FORM_MIXED_POISSON[_SCHUR] (hdiv_hex.cu): args and maps as include/fdb200.h lists them for the form and mode
+int fdb_launch_hdiv(fdb_kernel_s *k, fdb_int start, fdb_int end, int nlay, const fdb_int *subset, void *const *args,
+                    const fdb_int *const *maps);

@@ -298,7 +298,7 @@ static int device_pointers(const fdb_call_args *a, bool mat, void **args, const 
 // fdb_kernel_call hands its arguments to the launchers.
 enum { MODE_ACTION, MODE_MATRIX, MODE_DIAGONAL };
 enum { LAUNCH_HELMHOLTZ, LAUNCH_HELMHOLTZ_COEF, LAUNCH_ELASTICITY, LAUNCH_STOKES, LAUNCH_BOUNDARY, LAUNCH_DG_FACET,
-       LAUNCH_DG_TRANSPORT, LAUNCH_P_TRANSFER, LAUNCH_SPECTRAL };
+       LAUNCH_DG_TRANSPORT, LAUNCH_P_TRANSFER, LAUNCH_SPECTRAL, LAUNCH_HDIV };
 // the degree of the second space of a form on two spaces: the descriptor's degree - 1 (Stokes' pressure, the
 // default of a row that does not name one), or any lower degree of an instantiated (fine, coarse) pair (the
 // p-multigrid transfers)
@@ -374,6 +374,12 @@ static const fdb_hex_form hex_forms[] = {
      nullptr, FDB_INTEGRAL_CELL, SPACE2_PRESSURE},
     {FDB_FORM_SPECTRAL_HELMHOLTZ_COEF, "spectral_helmholtz_coef", 1, false, "kappa", 1, false, LAUNCH_SPECTRAL,
      {5, 0, 5}, 1, nullptr, FDB_INTEGRAL_CELL, SPACE2_PRESSURE},
+    // mixed Poisson on NCF_k x DQ_{k-1} (the descriptor is the flux space, the second space the DQ one), and its
+    // metric-free selfp Schur complement.  Device mode only, action and diagonal, no rank 2 (hdiv_call)
+    {FDB_FORM_MIXED_POISSON, "mixed_poisson", 1, false, nullptr, 0, false, LAUNCH_HDIV, {4, 0, 4}, 2, "y_u, u",
+     FDB_INTEGRAL_CELL, SPACE2_PRESSURE},
+    {FDB_FORM_MIXED_POISSON_SCHUR, "mixed_poisson_schur", 1, false, nullptr, 0, false, LAUNCH_HDIV, {4, 0, 4}, 2,
+     "w, t", FDB_INTEGRAL_CELL, SPACE2_PRESSURE},
 };
 
 // the (fine, coarse) degree pairs the transfer kernels instantiate (p_transfer_hex.cu)
@@ -499,8 +505,13 @@ static int kernel_create(const fdb_kernel_desc *d, const fdb_space2_desc *s2, fd
                   "pin the rule with dx(degree=2*p)", f->name, d->nq, d->degree);
         return 1;
     }
+    if (f->launcher == LAUNCH_HDIV && mode == MODE_MATRIX) {
+        set_error("fdb_kernel_create: %s has no rank-2 form: there is no assembled mixed matrix; use the action and "
+                  "the diagonal", f->name);
+        return 1;
+    }
     // (a mixed residual has no matrix or diagonal, nor has its Jacobian: the mixed-form message comes first)
-    if (f->space2 && mode != MODE_ACTION) {
+    if (f->space2 && mode != MODE_ACTION && f->launcher != LAUNCH_HDIV) {
         set_error("fdb_kernel_create: %s is a mixed form, a rank-1 action only: it has no assembled matrix or "
                   "diagonal", f->name);
         return 1;
@@ -557,8 +568,9 @@ static int kernel_create(const fdb_kernel_desc *d, const fdb_space2_desc *s2, fd
         set_error("fdb_kernel_create: rank must be 1 or 2");
         return 1;
     }
-    // (a transfer reads no coordinates: offset1 is not used)
-    if (d->cell == FDB_CELL_HEX_EXTRUDED && (!d->offset0 || (!d->offset1 && !transfer))) {
+    // (a transfer and the Schur complement of mixed Poisson read no coordinates: offset1 is not used)
+    const bool no_coords = transfer || d->form == FDB_FORM_MIXED_POISSON_SCHUR;
+    if (d->cell == FDB_CELL_HEX_EXTRUDED && (!d->offset0 || (!d->offset1 && !no_coords))) {
         set_error("fdb_kernel_create: extruded cells need offset0/offset1");
         return 1;
     }
@@ -605,6 +617,7 @@ static int kernel_create(const fdb_kernel_desc *d, const fdb_space2_desc *s2, fd
     // an interior-facet entry reads both cells: 2 (p+1)^3 dofs and 16 vertices
     const int sides = d->integral == FDB_INTEGRAL_INTERIOR_FACET ? 2 : 1;
     k->arity = sides * k->n1d * k->n1d * k->n1d;
+    if (f->launcher == LAUNCH_HDIV) k->arity = 3 * d->degree * d->degree * (d->degree + 1);    // NCF_k
     const int arity1 = sides * 8;
     memset(k->h_off0, 0, sizeof(k->h_off0));
     memset(k->h_off1, 0, sizeof(k->h_off1));
@@ -689,6 +702,38 @@ static int p_transfer_call(fdb_kernel_s *k, const fdb_call_args *a, int nlay)
                                  (const double *)a->args[1],
                                  form == FDB_FORM_P_RESTRICT ? (const double *)a->args[2] : nullptr,
                                  a->maps[fm], a->maps[1 - fm]);
+}
+
+// mixed Poisson (FDB_FORM_MIXED_POISSON[_SCHUR]): args and maps as include/fdb200.h lists them, device mode only.
+// The flux scatters (the action, the diagonal of alpha M and the Schur form's B^T pass) are coloured on the NCF map
+static int hdiv_call(fdb_kernel_s *k, const fdb_call_args *a, int nlay)
+{
+    const fdb_hex_form *f = k->hex;
+    const bool schur = k->desc.form == FDB_FORM_MIXED_POISSON_SCHUR;
+    const int mode = hex_mode(&k->desc);
+    static const char *const sig[2][2] = {{"y_sigma, coords, sigma, y_u, u", "d, coords"}, {"y_u, u, w, t", "d, w"}};
+    static const char *const mapsig[2][2] = {{"NCF map, coord map, DQ map", "NCF map, coord map"},
+                                             {"DQ map, NCF map", "DQ map, NCF map"}};
+    const int m = mode == MODE_ACTION ? 0 : 1;
+    const int want = schur ? (m ? 2 : 4) : (m ? 2 : 5);
+    const int want_maps = !schur && !m ? 3 : 2;
+    if (a->location != FDB_LOC_DEVICE) {
+        set_error("fdb_kernel_call: %s takes device-resident Dats only (no host-pointer mode)", f->name);
+        return 1;
+    }
+    if (a->nargs != want || a->nmaps != want_maps) {
+        set_error("fdb_kernel_call: %s %s expects %d device args (%s) and %d maps (%s), got %d/%d", f->name,
+                  mode_name[mode], want, sig[schur][m], want_maps, mapsig[schur][m], a->nargs, a->nmaps);
+        return 1;
+    }
+    if (k->desc.scatter == FDB_SCATTER_COLOURED && !(schur && m)) {
+        if (a->start != 0) {
+            set_error("fdb_kernel_call: coloured scatter needs start == 0");
+            return 1;
+        }
+        if (colouring_for(k, a, schur ? 1 : 0)) return 1;
+    }
+    return fdb_launch_hdiv(k, a->start, a->end, nlay, a->subset, a->args, a->maps);
 }
 
 extern "C" {
@@ -803,6 +848,7 @@ int fdb_kernel_call(fdb_kernel_t k, const fdb_call_args *a)
     // facets] on facets
     const fdb_hex_form *f = k->hex;
     if (f->launcher == LAUNCH_P_TRANSFER) return p_transfer_call(k, a, nlay);
+    if (f->launcher == LAUNCH_HDIV) return hdiv_call(k, a, nlay);
     const int mode = hex_mode(&k->desc);
     const bool transport_facets = f->launcher == LAUNCH_DG_TRANSPORT && k->desc.integral != FDB_INTEGRAL_CELL;
     if (f->integral != FDB_INTEGRAL_CELL && a->location != FDB_LOC_DEVICE) {

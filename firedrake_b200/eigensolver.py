@@ -64,6 +64,9 @@ class LinearEigenproblem:
     ``restrict=False``."""
 
     def __init__(self, A, M=None, bcs=(), bc_shift=0.0, restrict=True):
+        if any(getattr(getattr(F, "V", None), "family", "CG") == "NCF" for F in (A, M)):
+            raise NotImplementedError("the eigensolver does not take NCF (H(div)) spaces: MixedPoisson, the only "
+                                      "form on NCF, is indefinite")
         if isinstance(A, _MIXED) or isinstance(M, _MIXED):
             raise NotImplementedError(f"{type(A if isinstance(A, _MIXED) else M).__name__}: Taylor-Hood and mixed "
                                       f"forms are not implemented in the eigensolver")

@@ -469,6 +469,9 @@ class PTransfer:
 
     def __init__(self, Vc, Vf, scatter="atomic"):
         for W in (Vc, Vf):
+            if getattr(W, "family", "CG") == "NCF":
+                raise NotImplementedError("PTransfer does not take NCF (H(div)) spaces: the only form on NCF is "
+                                          "MixedPoisson")
             if getattr(W, "family", "CG") != "CG":
                 raise NotImplementedError("PTransfer: CG spaces only (there is no DQ p-multigrid)")
         if Vc.mesh is not Vf.mesh or Vc.cdim != Vf.cdim or not Vc.degree < Vf.degree:
@@ -635,6 +638,9 @@ class PMG(_LevelCycle):
                  coarse_rtol=1e-3, coarse_maxit=500, hierarchy=None, allreduce=None, scatter="atomic", seed=0,
                  level_pc="jacobi"):
         from .assemble import DirichletBC, FunctionSpace, assemble
+        if getattr(V, "family", "CG") == "NCF":
+            raise NotImplementedError("PMG does not take NCF (H(div)) spaces: the only form on NCF is "
+                                      "MixedPoisson")
         if getattr(V, "family", "CG") != "CG":
             raise NotImplementedError("PMG takes CG spaces (there is no DQ p-multigrid)")
         if allreduce is not None or V.dof_dset.halo is not None:

@@ -1434,6 +1434,15 @@ class Kernel:
     action (output, coordinates, u), diagonal (output, coordinates) at every degree.  "spectral_helmholtz_coef" adds a
     nodal kappa to the stiffness term, ``alpha*inner(kappa*grad u, grad v)*dx(GLL)``, as the LAST argument (READ,
     through the argument map) like "helmholtz_coef".  No rank 2; device-resident Dats only.
+
+    "mixed_poisson" is mixed Poisson on the H(div) pair NCF_k x DQ_{k-1} (``degree`` = k, 2..4), ``alpha*dot(sigma,
+    tau)*dx + div(tau)*u*dx + div(sigma)*v*dx``: the action (INC, READ, READ, INC, READ) = (flux output, coordinates,
+    sigma, DQ output, u) through the NCF, coordinate and DQ maps, and the diagonal of alpha*M (INC, READ) = (d,
+    coordinates).  "mixed_poisson_schur" is the metric-free selfp Schur complement S_p = B W B^T: the action (INC,
+    READ, READ, INC) = (DQ output, u, W, t) adds B^T u into the NCF scratch t and then B (W o t) into the output
+    (S_p u when t is zero on entry), the diagonal (INC, READ) = (d, W) adds diag(B W B^T).  Both are created with the
+    DQ space as the second space (the maps: NCF, coordinate, DQ for "mixed_poisson"; DQ, NCF for the Schur form).
+    Device-resident Dats only.
     """
     form: str = "helmholtz"
     degree: int = 1
@@ -1474,6 +1483,14 @@ class Kernel:
             if len(self.d) != 3:
                 raise ValueError("d holds the three coefficients of D(s) = d0 + d1 s + d2 s^2")
         spec = _FORMS.get(self.form)
+        if spec and spec.hdiv:
+            if self.form == "mixed_poisson":
+                acc = (INC, READ) if self.diagonal else (INC, READ, READ, INC, READ)
+            else:
+                acc = (INC, READ) if self.diagonal else (INC, READ, READ, INC)
+            object.__setattr__(self, "accesses", acc)
+            object.__setattr__(self, "name", self.form + ("_diagonal" if self.diagonal else ""))
+            return
         if spec and spec.transfer:
             acc = (INC, READ, READ) if self.form == "p_restrict" else (WRITE, READ)
             object.__setattr__(self, "accesses", acc)
@@ -1538,6 +1555,7 @@ class _Form(NamedTuple):
     velocity: bool = False      # reads b (3 values per vertex) through the coordinate map after u
     transfer: bool = False      # a p-multigrid degree transfer: fine and coarse maps, no coordinates
     gll: bool = False           # stated on the GLL rule at the nodes: the default element is the collocated GLL one
+    hdiv: bool = False          # a mixed Poisson form on NCF_k x DQ_{k-1}
 
 
 _FORMS = {"helmholtz": _Form(_lib.FORM_HELMHOLTZ),
@@ -1560,7 +1578,9 @@ _FORMS = {"helmholtz": _Form(_lib.FORM_HELMHOLTZ),
           "p_restrict": _Form(_lib.FORM_P_RESTRICT, transfer=True),
           "p_inject": _Form(_lib.FORM_P_INJECT, transfer=True),
           "spectral_helmholtz": _Form(_lib.FORM_SPECTRAL_HELMHOLTZ, gll=True),
-          "spectral_helmholtz_coef": _Form(_lib.FORM_SPECTRAL_HELMHOLTZ_COEF, coefficient=True, gll=True)}
+          "spectral_helmholtz_coef": _Form(_lib.FORM_SPECTRAL_HELMHOLTZ_COEF, coefficient=True, gll=True),
+          "mixed_poisson": _Form(_lib.FORM_MIXED_POISSON, hdiv=True),
+          "mixed_poisson_schur": _Form(_lib.FORM_MIXED_POISSON_SCHUR, hdiv=True)}
 _INTEGRALS = {"cell": _lib.INTEGRAL_CELL, "exterior_facet": _lib.INTEGRAL_EXTERIOR_FACET,
               "interior_facet": _lib.INTEGRAL_INTERIOR_FACET, "fused": _lib.INTEGRAL_FUSED}
 
@@ -1646,6 +1666,8 @@ class GlobalKernel:
             return h
         if _FORMS[lk.form].transfer:
             return self._compile_transfer()
+        if _FORMS[lk.form].hdiv:
+            return self._compile_hdiv()
         el = lk.element or (interval_element(lk.degree, quadrature="gll") if _FORMS[lk.form].gll
                              else interval_element(lk.degree))
         n = lk.degree + 1
@@ -1748,6 +1770,54 @@ class GlobalKernel:
             keep = [of, oc]
             d.offset0 = of.ctypes.data_as(C.POINTER(C.c_int32))
             s2.offset = oc.ctypes.data_as(C.POINTER(C.c_int32))
+        h = C.c_void_p()
+        _lib.check(_lib.lib().fdb_kernel_create_mixed(C.byref(d), C.byref(s2), C.byref(h)), "fdb_kernel_create_mixed")
+        del keep
+        self._handle = h
+        return h
+
+    def _compile_hdiv(self):
+        """fdb_kernel_create_mixed of a mixed Poisson form: the descriptor is NCF_k (degree k, nq = k+1, B / D the
+        CG_k tables at the Gauss points), the second space DQ_{k-1} (its Gauss-Legendre basis at the same points).
+        ``arguments``: the NCF, coordinate and DQ maps ("mixed_poisson", whatever the mode) or the DQ and NCF maps
+        ("mixed_poisson_schur")."""
+        from .fiat_lite import interval_element
+        lk = self.local_kernel
+        k = lk.degree
+        el = lk.element or interval_element(k)
+        d = _lib.KernelDesc()
+        d.form, d.rank, d.integral = _FORMS[lk.form].enum, lk.rank, _lib.INTEGRAL_CELL
+        d.cell = _lib.CELL_HEX_EXTRUDED if self.extruded else _lib.CELL_HEX
+        d.degree, d.nq, d.cdim = k, el.nq, lk.cdim
+        d.scatter = {"atomic": _lib.SCATTER_ATOMIC, "coloured": _lib.SCATTER_COLOURED}[self.scatter]
+        d.alpha, d.diagonal, d.affine_cells = lk.alpha, int(lk.diagonal), int(lk.affine)
+        n = k + 1
+        for q in range(el.nq):
+            d.wq[q], d.xq[q] = el.wq[q], el.xq[q]
+            for a in range(min(n, el.ndof)):
+                d.B[q * n + a] = el.B[q, a]
+                d.D[q * n + a] = el.D[q, a]
+        s2 = _lib.Space2Desc()
+        s2.degree = k - 1
+        if k >= 2:
+            elq = interval_element(k - 1, el.nq, "gl")
+            for q in range(el.nq):
+                for a in range(k):
+                    s2.B[q * k + a] = elq.B[q, a]
+        if lk.form == "mixed_poisson":
+            ms, mc, mu = self.arguments[0], self.arguments[1], self.arguments[2]
+        else:
+            mu, ms, mc = self.arguments[0], self.arguments[1], None
+        keep = []
+        if self.extruded:
+            if ms.offset is None or mu.offset is None or (mc is not None and mc.offset is None):
+                raise MapValueError("extruded parloop needs maps with offsets")
+            keep = [np.ascontiguousarray(m.offset, dtype=IntType) for m in (ms, mu)]
+            d.offset0 = keep[0].ctypes.data_as(C.POINTER(C.c_int32))
+            s2.offset = keep[1].ctypes.data_as(C.POINTER(C.c_int32))
+            if mc is not None:
+                keep.append(np.ascontiguousarray(mc.offset, dtype=IntType))
+                d.offset1 = keep[2].ctypes.data_as(C.POINTER(C.c_int32))
         h = C.c_void_p()
         _lib.check(_lib.lib().fdb_kernel_create_mixed(C.byref(d), C.byref(s2), C.byref(h)), "fdb_kernel_create_mixed")
         del keep

@@ -268,6 +268,9 @@ class FDMStar:
                                       f"alpha*kappa*grad.grad + beta*mass with the Gauss rule), not "
                                       f"{type(form).__name__}{' with ds terms' if type(form) is Form else ''}")
         V = form.V
+        if getattr(V, "family", "CG") == "NCF":
+            raise NotImplementedError("FDMStar does not take NCF (H(div)) spaces: the only form on NCF is "
+                                      "MixedPoisson")
         if getattr(V, "family", "CG") != "CG" or V.cdim != 1:
             raise NotImplementedError("FDMStar: scalar CG spaces only")
         if V.dof_dset.halo is not None:

@@ -202,6 +202,13 @@ class ExtrudedHexMesh:
             cache[degree] = ExtrudedDGFunctionSpace(self, degree)
         return cache[degree]
 
+    def hdiv_function_space(self, degree: int) -> "ExtrudedHDivFunctionSpace":
+        """NCF_k (k = 2..4), Firedrake's H(div) element on hexahedra in its default "spectral" variant."""
+        cache = self.__dict__.setdefault("_hdiv_fs_cache", {})
+        if degree not in cache:
+            cache[degree] = ExtrudedHDivFunctionSpace(self, degree)
+        return cache[degree]
+
     def _apply_warp(self, X):
         if self.warp == 0.0:
             return X
@@ -434,6 +441,100 @@ class ExtrudedDGFunctionSpace:
     def boundary_nodes(self, sub_domain):
         raise ValueError("a DQ space has no boundary nodes: every dof is interior to its cell.  Impose Dirichlet "
                          "conditions weakly (InteriorPenalty's weak_bcs and nitsche_load)")
+
+
+class ExtrudedHDivFunctionSpace:
+    """NCF_k (k = 2..4) on an :class:`ExtrudedHexMesh`: Firedrake's H(div) element on hexahedra in its default
+    "spectral" variant.  Component d of the reference field (the contravariant Piola pull-back sigma^ = det J J^-1
+    sigma) is CG_k on GLL nodes along axis d times DG_{k-1} on Gauss-Legendre nodes along the other two axes; a dof
+    is the value of one component at its node.
+
+    Local numbering is component-major: block d holds n0*n1*n2 dofs (n_d = k+1, the others k), index
+    ``(i0*n1 + i1)*n2 + i2`` with the CG index in FIAT entity order (0 at 0, 1 at 1, then the interior nodes) and
+    the GL indices in ascending position.  Arity 3 k^2 (k+1).
+
+    Global numbering follows :class:`ExtrudedFunctionSpace`'s entity columns in first-touch order: an x-normal
+    vertical face belongs to its base y-edge, a y-normal one to its base x-edge (``nz * k^2`` dofs per column), and a
+    base face holds its horizontal faces and the cell interiors as ``[hface_0, interior_0, hface_1, ..., hface_nz]``
+    (k^2 per face, 3 (k-1) k^2 per interior).  Every local dof has a constant layer offset.  All cells have the
+    reference orientation of the structured mesh, so two cells sharing a face parametrise it alike and see the same
+    sigma^.n^: no sign flips are needed."""
+
+    def __init__(self, mesh: ExtrudedHexMesh, degree: int):
+        k = int(degree)
+        if not 2 <= k <= 4:
+            raise ValueError(f"NCF degree {k} outside 2..4")
+        self.mesh = mesh
+        self.degree = k
+        self.arity = 3 * k * k * (k + 1)
+        nz = mesh.nz
+        NV, NEy, NEx, NF = mesh._nent
+        k2 = k * k
+        self.layer_stride = (3 * k - 2) * k2                       # hface + interior per layer of a base face
+        colsize = np.concatenate([np.zeros(NV, dtype=np.int64), np.full(NEy + NEx, nz * k2, dtype=np.int64),
+                                  np.full(NF, nz * self.layer_stride + k2, dtype=np.int64)])
+        order = np.argsort(mesh._rank, kind="stable")
+        start_sorted = np.concatenate([[0], np.cumsum(colsize[order])[:-1]])
+        ent_start = np.empty(mesh.num_entities, dtype=np.int64)
+        ent_start[order] = start_sorted
+        self._ent_start, self._ent_colsize = ent_start, colsize
+        self.node_count = int(colsize.sum())
+        self.owned_node_count, self.ghost_node_count = self.node_count, 0
+        if self.node_count >= 2 ** 31:
+            raise ValueError("node count exceeds int32 IntType")
+        ix, iy = mesh.cell_ix, mesh.cell_iy
+        cmap = np.empty((mesh.num_base_cells, self.arity), dtype=np.int64)
+        off = np.empty(self.arity, dtype=IntType)
+        face = ent_start[mesh._face(ix, iy)]
+        loc = 0
+        for d in range(3):
+            dims = [k + 1 if e == d else k for e in range(3)]
+            for i0 in range(dims[0]):
+                for i1 in range(dims[1]):
+                    for i2 in range(dims[2]):
+                        idx = (i0, i1, i2)
+                        a = idx[d]
+                        t0, t1 = [idx[e] for e in range(3) if e != d]   # the two GL indices, axis order
+                        within = t0 * k + t1
+                        if a >= 2:
+                            cmap[:, loc] = face + k2 + (d * (k - 1) + a - 2) * k2 + within
+                            off[loc] = self.layer_stride
+                        elif d == 2:
+                            cmap[:, loc] = face + a * self.layer_stride + within
+                            off[loc] = self.layer_stride
+                        else:
+                            ent = mesh._yedge(ix + a, iy) if d == 0 else mesh._xedge(ix, iy + a)
+                            cmap[:, loc] = ent_start[ent] + within
+                            off[loc] = k2
+                        loc += 1
+        self.cell_node_map = cmap.astype(IntType)
+        self.offset = off
+
+    def full_cell_node_list(self):
+        """(num_cells, arity) map with the layer loop expanded: row ``c*nz + l`` is column c, layer l."""
+        nz = self.mesh.nz
+        lay = np.arange(nz, dtype=np.int64)
+        full = (self.cell_node_map[:, None, :].astype(np.int64)
+                + lay[None, :, None] * self.offset[None, None, :])
+        return full.reshape(-1, self.arity).astype(IntType)
+
+    def boundary_nodes(self, sub_domain):
+        """The face dofs on a boundary: sub-domains 1..4 (x == 0, x == Lx, y == 0, y == Ly) and "bottom" / "top".
+        A DirichletBC on them is the flux condition sigma.n = 0."""
+        mesh, k2 = self.mesh, self.degree ** 2
+        nx, ny = mesh.nx, mesh.ny
+        if sub_domain in ("bottom", "top"):
+            st = self._ent_start[mesh._face(mesh.cell_ix, mesh.cell_iy)]
+            if sub_domain == "top":
+                st = st + mesh.nz * self.layer_stride
+            return np.sort((st[:, None] + np.arange(k2)[None, :]).ravel()).astype(IntType)
+        ents = {1: lambda: mesh._yedge(0, np.arange(ny)), 2: lambda: mesh._yedge(nx, np.arange(ny)),
+                3: lambda: mesh._xedge(np.arange(nx), 0), 4: lambda: mesh._xedge(np.arange(nx), ny)}
+        if sub_domain not in ents:
+            raise ValueError(f"unknown sub_domain {sub_domain!r}")
+        e = np.atleast_1d(ents[sub_domain]())
+        st, sz = self._ent_start[e], self._ent_colsize[e]
+        return np.sort(np.concatenate([np.arange(a, a + b) for a, b in zip(st, sz)])).astype(IntType)
 
 
 class UnitSquareTriMesh:

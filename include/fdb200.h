@@ -345,7 +345,7 @@ enum fdb_form {
                                                                             coloured is bit-reproducible)
                                      P_INJECT    [coarse WRITE, fine]       maps [coarse map, fine map]  */
     FDB_FORM_SPECTRAL_HELMHOLTZ = 20,
-    FDB_FORM_SPECTRAL_HELMHOLTZ_COEF = 21
+    FDB_FORM_SPECTRAL_HELMHOLTZ_COEF = 21,
                                 /* the spectral-element (SEM) Helmholtz operator on scalar CG_p, integrated
                                    with the GLL rule at the nodes themselves (mass lumping):
                                      alpha*inner(kappa*grad u, grad v)*dx(GLL) + beta*inner(u, v)*dx(GLL)
@@ -363,6 +363,37 @@ enum fdb_form {
                                                [y INC, coords, u, kappa]     SPECTRAL_HELMHOLTZ_COEF
                                      diagonal  [d INC, coords]               SPECTRAL_HELMHOLTZ
                                                [d INC, coords, kappa]        SPECTRAL_HELMHOLTZ_COEF      */
+    FDB_FORM_MIXED_POISSON = 22,
+                                /* mixed Poisson / Darcy on the H(div) pair NCF_k x DQ_{k-1} (k = 2..4; Firedrake's
+                                   "spectral" variants), symmetric and indefinite:
+                                     a((sigma, u), (tau, v)) = alpha*dot(sigma, tau)*dx + div(tau)*u*dx
+                                                               + div(sigma)*v*dx
+                                   A flux dof is one component of sigma^ = det J J^-1 sigma (the contravariant Piola
+                                   pull-back) at its node; component d is CG_k on GLL nodes along axis d and DG_{k-1}
+                                   on Gauss-Legendre nodes along the other two.  Local numbering component-major,
+                                   block d index (i0*n1 + i1)*n2 + i2 with n_d = k+1, n_e = k, the CG index in 1-D dof
+                                   numbering (0 at 0, 1 at 1, then the interior): arity 3 k^2 (k+1).  The descriptor
+                                   is NCF_k: degree k, cdim 1, nq == k+1, B / D the CG_k tables at the Gauss points,
+                                   offset0 the NCF map's layer offsets; fdb_space2_desc is DQ_{k-1}: degree k-1, B its
+                                   Gauss-Legendre basis at the same points (nq, k), offset the DQ map's.  det J > 0 is
+                                   assumed (the Piola identities then take det J out of B).  Rank 1 only, affine_cells
+                                   0, created by fdb_kernel_create_mixed; device mode, atomic or coloured scatter
+                                   (coloured is bit-reproducible), extruded and native hexes:
+                                     action    [y_sigma INC, coords, sigma, y_u INC, u]
+                                               maps [NCF map, coord map, DQ map]
+                                               y_sigma += alpha M sigma + B^T u,  y_u += B sigma
+                                     diagonal  [d INC, coords]   maps [NCF map, coord map]
+                                               d += diag(alpha M), one value per flux dof               */
+    FDB_FORM_MIXED_POISSON_SCHUR = 23
+                                /* the selfp Schur complement of FDB_FORM_MIXED_POISSON, S_p = B W B^T with W a
+                                   diagonal given as one value per flux dof (diag(alpha M)^-1, zero on flux-condition
+                                   rows).  Metric-free: no coordinates.  Same descriptor, second space, restrictions
+                                   and creation as FDB_FORM_MIXED_POISSON (alpha is not read):
+                                     action    [y_u INC, u, w, t INC]   maps [DQ map, NCF map]
+                                               t += B^T u (over the cells), then y_u += B (w o t) (a second pass):
+                                               y_u += S_p u when t is zero on entry
+                                     diagonal  [d INC, w]   maps [DQ map, NCF map]
+                                               d += diag(B W B^T), one pass                            */
 };
 
 enum fdb_cell {
@@ -453,7 +484,7 @@ typedef struct fdb_kernel_s *fdb_kernel_t;
  * kernel instantiation.  Fails (nonzero) for forms outside the supported set. */
 int fdb_kernel_create(const fdb_kernel_desc *desc, fdb_kernel_t *out);
 /* The same for a form on two spaces (FDB_FORM_STOKES, FDB_FORM_NAVIER_STOKES[_JACOBIAN], the
- * p-multigrid transfers FDB_FORM_P_*), which
+ * p-multigrid transfers FDB_FORM_P_*, FDB_FORM_MIXED_POISSON[_SCHUR]), which
  * fdb_kernel_create refuses; a form on one
  * space is refused here. */
 int fdb_kernel_create_mixed(const fdb_kernel_desc *desc, const fdb_space2_desc *space2, fdb_kernel_t *out);
