@@ -38,6 +38,8 @@ FORM_SPECTRAL_HELMHOLTZ = 20           # alpha*inner(grad u, grad v)*dx(GLL) + b
 FORM_SPECTRAL_HELMHOLTZ_COEF = 21      # the same with a trailing nodal kappa in the stiffness term
 FORM_MIXED_POISSON = 22                # alpha*dot(sigma, tau)*dx + div(tau)*u*dx + div(sigma)*v*dx on NCF_k x DQ_{k-1}
 FORM_MIXED_POISSON_SCHUR = 23          # its selfp Schur complement B W B^T (metric-free)
+FORM_BOUSSINESQ = 24                   # Navier-Stokes + buoyancy + temperature advection-diffusion (Rayleigh-Benard)
+FORM_BOUSSINESQ_JACOBIAN = 25          # its exact Gateaux derivative at (u0, T0)
 CELL_HEX_EXTRUDED = 1
 CELL_HEX = 2
 CELL_TRIANGLE = 3

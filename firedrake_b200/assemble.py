@@ -782,6 +782,173 @@ def assemble_navier_stokes_generic(F: "NavierStokes", up: op2.MixedDat, w: op2.M
     return tensor
 
 
+def boussinesq_kernel(degree, Ra, Pr, g=(0.0, 0.0, -1.0), jacobian=False, name=None):
+    """C source of the Boussinesq residual of :class:`Boussinesq` on Taylor-Hood Q_p-Q_(p-1) hexahedra with the
+    temperature in CG_(p-1) (arguments: y (INC) and upT, each the velocity's 3 END values (AoS), then the pressure's
+    and the temperature's (EN-1)^3, and the coordinates), or with ``jacobian`` of its Gateaux derivative's action at
+    (u0, T0) on (w, r, s) (arguments: y (INC), coords, wrs, u0 (3 END values), T0 ((EN-1)^3 values)).  The
+    independent statement of the hand-written FDB_FORM_BOUSSINESQ[_JACOBIAN] kernels, run through the generic wrapper
+    builder; the temperature is held like the pressure in an EN^3 block with a zero-padded table."""
+    from .codegen import CStringKernel
+    from .fiat_lite import interval_element
+    if not 2 <= degree <= 4:
+        raise NotImplementedError(f"the generic-path Boussinesq statement covers degrees 2..4, got degree {degree}")
+    if name is None:
+        name = "boussinesq_jacobian_action" if jacobian else "boussinesq_residual"
+    elq = interval_element(degree - 1, degree + 1)
+    n = degree + 1
+    bq = [[float(elq.B[q, a]) if a < n - 1 else 0.0 for a in range(n)] for q in range(n)]
+    dq = [[float(elq.D[q, a]) if a < n - 1 else 0.0 for a in range(n)] for q in range(n)]
+    table = lambda t: "{" + ", ".join("{" + ", ".join(repr(v) for v in r) + "}" for r in t) + "}"
+    bg = [float(Ra) / float(Pr) * float(c) for c in g]
+    kt = 1.0 / float(Pr)
+    args = ("double *y, const double *X, const double *up, const double *u, const double *tl" if jacobian else
+            "double *y, const double *X, const double *up")
+    # the linearisation point: its velocity UL, velocity gradient GU and temperature gradient TL0; u and T
+    # themselves for the residual
+    lin = """
+        double GL[3][3], gt0[3];
+        for (int d = 0; d < 3; ++d)
+            for (int k = 0; k < 3; ++k)
+                GL[d][k] = GU[d][0][q] * Jinv[0][k] + GU[d][1][q] * Jinv[1][k] + GU[d][2][q] * Jinv[2][k];
+        for (int k = 0; k < 3; ++k) gt0[k] = GT0[0][q] * Jinv[0][k] + GT0[1][q] * Jinv[1][k] + GT0[2][q] * Jinv[2][k];
+        for (int d = 0; d < 3; ++d)
+            cv[d] = Gp[d][0] * UL[0][q] + Gp[d][1] * UL[1][q] + Gp[d][2] * UL[2][q]
+                  + GL[d][0] * U[0][q] + GL[d][1] * U[1][q] + GL[d][2] * U[2][q];
+        const double tv = wd * (UL[0][q] * gt[0] + UL[1][q] * gt[1] + UL[2][q] * gt[2]
+                                + U[0][q] * gt0[0] + U[1][q] * gt0[1] + U[2][q] * gt0[2]);""" if jacobian else """
+        for (int d = 0; d < 3; ++d) cv[d] = Gp[d][0] * U[0][q] + Gp[d][1] * U[1][q] + Gp[d][2] * U[2][q];
+        const double tv = wd * (U[0][q] * gt[0] + U[1][q] * gt[1] + U[2][q] * gt[2]);"""
+    gather_u = """
+        for (int i = 0; i < END; ++i) c[i] = u[i * 3 + d];
+        el_tensor(EB, EB, EB, 0, c, UL[d]);
+        el_tensor(ED, EB, EB, 0, c, GU[d][0]);
+        el_tensor(EB, ED, EB, 0, c, GU[d][1]);
+        el_tensor(EB, EB, ED, 0, c, GU[d][2]);""" if jacobian else ""
+    gather_t0 = """
+    for (int i = 0; i < END; ++i) {
+        const int a = i / (EN * EN), b = (i / EN) % EN, e = i % EN;
+        c[i] = (a < ENP && b < ENP && e < ENP) ? tl[(a * ENP + b) * ENP + e] : 0.0;
+    }
+    el_tensor(EDQ, EQ, EQ, 0, c, GT0[0]);
+    el_tensor(EQ, EDQ, EQ, 0, c, GT0[1]);
+    el_tensor(EQ, EQ, EDQ, 0, c, GT0[2]);""" if jacobian else ""
+    decl_u = "double UL[3][END], GU[3][3][END], GT0[3][END];" if jacobian else ""
+    code = _vector_hex_tables(degree) + f"""#define ENP (EN - 1)
+#define NPD (ENP * ENP * ENP)
+static const double EQ[EN][EN] = {table(bq)};      /* EQ[q][a]: CG_(p-1) basis, zero last column */
+static const double EDQ[EN][EN] = {table(dq)};     /* its derivative */
+static const double BG[3] = {{{bg[0]!r}, {bg[1]!r}, {bg[2]!r}}};
+static void {name}({args})
+{{
+    double U[3][END], G[3][3][END], c[END], t[END], P[END], T[END], TV[END], GT[3][END];
+    {decl_u}
+    const double *pin = up + 3 * END, *tin = up + 3 * END + NPD;
+    for (int d = 0; d < 3; ++d) {{
+        for (int i = 0; i < END; ++i) c[i] = up[i * 3 + d];
+        el_tensor(EB, EB, EB, 0, c, U[d]);
+        el_tensor(ED, EB, EB, 0, c, G[d][0]);
+        el_tensor(EB, ED, EB, 0, c, G[d][1]);
+        el_tensor(EB, EB, ED, 0, c, G[d][2]);{gather_u}
+    }}
+    for (int i = 0; i < END; ++i) {{
+        const int a = i / (EN * EN), b = (i / EN) % EN, e = i % EN;
+        c[i] = (a < ENP && b < ENP && e < ENP) ? pin[(a * ENP + b) * ENP + e] : 0.0;
+    }}
+    el_tensor(EQ, EQ, EQ, 0, c, P);
+    for (int i = 0; i < END; ++i) {{
+        const int a = i / (EN * EN), b = (i / EN) % EN, e = i % EN;
+        c[i] = (a < ENP && b < ENP && e < ENP) ? tin[(a * ENP + b) * ENP + e] : 0.0;
+    }}
+    el_tensor(EQ, EQ, EQ, 0, c, TV);
+    el_tensor(EDQ, EQ, EQ, 0, c, GT[0]);
+    el_tensor(EQ, EDQ, EQ, 0, c, GT[1]);
+    el_tensor(EQ, EQ, EDQ, 0, c, GT[2]);{gather_t0}
+    for (int qx = 0; qx < EN; ++qx) for (int qy = 0; qy < EN; ++qy) for (int qz = 0; qz < EN; ++qz) {{
+        const int q = (qx * EN + qy) * EN + qz;
+        const double xi[3] = {{EX[qx], EX[qy], EX[qz]}};
+        double J[3][3] = {{{{0}}}};
+        for (int v = 0; v < 8; ++v) {{
+            const int b[3] = {{(v >> 2) & 1, (v >> 1) & 1, v & 1}};
+            for (int r = 0; r < 3; ++r) {{
+                double g = b[r] ? 1.0 : -1.0;
+                for (int e = 0; e < 3; ++e) if (e != r) g *= b[e] ? xi[e] : 1.0 - xi[e];
+                for (int k = 0; k < 3; ++k) J[k][r] += X[v * 3 + k] * g;
+            }}
+        }}
+        const double det = J[0][0] * (J[1][1] * J[2][2] - J[1][2] * J[2][1])
+                         - J[0][1] * (J[1][0] * J[2][2] - J[1][2] * J[2][0])
+                         + J[0][2] * (J[1][0] * J[2][1] - J[1][1] * J[2][0]);
+        double Jinv[3][3];
+        Jinv[0][0] = (J[1][1] * J[2][2] - J[1][2] * J[2][1]) / det;
+        Jinv[0][1] = (J[0][2] * J[2][1] - J[0][1] * J[2][2]) / det;
+        Jinv[0][2] = (J[0][1] * J[1][2] - J[0][2] * J[1][1]) / det;
+        Jinv[1][0] = (J[1][2] * J[2][0] - J[1][0] * J[2][2]) / det;
+        Jinv[1][1] = (J[0][0] * J[2][2] - J[0][2] * J[2][0]) / det;
+        Jinv[1][2] = (J[0][2] * J[1][0] - J[0][0] * J[1][2]) / det;
+        Jinv[2][0] = (J[1][0] * J[2][1] - J[1][1] * J[2][0]) / det;
+        Jinv[2][1] = (J[0][1] * J[2][0] - J[0][0] * J[2][1]) / det;
+        Jinv[2][2] = (J[0][0] * J[1][1] - J[0][1] * J[1][0]) / det;
+        const double wd = EW[qx] * EW[qy] * EW[qz] * fabs(det);
+        double Gp[3][3], S[3][3], cv[3], gt[3];
+        for (int d = 0; d < 3; ++d)
+            for (int k = 0; k < 3; ++k)
+                Gp[d][k] = G[d][0][q] * Jinv[0][k] + G[d][1][q] * Jinv[1][k] + G[d][2][q] * Jinv[2][k];
+        for (int k = 0; k < 3; ++k) gt[k] = GT[0][q] * Jinv[0][k] + GT[1][q] * Jinv[1][k] + GT[2][q] * Jinv[2][k];{lin}
+        for (int d = 0; d < 3; ++d)
+            for (int k = 0; k < 3; ++k)
+                S[d][k] = Gp[d][k] - (d == k ? P[q] : 0.0);
+        for (int d = 0; d < 3; ++d)
+            for (int m = 0; m < 3; ++m)
+                G[d][m][q] = wd * (Jinv[m][0] * S[d][0] + Jinv[m][1] * S[d][1] + Jinv[m][2] * S[d][2]);
+        for (int m = 0; m < 3; ++m)
+            GT[m][q] = {kt!r} * wd * (Jinv[m][0] * gt[0] + Jinv[m][1] * gt[1] + Jinv[m][2] * gt[2]);
+        for (int d = 0; d < 3; ++d) U[d][q] = wd * (cv[d] - BG[d] * TV[q]);
+        T[q] = -wd * (Gp[0][0] + Gp[1][1] + Gp[2][2]);
+        TV[q] = tv;
+    }}
+    for (int d = 0; d < 3; ++d) {{
+        el_tensor(EB, EB, EB, 1, U[d], c);
+        el_tensor(ED, EB, EB, 1, G[d][0], t);  for (int i = 0; i < END; ++i) c[i] += t[i];
+        el_tensor(EB, ED, EB, 1, G[d][1], t);  for (int i = 0; i < END; ++i) c[i] += t[i];
+        el_tensor(EB, EB, ED, 1, G[d][2], t);  for (int i = 0; i < END; ++i) c[i] += t[i];
+        for (int i = 0; i < END; ++i) y[i * 3 + d] += c[i];
+    }}
+    el_tensor(EQ, EQ, EQ, 1, T, c);
+    for (int a = 0; a < ENP; ++a) for (int b = 0; b < ENP; ++b) for (int e = 0; e < ENP; ++e)
+        y[3 * END + (a * ENP + b) * ENP + e] += c[(a * EN + b) * EN + e];
+    el_tensor(EQ, EQ, EQ, 1, TV, c);
+    el_tensor(EDQ, EQ, EQ, 1, GT[0], t);  for (int i = 0; i < END; ++i) c[i] += t[i];
+    el_tensor(EQ, EDQ, EQ, 1, GT[1], t);  for (int i = 0; i < END; ++i) c[i] += t[i];
+    el_tensor(EQ, EQ, EDQ, 1, GT[2], t);  for (int i = 0; i < END; ++i) c[i] += t[i];
+    for (int a = 0; a < ENP; ++a) for (int b = 0; b < ENP; ++b) for (int e = 0; e < ENP; ++e)
+        y[3 * END + NPD + (a * ENP + b) * ENP + e] += c[(a * EN + b) * EN + e];
+}}
+#undef NPD
+#undef ENP
+#undef END
+#undef EN
+"""
+    return CStringKernel(code, name)
+
+
+def assemble_boussinesq_generic(F: "Boussinesq", upT: op2.MixedDat, w: op2.MixedDat = None, tensor=None):
+    """The residual R(upT) of :class:`Boussinesq` (``w`` None) or the Jacobian action J(upT[0], upT[2]) w through the
+    generic wrapper path (:func:`boussinesq_kernel`): the cross-check and the baseline of the hand-written kernels."""
+    V = F.V
+    if tensor is None:
+        tensor = F.dat()
+    tensor.zero()
+    for d in tensor:
+        d.device_ptr
+    mm = op2.MixedMap(F.block_maps)
+    k = boussinesq_kernel(V.degree, F.Ra, F.Pr, F.g, jacobian=w is not None)
+    ins = ([w(op2.READ, mm), upT[0](op2.READ, V.cell_node_map), upT[2](op2.READ, F.temperature_map)]
+           if w is not None else [upT(op2.READ, mm)])
+    op2.par_loop(k, V.cell_set, tensor(op2.INC, mm), V.coordinates(op2.READ, V.coord_map), *ins)
+    return tensor
+
+
 def advection_diffusion_kernel(degree, alpha=1.0, beta=0.0, name="advection_diffusion_action"):
     """C source of the 1-form ``action(alpha*inner(grad(u), grad(v))*dx + inner(dot(b, grad(u)), v)*dx +
     beta*inner(u, v)*dx, u)`` on the scalar Q_p (x) P_p space, with the velocity b of 3 values per node
@@ -2800,14 +2967,161 @@ class NavierStokesJacobian:
         return op2.Kernel("navier_stokes_jacobian", degree=self.V.degree, mu=self.nu, beta=self.beta)
 
 
+def _temperature_map(V, Q, W, pressure_map):
+    """Check Boussinesq's temperature space ``W`` (a FunctionSpace object of its own, with the mesh, degree and
+    numbering of the pressure space ``Q``) and return its map on the velocity space's cell set, an alias of the
+    pressure map: the kernel reads T through Q's map."""
+    if W is Q:
+        raise ValueError("Boussinesq's temperature space W must be a FunctionSpace object of its own, not the "
+                         "pressure space Q, so that DirichletBC(W, ...) is a temperature condition")
+    if W.mesh is not Q.mesh or W.degree != Q.degree or W.cdim != 1 or getattr(W, "family", "CG") != "CG":
+        raise ValueError(f"Boussinesq's temperature space is scalar CG_(p-1) on the pressure space's mesh: got "
+                         f"{getattr(W, 'family', 'CG')} degree {W.degree}, cdim {W.cdim} for pressure degree "
+                         f"{Q.degree}")
+    if W.dof_dset.halo is not None or W.cell_set.owner_computes:
+        raise NotImplementedError("Boussinesq on a partitioned mesh is not implemented: the velocity, pressure "
+                                  "and temperature node sets need their own halo design")
+    same = (W.node_count == Q.node_count and W.V.arity == Q.V.arity and
+            np.array_equal(np.asarray(W.V.cell_node_map), np.asarray(Q.V.cell_node_map)) and
+            np.array_equal(np.asarray(W.V.offset), np.asarray(Q.V.offset)))
+    if not same:
+        raise ValueError("Boussinesq's temperature space must have the pressure space's numbering: the kernel "
+                         "reads T through the pressure map")
+    return op2.Map(V.cell_set, W.node_set, W.V.arity, W.V.cell_node_map, offset=W.V.offset, alias_of=pressure_map)
+
+
+@dataclass
+class Boussinesq:
+    """The residual of the Boussinesq approximation (Rayleigh-Benard convection, Firedrake's matrix-free
+    rayleigh-benard demo) on Taylor-Hood hexahedra: velocity ``V`` (vector CG_p), pressure ``Q`` (CG_{p-1}) and
+    temperature ``W`` (CG_{p-1}, a FunctionSpace object of its own with the numbering of ``Q``), p = 2..4:
+
+        R((u, p, T); (v, q, S)) = inner(grad u, grad v)*dx + inner(dot(grad u, u), v)*dx - p*div(v)*dx
+                                  - (Ra/Pr)*T*inner(g, v)*dx - q*div(u)*dx
+                                  + dot(grad T, u)*S*dx + (1/Pr)*inner(grad T, grad S)*dx
+
+    with the Stokes sign convention of :class:`NavierStokes` (the demo writes ``+ q*div(u)``, the same solution), so
+    that at Ra = 0 the (u, p) rows are ``NavierStokes(V, Q, nu=1)``.  ``g`` is a constant 3-vector, "down" the
+    extruded layers by default.  Vectors are 3-block MixedDats, ``F.dat(u, p, T)``; ``assemble(F, u=upT)`` is R,
+    ``F.jacobian(upT)`` the exact Newton Jacobian (reading upT[0] and upT[2] in place), and :func:`solve_nonlinear`
+    runs Newton with the demo's multiplicative fieldsplit.  A DirichletBC acts on the block of its space: on ``V``
+    the velocity, on ``W`` the temperature.  The (p+1)-point Gauss rule does not integrate the convective terms
+    exactly."""
+    V: FunctionSpace
+    Q: FunctionSpace
+    W: FunctionSpace
+    Ra: float
+    Pr: float
+    g: tuple = (0.0, 0.0, -1.0)
+    symmetric = False
+
+    def __post_init__(self):
+        for S in (self.V, self.Q, self.W):
+            _refuse_dq(S, "Boussinesq")
+            _refuse_ncf(S, "Boussinesq")
+        self.g = tuple(float(c) for c in self.g)
+        if len(self.g) != 3:
+            raise ValueError("g is a constant 3-vector")
+        if self.Pr == 0:
+            raise ValueError("the Prandtl number Pr must be nonzero")
+        self.pressure_map = _taylor_hood_pressure_map(self.V, self.Q, "Boussinesq")
+        self.temperature_map = _temperature_map(self.V, self.Q, self.W, self.pressure_map)
+
+    @property
+    def spaces(self):
+        return (self.V, self.Q, self.W)
+
+    @property
+    def block_maps(self):
+        return (self.V.cell_node_map, self.pressure_map, self.temperature_map)
+
+    @property
+    def bg(self):
+        """The buoyancy vector (Ra/Pr) g."""
+        return tuple(self.Ra / self.Pr * c for c in self.g)
+
+    @property
+    def kt(self):
+        return 1.0 / self.Pr
+
+    def dat(self, u=None, p=None, T=None):
+        """A (velocity, pressure, temperature) vector: ``op2.MixedDat([V.dat(u), Q.dat(p), W.dat(T)])``."""
+        return op2.MixedDat([self.V.dat(u), self.Q.dat(p), self.W.dat(T)])
+
+    def coefficient_args(self):
+        return []
+
+    def kernel(self, rank=1, diagonal=False):
+        if rank != 1 or diagonal:
+            raise ValueError("the Boussinesq residual is a 1-form: its operator is F.jacobian(upT), a matrix-free "
+                             "action")
+        return op2.Kernel("boussinesq", degree=self.V.degree, mu=1.0, beta=0.0, bg=self.bg, kt=self.kt)
+
+    def jacobian(self, upT: op2.MixedDat):
+        """The Gateaux derivative at (``upT[0]``, ``upT[2]``), read in place (a nonsymmetric bilinear form)."""
+        return BoussinesqJacobian(self, upT[0], upT[2])
+
+
+@dataclass
+class BoussinesqJacobian:
+    """J(u0, T0)[(w, r, s); (v, q, S)] = NavierStokesJacobian(V, Q, 1, 0, u0)[(w, r); (v, q)] - (Ra/Pr)*s*inner(g,
+    v)*dx + (dot(grad s, u0) + dot(grad T0, w))*S*dx + (1/Pr)*inner(grad s, grad S)*dx: the exact Newton Jacobian
+    of :class:`Boussinesq`, a nonsymmetric bilinear form on 3-block MixedDats (``assemble(J, u=wrs)``,
+    ``assemble(J, mat_type="matfree")``; no assembled matrix).  ``u0`` is read through the velocity map, ``T0``
+    through the pressure map."""
+    form: Boussinesq
+    u0: op2.Dat
+    T0: op2.Dat
+    symmetric = False
+
+    def __post_init__(self):
+        F = self.form
+        self.V, self.Q, self.W = F.V, F.Q, F.W
+        self.pressure_map, self.temperature_map = F.pressure_map, F.temperature_map
+
+    spaces = Boussinesq.spaces
+    block_maps = Boussinesq.block_maps
+    dat = Boussinesq.dat
+
+    def coefficient_args(self):
+        return [self.u0(op2.READ, self.V.cell_node_map), self.T0(op2.READ, self.temperature_map)]
+
+    def kernel(self, rank=1, diagonal=False):
+        if rank != 1 or diagonal:
+            raise NotImplementedError("the Boussinesq Jacobian is an action only: there is no assembled matrix or "
+                                      "diagonal (use mat_type='matfree')")
+        F = self.form
+        return op2.Kernel("boussinesq_jacobian", degree=self.V.degree, mu=1.0, beta=0.0, bg=F.bg, kt=F.kt)
+
+
 _TAYLOR_HOOD_FORMS = (Stokes, NavierStokes, NavierStokesJacobian)
 
 
+def _block_maps(F):
+    """The maps of the blocks of a mixed form's vectors: the first space's, the second space's and, for
+    :class:`Boussinesq`, the temperature's."""
+    return getattr(F, "block_maps", None) or (F.V.cell_node_map, F.pressure_map)
+
+
+def _bc_block(F, bc):
+    """The block of a mixed form's vectors that ``bc`` constrains: the one whose space is ``bc.V``.  A form on two
+    spaces that does not name its spaces constrains its first block."""
+    spaces = getattr(F, "spaces", None)
+    if spaces is None:
+        return 0
+    for i, S in enumerate(spaces):
+        if bc.V is S:
+            return i
+    raise ValueError(f"DirichletBC on a space that is not one of {type(F).__name__}'s: give it the form's own "
+                     f"FunctionSpace object")
+
+
 class StokesAssembler:
-    """Cached assembler of the action (velocity, pressure) -> (y_u, y_p) on MixedDats of a form on the
-    Taylor-Hood pair (:class:`Stokes`, :class:`NavierStokes`, :class:`NavierStokesJacobian`), the counterpart
-    of :class:`OneFormAssembler`: the parloop is built once and re-run; the form's coefficients (the Jacobian's
-    u) follow the pressure."""
+    """Cached assembler of the action (velocity, pressure[, temperature]) -> (y_u, y_p[, y_T]) on MixedDats of a
+    form on the Taylor-Hood pair (:class:`Stokes`, :class:`NavierStokes`, :class:`NavierStokesJacobian`,
+    :class:`Boussinesq`, :class:`BoussinesqJacobian`, and :class:`MixedPoisson`), the counterpart of
+    :class:`OneFormAssembler`: the parloop is built once and re-run; the form's coefficients (a Jacobian's
+    linearisation point) come last.  Each DirichletBC zeroes the rows of the block whose space is its own."""
 
     def __init__(self, form: Stokes, up: op2.MixedDat, bcs=(), scatter="atomic"):
         self.form, self.up, self.bcs = form, up, tuple(bcs)
@@ -2823,24 +3137,23 @@ class StokesAssembler:
             tensor = F.dat()
         if self._loop is None or self._tensor is not tensor:
             self._tensor = tensor
-            u, p = self.up
-            yu, yp = tensor
-            self._loop = op2.Parloop(self._gk, V.cell_set,
-                                     [yu(op2.INC, V.cell_node_map), V.coordinates(op2.READ, V.coord_map),
-                                      u(op2.READ, V.cell_node_map), yp(op2.INC, F.pressure_map),
-                                      p(op2.READ, F.pressure_map)] + F.coefficient_args(), location="device")
+            maps = _block_maps(F)
+            args = [tensor[0](op2.INC, maps[0]), V.coordinates(op2.READ, V.coord_map), self.up[0](op2.READ, maps[0])]
+            for y, x, m in zip(tensor.split()[1:], self.up.split()[1:], maps[1:]):
+                args += [y(op2.INC, m), x(op2.READ, m)]
+            self._loop = op2.Parloop(self._gk, V.cell_set, args + F.coefficient_args(), location="device")
         tensor.zero()
         self._loop()
         for bc in self.bcs:
-            bc.zero(tensor[0])
+            bc.zero(tensor[_bc_block(F, bc)])
         return tensor
 
 
 class StokesMatrixContext:
-    """Matrix-free operator of a Taylor-Hood form (:class:`Stokes`, :class:`NavierStokesJacobian`) on
-    MixedDats: ``mult`` zeroes the velocity-BC entries of x, applies the saddle-point action and writes x back
-    on the constrained velocity rows (identity there).  The Stokes operator is symmetric, so ``multTranspose``
-    is ``mult``; for a nonsymmetric form it raises."""
+    """Matrix-free operator of a Taylor-Hood form (:class:`Stokes`, :class:`NavierStokesJacobian`,
+    :class:`BoussinesqJacobian`) on MixedDats: ``mult`` zeroes the BC entries of x (each condition on the block of
+    its space), applies the action and writes x back on the constrained rows (identity there).  The Stokes operator
+    is symmetric, so ``multTranspose`` is ``mult``; for a nonsymmetric form it raises."""
 
     def __init__(self, form: Stokes, bcs=()):
         self.form, self.bcs = form, tuple(bcs)
@@ -2854,10 +3167,11 @@ class StokesMatrixContext:
             _lib.check(L.fdb_memcpy_d2d(a.device_ptr, b.device_ptr, b.nbytes))
             a._device_written()
         for bc in self.bcs:
-            bc.zero(self._x[0])
+            bc.zero(self._x[_bc_block(self.form, bc)])
         self._assembler.assemble(tensor=Y)
         for bc in self.bcs:
-            bc.set(Y[0], X[0])
+            i = _bc_block(self.form, bc)
+            bc.set(Y[i], X[i])
         return Y
 
     def multTranspose(self, X: op2.MixedDat, Y: op2.MixedDat):
@@ -3211,6 +3525,16 @@ def assemble(form: Form, u=None, tensor=None, bcs=(), mat_type="aij"):
             raise NotImplementedError(f"mat_type {mat_type!r}: MixedPoisson has no assembled matrix, use mat_type "
                                       f"'matfree'")
         return MixedPoissonMatrixContext(form, bcs)
+    if isinstance(form, (Boussinesq, BoussinesqJacobian)):
+        if u is not None:
+            return StokesAssembler(form, u, bcs).assemble(tensor)
+        if isinstance(form, Boussinesq):
+            raise ValueError("the Boussinesq residual is a 1-form: assemble(F, u=upT), or its operator "
+                             "assemble(F.jacobian(upT), mat_type='matfree')")
+        if mat_type != "matfree":
+            raise NotImplementedError(f"mat_type {mat_type!r}: the Boussinesq Jacobian has no assembled matrix, use "
+                                      f"mat_type 'matfree'")
+        return StokesMatrixContext(form, bcs)
     if isinstance(form, _TAYLOR_HOOD_FORMS):
         if u is not None:
             return StokesAssembler(form, u, bcs).assemble(tensor)
@@ -3754,11 +4078,17 @@ def solve_nonlinear(F, L: op2.Dat, u: op2.Dat, bcs=(), solver_parameters=None, h
     ``Form(W, nu, beta)`` per component, ``fieldsplit_1_pc_type`` "jacobi", the pressure mass over nu), built
     once per solve.  ``nullspace`` "constant" removes the pressure mean from the residual, from every
     preconditioned vector and from the final pressure.  A non-finite residual norm ends the solve with a
-    :class:`ConvergenceError` ("DIVERGED_FNORM_NAN").  The other forms take no ``nullspace``."""
+    :class:`ConvergenceError` ("DIVERGED_FNORM_NAN").
+
+    Boussinesq (``F`` a :class:`Boussinesq`): ``L`` and ``u`` are 3-block MixedDats (velocity, pressure,
+    temperature), each DirichletBC acts on the block of its space; Newton with the multiplicative fieldsplit of
+    Firedrake's Rayleigh-Benard demo, see :func:`_solve_boussinesq`.  The other forms take no ``nullspace``."""
     from . import _lib
     from . import mg as _mg
     if isinstance(F, NavierStokes):
         return _solve_navier_stokes(F, L, u, bcs, solver_parameters, hierarchy, nullspace)
+    if isinstance(F, Boussinesq):
+        return _solve_boussinesq(F, L, u, bcs, solver_parameters, hierarchy, nullspace)
     if nullspace is not None:
         raise NotImplementedError("nullspace is implemented for Navier-Stokes forms only")
     sp = {"snes_rtol": 1e-8, "snes_atol": 1e-50, "snes_max_it": 50, "ksp_type": "gmres",
@@ -4492,6 +4822,246 @@ def _solve_navier_stokes(F: NavierStokes, L: op2.MixedDat, up: op2.MixedDat, bcs
     if nullspace:
         remove_pressure_mean(up)
     return hist, kits
+
+
+# the options of the Boussinesq Newton solve (:func:`_solve_boussinesq`), flattened, with their defaults
+_BOUSSINESQ_OPTIONS = {"snes_rtol": 1e-8, "snes_atol": 1e-50, "snes_max_it": 50, "snes_type": "newtonls",
+                       "snes_linesearch_type": "basic", "mat_type": "matfree", "ksp_type": "fgmres",
+                       "ksp_gmres_restart": 30, "ksp_rtol": 1e-5, "ksp_max_it": 10000, "pc_type": "none",
+                       "pc_fieldsplit_type": "multiplicative", "pc_fieldsplit_0_fields": "0,1",
+                       "pc_fieldsplit_1_fields": "2",
+                       "fieldsplit_0_ksp_type": "preonly", "fieldsplit_0_ksp_rtol": 1e-2,
+                       "fieldsplit_0_ksp_max_it": 1000, "fieldsplit_0_ksp_gmres_restart": 30,
+                       "fieldsplit_0_pc_type": "fieldsplit", "fieldsplit_0_pc_fieldsplit_type": "schur",
+                       "fieldsplit_0_pc_fieldsplit_schur_fact_type": "lower",
+                       "fieldsplit_0_fieldsplit_0_ksp_type": "preonly", "fieldsplit_0_fieldsplit_0_pc_type": "jacobi",
+                       "fieldsplit_0_fieldsplit_1_ksp_type": "preonly", "fieldsplit_0_fieldsplit_1_pc_type": "jacobi",
+                       "fieldsplit_1_ksp_type": "preonly", "fieldsplit_1_ksp_rtol": 1e-4,
+                       "fieldsplit_1_ksp_max_it": 1000, "fieldsplit_1_ksp_gmres_restart": 30,
+                       "fieldsplit_1_pc_type": "jacobi"}
+_ASSEMBLED_PCS = ("lu", "cholesky", "ilu", "icc", "mumps", "hypre", "gamg", "redundant")
+
+
+def _boussinesq_options(solver_parameters):
+    """The flattened options of :func:`_solve_boussinesq` with their defaults; everything that is not built is
+    refused by name."""
+    given = _flatten("", solver_parameters or {})
+    sp = dict(_BOUSSINESQ_OPTIONS)
+    for k, v in given.items():
+        if k == "snes_monitor" or k.startswith("ksp_monitor") or "_ksp_monitor" in k:
+            continue                                    # accepted and ignored
+        if k.endswith("ksp_gmres_modifiedgramschmidt"):
+            continue                                    # the engine's GMRES orthogonalises by modified Gram-Schmidt
+        if k.endswith("pc_python_type"):
+            if v == "firedrake.PCDPC":
+                raise NotImplementedError(f"{k} 'firedrake.PCDPC': the pressure convection-diffusion Schur "
+                                          f"preconditioner was measured and set aside (DESIGN.md section 4.13); use "
+                                          f"fieldsplit_0_fieldsplit_1_pc_type 'jacobi'")
+            if v == "firedrake.AssembledPC":
+                raise NotImplementedError(f"{k} 'firedrake.AssembledPC': the Boussinesq operators have no assembled "
+                                          f"matrix; use 'jacobi' or 'mg'")
+            raise NotImplementedError(f"{k} {v!r}: not implemented for Boussinesq")
+        if k.endswith("assembled_pc_type") or (k.endswith("pc_type") and v in _ASSEMBLED_PCS):
+            raise NotImplementedError(f"{k} {v!r}: there is no assembled matrix to factorise or to coarsen "
+                                      f"algebraically; use 'jacobi' or 'mg'")
+        if k not in sp:
+            raise NotImplementedError(f"unknown Boussinesq solver option {k!r}")
+        sp[k] = v
+    if sp["mat_type"] != "matfree":
+        raise NotImplementedError(f"mat_type {sp['mat_type']!r}: the Boussinesq Jacobian has no assembled matrix, "
+                                  f"use mat_type 'matfree'")
+    if sp["snes_type"] != "newtonls" or sp["snes_linesearch_type"] != "basic":
+        raise NotImplementedError("snes_type 'newtonls' with snes_linesearch_type 'basic' (the full Newton step) only")
+    if sp["ksp_type"] not in ("fgmres", "gmres"):
+        raise NotImplementedError(f"ksp_type {sp['ksp_type']!r}: 'fgmres' or 'gmres' (both the engine's flexible "
+                                  f"GMRES)")
+    if sp["pc_type"] not in ("none", "fieldsplit"):
+        raise NotImplementedError(f"pc_type {sp['pc_type']!r}: 'none' or 'fieldsplit'")
+    if sp["pc_type"] == "fieldsplit":
+        if sp["pc_fieldsplit_type"] not in ("multiplicative", "additive"):
+            raise NotImplementedError(f"pc_fieldsplit_type {sp['pc_fieldsplit_type']!r}: 'multiplicative' or "
+                                      f"'additive' over the (u, p) and T splits (not 'symmetric_multiplicative', "
+                                      f"'schur' or 'full')")
+        if str(sp["pc_fieldsplit_0_fields"]).replace(" ", "") != "0,1" or str(sp["pc_fieldsplit_1_fields"]) != "2":
+            raise NotImplementedError(f"pc_fieldsplit_0_fields {sp['pc_fieldsplit_0_fields']!r}, "
+                                      f"pc_fieldsplit_1_fields {sp['pc_fieldsplit_1_fields']!r}: the splits are "
+                                      f"'0,1' (velocity and pressure) and '2' (temperature)")
+        for f in ("0", "1"):
+            if sp[f"fieldsplit_{f}_ksp_type"] not in ("preonly", "gmres", "fgmres"):
+                raise NotImplementedError(f"fieldsplit_{f}_ksp_type {sp[f'fieldsplit_{f}_ksp_type']!r}: 'preonly' or "
+                                          f"'gmres'")
+        if sp["fieldsplit_0_pc_type"] != "fieldsplit":
+            raise NotImplementedError(f"fieldsplit_0_pc_type {sp['fieldsplit_0_pc_type']!r}: 'fieldsplit' (the "
+                                      f"Schur fieldsplit of the Navier-Stokes block)")
+        if sp["fieldsplit_1_pc_type"] not in ("jacobi", "mg"):
+            raise NotImplementedError(f"fieldsplit_1_pc_type {sp['fieldsplit_1_pc_type']!r}: 'jacobi' or 'mg'")
+    return sp
+
+
+def _solve_boussinesq(F: Boussinesq, L: op2.MixedDat, upT: op2.MixedDat, bcs=(), solver_parameters=None,
+                      hierarchy=None, nullspace=None):
+    """Newton's method for :class:`Boussinesq` (``snes_type newtonls``, ``snes_linesearch_type basic``) on R(upT) =
+    F(upT) - L over 3-block MixedDats, with the options of Firedrake's Rayleigh-Benard demo, nested or flat:
+
+    - outer ``ksp_type`` "fgmres" (default) or "gmres": both are the engine's flexible, right-preconditioned GMRES
+      with modified Gram-Schmidt (:func:`gmres`), so ``ksp_gmres_modifiedgramschmidt`` is accepted;
+      ``ksp_rtol``, ``ksp_max_it``, ``ksp_gmres_restart``.
+    - ``pc_type`` "none" (default) or "fieldsplit" with ``pc_fieldsplit_0_fields`` "0,1" and ``pc_fieldsplit_1_fields``
+      "2", combined "multiplicative" (PETSc's block Gauss-Seidel: z_0 = P_0 r_0, then z_1 = P_1 (r_1 - J_10 z_0), with
+      J_10 z_0 the temperature block of one Jacobian action on (z_u, z_p, 0)) or "additive" (z_1 = P_1 r_1).
+    - ``fieldsplit_0``: ``ksp_type`` "preonly" or "gmres" (``ksp_rtol``, ``ksp_max_it``) on the Navier-Stokes
+      Jacobian ``NavierStokesJacobian(V, Q, 1, 0, u0)``, preconditioned by the Schur fieldsplit of
+      :func:`_solve_stokes` with its options under the ``fieldsplit_0_`` prefix (factorisation "diag", "lower" or
+      "upper"; velocity "jacobi" or "mg"; pressure "jacobi").
+    - ``fieldsplit_1``: ``ksp_type`` "preonly" or "gmres" on J_TT, applied as the temperature block of the Jacobian
+      action on (0, 0, s); ``pc_type`` "jacobi" or "mg" on the symmetric part ``Form(W, 1/Pr, 0)``, as for
+      :class:`AdvectionDiffusion`.  PETSc's Jacobi would take the diagonal of J_TT itself, which adds the diagonal of
+      the advection term u0 . grad S; the symmetric part's diagonal leaves it out.
+    - ``snes_monitor`` and ``ksp_monitor*`` are accepted and ignored.  AssembledPC, lu, mumps, hypre, ilu (there is
+      no assembled matrix), PCDPC (DESIGN.md section 4.13), an outer "schur", "full" or "symmetric_multiplicative",
+      other field groupings and unknown keys are refused by name.
+
+    ``nullspace`` "constant" removes the pressure mean (block 1) from the residual, every preconditioned vector and
+    the final pressure.  A non-finite residual norm raises :class:`ConvergenceError` ("DIVERGED_FNORM_NAN").  Returns
+    (Newton residual norms, outer GMRES iterations per Newton step, inner iterations per step as a list of
+    (fieldsplit_0, fieldsplit_1) totals)."""
+    sp = _boussinesq_options(solver_parameters)
+    if nullspace not in (None, "constant"):
+        raise NotImplementedError(f"nullspace {nullspace!r}: None or 'constant' (constant pressures)")
+    V, Q, W = F.V, F.Q, F.W
+    bcs = tuple(bcs)
+    blocks = [_bc_block(F, bc) for bc in bcs]
+    if any(b == 1 for b in blocks):
+        raise NotImplementedError("a DirichletBC on the pressure space: condition the velocity (V) or the "
+                                  "temperature (W)")
+    vbcs = tuple(bc for bc, b in zip(bcs, blocks) if b == 0)
+    tbcs = tuple(bc for bc, b in zip(bcs, blocks) if b == 2)
+    remove_pressure_mean = _pressure_mean_remover(Q) if nullspace else None
+    for d in upT:
+        d.device_ptr
+    for bc, b in zip(bcs, blocks):
+        bc.apply(upT[b])
+    R, du = F.dat(), F.dat()
+    res = StokesAssembler(F, upT, bcs)
+
+    def residual():
+        res.assemble(tensor=R)
+        R.axpy(-1.0, L)
+        for bc, b in zip(bcs, blocks):
+            bc.zero(R[b])
+        if nullspace:
+            remove_pressure_mean(R)
+        return R.norm()
+
+    def check_finite():
+        if not np.isfinite(hist[-1]):
+            raise ConvergenceError(f"Newton diverged: the residual norm is {hist[-1]} after {len(kits)} steps "
+                                   f"(DIVERGED_FNORM_NAN)", "DIVERGED_FNORM_NAN")
+
+    hist = [residual()]
+    kits, inner = [], []
+    check_finite()
+    tol = max(sp["snes_rtol"] * hist[0], sp["snes_atol"])
+    # J reads upT[0] and upT[2] in place: one matrix-free operator serves every step
+    A = StokesMatrixContext(F.jacobian(upT), bcs)
+    M, counts = _boussinesq_fieldsplit(F, upT, A, vbcs, tbcs, sp, hierarchy, remove_pressure_mean)
+    while hist[-1] > tol and len(kits) < sp["snes_max_it"]:
+        du.zero()
+        for d in du:
+            d.device_ptr
+        counts[:] = [0, 0]
+        its, _ = gmres(A, R, du, M, rtol=sp["ksp_rtol"], restart=sp["ksp_gmres_restart"], maxit=sp["ksp_max_it"])
+        for bc, b in zip(bcs, blocks):
+            bc.zero(du[b])
+        upT.axpy(-1.0, du)
+        kits.append(its)
+        inner.append(tuple(counts))
+        hist.append(residual())
+        check_finite()
+    if nullspace:
+        remove_pressure_mean(upT)
+    return hist, kits, inner
+
+
+def _boussinesq_fieldsplit(F, upT, A, vbcs, tbcs, sp, hierarchy, remove_pressure_mean):
+    """The outer preconditioner ``M(r, z)`` of :func:`_solve_boussinesq` (None for pc_type "none", or the constant
+    nullspace alone) and the list [fieldsplit_0 iterations, fieldsplit_1 iterations] that it counts into."""
+    V, Q, W = F.V, F.Q, F.W
+    counts = [0, 0]
+    if sp["pc_type"] != "fieldsplit":
+        M = None
+        if remove_pressure_mean is not None:
+            def M(r, z):
+                r.copy(z)
+                remove_pressure_mean(z)
+        return M, counts
+    # fieldsplit_0: the Navier-Stokes block with its Schur fieldsplit, options under "fieldsplit_0_"
+    pre = "fieldsplit_0_"
+    sp0 = {k[len(pre):]: v for k, v in sp.items() if k.startswith(pre)}
+    _check_fieldsplit(sp0, hierarchy)
+    up = op2.MixedDat([upT[0], upT[1]])
+    new0 = lambda: op2.MixedDat([V.dat(), Q.dat()])
+    P0 = _fieldsplit_pc(V, Q, 1.0, 0.0, up, vbcs, sp0, hierarchy, remove_pressure_mean)
+    if sp["fieldsplit_0_ksp_type"] == "preonly":
+        def S0(r, z):
+            P0(r, z)
+            counts[0] += 1
+    else:
+        A0 = StokesMatrixContext(NavierStokesJacobian(V, Q, 1.0, 0.0, upT[0], F.pressure_map), vbcs)
+
+        def S0(r, z):
+            its, _ = gmres(A0, r, z, P0, rtol=sp["fieldsplit_0_ksp_rtol"],
+                           restart=sp["fieldsplit_0_ksp_gmres_restart"], maxit=sp["fieldsplit_0_ksp_max_it"])
+            counts[0] += its
+    # fieldsplit_1: J_TT through the full Jacobian action on (0, 0, s), preconditioned on Form(W, 1/Pr, 0)
+    P1 = _preconditioner(Form(W, F.kt, 0.0), None, tbcs, {"pc_type": sp["fieldsplit_1_pc_type"]}, hierarchy)
+    x3, y3 = F.dat(), F.dat()
+    if sp["fieldsplit_1_ksp_type"] == "preonly":
+        def S1(r, z):
+            P1(r, z)
+            counts[1] += 1
+    else:
+        class _JTT:
+            def mult(self, s, y):
+                x3[0].zero()
+                x3[1].zero()
+                s.copy(x3[2])
+                A.mult(x3, y3)
+                y3[2].copy(y)
+
+        JTT = _JTT()
+
+        def S1(r, z):
+            its, _ = gmres(JTT, r, z, P1, rtol=sp["fieldsplit_1_ksp_rtol"],
+                           restart=sp["fieldsplit_1_ksp_gmres_restart"], maxit=sp["fieldsplit_1_ksp_max_it"])
+            counts[1] += its
+    M = _block_gauss_seidel(S0, S1, A, F.dat, sp["pc_fieldsplit_type"] == "multiplicative", remove_pressure_mean)
+    return M, counts
+
+
+def _block_gauss_seidel(S0, S1, A, new, multiplicative, remove_pressure_mean=None):
+    """``M(r, z)`` of PETSc's two-split fieldsplit over 3-block vectors, split 0 = blocks (0, 1), split 1 = block 2:
+    "multiplicative" is block Gauss-Seidel, the inverse of A's block lower triangle when S0 and S1 invert its
+    diagonal blocks: z_0 = S0(r_0), then z_1 = S1(r_1 - A_10 z_0), with A_10 z_0 the last block of ``A.mult`` on
+    (z_0, 0); "additive" is z_1 = S1(r_1).  ``new()`` makes the work vectors; ``remove_pressure_mean`` (the constant
+    nullspace) is applied to z_0."""
+    x3, y3 = new(), new()
+    r1 = new()[2]
+
+    def M(r, z):
+        z0 = op2.MixedDat([z[0], z[1]])
+        S0(op2.MixedDat([r[0], r[1]]), z0)
+        if remove_pressure_mean is not None:
+            remove_pressure_mean(z0)
+        r[2].copy(r1)
+        if multiplicative:
+            z[0].copy(x3[0])
+            z[1].copy(x3[1])
+            x3[2].zero()
+            A.mult(x3, y3)
+            r1.axpy(-1.0, y3[2])
+        S1(r1, z[2])
+    return M
 
 
 class DGAdvection:

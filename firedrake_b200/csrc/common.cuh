@@ -149,10 +149,13 @@ int fdb_launch_elasticity_matrix(fdb_kernel_s *k, fdb_int start, fdb_int end, in
                                  const fdb_int *map1, double *diag_out);
 // FDB_FORM_STOKES (elasticity_hex.cu): yu and u AoS with 3 values per node of map0, yp and p one value per
 // node of map2 (the pressure map).  FDB_FORM_NAVIER_STOKES[_JACOBIAN] run through it too: ulin is the
-// Jacobian's linearisation velocity (AoS through map0), NULL for the other two forms
+// Jacobian's linearisation velocity (AoS through map0), NULL for the other two forms.  FDB_FORM_BOUSSINESQ[_JACOBIAN]
+// also read t and write yt, one temperature value per node of map2, and the Jacobian reads its linearisation
+// temperature tlin through map2 (all three NULL for the other forms)
 int fdb_launch_stokes_action(fdb_kernel_s *k, fdb_int start, fdb_int end, int nlay, const fdb_int *subset,
                              double *yu, const double *coords, const double *u, double *yp, const double *p,
-                             const double *ulin, const fdb_int *map0, const fdb_int *map1, const fdb_int *map2);
+                             const double *ulin, const fdb_int *map0, const fdb_int *map1, const fdb_int *map2,
+                             double *yt = nullptr, const double *t = nullptr, const double *tlin = nullptr);
 // FDB_FORM_BOUNDARY_MASS (boundary_hex.cu): one exterior facet per iteration entry, facet[col] its local facet
 // number.  mat != NULL: the element matrices into mat; else x != NULL: the action into y; else the diagonal
 // into y (cdim values per node, the same in each component)

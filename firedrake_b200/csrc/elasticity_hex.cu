@@ -51,6 +51,20 @@
 // gains the convective term, w |det J| sum_k G[d][k] u_k (residual) or w |det J| sum_k (G_w[d][k] u_k +
 // G_u[d][k] w_k) (Jacobian).  The Jacobian gathers u into S_V as EL_JACOBIAN does (its forward passes share
 // S_F[3..9)), takes G_u from the collocated derivative of S_V, and keeps S_P / S_Q after S_V.
+//
+// FDB_FORM_BOUSSINESQ[_JACOBIAN] (DESIGN.md section 4.22) run with MODE EL_RB_RESIDUAL / EL_RB_JACOBIAN: the
+// Boussinesq (Rayleigh-Benard) system, Navier-Stokes coupled to a temperature T in CG_{p-1} on the pressure
+// numbering, with bg = (Ra/Pr) g and kT = 1/Pr,
+//     R((u, p, T); (v, q, S)) = NS((u, p); (v, q)) - T inner(bg, v)*dx + dot(grad T, u) S*dx
+//                               + kT inner(grad T, grad S)*dx
+//     J(u, T)[(w, r, s); ...]  = NS-Jacobian(u)[(w, r); (v, q)] - s inner(bg, v)*dx
+//                               + (dot(grad s, u) + dot(grad T, w)) S*dx + kT inner(grad s, grad S)*dx.
+// T (s, and the Jacobian's T) is gathered through map2 into a padded N^3 block like p and runs through the
+// Bq passes in two more per-slot buffers S_A / S_B (the Jacobian's T through S_TF as work, into S_T0); its
+// physical gradient comes from the collocated derivative Dt of the point values (exact: degree p-1 <= N-1).
+// The point stage subtracts bg T from the velocity value slot, and gives T's test function a value
+// u . grad T and three reference fluxes kT w |det J| J^{-1} J^{-T} grad^ T in S_TF; Dt^T and Bq^T take them
+// back, and the threads of the pressure dofs scatter into y_T.
 #include "common.cuh"
 
 namespace {
@@ -75,22 +89,34 @@ struct ElasParams {
     const fdb_int *row_lg, *col_lg;   // dof-level, NULL = identity
     const unsigned short *rank_tab;
     int nvar, nlay_total;
-    const double *u;             // EL_JACOBIAN, EL_NS_JACOBIAN: the linearisation point (AoS, node map)
+    const double *u;             // EL_JACOBIAN, EL_NS_JACOBIAN, EL_RB_JACOBIAN: the linearisation point (AoS, node map)
     // EL_STOKES, EL_NS_*: the pressure action output and input (one value per node of map2, (N-1)^3 per cell)
     double *yp;
     const double *xp;
     const fdb_int *map2, *off2;
     double Bq[N * N];            // pressure basis at the points, (N, N-1) padded with a zero last column
+    // EL_RB_*: the temperature output and input (through map2), the Jacobian's linearisation temperature, and
+    // the buoyancy vector (Ra/Pr) g; 1/Pr is lmbda
+    double *yt;
+    const double *xt, *t0;
+    double bg[3];
 };
 
-enum { EL_LINEAR = 0, EL_RESIDUAL = 1, EL_JACOBIAN = 2, EL_STOKES = 3, EL_NS_RESIDUAL = 4, EL_NS_JACOBIAN = 5 };
+enum { EL_LINEAR = 0, EL_RESIDUAL = 1, EL_JACOBIAN = 2, EL_STOKES = 3, EL_NS_RESIDUAL = 4, EL_NS_JACOBIAN = 5,
+       EL_RB_RESIDUAL = 6, EL_RB_JACOBIAN = 7 };
 
-// the modes that also gather u into S_V (a Jacobian's linearisation point), and those on the Taylor-Hood pair
-__host__ __device__ constexpr bool el_holds_u(int mode) { return mode == EL_JACOBIAN || mode == EL_NS_JACOBIAN; }
+// the modes that also gather u into S_V (a Jacobian's linearisation point), those on the Taylor-Hood pair, and
+// those with a temperature on the pressure numbering
+__host__ __device__ constexpr bool el_holds_u(int mode)
+{
+    return mode == EL_JACOBIAN || mode == EL_NS_JACOBIAN || mode == EL_RB_JACOBIAN;
+}
 __host__ __device__ constexpr bool el_pressure(int mode)
 {
-    return mode == EL_STOKES || mode == EL_NS_RESIDUAL || mode == EL_NS_JACOBIAN;
+    return mode == EL_STOKES || mode == EL_NS_RESIDUAL || mode == EL_NS_JACOBIAN || mode == EL_RB_RESIDUAL ||
+           mode == EL_RB_JACOBIAN;
 }
+__host__ __device__ constexpr bool el_temperature(int mode) { return mode == EL_RB_RESIDUAL || mode == EL_RB_JACOBIAN; }
 
 template <int N, int MODE = EL_LINEAR>
 struct ElasShape {
@@ -98,9 +124,12 @@ struct ElasShape {
     static constexpr int CPB = (256 / ND) > 0 ? 256 / ND : 1;          // cells (slots) per CTA
     static constexpr int THREADS = ((CPB * ND + 31) / 32) * 32;
     // doubles per slot: vertices, values at the points, work buffer, fluxes (9 per point); the Jacobians
-    // also hold u's values (S_V), the Taylor-Hood modes the pressure and its work buffer (S_P, S_Q, after S_V)
+    // also hold u's values (S_V), the Taylor-Hood modes the pressure and its work buffer (S_P, S_Q, after S_V),
+    // the Boussinesq modes the temperature's two buffers and three fluxes (S_A, S_B, S_TF) and the Jacobian's
+    // linearisation temperature (S_T0)
     static constexpr int SLOT = 24 + 3 * ND + 3 * ND + 9 * ND + (el_holds_u(MODE) ? 3 * ND : 0) +
-                                (el_pressure(MODE) ? 2 * ND : 0);
+                                (el_pressure(MODE) ? 2 * ND : 0) + (el_temperature(MODE) ? 5 * ND : 0) +
+                                (MODE == EL_RB_JACOBIAN ? ND : 0);
     static constexpr size_t SMEM = (size_t)CPB * SLOT * sizeof(double) + (size_t)CPB * ND * sizeof(int);
 };
 
@@ -141,7 +170,9 @@ elasticity_kernel(const __grid_constant__ ElasParams<N> P)
     constexpr int ND = S::ND;
     constexpr int CPB = S::CPB;
     constexpr bool JAC = el_holds_u(MODE);                 // EL_JACOBIAN, EL_NS_JACOBIAN: u in S_V
-    constexpr bool STK = el_pressure(MODE);                // EL_STOKES, EL_NS_*: the pressure space
+    constexpr bool STK = el_pressure(MODE);                // EL_STOKES, EL_NS_*, EL_RB_*: the pressure space
+    constexpr bool TMP = el_temperature(MODE);             // EL_RB_*: the temperature on the pressure numbering
+    constexpr bool RBJ = MODE == EL_RB_JACOBIAN;
     constexpr int NP = N - 1;                              // pressure dofs per axis (EL_STOKES, EL_NS_*)
     extern __shared__ __align__(16) unsigned char smem_raw[];
     const int slot = threadIdx.x / ND;
@@ -153,9 +184,13 @@ elasticity_kernel(const __grid_constant__ ElasParams<N> P)
     double *s_u = s_x + 24;                                // [3][ND]
     double *s_t = s_u + 3 * ND;                            // [3][ND]
     double *s_f = s_t + 3 * ND;                            // [3 d][3 m][ND]
-    double *s_v = s_f + 9 * ND;                            // [3][ND], EL_JACOBIAN and EL_NS_JACOBIAN only
-    double *s_p = s_f + 9 * ND + (MODE == EL_NS_JACOBIAN ? 3 * ND : 0);   // [ND], pressure modes: pressure
+    double *s_v = s_f + 9 * ND;                            // [3][ND], the modes that hold u only
+    double *s_p = s_f + 9 * ND + (MODE == EL_NS_JACOBIAN || RBJ ? 3 * ND : 0);   // [ND], pressure modes: pressure
     double *s_q = s_p + ND;                                // [ND], pressure modes: its work buffer
+    double *s_a = s_q + ND;                                // [ND], EL_RB_*: the temperature (s) and
+    double *s_b = s_a + ND;                                // [ND]  its work buffer
+    double *s_tf = s_b + ND;                               // [3 m][ND], EL_RB_*: its reference fluxes
+    double *s_t0 = s_tf + 3 * ND;                          // [ND], EL_RB_JACOBIAN: the linearisation temperature
     int *s_idx = reinterpret_cast<int *>(reinterpret_cast<double *>(smem_raw) + (size_t)CPB * S::SLOT) + sl * ND;
     const int qi = l / (N * N), qj = (l / N) % N, qk = l % N;
     // pressure modes: this thread's pressure dof, if its (i, j, k) is one
@@ -191,6 +226,8 @@ elasticity_kernel(const __grid_constant__ ElasParams<N> P)
                 if (pdof) gp = __ldg(P.map2 + (long long)col * (NP * NP * NP) + lp) + __ldg(P.off2 + lp) * layer;
                 s_p[l] = pdof ? __ldg(P.xp + gp) : 0.0;
             }
+            if (TMP) s_a[l] = pdof ? __ldg(P.xt + gp) : 0.0;
+            if (RBJ) s_t0[l] = pdof ? __ldg(P.t0 + gp) : 0.0;
             for (int i = l; i < 24; i += ND) {
                 const int v = i / 3, a = i - 3 * v;
                 const int gv = __ldg(P.map1 + (long long)col * 8 + v) + __ldg(P.off1 + v) * layer;
@@ -205,6 +242,8 @@ elasticity_kernel(const __grid_constant__ ElasParams<N> P)
                 for (int d = 0; d < 3; d++) s_v[d * ND + l] = 0.0;
             }
             if (STK) s_p[l] = 0.0;
+            if (TMP) s_a[l] = 0.0;
+            if (RBJ) s_t0[l] = 0.0;
             for (int i = l; i < 24; i += ND) s_x[i] = (double)(((i / 3) >> (2 - i % 3)) & 1);
         }
         __syncthreads();
@@ -219,6 +258,8 @@ elasticity_kernel(const __grid_constant__ ElasParams<N> P)
                     s_f[(3 + d) * ND + l] = pass1<N, 0, false>(P.B, s_v + d * ND, qi, qj, qk);
             }
             if (STK) s_q[l] = pass1<N, 0, false>(P.Bq, s_p, qi, qj, qk);
+            if (TMP) s_b[l] = pass1<N, 0, false>(P.Bq, s_a, qi, qj, qk);
+            if (RBJ) s_tf[l] = pass1<N, 0, false>(P.Bq, s_t0, qi, qj, qk);
         }
         __syncthreads();
         if (in_cta) {
@@ -230,6 +271,8 @@ elasticity_kernel(const __grid_constant__ ElasParams<N> P)
                     s_f[(6 + d) * ND + l] = pass1<N, 1, false>(P.B, s_f + (3 + d) * ND, qi, qj, qk);
             }
             if (STK) s_p[l] = pass1<N, 1, false>(P.Bq, s_q, qi, qj, qk);
+            if (TMP) s_a[l] = pass1<N, 1, false>(P.Bq, s_b, qi, qj, qk);
+            if (RBJ) s_tf[ND + l] = pass1<N, 1, false>(P.Bq, s_tf, qi, qj, qk);
         }
         __syncthreads();
         if (in_cta) {
@@ -241,10 +284,13 @@ elasticity_kernel(const __grid_constant__ ElasParams<N> P)
                     s_v[d * ND + l] = pass1<N, 2, false>(P.B, s_f + (6 + d) * ND, qi, qj, qk);
             }
             if (STK) s_q[l] = pass1<N, 2, false>(P.Bq, s_p, qi, qj, qk);
+            if (TMP) s_b[l] = pass1<N, 2, false>(P.Bq, s_a, qi, qj, qk);
+            if (RBJ) s_t0[l] = pass1<N, 2, false>(P.Bq, s_tf + ND, qi, qj, qk);
         }
         __syncthreads();
         // ---- point stage
         double mres[3] = {0.0, 0.0, 0.0};
+        double tres = 0.0;                                 // EL_RB_*: the temperature's test value
         if (in_cta) {
             double gh[3][3];                               // gh[d][m] = d u_d / d xi_m
 #pragma unroll
@@ -352,6 +398,35 @@ elasticity_kernel(const __grid_constant__ ElasParams<N> P)
                             cv[d] = fma((g0 * R[0][k] + g1 * R[1][k] + g2 * R[2][k]) * rdet, s_u[k * ND + l], cv[d]);
                     }
                 }
+                if (TMP) {
+                    // Boussinesq: buoyancy -bg T in the value slot; T's test value u . grad T (Jacobian: u0 . grad s
+                    // + w . grad T0) and fluxes kT w |det| J^{-1} grad T (grad s) in S_TF
+                    const double tv = s_b[l];
+                    double gt[3];
+                    {
+                        const double h0 = pass1<N, 0, false>(P.Dt, s_b, qi, qj, qk);
+                        const double h1 = pass1<N, 1, false>(P.Dt, s_b, qi, qj, qk);
+                        const double h2 = pass1<N, 2, false>(P.Dt, s_b, qi, qj, qk);
+#pragma unroll
+                        for (int k = 0; k < 3; k++) gt[k] = (h0 * R[0][k] + h1 * R[1][k] + h2 * R[2][k]) * rdet;
+                    }
+                    double tr = uq[0] * gt[0] + uq[1] * gt[1] + uq[2] * gt[2];
+                    if (RBJ) {
+                        const double h0 = pass1<N, 0, false>(P.Dt, s_t0, qi, qj, qk);
+                        const double h1 = pass1<N, 1, false>(P.Dt, s_t0, qi, qj, qk);
+                        const double h2 = pass1<N, 2, false>(P.Dt, s_t0, qi, qj, qk);
+#pragma unroll
+                        for (int k = 0; k < 3; k++)
+                            tr = fma((h0 * R[0][k] + h1 * R[1][k] + h2 * R[2][k]) * rdet, s_u[k * ND + l], tr);
+                    }
+                    tres = wd * tr;
+                    const double kw = P.lmbda * sw;
+#pragma unroll
+                    for (int m = 0; m < 3; m++)
+                        s_tf[m * ND + l] = kw * (R[m][0] * gt[0] + R[m][1] * gt[1] + R[m][2] * gt[2]);
+#pragma unroll
+                    for (int d = 0; d < 3; d++) cv[d] = fma(-P.bg[d], tv, cv[d]);
+                }
 #pragma unroll
                 for (int d = 0; d < 3; d++) {
                     double sg[3];
@@ -439,24 +514,31 @@ elasticity_kernel(const __grid_constant__ ElasParams<N> P)
                                   pass1<N, 2, true>(P.Dt, f + 2 * ND, qi, qj, qk);
             }
             if (STK) s_q[l] = pass1<N, 2, true>(P.Bq, s_p, qi, qj, qk);
+            if (TMP)
+                s_a[l] = tres + pass1<N, 0, true>(P.Dt, s_tf, qi, qj, qk) +
+                         pass1<N, 1, true>(P.Dt, s_tf + ND, qi, qj, qk) +
+                         pass1<N, 2, true>(P.Dt, s_tf + 2 * ND, qi, qj, qk);
         }
         __syncthreads();
         if (in_cta) {
 #pragma unroll
             for (int d = 0; d < 3; d++) s_u[d * ND + l] = pass1<N, 2, true>(P.B, s_t + d * ND, qi, qj, qk);
             if (STK) s_p[l] = pass1<N, 1, true>(P.Bq, s_q, qi, qj, qk);
+            if (TMP) s_b[l] = pass1<N, 2, true>(P.Bq, s_a, qi, qj, qk);
         }
         __syncthreads();
         if (in_cta) {
 #pragma unroll
             for (int d = 0; d < 3; d++) s_t[d * ND + l] = pass1<N, 1, true>(P.B, s_u + d * ND, qi, qj, qk);
+            if (TMP) s_a[l] = pass1<N, 1, true>(P.Bq, s_b, qi, qj, qk);
         }
         __syncthreads();
-        double out[3], outp = 0.0;
+        double out[3], outp = 0.0, outt = 0.0;
         if (in_cta) {
 #pragma unroll
             for (int d = 0; d < 3; d++) out[d] = pass1<N, 0, true>(P.B, s_t + d * ND, qi, qj, qk);
             if (STK) outp = pass1<N, 0, true>(P.Bq, s_p, qi, qj, qk);
+            if (TMP) outt = pass1<N, 0, true>(P.Bq, s_a, qi, qj, qk);
         }
         // ---- scatter (this thread's node, three components)
         if (valid) {
@@ -470,6 +552,10 @@ elasticity_kernel(const __grid_constant__ ElasParams<N> P)
                 if (pdof) {
                     if (ATOMIC) atomicAdd(P.yp + gp, outp);
                     else P.yp[gp] += outp;
+                }
+                if (TMP && pdof) {
+                    if (ATOMIC) atomicAdd(P.yt + gp, outt);
+                    else P.yt[gp] += outt;
                 }
             } else {
                 const int j = jb / 3, b = jb - 3 * (jb / 3);
@@ -543,8 +629,10 @@ void fill_tables(const fdb_kernel_s *k, ElasParams<N> &P)
         P.xq[i] = k->desc.xq[i];
     }
     if (k->desc.form == FDB_FORM_STOKES || k->desc.form == FDB_FORM_NAVIER_STOKES ||
-        k->desc.form == FDB_FORM_NAVIER_STOKES_JACOBIAN) {
+        k->desc.form == FDB_FORM_NAVIER_STOKES_JACOBIAN || k->desc.form == FDB_FORM_BOUSSINESQ ||
+        k->desc.form == FDB_FORM_BOUSSINESQ_JACOBIAN) {
         P.off2 = k->d_off2;
+        for (int d = 0; d < 3; d++) P.bg[d] = k->desc.dcoef[d];
         for (int q = 0; q < N; q++)
             for (int a = 0; a < N; a++) P.Bq[q * N + a] = a < N - 1 ? k->B2[q * (N - 1) + a] : 0.0;
     }
@@ -553,7 +641,7 @@ void fill_tables(const fdb_kernel_s *k, ElasParams<N> &P)
 template <int N, int MODE>
 int action_n(fdb_kernel_s *k, fdb_int start, fdb_int end, int nlay, const fdb_int *subset, double *y,
              const double *coords, const double *x, const double *u, const fdb_int *map0, const fdb_int *map1,
-             double *yp, const double *xp, const fdb_int *map2)
+             double *yp, const double *xp, const fdb_int *map2, double *yt, const double *xt, const double *t0)
 {
     fdb::Context &c = fdb::ctx();
     ElasParams<N> P;
@@ -568,6 +656,9 @@ int action_n(fdb_kernel_s *k, fdb_int start, fdb_int end, int nlay, const fdb_in
     P.yp = yp;
     P.xp = xp;
     P.map2 = map2;
+    P.yt = yt;
+    P.xt = xt;
+    P.t0 = t0;
     if (k->desc.scatter == FDB_SCATTER_ATOMIC) {
         P.collist = subset;
         P.col0 = start;
@@ -631,17 +722,22 @@ int matrix_n(fdb_kernel_s *k, fdb_int start, fdb_int end, int nlay, const fdb_in
 template <int MODE>
 int action_mode(fdb_kernel_s *k, fdb_int start, fdb_int end, int nlay, const fdb_int *subset, double *y,
                 const double *coords, const double *x, const double *u, const fdb_int *map0, const fdb_int *map1,
-                double *yp = nullptr, const double *xp = nullptr, const fdb_int *map2 = nullptr)
+                double *yp = nullptr, const double *xp = nullptr, const fdb_int *map2 = nullptr, double *yt = nullptr,
+                const double *xt = nullptr, const double *t0 = nullptr)
 {
     // the Taylor-Hood modes have no degree-1 instantiation (their pressure space would be CG_0)
     switch (k->n1d) {
     case 2:
         if constexpr (!el_pressure(MODE))
-            return action_n<2, MODE>(k, start, end, nlay, subset, y, coords, x, u, map0, map1, yp, xp, map2);
+            return action_n<2, MODE>(k, start, end, nlay, subset, y, coords, x, u, map0, map1, yp, xp, map2, yt, xt,
+                                     t0);
         break;
-    case 3: return action_n<3, MODE>(k, start, end, nlay, subset, y, coords, x, u, map0, map1, yp, xp, map2);
-    case 4: return action_n<4, MODE>(k, start, end, nlay, subset, y, coords, x, u, map0, map1, yp, xp, map2);
-    case 5: return action_n<5, MODE>(k, start, end, nlay, subset, y, coords, x, u, map0, map1, yp, xp, map2);
+    case 3:
+        return action_n<3, MODE>(k, start, end, nlay, subset, y, coords, x, u, map0, map1, yp, xp, map2, yt, xt, t0);
+    case 4:
+        return action_n<4, MODE>(k, start, end, nlay, subset, y, coords, x, u, map0, map1, yp, xp, map2, yt, xt, t0);
+    case 5:
+        return action_n<5, MODE>(k, start, end, nlay, subset, y, coords, x, u, map0, map1, yp, xp, map2, yt, xt, t0);
     }
     fdb::set_error("elasticity action: degree %d not instantiated (1..4)", k->n1d - 1);
     return 1;
@@ -680,7 +776,8 @@ int fdb_launch_elasticity_action(fdb_kernel_s *k, fdb_int start, fdb_int end, in
 
 int fdb_launch_stokes_action(fdb_kernel_s *k, fdb_int start, fdb_int end, int nlay, const fdb_int *subset,
                              double *yu, const double *coords, const double *u, double *yp, const double *p,
-                             const double *ulin, const fdb_int *map0, const fdb_int *map1, const fdb_int *map2)
+                             const double *ulin, const fdb_int *map0, const fdb_int *map1, const fdb_int *map2,
+                             double *yt, const double *t, const double *tlin)
 {
     switch (k->desc.form) {
     case FDB_FORM_STOKES:
@@ -691,6 +788,12 @@ int fdb_launch_stokes_action(fdb_kernel_s *k, fdb_int start, fdb_int end, int nl
     case FDB_FORM_NAVIER_STOKES_JACOBIAN:
         return action_mode<EL_NS_JACOBIAN>(k, start, end, nlay, subset, yu, coords, u, ulin, map0, map1, yp, p,
                                            map2);
+    case FDB_FORM_BOUSSINESQ:
+        return action_mode<EL_RB_RESIDUAL>(k, start, end, nlay, subset, yu, coords, u, nullptr, map0, map1, yp, p,
+                                           map2, yt, t);
+    case FDB_FORM_BOUSSINESQ_JACOBIAN:
+        return action_mode<EL_RB_JACOBIAN>(k, start, end, nlay, subset, yu, coords, u, ulin, map0, map1, yp, p,
+                                           map2, yt, t, tlin);
     }
     fdb::set_error("stokes action: form %d is not a Taylor-Hood form", k->desc.form);
     return 1;

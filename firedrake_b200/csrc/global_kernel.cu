@@ -316,7 +316,7 @@ struct fdb_hex_form {
     bool residual;            // a 1-form action only
     int launcher;             // fdb_launch_helmholtz_*, fdb_launch_helmholtz_coef_* (which also run the
                               // nonlinear diffusion and advection-diffusion forms), fdb_launch_elasticity_*
-                              // fdb_launch_stokes_action (which also runs the Navier-Stokes forms),
+                              // fdb_launch_stokes_action (which also runs the Navier-Stokes and Boussinesq forms),
                               // fdb_launch_boundary_mass, fdb_launch_dg_facet (the DG facet forms),
                               // fdb_launch_dg_transport or fdb_launch_spectral_helmholtz
     int max_degree[3];        // per mode: action, matrix, diagonal
@@ -326,6 +326,10 @@ struct fdb_hex_form {
     int integral;             // enum fdb_integral: facet forms run in device mode only; -1: the descriptor's
                               // integral (cell, exterior or interior facet) selects the term
     int space2_degree;        // SPACE2_*: the degree the second space must have (read when space2 is set)
+    const char *field3;       // the arguments of a third field on the second space's map (output and input, after
+                              // the second space's: Boussinesq's temperature), or NULL
+    int ncoef;                // the number of trailing coefficient arguments when coef names more than one
+                              // (Boussinesq's Jacobian: u0, T0), 0: one
 };
 
 static const fdb_hex_form hex_forms[] = {
@@ -348,6 +352,12 @@ static const fdb_hex_form hex_forms[] = {
     {FDB_FORM_NAVIER_STOKES, "navier_stokes", 3, false, nullptr, 0, true, LAUNCH_STOKES, {4, 0, 0}, 2, "y_p, p", FDB_INTEGRAL_CELL},
     {FDB_FORM_NAVIER_STOKES_JACOBIAN, "navier_stokes_jacobian", 3, false, "u", 3, false, LAUNCH_STOKES, {4, 0, 0}, 2,
      "y_p, p", FDB_INTEGRAL_CELL},
+    // Navier-Stokes coupled to a temperature in CG_{p-1} on the pressure map: [y_u, coords, u, y_p, p, y_T, T]; the
+    // Jacobian reads its linearisation point (u0 through the velocity map, T0 through the pressure map) last
+    {FDB_FORM_BOUSSINESQ, "boussinesq", 3, false, nullptr, 0, true, LAUNCH_STOKES, {4, 0, 0}, 2, "y_p, p",
+     FDB_INTEGRAL_CELL, SPACE2_PRESSURE, "y_T, T"},
+    {FDB_FORM_BOUSSINESQ_JACOBIAN, "boussinesq_jacobian", 3, false, "u0, T0", 3, false, LAUNCH_STOKES, {4, 0, 0}, 2,
+     "y_p, p", FDB_INTEGRAL_CELL, SPACE2_PRESSURE, "y_T, s", 2},
     // gamma*inner(u, v)*ds: one exterior facet of one cell per entry, its local facet number last
     {FDB_FORM_BOUNDARY_MASS, "boundary_mass", -1, false, "facet", 1, false, LAUNCH_BOUNDARY, {5, 4, 5}, 1, nullptr,
      FDB_INTEGRAL_EXTERIOR_FACET},
@@ -840,7 +850,9 @@ int fdb_kernel_call(fdb_kernel_t k, const fdb_call_args *a)
     // the form's trailing coefficient; maps = [V map, coord map].  A form on two spaces (Stokes) has the
     // output and input of the second space after x and a third map: [y, coords, x, y2, x2], [V map, coord
     // map, second map]; with a trailing coefficient as well (the Navier-Stokes Jacobian's u) the coefficient
-    // comes last: [y, coords, x, y2, x2, coef]
+    // comes last: [y, coords, x, y2, x2, coef]; a third field on the second map (Boussinesq's temperature) comes
+    // after the second space's arguments, and its coefficients (several: u0, T0) last: [y, coords, x, y2, x2, y3,
+    // x3, coef...]
     // an exterior-facet form (boundary_mass): the trailing argument is the uint32 local facet number of each
     // entry, [y, coords, x, facet] / [mat, coords, facet] / [d, coords, facet]; an interior-facet form
     // (interior_penalty): the two local facet numbers ('+', '-') of each entry, [y, coords, x, facets]; dg_transport
@@ -856,7 +868,9 @@ int fdb_kernel_call(fdb_kernel_t k, const fdb_call_args *a)
                   f->name);
         return 1;
     }
-    const int want = (mode == MODE_ACTION ? 3 : 2) + (f->coef ? 1 : 0) + (f->space2 ? 2 : 0) + (transport_facets ? 1 : 0);
+    const int ncoef = f->coef ? (f->ncoef ? f->ncoef : 1) : 0;
+    const int want = (mode == MODE_ACTION ? 3 : 2) + ncoef + (f->space2 ? 2 : 0) + (f->field3 ? 2 : 0) +
+                     (transport_facets ? 1 : 0);
     const int want_maps = f->space2 ? 3 : 2;
     const bool device_only = mode == MODE_DIAGONAL || f->space2 || f->integral != FDB_INTEGRAL_CELL;
     if (f->launcher == LAUNCH_SPECTRAL && a->location != FDB_LOC_DEVICE) {
@@ -865,9 +879,9 @@ int fdb_kernel_call(fdb_kernel_t k, const fdb_call_args *a)
     }
     if (a->nargs != want || a->nmaps != want_maps || (device_only && a->location != FDB_LOC_DEVICE)) {
         static const char *const args[] = {"y, coords, x", "mat, coords", "d, coords"};
-        set_error("fdb_kernel_call: %s %s expects %d %sargs (%s%s%s%s%s) and %d maps, got %d/%d", f->name,
+        set_error("fdb_kernel_call: %s %s expects %d %sargs (%s%s%s%s%s%s%s) and %d maps, got %d/%d", f->name,
                   mode_name[mode], want, device_only ? "device " : "", args[mode], f->space2 ? ", " : "",
-                  f->space2 ? f->space2 : "", f->coef ? ", " : "",
+                  f->space2 ? f->space2 : "", f->field3 ? ", " : "", f->field3 ? f->field3 : "", f->coef ? ", " : "",
                   transport_facets ? "b, facets" : (f->coef ? f->coef : ""), want_maps, a->nargs,
                   a->nmaps);
         return 1;
@@ -912,12 +926,12 @@ int fdb_kernel_call(fdb_kernel_t k, const fdb_call_args *a)
         int rc = pipelined_host_action(k, a, nlay);
         if (rc >= 0) return rc;      // -1: not applicable, fall through to the monolithic path
     }
-    void *dargs[6];
+    void *dargs[9];
     const fdb_int *dmaps[3];
     const fdb_int *dsubset;
     if (device_pointers(a, mat != nullptr, dargs, dmaps, &dsubset)) return 1;
     const double *coords = (const double *)dargs[1];
-    const double *coef = f->coef ? (const double *)dargs[want - 1] : nullptr;
+    const double *coef = f->coef ? (const double *)dargs[want - ncoef] : nullptr;
     // dg_transport: b, and on facets the local facet numbers after it
     const double *vel = f->launcher == LAUNCH_DG_TRANSPORT ? (const double *)dargs[mode == MODE_ACTION ? 3 : 2] : nullptr;
     const unsigned *tfacets = transport_facets ? (const unsigned *)dargs[want - 1] : nullptr;
@@ -1007,7 +1021,10 @@ int fdb_kernel_call(fdb_kernel_t k, const fdb_call_args *a)
         break;
     default:
         rc = fdb_launch_stokes_action(k, a->start, a->end, nlay, dsubset, out, coords, x, (double *)dargs[3],
-                                      (const double *)dargs[4], coef, dmaps[0], dmaps[1], dmaps[2]);
+                                      (const double *)dargs[4], coef, dmaps[0], dmaps[1], dmaps[2],
+                                      f->field3 ? (double *)dargs[5] : nullptr,
+                                      f->field3 ? (const double *)dargs[6] : nullptr,
+                                      ncoef > 1 ? (const double *)dargs[want - 1] : nullptr);
     }
     if (rc) return rc;
     if (a->location == FDB_LOC_HOST && a->writeback) {

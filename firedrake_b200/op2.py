@@ -245,11 +245,16 @@ def _as_dataset(s):
 class Map:
     """``values`` has shape (iterset.total_size, arity); for extruded iteration
     sets each row addresses the BOTTOM cell of a column and ``offset[i]`` is
-    added per layer (pyop2/types/map.py:36-56)."""
+    added per layer (pyop2/types/map.py:36-56).
+
+    ``alias_of``: another Map with the same values and offsets onto a set of the same size (a field numbered like
+    another, e.g. Boussinesq's temperature on the pressure numbering).  A hand-written kernel call then passes that
+    map in its place, so both fields are read through one device map."""
     _ids = itertools.count()
 
-    def __init__(self, iterset, toset, arity, values, name=None, offset=None, offset_quotient=None):
+    def __init__(self, iterset, toset, arity, values, name=None, offset=None, offset_quotient=None, alias_of=None):
         self.iterset, self.toset, self.arity = iterset, toset, int(arity)
+        self.alias_of = alias_of
         v = np.ascontiguousarray(np.asarray(values, dtype=IntType).reshape(-1, self.arity))
         if v.shape[0] != iterset.total_size:
             raise MapValueError(f"map has {v.shape[0]} rows, iterset has {iterset.total_size}")
@@ -1398,6 +1403,14 @@ class Kernel:
     argument: (INC, READ, READ, INC, READ, READ) = (velocity output, coordinates, w, pressure output, r, u).
     Neither is symmetric; both are rank-1 actions only.
 
+    "boussinesq" is the Boussinesq (Rayleigh-Benard) residual on the same spaces with a temperature T in CG_{p-1} on
+    the pressure numbering: "navier_stokes" with ``mu`` = nu, plus ``-T*inner(bg, v)*dx + dot(grad T, u)*S*dx +
+    kt*inner(grad T, grad S)*dx`` with the buoyancy vector ``bg`` = (Ra/Pr) g and ``kt`` = 1/Pr; arguments (INC, READ,
+    READ, INC, READ, INC, READ) = (velocity output, coordinates, u, pressure output, p, temperature output, T), the
+    temperature through the pressure map.  "boussinesq_jacobian" is its Gateaux derivative at (u0, T0) applied to
+    (w, r, s), with u0 and T0 LAST: (velocity output, coordinates, w, pressure output, r, temperature output, s, u0,
+    T0).  Rank-1 actions only.
+
     "boundary_mass" is the exterior-facet integral ``alpha*inner(u, v)*ds`` (gamma = ``alpha``) on a scalar or
     vector (``cdim=3``) space, with ``integral="exterior_facet"``.  The iteration set has one entry per facet of
     a cell: its maps are the owning cells' rows, and the LAST argument is a uint32 Dat of the local facet numbers
@@ -1467,6 +1480,8 @@ class Kernel:
     c_out: float = 1.0              # dg_transport (exterior facets): the max(b.n, 0) and min(b.n, 0) coefficients
     c_in: float = 0.0
     coarse_degree: int = 0          # p_prolong / p_restrict / p_inject: the coarse space's degree q
+    bg: tuple = (0.0, 0.0, 0.0)     # boussinesq[_jacobian]: the buoyancy vector (Ra/Pr) g
+    kt: float = 0.0                 # boussinesq[_jacobian]: the temperature diffusivity 1/Pr
 
     def __new__(cls, *args, **kwargs):
         # ``op2.Kernel(code, name)`` with C source (pyop2/local_kernel.py:33-43) builds the
@@ -1501,7 +1516,13 @@ class Kernel:
             # refuses)
             if self.cdim == 1:
                 object.__setattr__(self, "cdim", 3)
-            acc = (INC, READ, READ, INC, READ) + ((READ,) if spec.coefficient else ())
+            if spec.temperature:
+                object.__setattr__(self, "bg", tuple(float(c) for c in self.bg))
+                if len(self.bg) != 3:
+                    raise ValueError("bg is the buoyancy vector (Ra/Pr) g, three values")
+                acc = (INC, READ, READ, INC, READ, INC, READ) + ((READ, READ) if spec.coefficient else ())
+            else:
+                acc = (INC, READ, READ, INC, READ) + ((READ,) if spec.coefficient else ())
             object.__setattr__(self, "accesses", acc)
             return
         if spec and spec.residual:
@@ -1556,6 +1577,7 @@ class _Form(NamedTuple):
     transfer: bool = False      # a p-multigrid degree transfer: fine and coarse maps, no coordinates
     gll: bool = False           # stated on the GLL rule at the nodes: the default element is the collocated GLL one
     hdiv: bool = False          # a mixed Poisson form on NCF_k x DQ_{k-1}
+    temperature: bool = False   # also reads and writes a temperature on the pressure map (Boussinesq)
 
 
 _FORMS = {"helmholtz": _Form(_lib.FORM_HELMHOLTZ),
@@ -1580,7 +1602,10 @@ _FORMS = {"helmholtz": _Form(_lib.FORM_HELMHOLTZ),
           "spectral_helmholtz": _Form(_lib.FORM_SPECTRAL_HELMHOLTZ, gll=True),
           "spectral_helmholtz_coef": _Form(_lib.FORM_SPECTRAL_HELMHOLTZ_COEF, coefficient=True, gll=True),
           "mixed_poisson": _Form(_lib.FORM_MIXED_POISSON, hdiv=True),
-          "mixed_poisson_schur": _Form(_lib.FORM_MIXED_POISSON_SCHUR, hdiv=True)}
+          "mixed_poisson_schur": _Form(_lib.FORM_MIXED_POISSON_SCHUR, hdiv=True),
+          "boussinesq": _Form(_lib.FORM_BOUSSINESQ, residual=True, pressure=True, temperature=True),
+          "boussinesq_jacobian": _Form(_lib.FORM_BOUSSINESQ_JACOBIAN, coefficient=True, pressure=True,
+                                       temperature=True)}
 _INTEGRALS = {"cell": _lib.INTEGRAL_CELL, "exterior_facet": _lib.INTEGRAL_EXTERIOR_FACET,
               "interior_facet": _lib.INTEGRAL_INTERIOR_FACET, "fused": _lib.INTEGRAL_FUSED}
 
@@ -1694,6 +1719,9 @@ class GlobalKernel:
             d.dcoef[0], d.dcoef[1], d.dcoef[2] = lk.c_out, lk.c_in, 0.0
         if spec.lame:
             d.alpha, d.lmbda = lk.mu, lk.lmbda
+        if spec.temperature:
+            d.dcoef[0], d.dcoef[1], d.dcoef[2] = lk.bg
+            d.lmbda = lk.kt
         s2 = None
         if spec.pressure:
             d.alpha = lk.mu
@@ -1963,8 +1991,9 @@ class Parloop:
         out = self.args[0].data
         maps = []
         for a in self.args:
-            if a.map is not None and a.map not in maps:
-                maps.append(a.map)       # distinct maps, first-use order
+            m = getattr(a.map, "alias_of", None) or a.map
+            if m is not None and m not in maps:
+                maps.append(m)           # distinct maps, first-use order
         if isinstance(out, Mat):
             # replace_lgmaps (pyop2/parloop.py:279-314): BC-masked maps for this loop only
             L = _lib.lib()

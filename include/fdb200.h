@@ -384,7 +384,7 @@ enum fdb_form {
                                                y_sigma += alpha M sigma + B^T u,  y_u += B sigma
                                      diagonal  [d INC, coords]   maps [NCF map, coord map]
                                                d += diag(alpha M), one value per flux dof               */
-    FDB_FORM_MIXED_POISSON_SCHUR = 23
+    FDB_FORM_MIXED_POISSON_SCHUR = 23,
                                 /* the selfp Schur complement of FDB_FORM_MIXED_POISSON, S_p = B W B^T with W a
                                    diagonal given as one value per flux dof (diag(alpha M)^-1, zero on flux-condition
                                    rows).  Metric-free: no coordinates.  Same descriptor, second space, restrictions
@@ -394,6 +394,34 @@ enum fdb_form {
                                                y_u += S_p u when t is zero on entry
                                      diagonal  [d INC, w]   maps [DQ map, NCF map]
                                                d += diag(B W B^T), one pass                            */
+    FDB_FORM_BOUSSINESQ = 24,
+                                /* residual of the Boussinesq (Rayleigh-Benard) system on the Taylor-Hood spaces
+                                   of FDB_FORM_STOKES with a temperature T in scalar CG_{p-1} on the PRESSURE
+                                   numbering (one value per node of maps[2]; NOT symmetric):
+                                     R((u, p, T); (v, q, S)) = nu*inner(grad u, grad v)*dx + beta*inner(u, v)*dx
+                                                               + inner(dot(grad u, u), v)*dx
+                                                               - p*div(v)*dx - T*inner(bg, v)*dx
+                                                               - q*div(u)*dx
+                                                               + dot(grad T, u)*S*dx
+                                                               + kT*inner(grad T, grad S)*dx
+                                   nu = alpha, bg = dcoef[0..2] (the buoyancy vector (Ra/Pr) g), kT = lmbda
+                                   (1/Pr).  The (u, p) rows are FDB_FORM_NAVIER_STOKES when bg = 0.  The
+                                   convective terms are not integrated exactly by the nq = p+1 rule.  Same
+                                   spaces, creation (fdb_kernel_create_mixed, the pressure space as the second
+                                   space) and restrictions as FDB_FORM_STOKES:
+                                     action  [y_u INC, coords, u, y_p INC, p, y_T INC, T]
+                                             maps [V map, coord map, Q map]                       */
+    FDB_FORM_BOUSSINESQ_JACOBIAN = 25
+                                /* its Gateaux derivative at (u0, T0) (exact Newton Jacobian, NOT symmetric),
+                                   applied to the direction (w, r, s):
+                                     J[(w, r, s); (v, q, S)] = FDB_FORM_NAVIER_STOKES_JACOBIAN at u0 on (w, r)
+                                                               - s*inner(bg, v)*dx
+                                                               + dot(grad s, u0)*S*dx + dot(grad T0, w)*S*dx
+                                                               + kT*inner(grad s, grad S)*dx
+                                   Parameters and restrictions as FDB_FORM_BOUSSINESQ.  The linearisation point
+                                   comes LAST: u0 through maps[0], T0 through maps[2]:
+                                     action  [y_u INC, coords, w, y_p INC, r, y_T INC, s, u0, T0]
+                                             maps [V map, coord map, Q map]                       */
 };
 
 enum fdb_cell {
@@ -456,15 +484,17 @@ typedef struct fdb_kernel_desc {
     /* FDB_FORM_NONLINEAR_DIFFUSION[_JACOBIAN]: D(s) = dcoef[0] + dcoef[1] s + dcoef[2] s^2.
      * FDB_FORM_DG_BOUNDARY: c_m = dcoef[0], c_s = dcoef[1].
      * FDB_FORM_DG_TRANSPORT (exterior facets): c_out = dcoef[0], c_in = dcoef[1].
+     * FDB_FORM_BOUSSINESQ[_JACOBIAN]: the buoyancy vector (Ra/Pr) g = dcoef[0..2].
      * Ignored by every other form (a zeroed descriptor stays valid for them). */
     double dcoef[3];
     /* FDB_FORM_ELASTICITY, FDB_FORM_HYPERELASTICITY[_JACOBIAN]: the Lame parameter lambda (mu is
-     * alpha).  Ignored by every other form. */
+     * alpha).  FDB_FORM_BOUSSINESQ[_JACOBIAN]: the temperature diffusivity 1/Pr.  Ignored by every other
+     * form. */
     double lmbda;
 } fdb_kernel_desc;
 
-/* The second space of a form on two spaces (FDB_FORM_STOKES, FDB_FORM_NAVIER_STOKES[_JACOBIAN]: the
- * pressure space), passed to
+/* The second space of a form on two spaces (FDB_FORM_STOKES, FDB_FORM_NAVIER_STOKES[_JACOBIAN],
+ * FDB_FORM_BOUSSINESQ[_JACOBIAN]: the pressure space, which also numbers the temperature), passed to
  * fdb_kernel_create_mixed next to the descriptor of the first (argument) space, which keeps its
  * layout.  degree: the second space's polynomial degree (Stokes: the velocity degree minus 1);
  * B: its basis at the descriptor's nq Gauss points, row-major (nq, degree+1), 1-D dof numbering;
@@ -483,8 +513,8 @@ typedef struct fdb_kernel_s *fdb_kernel_t;
  * "compile" = validate the descriptor, precompute tables, pick the sm_90a
  * kernel instantiation.  Fails (nonzero) for forms outside the supported set. */
 int fdb_kernel_create(const fdb_kernel_desc *desc, fdb_kernel_t *out);
-/* The same for a form on two spaces (FDB_FORM_STOKES, FDB_FORM_NAVIER_STOKES[_JACOBIAN], the
- * p-multigrid transfers FDB_FORM_P_*, FDB_FORM_MIXED_POISSON[_SCHUR]), which
+/* The same for a form on two spaces (FDB_FORM_STOKES, FDB_FORM_NAVIER_STOKES[_JACOBIAN],
+ * FDB_FORM_BOUSSINESQ[_JACOBIAN], the p-multigrid transfers FDB_FORM_P_*, FDB_FORM_MIXED_POISSON[_SCHUR]), which
  * fdb_kernel_create refuses; a form on one
  * space is refused here. */
 int fdb_kernel_create_mixed(const fdb_kernel_desc *desc, const fdb_space2_desc *space2, fdb_kernel_t *out);
