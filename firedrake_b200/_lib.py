@@ -40,6 +40,8 @@ FORM_MIXED_POISSON = 22                # alpha*dot(sigma, tau)*dx + div(tau)*u*d
 FORM_MIXED_POISSON_SCHUR = 23          # its selfp Schur complement B W B^T (metric-free)
 FORM_BOUSSINESQ = 24                   # Navier-Stokes + buoyancy + temperature advection-diffusion (Rayleigh-Benard)
 FORM_BOUSSINESQ_JACOBIAN = 25          # its exact Gateaux derivative at (u0, T0)
+FORM_MIXED_POISSON_HYBRID = 26         # mixed Poisson hybridised: the condensed trace matrix (rank 2), its load (rank 1)
+FORM_MIXED_POISSON_RECONSTRUCT = 27    # (sigma, u) cell by cell from the trace multiplier lambda
 CELL_HEX_EXTRUDED = 1
 CELL_HEX = 2
 CELL_TRIANGLE = 3
@@ -175,6 +177,7 @@ SIGNATURES = {
     "fdb_mat_set_lgmaps": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p]),
     "fdb_mat_set_diagonal": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_double]),
     "fdb_mat_mult": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p]),
+    "fdb_mat_get_diagonal": (C.c_int, [C.c_void_p, C.c_void_p]),
     "fdb_mat_get_csr": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "fdb_dat_zero_nodes": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int32]),
     "fdb_dat_set_nodes": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int32]),

@@ -37,15 +37,25 @@ class FunctionSpace:
     element.
 
     ``family="NCF"``: the H(div) space NCF_k (k = 2..4, ``mesh.hdiv_function_space``), the flux space of
-    :class:`MixedPoisson`; no other form takes it."""
+    :class:`MixedPoisson`; no other form takes it.
+
+    ``family="HDiv Trace"``: Firedrake's trace space of degree k - 1 (1..3, ``mesh.trace_function_space``), Q_{k-1}
+    on every face, the multiplier space of :class:`HybridizationPC`; no form takes it."""
 
     def __init__(self, mesh, degree, cdim=1, partition=None, family="CG"):
         self.mesh, self.degree, self.cdim = mesh, degree, cdim
-        if family not in ("CG", "DQ", "NCF"):
-            raise ValueError(f"family {family!r}: 'CG', 'DQ' or 'NCF'")
+        if family not in ("CG", "DQ", "NCF", "HDiv Trace"):
+            raise ValueError(f"family {family!r}: 'CG', 'DQ', 'NCF' or 'HDiv Trace'")
         self.family = family
         self.element = None
-        if family == "NCF":
+        if family == "HDiv Trace":
+            if cdim != 1:
+                raise NotImplementedError("an HDiv Trace space is scalar (cdim 1)")
+            if partition is not None:
+                raise NotImplementedError("partitioned HDiv Trace spaces are not implemented: their NCF flux spaces "
+                                          "are not partitioned")
+            self.V = V = mesh.trace_function_space(degree)
+        elif family == "NCF":
             if cdim != 1:
                 raise NotImplementedError("an NCF space has one value per dof (cdim 1): its dofs are the "
                                           "components of the Piola-mapped field")
@@ -128,6 +138,9 @@ def _refuse_dq(V, what, why="it is stated on CG spaces only"):
 
 
 def _refuse_ncf(V, what):
+    if getattr(V, "family", "CG") == "HDiv Trace":
+        raise NotImplementedError(f"{what} does not take HDiv Trace spaces: the trace space is the multiplier space "
+                                  f"of HybridizationPC")
     if getattr(V, "family", "CG") == "NCF":
         raise NotImplementedError(f"{what} does not take NCF (H(div)) spaces: the only form on NCF is MixedPoisson")
 
@@ -3448,6 +3461,328 @@ def assemble_mixed_poisson_generic(F: MixedPoisson, up: op2.MixedDat, tensor=Non
     return tensor
 
 
+def hybridization_kernel(degree, alpha=1.0, name=None):
+    """C source of the condensed trace matrix H_K = C^ K_K^-1 C^^T of one cell on the generic wrapper path
+    (arguments: the 6k^2 x 6k^2 local tensor (INC, through the trace map) and the coordinates).  Every flux basis
+    function is tabulated at every Gauss point and alpha M, B assembled as dense sums over the points; then a dense
+    Cholesky factorisation of alpha M, Y = (alpha M)^-1 [B^T C^T], and the Cholesky-factored S_B = B Y_B give
+    H_K = C Y_C - (B Y_C)^T S_B^-1 (B Y_C).  The independent statement of the hand-written HY_CONDENSE kernel (a
+    bordered LDL^T elimination) and its speed baseline.  k = 2 only: at k = 3 the dense local arrays (about 170 KB)
+    do not fit a thread's stack."""
+    from .codegen import CStringKernel
+    from .fiat_lite import gauss_legendre, interval_element
+    k = degree
+    if k != 2:
+        raise NotImplementedError(f"the generic-path hybridisation statement covers degree 2 only, got {k}: at k = 3 "
+                                  f"its dense local arrays (about 170 KB per thread) do not fit a thread's stack")
+    name = name or f"hybrid_condense{k}"
+    cg, dg = interval_element(k), interval_element(k - 1, k + 1, "gl")
+    _, wg = gauss_legendre(k)
+    vec = lambda a: "{" + ", ".join(repr(float(v)) for v in a) + "}"
+    tab = lambda a: "{" + ", ".join(vec(r) for r in a) + "}"
+    ns, nu, nf = 3 * k * k * (k + 1), k ** 3, 6 * k * k
+    code = f"""
+#define YQ {k + 1}
+#define YK {k}
+#define YS {ns}
+#define YU {nu}
+#define YF {nf}
+static const double YX[YQ] = {vec(cg.xq)}, YW[YQ] = {vec(cg.wq)}, YWG[YK] = {vec(wg)};
+static const double YC[YQ][YK + 1] = {tab(cg.B)}, YD[YQ][YK + 1] = {tab(cg.D)}, YG[YQ][YK] = {tab(dg.B)};
+/* (component, 1-D indices) of flux dof j, component-major, block index (i0 * n1 + i1) * n2 + i2 */
+static void hy_dof(int j, int *d, int *i)
+{{
+    *d = j / (YK * YK * (YK + 1));
+    const int r = j % (YK * YK * (YK + 1)), n1 = *d == 1 ? YK + 1 : YK, n2 = *d == 2 ? YK + 1 : YK;
+    i[0] = r / (n1 * n2); i[1] = (r / n2) % n1; i[2] = r % n2;
+}}
+/* the flux dof of trace dof t (face 2d + s, GL indices t0, t1 in axis order) and its coupling o w_t0 w_t1 */
+static int hy_face(int t, double *c)
+{{
+    const int f = t / (YK * YK), r = t % (YK * YK), d = f / 2, s = f % 2, t0 = r / YK, t1 = r % YK;
+    int idx[3];
+    idx[d] = s; idx[d == 0 ? 1 : 0] = t0; idx[d == 2 ? 1 : 2] = t1;
+    const int n1 = d == 1 ? YK + 1 : YK, n2 = d == 2 ? YK + 1 : YK;
+    *c = (s ? 1.0 : -1.0) * YWG[t0] * YWG[t1];
+    return d * YK * YK * (YK + 1) + (idx[0] * n1 + idx[1]) * n2 + idx[2];
+}}
+static void {name}(double *Hl, const double *X)
+{{
+    double A[YS][YS], Bm[YU][YS], Y[YS][YU + YF], SB[YU][YU], P[YU][YF];
+    for (int i = 0; i < YS; ++i) for (int j = 0; j < YS; ++j) A[i][j] = 0.0;
+    for (int v = 0; v < YU; ++v) for (int j = 0; j < YS; ++j) Bm[v][j] = 0.0;
+    for (int qx = 0; qx < YQ; ++qx) for (int qy = 0; qy < YQ; ++qy) for (int qz = 0; qz < YQ; ++qz) {{
+        const int q[3] = {{qx, qy, qz}};
+        const double xi[3] = {{YX[qx], YX[qy], YX[qz]}};
+        double J[3][3] = {{{{0}}}};
+        for (int v = 0; v < 8; ++v) {{
+            const int b[3] = {{(v >> 2) & 1, (v >> 1) & 1, v & 1}};
+            for (int r = 0; r < 3; ++r) {{
+                double gr = b[r] ? 1.0 : -1.0;
+                for (int e = 0; e < 3; ++e) if (e != r) gr *= b[e] ? xi[e] : 1.0 - xi[e];
+                for (int c = 0; c < 3; ++c) J[c][r] += X[v * 3 + c] * gr;
+            }}
+        }}
+        const double det = J[0][0] * (J[1][1] * J[2][2] - J[1][2] * J[2][1])
+                         - J[0][1] * (J[1][0] * J[2][2] - J[1][2] * J[2][0])
+                         + J[0][2] * (J[1][0] * J[2][1] - J[1][1] * J[2][0]);
+        const double w = YW[qx] * YW[qy] * YW[qz];
+        double G[3][3], phi[YS], dv[YS], psi[YU];
+        for (int a = 0; a < 3; ++a) for (int b = 0; b < 3; ++b)
+            G[a][b] = {float(alpha)!r} * w / det * (J[0][a] * J[0][b] + J[1][a] * J[1][b] + J[2][a] * J[2][b]);
+        for (int j = 0; j < YS; ++j) {{
+            int d, i[3];
+            hy_dof(j, &d, i);
+            phi[j] = 1.0; dv[j] = 1.0;
+            for (int e = 0; e < 3; ++e) {{
+                phi[j] *= e == d ? YC[q[e]][i[e]] : YG[q[e]][i[e]];
+                dv[j] *= e == d ? YD[q[e]][i[e]] : YG[q[e]][i[e]];
+            }}
+        }}
+        for (int a = 0; a < YK; ++a) for (int b = 0; b < YK; ++b) for (int c = 0; c < YK; ++c)
+            psi[(a * YK + b) * YK + c] = YG[qx][a] * YG[qy][b] * YG[qz][c];
+        for (int i = 0; i < YS; ++i) {{
+            int di, ii[3];
+            hy_dof(i, &di, ii);
+            for (int j = 0; j < YS; ++j) {{
+                int dj, jj[3];
+                hy_dof(j, &dj, jj);
+                A[i][j] += G[di][dj] * phi[i] * phi[j];
+            }}
+            for (int v = 0; v < YU; ++v) Bm[v][i] += w * psi[v] * dv[i];
+        }}
+    }}
+    /* Cholesky A = L L^T in place (lower triangle) */
+    for (int j = 0; j < YS; ++j) {{
+        double s = A[j][j];
+        for (int m = 0; m < j; ++m) s -= A[j][m] * A[j][m];
+        A[j][j] = sqrt(s);
+        for (int i = j + 1; i < YS; ++i) {{
+            double t = A[i][j];
+            for (int m = 0; m < j; ++m) t -= A[i][m] * A[j][m];
+            A[i][j] = t / A[j][j];
+        }}
+    }}
+    /* Y = A^-1 [B^T C^T] */
+    for (int i = 0; i < YS; ++i) for (int c = 0; c < YU + YF; ++c) Y[i][c] = c < YU ? Bm[c][i] : 0.0;
+    for (int t = 0; t < YF; ++t) {{
+        double ct;
+        const int i = hy_face(t, &ct);
+        Y[i][YU + t] = ct;
+    }}
+    for (int c = 0; c < YU + YF; ++c) {{
+        for (int i = 0; i < YS; ++i) {{
+            double s = Y[i][c];
+            for (int m = 0; m < i; ++m) s -= A[i][m] * Y[m][c];
+            Y[i][c] = s / A[i][i];
+        }}
+        for (int i = YS - 1; i >= 0; --i) {{
+            double s = Y[i][c];
+            for (int m = i + 1; m < YS; ++m) s -= A[m][i] * Y[m][c];
+            Y[i][c] = s / A[i][i];
+        }}
+    }}
+    /* S_B = B Y_B (Cholesky in place), P = B Y_C, then P <- S_B^-1 P */
+    for (int v = 0; v < YU; ++v) {{
+        for (int u = 0; u < YU; ++u) {{
+            double s = 0.0;
+            for (int j = 0; j < YS; ++j) s += Bm[v][j] * Y[j][u];
+            SB[v][u] = s;
+        }}
+        for (int t = 0; t < YF; ++t) {{
+            double s = 0.0;
+            for (int j = 0; j < YS; ++j) s += Bm[v][j] * Y[j][YU + t];
+            P[v][t] = s;
+        }}
+    }}
+    for (int j = 0; j < YU; ++j) {{
+        double s = SB[j][j];
+        for (int m = 0; m < j; ++m) s -= SB[j][m] * SB[j][m];
+        SB[j][j] = sqrt(s);
+        for (int i = j + 1; i < YU; ++i) {{
+            double t = SB[i][j];
+            for (int m = 0; m < j; ++m) t -= SB[i][m] * SB[j][m];
+            SB[i][j] = t / SB[j][j];
+        }}
+    }}
+    double W[YU][YF];
+    for (int c = 0; c < YF; ++c) {{
+        for (int i = 0; i < YU; ++i) {{
+            double s = P[i][c];
+            for (int m = 0; m < i; ++m) s -= SB[i][m] * W[m][c];
+            W[i][c] = s / SB[i][i];
+        }}
+        for (int i = YU - 1; i >= 0; --i) {{
+            double s = W[i][c];
+            for (int m = i + 1; m < YU; ++m) s -= SB[m][i] * W[m][c];
+            W[i][c] = s / SB[i][i];
+        }}
+    }}
+    /* H = C Y_C - P^T S_B^-1 P */
+    for (int t = 0; t < YF; ++t) {{
+        double ct;
+        const int i = hy_face(t, &ct);
+        for (int u = 0; u < YF; ++u) {{
+            double h = ct * Y[i][YU + u];
+            for (int v = 0; v < YU; ++v) h -= P[v][t] * W[v][u];
+            Hl[t * YF + u] += h;
+        }}
+    }}
+}}
+#undef YQ
+#undef YK
+#undef YS
+#undef YU
+#undef YF
+"""
+    return CStringKernel(code, name)
+
+
+def assemble_hybrid_trace_generic(pc: "HybridizationPC", tensor: op2.Mat = None):
+    """The trace matrix H of ``pc`` through the generic wrapper path (:func:`hybridization_kernel`, k = 2) into
+    ``tensor`` (a new Mat on ``pc.mat``'s sparsity if None), with the same masked lgmaps and unit diagonal on the
+    natural-condition faces: the cross-check and the baseline of the hand-written HY_CONDENSE kernel."""
+    from . import codegen
+    F, T = pc.form, pc.trace
+    S = F.Sigma
+    if tensor is None:
+        tensor = op2.Mat(pc.mat.sparsity)
+    tensor.zero()
+    lg = np.arange(T.node_count, dtype=np.int32)
+    lg[pc.natural_nodes] = -1
+    codegen.par_loop(hybridization_kernel(S.degree, F.alpha), S.cell_set,
+                     tensor(op2.INC, (pc.trace_map, pc.trace_map), lgmaps=(lg, lg)),
+                     S.coordinates(op2.READ, S.coord_map))
+    tensor.set_local_diagonal_entries(pc.natural_nodes, 1.0)
+    tensor.assemble()
+    return tensor
+
+
+class HybridizationPC:
+    """Firedrake's ``HybridizationPC`` for :class:`MixedPoisson` (NCF_k x DQ_{k-1}, k = 2..3): the flux space is broken
+    cell by cell, normal continuity is enforced by a multiplier lambda in the HDiv-trace space ``trace`` (degree
+    k - 1), and every local unknown is eliminated, which leaves one symmetric positive (semi-)definite system H lambda
+    = r on the faces.  Its solution reconstructs the SAME (sigma, u) as the mixed system.
+
+    - ``w``: one value per flux dof, 1 / the number of cells holding it (1/2 on interior faces): the load split
+      f_K = (w o L[0], L[1]) and the average of the two sides' sigma_K.
+    - ``mat``: the trace matrix H (an :class:`op2.Mat`, assembled once on the device, form "mixed_poisson_hybrid" at
+      rank 2).  Faces under a flux condition (``bcs``, ``DirichletBC(Sigma, 0.0, s)``) keep free multipliers, whose
+      rows enforce sigma.n = 0; every other boundary face is a natural-condition face with lambda = 0: masked by the
+      lgmaps, with a unit diagonal.
+    - ``forward(L) -> r``, ``trace_solve(r, lam)`` (CG) and ``backward(lam, L, up)``.
+
+    Every kernel recomputes the local factorisations (csrc/hybrid_hex.cu); device mode only."""
+
+    def __init__(self, F: MixedPoisson, bcs=()):
+        S, Q = F.Sigma, F.Q
+        k = S.degree
+        if k == 4:
+            raise NotImplementedError("HybridizationPC: NCF degree 4 is not built: its local flux mass matrix alone "
+                                      "(240^2 doubles, 460 KB) exceeds the 227 KB of shared memory of an SM; degrees "
+                                      "2..3")
+        if not 2 <= k <= 3:
+            raise NotImplementedError(f"HybridizationPC: NCF degree {k} outside 2..3")
+        self.form, self.bcs = F, tuple(bcs)
+        for bc in self.bcs:
+            if bc.V is not S:
+                raise ValueError("MixedPoisson's DirichletBCs are flux conditions on its NCF space")
+        self.trace = T = FunctionSpace(S.mesh, k - 1, family="HDiv Trace")
+        self.trace_map = op2.Map(S.cell_set, T.node_set, T.V.arity, T.V.cell_node_map, offset=T.V.offset)
+        self._maps = [self.trace_map, S.coord_map, S.cell_node_map, F.pressure_map]
+        counts = np.bincount(S.V.full_cell_node_list().ravel(), minlength=S.node_count)
+        self.w = S.dat(1.0 / counts)
+        flux = [s for bc in self.bcs for s in bc.sub_domains]
+        natural = [s for s in _BOUNDARY_SUB_DOMAINS if not any(_same_name(s, t) for t in flux)]
+        self.natural_nodes = (np.unique(np.concatenate([T.boundary_nodes(s) for s in natural])).astype(np.int32)
+                              if natural else np.zeros(0, dtype=np.int32))
+        self._natural = op2.Subset(T.node_set, self.natural_nodes)
+        self.mat = op2.Mat(op2.Sparsity((T.node_set, T.node_set), [(self.trace_map, self.trace_map, None)]))
+        self._gk = {rank: op2.GlobalKernel(op2.Kernel("mixed_poisson_hybrid", degree=k, alpha=F.alpha, rank=rank),
+                                           self._maps, extruded=True) for rank in (1, 2)}
+        self._gkr = op2.GlobalKernel(op2.Kernel("mixed_poisson_reconstruct", degree=k, alpha=F.alpha), self._maps,
+                                     extruded=True)
+        self.assemble()
+        self._dinv = self._ones = None
+
+    def assemble(self):
+        """H into ``mat``: zero, one condensation pass over the cells, unit diagonal on the natural faces."""
+        S, T = self.form.Sigma, self.trace
+        lg = np.arange(T.node_count, dtype=np.int32)
+        lg[self.natural_nodes] = -1
+        self.mat.zero()
+        op2.Parloop(self._gk[2], S.cell_set, [self.mat(op2.INC, (self.trace_map, self.trace_map), lgmaps=(lg, lg)),
+                                              S.coordinates(op2.READ, S.coord_map)])()
+        self.mat.set_local_diagonal_entries(self.natural_nodes, 1.0)
+        self.mat.assemble()
+        return self.mat
+
+    def forward(self, L: op2.MixedDat, r: op2.Dat = None):
+        """r = sum_K C K_K^-1 (w o L[0], L[1]), zero on the natural-condition faces."""
+        S, F = self.form.Sigma, self.form
+        if r is None:
+            r = self.trace.dat()
+        r.zero()
+        r.device_ptr
+        op2.Parloop(self._gk[1], S.cell_set,
+                    [r(op2.INC, self.trace_map), S.coordinates(op2.READ, S.coord_map), L[0](op2.READ, S.cell_node_map),
+                     self.w(op2.READ, S.cell_node_map), L[1](op2.READ, F.pressure_map)])()
+        r.zero(self._natural)
+        return r
+
+    def diagonal_inverse(self):
+        """diag(H)^-1 (the trace CG's Jacobi preconditioner), one device pass over the CSR."""
+        from . import _lib
+        if self._dinv is None:
+            from . import mg as _mg
+            d = self.trace.dat()
+            _lib.check(_lib.lib().fdb_mat_get_diagonal(self.mat.handle, d.device_ptr), "fdb_mat_get_diagonal")
+            d._device_written()
+            op2.par_loop(_mg.reciprocal_kernel(1), self.trace.node_set, d(op2.RW))
+            self._dinv = d
+        return self._dinv
+
+    def trace_solve(self, r: op2.Dat, lam: op2.Dat, rtol=1e-8, maxit=10000, pc_type="jacobi", nullspace=False):
+        """CG on H lam = r from lam = 0, Jacobi-preconditioned (``pc_type`` "jacobi") or not ("none").  With
+        ``nullspace`` (flux conditions on the whole boundary, H 1 = 0) the plain mean is removed from r and from every
+        preconditioned vector.  Returns (iterations, residual history)."""
+        from . import _lib
+        from . import mg as _mg
+        lib = _lib.lib()
+        n = r._data.size
+        if nullspace and self._ones is None:
+            self._ones = self.trace.dat(np.ones(n))
+        ones = self._ones
+        if nullspace:
+            r.axpy(-r.inner(ones) / n, ones)
+        dinv = self.diagonal_inverse() if pc_type == "jacobi" else None
+
+        def M(x, z):
+            if dinv is not None:
+                _lib.check(lib.fdb_vec_pointwise_mult(n, x.device_ptr, dinv.device_ptr, z.device_ptr))
+                z._device_written()
+            else:
+                x.copy(z)
+            if nullspace:
+                z.axpy(-z.inner(ones) / n, ones)
+
+        lam.zero()
+        lam.device_ptr
+        return _mg.pcg(self.mat, r, lam, M, rtol=rtol, maxit=maxit)
+
+    def backward(self, lam: op2.Dat, L: op2.MixedDat, up: op2.MixedDat):
+        """(sigma, u) = sum_K (w o sigma_K, u_K), (sigma_K, u_K) = K_K^-1 ((w o L[0], L[1]) - C^T lam)."""
+        S, F = self.form.Sigma, self.form
+        up.zero()
+        for d in up:
+            d.device_ptr
+        op2.Parloop(self._gkr, S.cell_set,
+                    [up[0](op2.INC, S.cell_node_map), S.coordinates(op2.READ, S.coord_map),
+                     lam(op2.READ, self.trace_map), L[0](op2.READ, S.cell_node_map), self.w(op2.READ, S.cell_node_map),
+                     up[1](op2.INC, F.pressure_map), L[1](op2.READ, F.pressure_map)])()
+        return up
+
+
 class ConvergenceError(RuntimeError):
     """A nonlinear solve that cannot go on (firedrake.exceptions.ConvergenceError); ``reason`` is the
     SNES converged reason, e.g. "DIVERGED_FNORM_NAN"."""
@@ -4649,6 +4984,10 @@ def _solve_mixed_poisson(F: MixedPoisson, L: op2.MixedDat, up: op2.MixedDat, bcs
     (iterations, residual history)."""
     from . import _lib
     from . import mg as _mg
+    flat = _flatten("", solver_parameters or {})
+    if flat.get("pc_type") == "python" or "pc_python_type" in flat or any(k.startswith("hybridization")
+                                                                           for k in flat):
+        return _solve_mixed_poisson_hybrid(F, L, up, bcs, flat, nullspace)
     sp = dict(_MIXED_POISSON_OPTIONS)
     sp.update(solver_parameters or {})
     _check_mixed_poisson_options(sp)
@@ -4751,6 +5090,108 @@ def _solve_mixed_poisson(F: MixedPoisson, L: op2.MixedDat, up: op2.MixedDat, bcs
             r.copy(z)
             remove_mean(z)
     its, hist = gmres(A, b, up, M, rtol=sp["ksp_rtol"], restart=sp["ksp_gmres_restart"], maxit=sp["ksp_max_it"])
+    if nullspace:
+        remove_mean(up)
+    for bc in bcs:
+        bc.apply(up[0])
+    return its, hist
+
+
+_HYBRID_OPTIONS = {"mat_type": "matfree", "ksp_type": "preonly", "ksp_rtol": 1e-8, "ksp_max_it": 1000,
+                   "ksp_gmres_restart": 30, "pc_type": None, "pc_python_type": None,
+                   "hybridization_ksp_type": "cg", "hybridization_pc_type": "jacobi", "hybridization_ksp_rtol": 1e-8,
+                   "hybridization_ksp_max_it": 10000, "hybridization_mat_type": "aij"}
+
+
+def _check_hybrid_options(sp):
+    """The options of :func:`_solve_mixed_poisson_hybrid` (flattened): Firedrake's HybridizationPC with a CG trace
+    solve."""
+    for key in sp:
+        if "localsolve" in key:
+            raise NotImplementedError(f"option {key!r}: the Slate localsolve options are not implemented; the local "
+                                      f"systems are eliminated by batched dense factorisations on the device")
+        if key not in _HYBRID_OPTIONS:
+            raise NotImplementedError(f"option {key!r} is not implemented for HybridizationPC")
+    if sp["pc_type"] != "python":
+        raise NotImplementedError(f"pc_type {sp['pc_type']!r}: the hybridization options need pc_type 'python' with "
+                                  f"pc_python_type 'firedrake.HybridizationPC'")
+    if sp["pc_python_type"] is None:
+        raise NotImplementedError("pc_type 'python' needs pc_python_type: MixedPoisson takes "
+                                  "'firedrake.HybridizationPC'")
+    if sp["pc_python_type"] != "firedrake.HybridizationPC":
+        raise NotImplementedError(f"pc_python_type {sp['pc_python_type']!r}: MixedPoisson takes "
+                                  f"'firedrake.HybridizationPC' (or pc_type 'fieldsplit' for the Schur fieldsplit)")
+    if sp["mat_type"] != "matfree":
+        raise NotImplementedError(f"mat_type {sp['mat_type']!r}: MixedPoisson has no assembled matrix, use 'matfree'")
+    if sp["ksp_type"] == "cg":
+        raise ValueError("ksp_type cg needs a positive definite operator, and the mixed Poisson operator is "
+                         "indefinite: use preonly or gmres")
+    if sp["ksp_type"] not in ("preonly", "gmres"):
+        raise NotImplementedError(f"ksp_type {sp['ksp_type']!r}: HybridizationPC runs with preonly or gmres")
+    if sp["hybridization_ksp_type"] == "preonly":
+        raise NotImplementedError("hybridization_ksp_type 'preonly' needs a direct solver of the trace system, which "
+                                  "is not implemented: use 'cg'")
+    if sp["hybridization_ksp_type"] != "cg":
+        raise NotImplementedError(f"hybridization_ksp_type {sp['hybridization_ksp_type']!r}: the trace system is "
+                                  f"symmetric positive (semi-)definite, solved with 'cg'")
+    if sp["hybridization_pc_type"] not in ("jacobi", "none"):
+        raise NotImplementedError(f"hybridization_pc_type {sp['hybridization_pc_type']!r}: 'jacobi' or 'none'; direct "
+                                  f"solvers and scalable trace preconditioners (GTMG, AMG, multigrid) are not "
+                                  f"implemented")
+    if sp["hybridization_mat_type"] != "aij":
+        raise NotImplementedError(f"hybridization_mat_type {sp['hybridization_mat_type']!r}: the trace operator is "
+                                  f"assembled, 'aij'")
+
+
+def _solve_mixed_poisson_hybrid(F: MixedPoisson, L: op2.MixedDat, up: op2.MixedDat, bcs, flat, nullspace):
+    """:func:`_solve_mixed_poisson` with Firedrake's hybridisation options (nested under "hybridization" or flat):
+
+        {"mat_type": "matfree", "ksp_type": "preonly", "pc_type": "python",
+         "pc_python_type": "firedrake.HybridizationPC",
+         "hybridization": {"ksp_type": "cg", "pc_type": "jacobi", "ksp_rtol": 1e-10}}
+
+    ``ksp_type`` "preonly": one elimination (:meth:`HybridizationPC.forward`), the trace CG and one reconstruction;
+    the returned (iterations, residual history) are the trace CG's.  "gmres": :class:`HybridizationPC` as the right
+    preconditioner of the matrix-free mixed operator (``ksp_rtol``, ``ksp_max_it``, ``ksp_gmres_restart``).
+    ``hybridization_pc_type`` "jacobi" (the CSR diagonal) or "none", ``hybridization_ksp_rtol`` /
+    ``_max_it``.  ``nullspace`` "constant" as for the Schur solve.  Every other option is refused by name."""
+    sp = dict(_HYBRID_OPTIONS)
+    sp.update(flat)
+    _check_hybrid_options(sp)
+    if nullspace not in (None, "constant"):
+        raise NotImplementedError(f"nullspace {nullspace!r}: None or 'constant' (constant u)")
+    bcs = tuple(bcs)
+    pc = HybridizationPC(F, bcs)
+    Q = F.Q
+    remove_mean = _pressure_mean_remover(Q) if nullspace else None
+    b = F.dat()
+    L.copy(b)
+    for bc in bcs:
+        bc.zero(b[0])
+    if nullspace:
+        remove_mean(b)
+    r, lam = pc.trace.dat(), pc.trace.dat()
+    rtol, maxit, pct = sp["hybridization_ksp_rtol"], sp["hybridization_ksp_max_it"], sp["hybridization_pc_type"]
+
+    def M(x, z):
+        pc.forward(x, r)
+        pc.trace_solve(r, lam, rtol, maxit, pct, bool(nullspace))
+        pc.backward(lam, x, z)
+        for bc in bcs:
+            bc.set(z[0], x[0])
+        if nullspace:
+            remove_mean(z)
+
+    if sp["ksp_type"] == "preonly":
+        pc.forward(b, r)
+        its, hist = pc.trace_solve(r, lam, rtol, maxit, pct, bool(nullspace))
+        pc.backward(lam, b, up)
+    else:
+        A = MixedPoissonMatrixContext(F, bcs)
+        up.zero()
+        for d in up:
+            d.device_ptr
+        its, hist = gmres(A, b, up, M, rtol=sp["ksp_rtol"], restart=sp["ksp_gmres_restart"], maxit=sp["ksp_max_it"])
     if nullspace:
         remove_mean(up)
     for bc in bcs:

@@ -187,3 +187,6 @@ int fdb_launch_spectral_helmholtz(fdb_kernel_s *k, fdb_int start, fdb_int end, i
 // FDB_FORM_MIXED_POISSON[_SCHUR] (hdiv_hex.cu): args and maps as include/fdb200.h lists them for the form and mode
 int fdb_launch_hdiv(fdb_kernel_s *k, fdb_int start, fdb_int end, int nlay, const fdb_int *subset, void *const *args,
                     const fdb_int *const *maps);
+// FDB_FORM_MIXED_POISSON_HYBRID / _RECONSTRUCT (hybrid_hex.cu): args and maps as include/fdb200.h lists them
+int fdb_launch_hybrid(fdb_kernel_s *k, fdb_int start, fdb_int end, int nlay, const fdb_int *subset, void *const *args,
+                      const fdb_int *const *maps);

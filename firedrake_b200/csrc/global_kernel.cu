@@ -298,7 +298,7 @@ static int device_pointers(const fdb_call_args *a, bool mat, void **args, const 
 // fdb_kernel_call hands its arguments to the launchers.
 enum { MODE_ACTION, MODE_MATRIX, MODE_DIAGONAL };
 enum { LAUNCH_HELMHOLTZ, LAUNCH_HELMHOLTZ_COEF, LAUNCH_ELASTICITY, LAUNCH_STOKES, LAUNCH_BOUNDARY, LAUNCH_DG_FACET,
-       LAUNCH_DG_TRANSPORT, LAUNCH_P_TRANSFER, LAUNCH_SPECTRAL, LAUNCH_HDIV };
+       LAUNCH_DG_TRANSPORT, LAUNCH_P_TRANSFER, LAUNCH_SPECTRAL, LAUNCH_HDIV, LAUNCH_HYBRID };
 // the degree of the second space of a form on two spaces: the descriptor's degree - 1 (Stokes' pressure, the
 // default of a row that does not name one), or any lower degree of an instantiated (fine, coarse) pair (the
 // p-multigrid transfers)
@@ -390,6 +390,12 @@ static const fdb_hex_form hex_forms[] = {
      FDB_INTEGRAL_CELL, SPACE2_PRESSURE},
     {FDB_FORM_MIXED_POISSON_SCHUR, "mixed_poisson_schur", 1, false, nullptr, 0, false, LAUNCH_HDIV, {4, 0, 4}, 2,
      "w, t", FDB_INTEGRAL_CELL, SPACE2_PRESSURE},
+    // its hybridisation on the HDiv-trace space: the condensed trace matrix (rank 2) and the elimination of the load
+    // (rank 1), and the reconstruction of (sigma, u) from lambda.  Device mode, atomic scatter, k = 2..3 (hybrid_call)
+    {FDB_FORM_MIXED_POISSON_HYBRID, "mixed_poisson_hybrid", 1, false, nullptr, 0, false, LAUNCH_HYBRID, {3, 3, 0}, 2,
+     "f_sigma, w, f_u", FDB_INTEGRAL_CELL, SPACE2_PRESSURE},
+    {FDB_FORM_MIXED_POISSON_RECONSTRUCT, "mixed_poisson_reconstruct", 1, false, nullptr, 0, false, LAUNCH_HYBRID,
+     {3, 0, 0}, 2, "lambda, f_sigma, w, y_u, f_u", FDB_INTEGRAL_CELL, SPACE2_PRESSURE},
 };
 
 // the (fine, coarse) degree pairs the transfer kernels instantiate (p_transfer_hex.cu)
@@ -520,8 +526,29 @@ static int kernel_create(const fdb_kernel_desc *d, const fdb_space2_desc *s2, fd
                   "the diagonal", f->name);
         return 1;
     }
+    if (f->launcher == LAUNCH_HYBRID) {
+        if (d->degree == 4) {
+            set_error("fdb_kernel_create: %s: degree 4 is not built: its local flux mass matrix alone (240^2 doubles, "
+                      "460 KB) exceeds the 227 KB of shared memory of an SM; degrees 2..3", f->name);
+            return 1;
+        }
+        if (mode == MODE_DIAGONAL) {
+            set_error("fdb_kernel_create: %s has no diagonal form: the trace matrix is assembled (rank 2)", f->name);
+            return 1;
+        }
+        if (mode == MODE_MATRIX && d->form != FDB_FORM_MIXED_POISSON_HYBRID) {
+            set_error("fdb_kernel_create: %s has no rank-2 form: it is the rank-1 reconstruction of (sigma, u); the "
+                      "trace matrix is mixed_poisson_hybrid at rank 2", f->name);
+            return 1;
+        }
+        if (d->scatter != FDB_SCATTER_ATOMIC) {
+            set_error("fdb_kernel_create: %s takes atomic scatter only: every entry receives at most two cell "
+                      "contributions, so the atomic sums are already bit-reproducible", f->name);
+            return 1;
+        }
+    }
     // (a mixed residual has no matrix or diagonal, nor has its Jacobian: the mixed-form message comes first)
-    if (f->space2 && mode != MODE_ACTION && f->launcher != LAUNCH_HDIV) {
+    if (f->space2 && mode != MODE_ACTION && f->launcher != LAUNCH_HDIV && f->launcher != LAUNCH_HYBRID) {
         set_error("fdb_kernel_create: %s is a mixed form, a rank-1 action only: it has no assembled matrix or "
                   "diagonal", f->name);
         return 1;
@@ -628,6 +655,8 @@ static int kernel_create(const fdb_kernel_desc *d, const fdb_space2_desc *s2, fd
     const int sides = d->integral == FDB_INTEGRAL_INTERIOR_FACET ? 2 : 1;
     k->arity = sides * k->n1d * k->n1d * k->n1d;
     if (f->launcher == LAUNCH_HDIV) k->arity = 3 * d->degree * d->degree * (d->degree + 1);    // NCF_k
+    // the hybrid forms: offset0 holds the trace map's 6k^2 layer offsets, then the NCF map's 3k^2(k+1)
+    if (f->launcher == LAUNCH_HYBRID) k->arity = 6 * d->degree * d->degree + 3 * d->degree * d->degree * (d->degree + 1);
     const int arity1 = sides * 8;
     memset(k->h_off0, 0, sizeof(k->h_off0));
     memset(k->h_off1, 0, sizeof(k->h_off1));
@@ -746,6 +775,32 @@ static int hdiv_call(fdb_kernel_s *k, const fdb_call_args *a, int nlay)
     return fdb_launch_hdiv(k, a->start, a->end, nlay, a->subset, a->args, a->maps);
 }
 
+// the hybridised mixed Poisson forms (FDB_FORM_MIXED_POISSON_HYBRID / _RECONSTRUCT): args and maps as include/fdb200.h
+// lists them, device mode only, atomic scatter
+static int hybrid_call(fdb_kernel_s *k, const fdb_call_args *a, int nlay)
+{
+    const fdb_hex_form *f = k->hex;
+    const int mode = hex_mode(&k->desc);
+    const bool reconstruct = k->desc.form == FDB_FORM_MIXED_POISSON_RECONSTRUCT;
+    const char *sig = mode == MODE_MATRIX ? "H mat, coords"
+                      : (reconstruct ? "y_sigma, coords, lambda, f_sigma, w, y_u, f_u" : "r, coords, f_sigma, w, f_u");
+    const char *mapsig = mode == MODE_MATRIX ? "trace map, coord map"
+                         : (reconstruct ? "NCF map, coord map, trace map, DQ map"
+                                        : "trace map, coord map, NCF map, DQ map");
+    const int want = mode == MODE_MATRIX ? 2 : (reconstruct ? 7 : 5);
+    const int want_maps = mode == MODE_MATRIX ? 2 : 4;
+    if (a->location != FDB_LOC_DEVICE) {
+        set_error("fdb_kernel_call: %s takes device-resident Dats only (no host-pointer mode)", f->name);
+        return 1;
+    }
+    if (a->nargs != want || a->nmaps != want_maps) {
+        set_error("fdb_kernel_call: %s %s expects %d device args (%s) and %d maps (%s), got %d/%d", f->name,
+                  mode_name[mode], want, sig, want_maps, mapsig, a->nargs, a->nmaps);
+        return 1;
+    }
+    return fdb_launch_hybrid(k, a->start, a->end, nlay, a->subset, a->args, a->maps);
+}
+
 extern "C" {
 
 int fdb_kernel_create(const fdb_kernel_desc *d, fdb_kernel_t *out)
@@ -861,6 +916,7 @@ int fdb_kernel_call(fdb_kernel_t k, const fdb_call_args *a)
     const fdb_hex_form *f = k->hex;
     if (f->launcher == LAUNCH_P_TRANSFER) return p_transfer_call(k, a, nlay);
     if (f->launcher == LAUNCH_HDIV) return hdiv_call(k, a, nlay);
+    if (f->launcher == LAUNCH_HYBRID) return hybrid_call(k, a, nlay);
     const int mode = hex_mode(&k->desc);
     const bool transport_facets = f->launcher == LAUNCH_DG_TRANSPORT && k->desc.integral != FDB_INTEGRAL_CELL;
     if (f->integral != FDB_INTEGRAL_CELL && a->location != FDB_LOC_DEVICE) {

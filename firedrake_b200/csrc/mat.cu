@@ -143,6 +143,24 @@ __global__ void k_spmv(fdb_int nrows, const long long *__restrict__ rowptr,
     }
 }
 
+// d[r] = A[r][r] (0 where the pattern has no diagonal entry), scalar matrices
+__global__ void k_get_diag(const long long *__restrict__ rowptr, const fdb_int *__restrict__ colidx,
+                           const double *__restrict__ vals, fdb_int n, double *__restrict__ d)
+{
+    for (fdb_int r = blockIdx.x * blockDim.x + threadIdx.x; r < n; r += gridDim.x * blockDim.x) {
+        long long lo = rowptr[r], hi = rowptr[r + 1];
+        if (hi == lo) {
+            d[r] = 0.0;
+            continue;
+        }
+        while (hi - lo > 1) {
+            long long mid = (lo + hi) >> 1;
+            if (colidx[mid] <= r) lo = mid; else hi = mid;
+        }
+        d[r] = colidx[lo] == r ? vals[lo] : 0.0;
+    }
+}
+
 __global__ void k_set_diag(const long long *__restrict__ rowptr, const fdb_int *__restrict__ colidx,
                            double *__restrict__ vals, const fdb_int *__restrict__ rows, fdb_int n,
                            double value)
@@ -584,6 +602,20 @@ int fdb_mat_set_diagonal_blocked(fdb_mat_t m, const fdb_int *rows_host, fdb_int 
     FDB_LAUNCH_CHECK();
     FDB_CUDA(cudaStreamSynchronize(st));
     cudaFree(d_rows);
+    return 0;
+}
+
+int fdb_mat_get_diagonal(fdb_mat_t m, double *d)
+{
+    if (require_init()) return 1;
+    if (m->bs != 1) {
+        set_error("fdb_mat_get_diagonal: scalar matrices only (block size %d)", m->bs);
+        return 1;
+    }
+    if (materialise_zero(m)) return 1;
+    if (m->nrows <= 0) return 0;
+    k_get_diag<<<grid1d(m->nrows), 256, 0, ctx().stream>>>(m->d_rowptr, m->d_colidx, m->d_vals, m->nrows, d);
+    FDB_LAUNCH_CHECK();
     return 0;
 }
 

@@ -1456,6 +1456,14 @@ class Kernel:
     (S_p u when t is zero on entry), the diagonal (INC, READ) = (d, W) adds diag(B W B^T).  Both are created with the
     DQ space as the second space (the maps: NCF, coordinate, DQ for "mixed_poisson"; DQ, NCF for the Schur form).
     Device-resident Dats only.
+
+    "mixed_poisson_hybrid" is the hybridisation of "mixed_poisson" on the HDiv-trace space (``degree`` = k, 2..3): at
+    rank 2 the condensed trace matrix H = sum_K C K_K^-1 C^T (INC Mat through the trace map, coordinates); at rank 1
+    the eliminated load r = sum_K C K_K^-1 f_K (INC, READ, READ, READ, READ) = (r, coordinates, sigma load, w, u load)
+    through the trace, coordinate, NCF and DQ maps, f_K = (w o sigma load, u load).  "mixed_poisson_reconstruct"
+    gives (sigma, u) cell by cell from the multiplier: (INC, READ, READ, READ, READ, INC, READ) = (sigma output,
+    coordinates, lambda, sigma load, w, u output, u load), sigma output += w o sigma_K, u output += u_K.  The
+    GlobalKernel's ``arguments`` are always [trace map, coordinate map, NCF map, DQ map].  Device-resident Dats only.
     """
     form: str = "helmholtz"
     degree: int = 1
@@ -1498,6 +1506,14 @@ class Kernel:
             if len(self.d) != 3:
                 raise ValueError("d holds the three coefficients of D(s) = d0 + d1 s + d2 s^2")
         spec = _FORMS.get(self.form)
+        if spec and spec.hybrid:
+            if self.form == "mixed_poisson_reconstruct":
+                acc = (INC, READ, READ, READ, READ, INC, READ)
+            else:
+                acc = (INC, READ) if self.rank == 2 else (INC, READ, READ, READ, READ)
+            object.__setattr__(self, "accesses", acc)
+            object.__setattr__(self, "name", self.form + ("_matrix" if self.rank == 2 else ""))
+            return
         if spec and spec.hdiv:
             if self.form == "mixed_poisson":
                 acc = (INC, READ) if self.diagonal else (INC, READ, READ, INC, READ)
@@ -1578,6 +1594,7 @@ class _Form(NamedTuple):
     gll: bool = False           # stated on the GLL rule at the nodes: the default element is the collocated GLL one
     hdiv: bool = False          # a mixed Poisson form on NCF_k x DQ_{k-1}
     temperature: bool = False   # also reads and writes a temperature on the pressure map (Boussinesq)
+    hybrid: bool = False        # the hybridised mixed Poisson forms on the HDiv-trace space
 
 
 _FORMS = {"helmholtz": _Form(_lib.FORM_HELMHOLTZ),
@@ -1605,7 +1622,9 @@ _FORMS = {"helmholtz": _Form(_lib.FORM_HELMHOLTZ),
           "mixed_poisson_schur": _Form(_lib.FORM_MIXED_POISSON_SCHUR, hdiv=True),
           "boussinesq": _Form(_lib.FORM_BOUSSINESQ, residual=True, pressure=True, temperature=True),
           "boussinesq_jacobian": _Form(_lib.FORM_BOUSSINESQ_JACOBIAN, coefficient=True, pressure=True,
-                                       temperature=True)}
+                                       temperature=True),
+          "mixed_poisson_hybrid": _Form(_lib.FORM_MIXED_POISSON_HYBRID, hdiv=True, hybrid=True),
+          "mixed_poisson_reconstruct": _Form(_lib.FORM_MIXED_POISSON_RECONSTRUCT, hdiv=True, hybrid=True)}
 _INTEGRALS = {"cell": _lib.INTEGRAL_CELL, "exterior_facet": _lib.INTEGRAL_EXTERIOR_FACET,
               "interior_facet": _lib.INTEGRAL_INTERIOR_FACET, "fused": _lib.INTEGRAL_FUSED}
 
@@ -1832,15 +1851,21 @@ class GlobalKernel:
             for q in range(el.nq):
                 for a in range(k):
                     s2.B[q * k + a] = elq.B[q, a]
-        if lk.form == "mixed_poisson":
+        mt = None
+        if _FORMS[lk.form].hybrid:
+            # the trace map's offsets first, then the NCF map's (include/fdb200.h)
+            mt, mc, ms, mu = self.arguments[:4]
+        elif lk.form == "mixed_poisson":
             ms, mc, mu = self.arguments[0], self.arguments[1], self.arguments[2]
         else:
             mu, ms, mc = self.arguments[0], self.arguments[1], None
         keep = []
         if self.extruded:
-            if ms.offset is None or mu.offset is None or (mc is not None and mc.offset is None):
+            if ms.offset is None or mu.offset is None or (mc is not None and mc.offset is None) or \
+                    (mt is not None and mt.offset is None):
                 raise MapValueError("extruded parloop needs maps with offsets")
-            keep = [np.ascontiguousarray(m.offset, dtype=IntType) for m in (ms, mu)]
+            off0 = ms.offset if mt is None else np.concatenate([mt.offset, ms.offset])
+            keep = [np.ascontiguousarray(off0, dtype=IntType), np.ascontiguousarray(mu.offset, dtype=IntType)]
             d.offset0 = keep[0].ctypes.data_as(C.POINTER(C.c_int32))
             s2.offset = keep[1].ctypes.data_as(C.POINTER(C.c_int32))
             if mc is not None:

@@ -209,6 +209,14 @@ class ExtrudedHexMesh:
             cache[degree] = ExtrudedHDivFunctionSpace(self, degree)
         return cache[degree]
 
+    def trace_function_space(self, degree: int) -> "ExtrudedTraceFunctionSpace":
+        """Firedrake's "HDiv Trace" space of degree ``degree`` = k - 1 (1..3): Q_{k-1} on every face, the Lagrange
+        multiplier of the hybridised NCF_k x DQ_{k-1} mixed Poisson problem."""
+        cache = self.__dict__.setdefault("_trace_fs_cache", {})
+        if degree not in cache:
+            cache[degree] = ExtrudedTraceFunctionSpace(self, degree)
+        return cache[degree]
+
     def _apply_warp(self, X):
         if self.warp == 0.0:
             return X
@@ -527,6 +535,75 @@ class ExtrudedHDivFunctionSpace:
             st = self._ent_start[mesh._face(mesh.cell_ix, mesh.cell_iy)]
             if sub_domain == "top":
                 st = st + mesh.nz * self.layer_stride
+            return np.sort((st[:, None] + np.arange(k2)[None, :]).ravel()).astype(IntType)
+        ents = {1: lambda: mesh._yedge(0, np.arange(ny)), 2: lambda: mesh._yedge(nx, np.arange(ny)),
+                3: lambda: mesh._xedge(np.arange(nx), 0), 4: lambda: mesh._xedge(np.arange(nx), ny)}
+        if sub_domain not in ents:
+            raise ValueError(f"unknown sub_domain {sub_domain!r}")
+        e = np.atleast_1d(ents[sub_domain]())
+        st, sz = self._ent_start[e], self._ent_colsize[e]
+        return np.sort(np.concatenate([np.arange(a, a + b) for a, b in zip(st, sz)])).astype(IntType)
+
+
+class ExtrudedTraceFunctionSpace:
+    """Firedrake's "HDiv Trace" space of degree k - 1 (k = 2..4) on an :class:`ExtrudedHexMesh`: Q_{k-1} on every
+    face of the mesh, its k^2 dofs the values at the k x k Gauss-Legendre points of the face -- the points of the NCF_k
+    face dofs of that face.
+
+    Local numbering (arity 6k^2): face ``2d + s`` (normal axis d, side s), then ``t0 * k + t1`` with the two GL
+    indices in axis order: exactly the order of the NCF_k face dofs of component d at CG index s
+    (:class:`ExtrudedHDivFunctionSpace`).  Global numbering: the NCF_k entity columns with the cell interiors removed,
+    in the same first-touch order: a base edge holds its ``nz`` vertical faces (``nz * k^2`` dofs), a base face its
+    ``nz + 1`` horizontal faces (``(nz + 1) * k^2``).  Every local dof has the layer offset k^2."""
+
+    def __init__(self, mesh: ExtrudedHexMesh, degree: int):
+        p = int(degree)
+        if not 1 <= p <= 3:
+            raise ValueError(f"HDiv Trace degree {p} outside 1..3")
+        self.mesh = mesh
+        self.degree = p
+        self.k = k = p + 1
+        k2 = k * k
+        self.arity = 6 * k2
+        nz = mesh.nz
+        NV, NEy, NEx, NF = mesh._nent
+        colsize = np.concatenate([np.zeros(NV, dtype=np.int64), np.full(NEy + NEx, nz * k2, dtype=np.int64),
+                                  np.full(NF, (nz + 1) * k2, dtype=np.int64)])
+        order = np.argsort(mesh._rank, kind="stable")
+        start_sorted = np.concatenate([[0], np.cumsum(colsize[order])[:-1]])
+        ent_start = np.empty(mesh.num_entities, dtype=np.int64)
+        ent_start[order] = start_sorted
+        self._ent_start, self._ent_colsize = ent_start, colsize
+        self.node_count = int(colsize.sum())
+        self.owned_node_count, self.ghost_node_count = self.node_count, 0
+        if self.node_count >= 2 ** 31:
+            raise ValueError("node count exceeds int32 IntType")
+        ix, iy = mesh.cell_ix, mesh.cell_iy
+        within = np.arange(k2, dtype=np.int64)
+        starts = [ent_start[mesh._yedge(ix, iy)], ent_start[mesh._yedge(ix + 1, iy)],
+                  ent_start[mesh._xedge(ix, iy)], ent_start[mesh._xedge(ix, iy + 1)],
+                  ent_start[mesh._face(ix, iy)], ent_start[mesh._face(ix, iy)] + k2]
+        self.cell_node_map = np.concatenate([st[:, None] + within[None, :] for st in starts],
+                                            axis=1).astype(IntType)
+        self.offset = np.full(self.arity, k2, dtype=IntType)
+
+    def full_cell_node_list(self):
+        """(num_cells, arity) map with the layer loop expanded: row ``c*nz + l`` is column c, layer l."""
+        nz = self.mesh.nz
+        lay = np.arange(nz, dtype=np.int64)
+        full = (self.cell_node_map[:, None, :].astype(np.int64)
+                + lay[None, :, None] * self.offset[None, None, :])
+        return full.reshape(-1, self.arity).astype(IntType)
+
+    def boundary_nodes(self, sub_domain):
+        """The trace dofs on a boundary: sub-domains 1..4 (x == 0, x == Lx, y == 0, y == Ly) and "bottom" / "top",
+        the names of the NCF space's."""
+        mesh, k2 = self.mesh, self.k ** 2
+        nx, ny = mesh.nx, mesh.ny
+        if sub_domain in ("bottom", "top"):
+            st = self._ent_start[mesh._face(mesh.cell_ix, mesh.cell_iy)]
+            if sub_domain == "top":
+                st = st + mesh.nz * k2
             return np.sort((st[:, None] + np.arange(k2)[None, :]).ravel()).astype(IntType)
         ents = {1: lambda: mesh._yedge(0, np.arange(ny)), 2: lambda: mesh._yedge(nx, np.arange(ny)),
                 3: lambda: mesh._xedge(np.arange(nx), 0), 4: lambda: mesh._xedge(np.arange(nx), ny)}

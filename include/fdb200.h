@@ -411,7 +411,7 @@ enum fdb_form {
                                    space) and restrictions as FDB_FORM_STOKES:
                                      action  [y_u INC, coords, u, y_p INC, p, y_T INC, T]
                                              maps [V map, coord map, Q map]                       */
-    FDB_FORM_BOUSSINESQ_JACOBIAN = 25
+    FDB_FORM_BOUSSINESQ_JACOBIAN = 25,
                                 /* its Gateaux derivative at (u0, T0) (exact Newton Jacobian, NOT symmetric),
                                    applied to the direction (w, r, s):
                                      J[(w, r, s); (v, q, S)] = FDB_FORM_NAVIER_STOKES_JACOBIAN at u0 on (w, r)
@@ -422,6 +422,32 @@ enum fdb_form {
                                    comes LAST: u0 through maps[0], T0 through maps[2]:
                                      action  [y_u INC, coords, w, y_p INC, r, y_T INC, s, u0, T0]
                                              maps [V map, coord map, Q map]                       */
+    FDB_FORM_MIXED_POISSON_HYBRID = 26,
+    FDB_FORM_MIXED_POISSON_RECONSTRUCT = 27,
+                                /* hybridisation of FDB_FORM_MIXED_POISSON (k = 2..3): the flux space broken cell by
+                                   cell, normal continuity enforced by lambda in the HDiv-trace space (Q_{k-1} on each
+                                   face, k^2 dofs at its Gauss-Legendre points; local numbering face 2d + s, then
+                                   t0 * k + t1 with the two GL indices in axis order: 6k^2 per cell).  With K_K the
+                                   cell's [[alpha M, B^T], [B, 0]] and C^ = [C 0], C[t][sigma-dof(t)] = o_t w_t0 w_t1
+                                   (o = -1 on side s = 0, +1 on s = 1; w the k-point GL weights):
+                                     H = sum_K C^ K_K^-1 C^^T   (symmetric positive semi-definite)
+                                     r = sum_K C^ K_K^-1 f_K,   (sigma_K, u_K) = K_K^-1 (f_K - C^^T lambda)
+                                   f_K = (w o f_sigma, f_u) gathered through the NCF and DQ maps, w one value per
+                                   flux dof.  Descriptor, second space and creation (fdb_kernel_create_mixed) as
+                                   FDB_FORM_MIXED_POISSON, except that offset0 holds the trace map's 6k^2 layer
+                                   offsets FOLLOWED by the NCF map's 3k^2(k+1) (offset1 the coordinate map's, the
+                                   second space's offset the DQ map's).  Degree 4 is refused (its local flux mass
+                                   matrix exceeds the shared memory of an SM).  Device mode, atomic scatter only
+                                   (every entry receives at most two cell contributions: bit-reproducible), extruded
+                                   and native hexes, no diagonal:
+                                     HYBRID       rank 2  [H mat INC, coords]   maps [trace map, coord map]
+                                                          H += H_K through the Mat's lgmaps (masked rows and
+                                                          columns are skipped)
+                                                  rank 1  [r INC, coords, f_sigma, w, f_u]
+                                                          maps [trace map, coord map, NCF map, DQ map]
+                                     RECONSTRUCT  rank 1  [y_sigma INC, coords, lambda, f_sigma, w, y_u INC, f_u]
+                                                          maps [NCF map, coord map, trace map, DQ map]
+                                                          y_sigma += w o sigma_K, y_u += u_K               */
 };
 
 enum fdb_cell {
@@ -703,6 +729,9 @@ int fdb_mat_set_diagonal(fdb_mat_t m, const fdb_int *rows_host, fdb_int n, doubl
 /* rows are NODE rows; idx = component to set, -1 = every component (the `idx` argument of
  * set_local_diagonal_entries, pyop2/types/mat.py:897-937) */
 int fdb_mat_set_diagonal_blocked(fdb_mat_t m, const fdb_int *rows_host, fdb_int n, double value, int idx);
+/* d[r] = A[r][r] into a device array of nrows doubles (0 where the pattern has no diagonal entry), scalar
+ * matrices: the Jacobi preconditioner of an assembled operator (HybridizationPC's trace CG) */
+int fdb_mat_get_diagonal(fdb_mat_t m, double *d);
 /* y = A x on device pointers (cross-check of assembled vs matrix-free action) */
 int fdb_mat_mult(fdb_mat_t m, const double *x, double *y);
 /* copy the CSR arrays to the host (any pointer may be NULL); rowptr is int64 */
