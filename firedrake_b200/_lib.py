@@ -42,6 +42,8 @@ FORM_BOUSSINESQ = 24                   # Navier-Stokes + buoyancy + temperature 
 FORM_BOUSSINESQ_JACOBIAN = 25          # its exact Gateaux derivative at (u0, T0)
 FORM_MIXED_POISSON_HYBRID = 26         # mixed Poisson hybridised: the condensed trace matrix (rank 2), its load (rank 1)
 FORM_MIXED_POISSON_RECONSTRUCT = 27    # (sigma, u) cell by cell from the trace multiplier lambda
+FORM_TRACE_PROLONG = 28                # CG1 vertex values -> HDiv-trace face points (GTMG)
+FORM_TRACE_RESTRICT = 29               # its transpose, HDiv trace -> CG1
 CELL_HEX_EXTRUDED = 1
 CELL_HEX = 2
 CELL_TRIANGLE = 3

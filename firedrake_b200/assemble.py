@@ -3694,6 +3694,7 @@ class HybridizationPC:
         self.w = S.dat(1.0 / counts)
         flux = [s for bc in self.bcs for s in bc.sub_domains]
         natural = [s for s in _BOUNDARY_SUB_DOMAINS if not any(_same_name(s, t) for t in flux)]
+        self.natural_sub_domains = tuple(natural)
         self.natural_nodes = (np.unique(np.concatenate([T.boundary_nodes(s) for s in natural])).astype(np.int32)
                               if natural else np.zeros(0, dtype=np.int32))
         self._natural = op2.Subset(T.node_set, self.natural_nodes)
@@ -3742,9 +3743,11 @@ class HybridizationPC:
             self._dinv = d
         return self._dinv
 
-    def trace_solve(self, r: op2.Dat, lam: op2.Dat, rtol=1e-8, maxit=10000, pc_type="jacobi", nullspace=False):
-        """CG on H lam = r from lam = 0, Jacobi-preconditioned (``pc_type`` "jacobi") or not ("none").  With
-        ``nullspace`` (flux conditions on the whole boundary, H 1 = 0) the plain mean is removed from r and from every
+    def trace_solve(self, r: op2.Dat, lam: op2.Dat, rtol=1e-8, maxit=10000, pc_type="jacobi", nullspace=False,
+                    cycle=None):
+        """CG on H lam = r from lam = 0, Jacobi-preconditioned (``pc_type`` "jacobi") or not ("none"), or, when
+        ``cycle`` (an :class:`mg.GTMG` on this object) is given, preconditioned by one GTMG cycle.  With ``nullspace``
+        (flux conditions on the whole boundary, H 1 = 0) the plain mean is removed from r and from every
         preconditioned vector.  Returns (iterations, residual history)."""
         from . import _lib
         from . import mg as _mg
@@ -3755,10 +3758,12 @@ class HybridizationPC:
         ones = self._ones
         if nullspace:
             r.axpy(-r.inner(ones) / n, ones)
-        dinv = self.diagonal_inverse() if pc_type == "jacobi" else None
+        dinv = self.diagonal_inverse() if pc_type == "jacobi" and cycle is None else None
 
         def M(x, z):
-            if dinv is not None:
+            if cycle is not None:
+                cycle(x, z)
+            elif dinv is not None:
                 _lib.check(lib.fdb_vec_pointwise_mult(n, x.device_ptr, dinv.device_ptr, z.device_ptr))
                 z._device_written()
             else:
@@ -4635,7 +4640,7 @@ def solve(form: Form, L: op2.Dat, u: op2.Dat, bcs=(), solver_parameters=None, hi
     if isinstance(form, Stokes):
         return _solve_stokes(form, L, u, bcs, solver_parameters, hierarchy, nullspace)
     if isinstance(form, MixedPoisson):
-        return _solve_mixed_poisson(form, L, u, bcs, solver_parameters, nullspace)
+        return _solve_mixed_poisson(form, L, u, bcs, solver_parameters, nullspace, hierarchy=hierarchy)
     if nullspace is not None:
         raise NotImplementedError("nullspace is implemented for MixedPoisson and Stokes forms only")
     symmetric = getattr(form, "symmetric", True)
@@ -4963,7 +4968,7 @@ def _check_mixed_poisson_options(sp):
 
 
 def _solve_mixed_poisson(F: MixedPoisson, L: op2.MixedDat, up: op2.MixedDat, bcs=(), solver_parameters=None,
-                         nullspace=None):
+                         nullspace=None, hierarchy=None):
     """``solve(a == L, up, bcs=bcs, solver_parameters=..., nullspace=...)`` for :class:`MixedPoisson`, with the
     options of Firedrake's saddle_point_pc demo, "Schur complement with S_p":
 
@@ -4987,7 +4992,7 @@ def _solve_mixed_poisson(F: MixedPoisson, L: op2.MixedDat, up: op2.MixedDat, bcs
     flat = _flatten("", solver_parameters or {})
     if flat.get("pc_type") == "python" or "pc_python_type" in flat or any(k.startswith("hybridization")
                                                                            for k in flat):
-        return _solve_mixed_poisson_hybrid(F, L, up, bcs, flat, nullspace)
+        return _solve_mixed_poisson_hybrid(F, L, up, bcs, flat, nullspace, hierarchy)
     sp = dict(_MIXED_POISSON_OPTIONS)
     sp.update(solver_parameters or {})
     _check_mixed_poisson_options(sp)
@@ -5100,7 +5105,60 @@ def _solve_mixed_poisson(F: MixedPoisson, L: op2.MixedDat, up: op2.MixedDat, bcs
 _HYBRID_OPTIONS = {"mat_type": "matfree", "ksp_type": "preonly", "ksp_rtol": 1e-8, "ksp_max_it": 1000,
                    "ksp_gmres_restart": 30, "pc_type": None, "pc_python_type": None,
                    "hybridization_ksp_type": "cg", "hybridization_pc_type": "jacobi", "hybridization_ksp_rtol": 1e-8,
-                   "hybridization_ksp_max_it": 10000, "hybridization_mat_type": "aij"}
+                   "hybridization_ksp_max_it": 10000, "hybridization_mat_type": "aij",
+                   "hybridization_pc_python_type": None}
+# the GTMG trace preconditioner's levels and coarse solve (hybridization_pc_python_type "firedrake.GTMGPC"): the
+# p-multigrid keys and defaults under the prefix "hybridization_gt_"
+_GTMG_KEYS = {"hybridization_gt_" + k[len("pmg_"):]: v for k, v in _PMG_KEYS.items() if k != "pmg_mg_coarse_degree"}
+
+
+def _check_gtmg_options(sp):
+    """The ``hybridization_gt_*`` keys of :func:`_check_hybrid_options`, refused by name where the engine's GTMG
+    differs from Firedrake's."""
+    for key in sorted(k for k in sp if k.startswith("hybridization_gt_")):
+        if key == "hybridization_gt_pc_mg_galerkin":
+            raise NotImplementedError("hybridization_gt_pc_mg_galerkin: the coarse operator is the rediscretised CG1 "
+                                      "Laplacian Form(P1, 1/alpha, 0); a Galerkin P^T H P is not built")
+        if key == "hybridization_gt_pc_mg_type":
+            if sp[key] != "multiplicative":
+                raise NotImplementedError(f"hybridization_gt_pc_mg_type {sp[key]!r}: the two-level cycle is "
+                                          f"'multiplicative' ('full' is not implemented)")
+            continue
+        if key == "hybridization_gt_mg_coarse_pc_mg_type" or key.startswith("hybridization_gt_mg_coarse_mg_levels_"):
+            raise NotImplementedError(f"{key}: the coarse V-cycle (mg_coarse pc_type 'mg') has the engine's fixed "
+                                      f"damped-Jacobi smoother and multiplicative cycle; its options are not taken")
+        if key not in _GTMG_KEYS:
+            raise NotImplementedError(f"unknown GTMG option {key}: the supported ones are "
+                                      f"{', '.join(_GTMG_KEYS)} and hybridization_gt_pc_mg_type 'multiplicative'")
+    o = dict(_GTMG_KEYS, **{k: v for k, v in sp.items() if k in _GTMG_KEYS})
+    if o["hybridization_gt_mg_coarse_pc_type"] in _DIRECT:
+        raise NotImplementedError(f"hybridization_gt_mg_coarse_pc_type {o['hybridization_gt_mg_coarse_pc_type']!r}: "
+                                  f"direct coarse solvers are not implemented; cg with jacobi or none, or preonly "
+                                  f"with mg")
+    if o["hybridization_gt_mg_levels_pc_type"] != "jacobi":
+        raise NotImplementedError(f"hybridization_gt_mg_levels_pc_type {o['hybridization_gt_mg_levels_pc_type']!r}: "
+                                  f"the trace smoother is Jacobi-preconditioned ('jacobi')")
+    if o["hybridization_gt_mg_levels_ksp_type"] not in ("chebyshev", "richardson"):
+        raise NotImplementedError(f"hybridization_gt_mg_levels_ksp_type {o['hybridization_gt_mg_levels_ksp_type']!r}: "
+                                  f"'chebyshev' or 'richardson'")
+    pair = (o["hybridization_gt_mg_coarse_ksp_type"], o["hybridization_gt_mg_coarse_pc_type"])
+    if pair not in (("cg", "jacobi"), ("cg", "none"), ("preonly", "mg")):
+        raise NotImplementedError(f"hybridization_gt_mg_coarse ksp_type {pair[0]!r} with pc_type {pair[1]!r}: cg with "
+                                  f"jacobi or none, or preonly with mg")
+    return o
+
+
+def _gtmg(pc, sp, hierarchy, nullspace):
+    """The :class:`mg.GTMG` of the checked hybridisation options ``sp``."""
+    from . import mg as _mg
+    o = _check_gtmg_options(sp)
+    est = tuple(float(v) for v in str(o["hybridization_gt_mg_levels_ksp_chebyshev_esteig"]).split(","))
+    return _mg.GTMG(pc, nullspace=nullspace, smoother=o["hybridization_gt_mg_levels_ksp_type"],
+                    nu=int(o["hybridization_gt_mg_levels_ksp_max_it"]), esteig=est,
+                    coarse_ksp=o["hybridization_gt_mg_coarse_ksp_type"],
+                    coarse_pc=o["hybridization_gt_mg_coarse_pc_type"],
+                    coarse_rtol=float(o["hybridization_gt_mg_coarse_ksp_rtol"]),
+                    coarse_maxit=int(o["hybridization_gt_mg_coarse_ksp_max_it"]), hierarchy=hierarchy)
 
 
 def _check_hybrid_options(sp):
@@ -5110,7 +5168,7 @@ def _check_hybrid_options(sp):
         if "localsolve" in key:
             raise NotImplementedError(f"option {key!r}: the Slate localsolve options are not implemented; the local "
                                       f"systems are eliminated by batched dense factorisations on the device")
-        if key not in _HYBRID_OPTIONS:
+        if key not in _HYBRID_OPTIONS and not key.startswith("hybridization_gt_"):
             raise NotImplementedError(f"option {key!r} is not implemented for HybridizationPC")
     if sp["pc_type"] != "python":
         raise NotImplementedError(f"pc_type {sp['pc_type']!r}: the hybridization options need pc_type 'python' with "
@@ -5134,16 +5192,31 @@ def _check_hybrid_options(sp):
     if sp["hybridization_ksp_type"] != "cg":
         raise NotImplementedError(f"hybridization_ksp_type {sp['hybridization_ksp_type']!r}: the trace system is "
                                   f"symmetric positive (semi-)definite, solved with 'cg'")
-    if sp["hybridization_pc_type"] not in ("jacobi", "none"):
-        raise NotImplementedError(f"hybridization_pc_type {sp['hybridization_pc_type']!r}: 'jacobi' or 'none'; direct "
-                                  f"solvers and scalable trace preconditioners (GTMG, AMG, multigrid) are not "
-                                  f"implemented")
+    gt = sorted(k for k in sp if k.startswith("hybridization_gt_"))
+    if sp["hybridization_pc_type"] == "python":
+        ppt = sp["hybridization_pc_python_type"]
+        if ppt is None:
+            raise NotImplementedError("hybridization_pc_type 'python' needs hybridization_pc_python_type: the trace "
+                                      "system takes 'firedrake.GTMGPC'")
+        if ppt != "firedrake.GTMGPC":
+            raise NotImplementedError(f"hybridization_pc_python_type {ppt!r}: the trace system takes "
+                                      f"'firedrake.GTMGPC'")
+        _check_gtmg_options(sp)
+    elif sp["hybridization_pc_type"] not in ("jacobi", "none"):
+        raise NotImplementedError(f"hybridization_pc_type {sp['hybridization_pc_type']!r}: 'jacobi', 'none' or "
+                                  f"'python' with 'firedrake.GTMGPC'; direct solvers and other scalable trace "
+                                  f"preconditioners (AMG, multigrid) are not implemented")
+    elif sp["hybridization_pc_python_type"] is not None or gt:
+        what = "hybridization_pc_python_type" if sp["hybridization_pc_python_type"] is not None else gt[0]
+        raise NotImplementedError(f"{what} needs hybridization_pc_type 'python' with hybridization_pc_python_type "
+                                  f"'firedrake.GTMGPC'")
     if sp["hybridization_mat_type"] != "aij":
         raise NotImplementedError(f"hybridization_mat_type {sp['hybridization_mat_type']!r}: the trace operator is "
                                   f"assembled, 'aij'")
 
 
-def _solve_mixed_poisson_hybrid(F: MixedPoisson, L: op2.MixedDat, up: op2.MixedDat, bcs, flat, nullspace):
+def _solve_mixed_poisson_hybrid(F: MixedPoisson, L: op2.MixedDat, up: op2.MixedDat, bcs, flat, nullspace,
+                                hierarchy=None):
     """:func:`_solve_mixed_poisson` with Firedrake's hybridisation options (nested under "hybridization" or flat):
 
         {"mat_type": "matfree", "ksp_type": "preonly", "pc_type": "python",
@@ -5154,7 +5227,11 @@ def _solve_mixed_poisson_hybrid(F: MixedPoisson, L: op2.MixedDat, up: op2.MixedD
     the returned (iterations, residual history) are the trace CG's.  "gmres": :class:`HybridizationPC` as the right
     preconditioner of the matrix-free mixed operator (``ksp_rtol``, ``ksp_max_it``, ``ksp_gmres_restart``).
     ``hybridization_pc_type`` "jacobi" (the CSR diagonal) or "none", ``hybridization_ksp_rtol`` /
-    ``_max_it``.  ``nullspace`` "constant" as for the Schur solve.  Every other option is refused by name."""
+    ``_max_it``.  ``hybridization_pc_type`` "python" with ``hybridization_pc_python_type`` "firedrake.GTMGPC"
+    preconditions the trace CG with one :class:`mg.GTMG` cycle, configured by the ``hybridization_gt_mg_levels_*`` /
+    ``hybridization_gt_mg_coarse_*`` keys of ``_GTMG_KEYS`` (nested under "gt" or flat); coarse "preonly" / "mg" needs
+    ``hierarchy``, a mg.MeshHierarchy whose finest mesh is the problem's.  ``nullspace`` "constant" as for the Schur
+    solve.  Every other option is refused by name."""
     sp = dict(_HYBRID_OPTIONS)
     sp.update(flat)
     _check_hybrid_options(sp)
@@ -5172,10 +5249,11 @@ def _solve_mixed_poisson_hybrid(F: MixedPoisson, L: op2.MixedDat, up: op2.MixedD
         remove_mean(b)
     r, lam = pc.trace.dat(), pc.trace.dat()
     rtol, maxit, pct = sp["hybridization_ksp_rtol"], sp["hybridization_ksp_max_it"], sp["hybridization_pc_type"]
+    cycle = _gtmg(pc, sp, hierarchy, bool(nullspace)) if pct == "python" else None
 
     def M(x, z):
         pc.forward(x, r)
-        pc.trace_solve(r, lam, rtol, maxit, pct, bool(nullspace))
+        pc.trace_solve(r, lam, rtol, maxit, pct, bool(nullspace), cycle)
         pc.backward(lam, x, z)
         for bc in bcs:
             bc.set(z[0], x[0])
@@ -5184,7 +5262,7 @@ def _solve_mixed_poisson_hybrid(F: MixedPoisson, L: op2.MixedDat, up: op2.MixedD
 
     if sp["ksp_type"] == "preonly":
         pc.forward(b, r)
-        its, hist = pc.trace_solve(r, lam, rtol, maxit, pct, bool(nullspace))
+        its, hist = pc.trace_solve(r, lam, rtol, maxit, pct, bool(nullspace), cycle)
         pc.backward(lam, b, up)
     else:
         A = MixedPoissonMatrixContext(F, bcs)

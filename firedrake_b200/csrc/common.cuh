@@ -190,3 +190,7 @@ int fdb_launch_hdiv(fdb_kernel_s *k, fdb_int start, fdb_int end, int nlay, const
 // FDB_FORM_MIXED_POISSON_HYBRID / _RECONSTRUCT (hybrid_hex.cu): args and maps as include/fdb200.h lists them
 int fdb_launch_hybrid(fdb_kernel_s *k, fdb_int start, fdb_int end, int nlay, const fdb_int *subset, void *const *args,
                       const fdb_int *const *maps);
+// FDB_FORM_TRACE_PROLONG / _RESTRICT (trace_transfer_hex.cu): out, in, w (restrict only), the trace and CG1 maps
+int fdb_launch_trace_transfer(fdb_kernel_s *k, fdb_int start, fdb_int end, int nlay, const fdb_int *subset,
+                              double *out, const double *in, const double *w, const fdb_int *mapt,
+                              const fdb_int *mapv);

@@ -79,9 +79,8 @@ void endpoint_tables(int n, const double *B, const double *xq, double *Bend)
 // colour share a dof column: the deterministic fallback of the north_star
 // ("warp-aggregated atomic kernel with a colouring fallback").  Host side,
 // once per map.
-int build_colouring(fdb_kernel_s *k, const fdb_int *h_map, fdb_int ncols)
+int build_colouring(fdb_kernel_s *k, const fdb_int *h_map, fdb_int ncols, int arity)
 {
-    const int arity = k->arity;
     fdb_int maxnode = 0;
     for (long long i = 0; i < (long long)ncols * arity; i++) maxnode = std::max(maxnode, h_map[i]);
     // node -> bitmask of colours already used by a column touching it
@@ -298,11 +297,12 @@ static int device_pointers(const fdb_call_args *a, bool mat, void **args, const 
 // fdb_kernel_call hands its arguments to the launchers.
 enum { MODE_ACTION, MODE_MATRIX, MODE_DIAGONAL };
 enum { LAUNCH_HELMHOLTZ, LAUNCH_HELMHOLTZ_COEF, LAUNCH_ELASTICITY, LAUNCH_STOKES, LAUNCH_BOUNDARY, LAUNCH_DG_FACET,
-       LAUNCH_DG_TRANSPORT, LAUNCH_P_TRANSFER, LAUNCH_SPECTRAL, LAUNCH_HDIV, LAUNCH_HYBRID };
+       LAUNCH_DG_TRANSPORT, LAUNCH_P_TRANSFER, LAUNCH_SPECTRAL, LAUNCH_HDIV, LAUNCH_HYBRID, LAUNCH_TRACE_TRANSFER };
 // the degree of the second space of a form on two spaces: the descriptor's degree - 1 (Stokes' pressure, the
 // default of a row that does not name one), or any lower degree of an instantiated (fine, coarse) pair (the
-// p-multigrid transfers)
+// p-multigrid transfers), or CG1 (the trace transfers)
 enum { SPACE2_PRESSURE = 0, SPACE2_COARSER };
+enum { SPACE2_CG1 = SPACE2_COARSER + 1 };
 
 struct fdb_hex_form {
     int form;                 // enum fdb_form
@@ -396,6 +396,12 @@ static const fdb_hex_form hex_forms[] = {
      "f_sigma, w, f_u", FDB_INTEGRAL_CELL, SPACE2_PRESSURE},
     {FDB_FORM_MIXED_POISSON_RECONSTRUCT, "mixed_poisson_reconstruct", 1, false, nullptr, 0, false, LAUNCH_HYBRID,
      {3, 0, 0}, 2, "lambda, f_sigma, w, y_u, f_u", FDB_INTEGRAL_CELL, SPACE2_PRESSURE},
+    // the GTMG transfers between CG1 and that trace space: the descriptor is the trace space (degree k - 1), the
+    // second space CG1.  Device mode only, rank 1, no diagonal (trace_transfer_call)
+    {FDB_FORM_TRACE_PROLONG, "trace_prolong", 1, false, nullptr, 0, false, LAUNCH_TRACE_TRANSFER, {2, 0, 0}, 1, "c",
+     FDB_INTEGRAL_CELL, SPACE2_CG1},
+    {FDB_FORM_TRACE_RESTRICT, "trace_restrict", 1, false, nullptr, 0, false, LAUNCH_TRACE_TRANSFER, {2, 0, 0}, 1,
+     "lambda, w", FDB_INTEGRAL_CELL, SPACE2_CG1},
 };
 
 // the (fine, coarse) degree pairs the transfer kernels instantiate (p_transfer_hex.cu)
@@ -484,6 +490,24 @@ static int kernel_create(const fdb_kernel_desc *d, const fdb_space2_desc *s2, fd
         return 1;
     }
     const bool transfer = f->launcher == LAUNCH_P_TRANSFER;
+    const bool trace = f->launcher == LAUNCH_TRACE_TRANSFER;
+    if (trace) {
+        if (d->degree < 1 || d->degree > 2) {
+            set_error("fdb_kernel_create_mixed: %s: trace degree %d not instantiated: the hybridised trace spaces of "
+                      "k = 2, 3 (trace degrees 1, 2)", f->name, d->degree);
+            return 1;
+        }
+        if (mode != MODE_ACTION) {
+            set_error("fdb_kernel_create_mixed: %s is a transfer, a rank-1 map between CG1 and the trace space: it "
+                      "has no rank-2 or diagonal form", f->name);
+            return 1;
+        }
+        if (s2->degree != 1) {
+            set_error("fdb_kernel_create_mixed: %s: the second space must be CG1, the vertex values (degree 1), got "
+                      "degree %d", f->name, s2->degree);
+            return 1;
+        }
+    }
     if (f->launcher == LAUNCH_SPECTRAL) {
         // the GLL rule in dof order: the points are the nodes (dof 0 at 0, dof 1 at 1), so B is the identity
         if (d->rank == 2) {
@@ -606,7 +630,7 @@ static int kernel_create(const fdb_kernel_desc *d, const fdb_space2_desc *s2, fd
         return 1;
     }
     // (a transfer and the Schur complement of mixed Poisson read no coordinates: offset1 is not used)
-    const bool no_coords = transfer || d->form == FDB_FORM_MIXED_POISSON_SCHUR;
+    const bool no_coords = transfer || trace || d->form == FDB_FORM_MIXED_POISSON_SCHUR;
     if (d->cell == FDB_CELL_HEX_EXTRUDED && (!d->offset0 || (!d->offset1 && !no_coords))) {
         set_error("fdb_kernel_create: extruded cells need offset0/offset1");
         return 1;
@@ -657,6 +681,7 @@ static int kernel_create(const fdb_kernel_desc *d, const fdb_space2_desc *s2, fd
     if (f->launcher == LAUNCH_HDIV) k->arity = 3 * d->degree * d->degree * (d->degree + 1);    // NCF_k
     // the hybrid forms: offset0 holds the trace map's 6k^2 layer offsets, then the NCF map's 3k^2(k+1)
     if (f->launcher == LAUNCH_HYBRID) k->arity = 6 * d->degree * d->degree + 3 * d->degree * d->degree * (d->degree + 1);
+    if (trace) k->arity = 6 * k->n1d * k->n1d;                                      // the trace map: 6k^2
     const int arity1 = sides * 8;
     memset(k->h_off0, 0, sizeof(k->h_off0));
     memset(k->h_off1, 0, sizeof(k->h_off1));
@@ -672,7 +697,7 @@ static int kernel_create(const fdb_kernel_desc *d, const fdb_space2_desc *s2, fd
         if (s2->offset) memcpy(k->h_off2, s2->offset, sizeof(fdb_int) * arity2);
         memcpy(k->B2, s2->B, sizeof(k->B2));
     }
-    if (!transfer && collocated_derivative(k->n1d, d->B, d->D, k->Dt)) {
+    if (!transfer && !trace && collocated_derivative(k->n1d, d->B, d->D, k->Dt)) {
         set_error("fdb_kernel_create: basis table B is singular");
         delete k;
         return 1;
@@ -697,19 +722,20 @@ static int kernel_create(const fdb_kernel_desc *d, const fdb_space2_desc *s2, fd
 
 // the colouring plan of the call's map m (arity k->arity), rebuilt when the map, its generation or the range
 // changes.  It covers columns [0, end): the map is copied to the host if needed
-static int colouring_for(fdb_kernel_s *k, const fdb_call_args *a, int m)
+static int colouring_for(fdb_kernel_s *k, const fdb_call_args *a, int m, int arity = 0)
 {
+    if (!arity) arity = k->arity;
     if (k->colour_map_key == (const void *)a->maps[m] && k->colour_map_gen == map_ver(a, m) &&
         k->colour_end == a->end)
         return 0;
     std::vector<fdb_int> hmap;
     const fdb_int *src = a->maps[m];
     if (a->location == FDB_LOC_DEVICE) {
-        hmap.resize((size_t)a->end * k->arity);
+        hmap.resize((size_t)a->end * arity);
         FDB_CUDA(cudaMemcpy(hmap.data(), a->maps[m], sizeof(fdb_int) * hmap.size(), cudaMemcpyDeviceToHost));
         src = hmap.data();
     }
-    if (build_colouring(k, src, a->end)) return 1;
+    if (build_colouring(k, src, a->end, arity)) return 1;
     k->colour_map_key = (const void *)a->maps[m];
     k->colour_map_gen = map_ver(a, m);
     k->colour_end = a->end;
@@ -741,6 +767,36 @@ static int p_transfer_call(fdb_kernel_s *k, const fdb_call_args *a, int nlay)
                                  (const double *)a->args[1],
                                  form == FDB_FORM_P_RESTRICT ? (const double *)a->args[2] : nullptr,
                                  a->maps[fm], a->maps[1 - fm]);
+}
+
+// the GTMG trace transfers: args and maps in first-use order (include/fdb200.h), device mode only.  A coloured
+// restriction is coloured on the CG1 map (8 vertices per cell): cells that share a vertex must not run together
+static int trace_transfer_call(fdb_kernel_s *k, const fdb_call_args *a, int nlay)
+{
+    const bool prolong = k->desc.form == FDB_FORM_TRACE_PROLONG;
+    const fdb_hex_form *f = k->hex;
+    const int want = prolong ? 2 : 3;
+    if (a->location != FDB_LOC_DEVICE) {
+        set_error("fdb_kernel_call: %s takes device-resident Dats only (no host-pointer mode)", f->name);
+        return 1;
+    }
+    if (a->nargs != want || a->nmaps != 2) {
+        set_error("fdb_kernel_call: %s expects %d device args (%s) and 2 maps (%s), got %d/%d", f->name, want,
+                  prolong ? "lambda, c" : "c, lambda, w", prolong ? "trace map, CG1 map" : "CG1 map, trace map",
+                  a->nargs, a->nmaps);
+        return 1;
+    }
+    const int tm = prolong ? 0 : 1;      // the trace map's slot
+    if (!prolong && k->desc.scatter == FDB_SCATTER_COLOURED) {
+        if (a->start != 0) {
+            set_error("fdb_kernel_call: coloured scatter needs start == 0");
+            return 1;
+        }
+        if (colouring_for(k, a, 1 - tm, 8)) return 1;
+    }
+    return fdb_launch_trace_transfer(k, a->start, a->end, nlay, a->subset, (double *)a->args[0],
+                                     (const double *)a->args[1], prolong ? nullptr : (const double *)a->args[2],
+                                     a->maps[tm], a->maps[1 - tm]);
 }
 
 // mixed Poisson (FDB_FORM_MIXED_POISSON[_SCHUR]): args and maps as include/fdb200.h lists them, device mode only.
@@ -917,6 +973,7 @@ int fdb_kernel_call(fdb_kernel_t k, const fdb_call_args *a)
     if (f->launcher == LAUNCH_P_TRANSFER) return p_transfer_call(k, a, nlay);
     if (f->launcher == LAUNCH_HDIV) return hdiv_call(k, a, nlay);
     if (f->launcher == LAUNCH_HYBRID) return hybrid_call(k, a, nlay);
+    if (f->launcher == LAUNCH_TRACE_TRANSFER) return trace_transfer_call(k, a, nlay);
     const int mode = hex_mode(&k->desc);
     const bool transport_facets = f->launcher == LAUNCH_DG_TRANSPORT && k->desc.integral != FDB_INTEGRAL_CELL;
     if (f->integral != FDB_INTEGRAL_CELL && a->location != FDB_LOC_DEVICE) {

@@ -613,7 +613,71 @@ def chebyshev_coefficients(emin, emax, k):
     return out
 
 
-class PMG(_LevelCycle):
+class _SmoothedCycle(_LevelCycle):
+    """The parts of a cycle with Chebyshev- or Richardson-Jacobi smoothing and a CG / V-cycle coarse solve, shared by
+    :class:`PMG` and :class:`GTMG`.  A subclass sets, besides :class:`_LevelCycle`'s attributes, ``smoother``,
+    ``stars`` (None per level, or a vertex-star relaxation), ``bounds`` (:meth:`_estimate_bounds`), ``coarse_mg`` /
+    ``_coarse_top``, ``coarse_pc``, ``coarse_rtol``, ``coarse_maxit`` and a work vector "d" on every level."""
+
+    def _estimate_bounds(self, esteig, esteig_steps, seed):
+        """The Chebyshev bounds [a lmin + b lmax, c lmin + d lmax] of P^-1 A on every smoothed level (P = D, or the
+        level's star), lmin / lmax from :func:`jacobi_lanczos_bounds` with a right-hand side seeded by ``seed``."""
+        a, b_, c, d_ = esteig
+        rng = np.random.default_rng(seed)
+        for l in range(1, len(self.spaces)):
+            W = self.spaces[l]
+            shape = (W.node_count, W.cdim) if W.cdim > 1 else (W.node_count,)
+            rhs = W.dat(rng.standard_normal(shape))
+            for bc in self.bcs[l]:
+                bc.zero(rhs)
+            star = self.stars[l]
+            lmin, lmax = jacobi_lanczos_bounds(self.ops[l], self.invdiag[l], rhs, esteig_steps,
+                                               M=None if star is None else star.apply)
+            self.bounds[l] = (a * lmin + b_ * lmax, c * lmin + d_ * lmax)
+
+    def _smooth(self, l, b, x):
+        if self.smoother == "richardson":
+            return super()._smooth(l, b, x)
+        # one action and one fused vector pass per iteration
+        from . import _lib
+        L = _lib.lib()
+        A, w = self.ops[l], self._work[l]
+        n = b._data.size
+        if self.stars[l] is not None:
+            # z = P^-1 (b - A x); d = c_d d + c_z z; x += d
+            for cd, cz in chebyshev_coefficients(*self.bounds[l], self.nu):
+                A.mult(x, w["t"])
+                _lib.check(L.fdb_vec_aypx(n, -1.0, b.device_ptr, w["t"].device_ptr))
+                _touched(w["t"])
+                self.stars[l].apply(w["t"], w["s"])
+                _lib.check(L.fdb_vec_chebyshev(n, cd, cz, w["s"].device_ptr, w["zero"].device_ptr,
+                                               w["one"].device_ptr, w["d"].device_ptr, x.device_ptr))
+                _touched(w["d"], x)
+            return
+        for cd, cz in chebyshev_coefficients(*self.bounds[l], self.nu):
+            A.mult(x, w["t"])
+            _lib.check(L.fdb_vec_chebyshev(n, cd, cz, b.device_ptr, w["t"].device_ptr, self.invdiag[l].device_ptr,
+                                           w["d"].device_ptr, x.device_ptr))
+            _touched(w["d"], x)
+
+    def _coarse_solve(self, b, x):
+        from . import _lib
+        from .assemble import cg
+        if self.coarse_mg is not None:
+            self.coarse_mg.apply(self._coarse_top, b, x)
+        elif self.coarse_pc == "none":
+            cg(self.ops[0], b, x, rtol=self.coarse_rtol, maxit=self.coarse_maxit)
+        else:
+            L, d, n = _lib.lib(), self.invdiag[0], b._data.size
+
+            def M(r, z):
+                _lib.check(L.fdb_vec_pointwise_mult(n, r.device_ptr, d.device_ptr, z.device_ptr))
+                _touched(z)
+            pcg(self.ops[0], b, x, M, rtol=self.coarse_rtol, maxit=self.coarse_maxit)
+        _touched(x)
+
+
+class PMG(_SmoothedCycle):
     """p-multigrid on one mesh (Firedrake's ``firedrake.PMGPC`` / ``firedrake.P1PC``): the levels are CG spaces of
     falling degree on ``V.mesh`` (:func:`pmg_degrees`), the operators rediscretised on every level, the transfers
     :class:`PTransfer`.  The cycle is :class:`VCycle`'s (``_LevelCycle.apply``); the top level is ``len(ops) - 1``.
@@ -710,56 +774,194 @@ class PMG(_LevelCycle):
         # Chebyshev bounds of D^-1 A on every smoothed level
         self.bounds = [None] * len(spaces)
         if smoother == "chebyshev":
-            a, b_, c, d_ = esteig
-            rng = np.random.default_rng(seed)
-            for l in range(1, len(spaces)):
-                W = spaces[l]
-                shape = (W.node_count, W.cdim) if W.cdim > 1 else (W.node_count,)
-                rhs = W.dat(rng.standard_normal(shape))
-                for bc in self.bcs[l]:
-                    bc.zero(rhs)
-                star = self.stars[l]
-                lmin, lmax = jacobi_lanczos_bounds(self.ops[l], self.invdiag[l], rhs, esteig_steps,
-                                                   M=None if star is None else star.apply)
-                self.bounds[l] = (a * lmin + b_ * lmax, c * lmin + d_ * lmax)
+            self._estimate_bounds(esteig, esteig_steps, seed)
 
-    def _smooth(self, l, b, x):
-        if self.smoother == "richardson":
-            return super()._smooth(l, b, x)
-        # one action and one fused vector pass per iteration
-        from . import _lib
-        L = _lib.lib()
-        A, w = self.ops[l], self._work[l]
-        n = b._data.size
-        if self.stars[l] is not None:
-            # z = P^-1 (b - A x); d = c_d d + c_z z; x += d
-            for cd, cz in chebyshev_coefficients(*self.bounds[l], self.nu):
-                A.mult(x, w["t"])
-                _lib.check(L.fdb_vec_aypx(n, -1.0, b.device_ptr, w["t"].device_ptr))
-                _touched(w["t"])
-                self.stars[l].apply(w["t"], w["s"])
-                _lib.check(L.fdb_vec_chebyshev(n, cd, cz, w["s"].device_ptr, w["zero"].device_ptr,
-                                               w["one"].device_ptr, w["d"].device_ptr, x.device_ptr))
-                _touched(w["d"], x)
-            return
-        for cd, cz in chebyshev_coefficients(*self.bounds[l], self.nu):
-            A.mult(x, w["t"])
-            _lib.check(L.fdb_vec_chebyshev(n, cd, cz, b.device_ptr, w["t"].device_ptr, self.invdiag[l].device_ptr,
-                                           w["d"].device_ptr, x.device_ptr))
-            _touched(w["d"], x)
+
+# ---------------------------------------------------------- GTMG for the trace system
+def trace_transfer_kernels(k):
+    """(prolong, restrict): the transfers between CG1 and the HDiv-trace space of degree k - 1 (k = 2, 3) as plain C
+    on the generic wrapper path, the statement that csrc/trace_transfer_hex.cu is checked against and the baseline it
+    is measured against.  prolong(lambda WRITE, c READ): trace dof (face 2d + s, GL indices t0, t1 along the
+    tangential axes e0 < e1) = sum over the face's 4 vertices of P1[t0][a_e0] P1[t1][a_e1] c; restrict(c INC, lambda
+    READ, w READ) adds the transpose applied to w * lambda."""
+    if k not in (2, 3):
+        raise NotImplementedError(f"trace transfers: k = {k}: the hybridised trace spaces are k = 2, 3")
+    table = f"static const double P1[{k}][2] = {_table(op2.trace_transfer_table(k))};\n"
+    loop = f"""
+    for (int d = 0; d < 3; ++d) {{
+        const int e0 = d == 0 ? 1 : 0, e1 = d == 2 ? 1 : 2;
+        for (int s = 0; s < 2; ++s)
+            for (int t0 = 0; t0 < {k}; ++t0)
+                for (int t1 = 0; t1 < {k}; ++t1) {{
+                    const int t = (2 * d + s) * {k * k} + t0 * {k} + t1;
+                    BODY
+                }}
+    }}"""
+    vert = ("const int lv = (s << (2 - d)) | ((b >> 1) << (2 - e0)) | ((b & 1) << (2 - e1));\n"
+            "                        const double p = P1[t0][b >> 1] * P1[t1][b & 1];")
+    pro = loop.replace("BODY", f"""double v = 0.0;
+                    for (int b = 0; b < 4; ++b) {{
+                        {vert}
+                        v += p * c[lv];
+                    }}
+                    lam[t] = v;""")
+    res = loop.replace("BODY", f"""const double wl = w[t] * lam[t];
+                    for (int b = 0; b < 4; ++b) {{
+                        {vert}
+                        c[lv] += p * wl;
+                    }}""")
+    return (CStringKernel(table + f"static void trace_prolong(double *lam, const double *c)\n{{{pro}\n}}\n",
+                          "trace_prolong"),
+            CStringKernel(table + f"static void trace_restrict(double *c, const double *lam, const double *w)\n"
+                                  f"{{{res}\n}}\n", "trace_restrict"))
+
+
+class TraceTransfer:
+    """prolong / restrict between CG1 (``Vc``, ``FunctionSpace(mesh, 1)`` by default) and the HDiv-trace space of a
+    :class:`assemble.HybridizationPC`, with :class:`TransferManager`'s interface, on the hand-written kernels of
+    csrc/trace_transfer_hex.cu (forms "trace_prolong", "trace_restrict").  prolong is lambda = P c, the trilinear
+    interpolant of the vertex values at every trace dof's face point; restrict is c = P^T lambda (exactly: every trace
+    dof is weighted by 1 / the number of cells holding it).  ``scatter``: "atomic" or "coloured" (bit-reproducible)
+    for the restriction.  ``prolong_generic`` / ``restrict_generic`` run :func:`trace_transfer_kernels` on the generic
+    wrapper path."""
+
+    def __init__(self, pc, Vc=None, scatter="atomic"):
+        from .assemble import FunctionSpace
+        S = pc.form.Sigma
+        if Vc is None:
+            Vc = FunctionSpace(S.mesh, 1)
+        if getattr(Vc, "family", "CG") != "CG" or Vc.degree != 1 or Vc.cdim != 1 or Vc.mesh is not S.mesh:
+            raise ValueError("TraceTransfer: the coarse space is scalar CG1 on the hybridised problem's mesh")
+        if Vc.dof_dset.halo is not None:
+            raise NotImplementedError("TraceTransfer: partitioned spaces are not supported")
+        self.pc, self.Vc, self.Vf, self.scatter = pc, Vc, pc.trace, scatter
+        self.k = S.degree
+        self.cell_set = S.cell_set
+        self.cmap = op2.Map(S.cell_set, Vc.node_set, 8, Vc.V.cell_node_map, offset=Vc.V.offset, name="trace_cg1")
+        self.tmap = pc.trace_map
+        counts = np.bincount(pc.trace.V.full_cell_node_list().ravel(), minlength=pc.trace.node_count)
+        self.weight = pc.trace.dat(1.0 / counts)
+        kw = dict(degree=self.k - 1, coarse_degree=1)
+        self._gk = {f: op2.GlobalKernel(op2.Kernel(f, **kw), maps, extruded=True,
+                                        scatter=scatter if f == "trace_restrict" else "atomic")
+                    for f, maps in (("trace_prolong", [self.tmap, self.cmap]),
+                                    ("trace_restrict", [self.cmap, self.tmap]))}
+        self._generic = None
+
+    def prolong(self, coarse: op2.Dat, fine: op2.Dat):
+        op2.Parloop(self._gk["trace_prolong"], self.cell_set, [fine(op2.WRITE, self.tmap),
+                                                               coarse(op2.READ, self.cmap)])()
+        return fine
+
+    def restrict(self, fine_dual: op2.Dat, coarse_dual: op2.Dat):
+        coarse_dual.zero()
+        coarse_dual.device_ptr                      # materialise the zero on the device
+        op2.Parloop(self._gk["trace_restrict"], self.cell_set,
+                    [coarse_dual(op2.INC, self.cmap), fine_dual(op2.READ, self.tmap),
+                     self.weight(op2.READ, self.tmap)])()
+        return coarse_dual
+
+    def prolong_generic(self, coarse: op2.Dat, fine: op2.Dat):
+        if self._generic is None:
+            self._generic = trace_transfer_kernels(self.k)
+        op2.par_loop(self._generic[0], self.cell_set, fine(op2.WRITE, self.tmap), coarse(op2.READ, self.cmap))
+        return fine
+
+    def restrict_generic(self, fine_dual: op2.Dat, coarse_dual: op2.Dat):
+        if self._generic is None:
+            self._generic = trace_transfer_kernels(self.k)
+        coarse_dual.zero()
+        op2.par_loop(self._generic[1], self.cell_set, coarse_dual(op2.INC, self.cmap), fine_dual(op2.READ, self.tmap),
+                     self.weight(op2.READ, self.tmap))
+        return coarse_dual
+
+
+class _TraceNatural:
+    """The trace level's "boundary condition": zero the natural-condition faces' multipliers (lambda = 0 there)."""
+
+    def __init__(self, pc):
+        self.pc = pc
+
+    def zero(self, d):
+        d.zero(self.pc._natural)
+
+
+class GTMG(_SmoothedCycle):
+    """Gopalakrishnan and Tan's non-nested two-level cycle for the trace system H lambda = r of an
+    :class:`assemble.HybridizationPC` (Firedrake's ``firedrake.GTMGPC``).  Level 1 is the trace space: operator
+    ``pc.mat``, Jacobi diagonal ``pc.diagonal_inverse()``, its natural-condition faces held at zero.  Level 0 is CG1 on
+    the same mesh with the rediscretised Laplacian ``Form(P1, 1/alpha, 0.0)`` and Dirichlet conditions on the
+    natural sub-domains; the transfers are :class:`TraceTransfer`.  For an affine p, (P p)^T H (P p) = p^T A p /
+    alpha: the local problem with affine trace data has the constant flux grad(lambda)/alpha as its exact solution,
+    so this coarse operator needs no fitted scale.
+
+    Unlike Firedrake, the engine builds the coarse space and operator itself: no ``appctx`` callbacks
+    (``get_coarse_space``, ``get_coarse_operator``, ``coarse_space_bcs``) are read.
+
+    Smoothing, bounds and coarse solves are :class:`PMG`'s: ``smoother`` "chebyshev" (``nu`` iterations, bounds
+    ``esteig`` of D^-1 H from ``esteig_steps`` Lanczos steps) or "richardson" (``omega``); ``coarse_ksp`` /
+    ``coarse_pc`` "cg" with "jacobi" or "none" to ``coarse_rtol`` / ``coarse_maxit``, or "preonly" with "mg": one
+    :class:`VCycle` on ``hierarchy``, whose finest mesh must be the problem's.  ``nullspace``: flux conditions on the
+    whole boundary (H 1 = 0, P 1 = 1): the coarse problem is the singular Neumann Laplacian, and the plain mean of its
+    right-hand side is removed so that it stays consistent; the caller's CG projects the preconditioned vector."""
+
+    def __init__(self, pc, nullspace=False, smoother="chebyshev", nu=2, omega=0.8, esteig=(0.0, 0.1, 0.0, 1.1),
+                 esteig_steps=10, coarse_ksp="cg", coarse_pc="jacobi", coarse_rtol=1e-3, coarse_maxit=500,
+                 hierarchy=None, scatter="atomic", seed=0):
+        from .assemble import DirichletBC, Form, FunctionSpace, assemble
+        if smoother not in ("chebyshev", "richardson"):
+            raise NotImplementedError(f"GTMG level smoother {smoother!r}: 'chebyshev' or 'richardson'")
+        if (coarse_ksp, coarse_pc) not in (("cg", "jacobi"), ("cg", "none"), ("preonly", "mg")):
+            raise NotImplementedError(f"GTMG coarse solve ksp_type {coarse_ksp!r} with pc_type {coarse_pc!r}: cg with "
+                                      f"jacobi or none, or preonly with mg")
+        F = pc.form
+        mesh = F.Sigma.mesh
+        self.nu, self.omega, self.smoother = nu, omega, smoother
+        self.coarse_ksp, self.coarse_pc = coarse_ksp, coarse_pc
+        self.coarse_rtol, self.coarse_maxit = coarse_rtol, coarse_maxit
+        self.nullspace = nullspace
+        natural = pc.natural_sub_domains
+
+        def make_form(V):
+            return Form(V, 1.0 / F.alpha, 0.0)
+
+        self.coarse_mg = None
+        if coarse_pc == "mg":
+            if hierarchy is None or hierarchy[len(hierarchy) - 1] is not mesh:
+                raise ValueError("GTMG coarse pc_type mg needs a mesh hierarchy whose finest mesh is the hybridised "
+                                 "problem's mesh")
+            self.coarse_mg = VCycle(hierarchy, 1, make_form, natural, omega=omega)
+            self._coarse_top = len(hierarchy) - 1
+            V1 = self.coarse_mg.spaces[-1]
+            bcs0 = self.coarse_mg.bcs[-1]
+            A0, d0 = self.coarse_mg.ops[-1], self.coarse_mg.invdiag[-1]
+        else:
+            V1 = FunctionSpace(mesh, 1)
+            bcs0 = [DirichletBC(V1, 0.0, s) for s in natural]
+            A0 = assemble(make_form(V1), bcs=bcs0, mat_type="matfree")
+            d0 = A0.getDiagonal(V1.dat())
+            op2.par_loop(reciprocal_kernel(1), V1.node_set, d0(op2.RW))
+        self.pc = pc
+        self.spaces = [V1, pc.trace]
+        self.bcs = [bcs0, [_TraceNatural(pc)]]
+        self.transfers = [TraceTransfer(pc, V1, scatter)]
+        self.ops = [A0, pc.mat]
+        self.invdiag = [d0, pc.diagonal_inverse()]
+        self.stars = [None, None]
+        self._work = [dict(r=W.dat(), e=W.dat(), t=W.dat(), b=W.dat(), x=W.dat(), d=W.dat()) for W in self.spaces]
+        self._ones = V1.dat(np.ones(V1.node_count)) if nullspace else None
+        self.top = 1
+        self.bounds = [None, None]
+        if smoother == "chebyshev":
+            self._estimate_bounds(esteig, esteig_steps, seed)
 
     def _coarse_solve(self, b, x):
-        from . import _lib
-        from .assemble import cg
-        if self.coarse_mg is not None:
-            self.coarse_mg.apply(self._coarse_top, b, x)
-        elif self.coarse_pc == "none":
-            cg(self.ops[0], b, x, rtol=self.coarse_rtol, maxit=self.coarse_maxit)
-        else:
-            L, d, n = _lib.lib(), self.invdiag[0], b._data.size
+        if self.nullspace:
+            b.axpy(-b.inner(self._ones) / b._data.size, self._ones)
+        super()._coarse_solve(b, x)
 
-            def M(r, z):
-                _lib.check(L.fdb_vec_pointwise_mult(n, r.device_ptr, d.device_ptr, z.device_ptr))
-                _touched(z)
-            pcg(self.ops[0], b, x, M, rtol=self.coarse_rtol, maxit=self.coarse_maxit)
-        _touched(x)
+    def __call__(self, r, z):
+        """z = one cycle applied to r, from z = 0."""
+        z.zero()
+        z.device_ptr
+        return self.apply(self.top, r, z)

@@ -1464,6 +1464,12 @@ class Kernel:
     gives (sigma, u) cell by cell from the multiplier: (INC, READ, READ, READ, READ, INC, READ) = (sigma output,
     coordinates, lambda, sigma load, w, u output, u load), sigma output += w o sigma_K, u output += u_K.  The
     GlobalKernel's ``arguments`` are always [trace map, coordinate map, NCF map, DQ map].  Device-resident Dats only.
+
+    "trace_prolong" and "trace_restrict" are the transfers of the GTMG cycle between CG1 (vertex values) and the
+    HDiv-trace space of degree ``degree`` = k - 1 (1..2) on the same cells: prolong (trace WRITE, CG1 READ), the
+    trilinear interpolant of the vertex values at every trace dof's face point, and restrict (CG1 INC, trace READ, w
+    READ: ``c += P^T (w * lambda)``, w one value per trace dof).  The trace Dats go through the trace map, the CG1 ones
+    through the CG1 map; no coordinates.  Device-resident Dats only.
     """
     form: str = "helmholtz"
     degree: int = 1
@@ -1523,7 +1529,7 @@ class Kernel:
             object.__setattr__(self, "name", self.form + ("_diagonal" if self.diagonal else ""))
             return
         if spec and spec.transfer:
-            acc = (INC, READ, READ) if self.form == "p_restrict" else (WRITE, READ)
+            acc = (INC, READ, READ) if self.form in ("p_restrict", "trace_restrict") else (WRITE, READ)
             object.__setattr__(self, "accesses", acc)
             object.__setattr__(self, "name", self.form)
             return
@@ -1591,6 +1597,7 @@ class _Form(NamedTuple):
     facet: bool = False         # an exterior-facet integral: the local facet numbers come last, the integral as given
     velocity: bool = False      # reads b (3 values per vertex) through the coordinate map after u
     transfer: bool = False      # a p-multigrid degree transfer: fine and coarse maps, no coordinates
+    trace: bool = False         # a GTMG transfer between CG1 and the HDiv-trace space (with transfer)
     gll: bool = False           # stated on the GLL rule at the nodes: the default element is the collocated GLL one
     hdiv: bool = False          # a mixed Poisson form on NCF_k x DQ_{k-1}
     temperature: bool = False   # also reads and writes a temperature on the pressure map (Boussinesq)
@@ -1624,7 +1631,9 @@ _FORMS = {"helmholtz": _Form(_lib.FORM_HELMHOLTZ),
           "boussinesq_jacobian": _Form(_lib.FORM_BOUSSINESQ_JACOBIAN, coefficient=True, pressure=True,
                                        temperature=True),
           "mixed_poisson_hybrid": _Form(_lib.FORM_MIXED_POISSON_HYBRID, hdiv=True, hybrid=True),
-          "mixed_poisson_reconstruct": _Form(_lib.FORM_MIXED_POISSON_RECONSTRUCT, hdiv=True, hybrid=True)}
+          "mixed_poisson_reconstruct": _Form(_lib.FORM_MIXED_POISSON_RECONSTRUCT, hdiv=True, hybrid=True),
+          "trace_prolong": _Form(_lib.FORM_TRACE_PROLONG, transfer=True, trace=True),
+          "trace_restrict": _Form(_lib.FORM_TRACE_RESTRICT, transfer=True, trace=True)}
 _INTEGRALS = {"cell": _lib.INTEGRAL_CELL, "exterior_facet": _lib.INTEGRAL_EXTERIOR_FACET,
               "interior_facet": _lib.INTEGRAL_INTERIOR_FACET, "fused": _lib.INTEGRAL_FUSED}
 
@@ -1643,6 +1652,14 @@ def p_transfer_tables(p, q):
         T[:2] = 0.0
         T[0, 0] = T[1, 1] = 1.0
     return P, R
+
+
+def trace_transfer_table(k):
+    """(k, 2): the CG1 basis (1 - x, x) at the k Gauss-Legendre points on [0, 1], ascending (the points of the trace
+    dofs along each tangential axis)."""
+    from .fiat_lite import gauss_legendre
+    x, _ = gauss_legendre(k)
+    return np.stack([1.0 - x, x], axis=1)
 
 
 class GlobalKernel:
@@ -1785,7 +1802,8 @@ class GlobalKernel:
     def _compile_transfer(self):
         """fdb_kernel_create_mixed of a p-multigrid transfer: R in the descriptor's B (nq = q+1), P in the second
         space's (include/fdb200.h).  The maps come in first-use order: prolong (fine, coarse), restrict and inject
-        (coarse, fine)."""
+        (coarse, fine).  A trace transfer takes the trace space for the fine one (``degree`` = k - 1, ``coarse_degree``
+        = 1) and only the CG1 table (:func:`trace_transfer_table`)."""
         from .fiat_lite import interval_element
         lk = self.local_kernel
         d = _lib.KernelDesc()
@@ -1795,7 +1813,11 @@ class GlobalKernel:
         d.scatter = {"atomic": _lib.SCATTER_ATOMIC, "coloured": _lib.SCATTER_COLOURED}[self.scatter]
         s2 = _lib.Space2Desc()
         s2.degree = lk.coarse_degree
-        if lk.element is None and lk.coarse_degree >= 1:
+        if _FORMS[lk.form].trace:
+            # the trace space (degree k - 1, nq = k) and CG1: its basis (1 - x, x) at the k Gauss-Legendre points
+            d.nq = lk.degree + 1
+            P, R = trace_transfer_table(lk.degree + 1), None
+        elif lk.element is None and lk.coarse_degree >= 1:
             P, R = p_transfer_tables(lk.degree, lk.coarse_degree)
         else:                               # another fine element (the engine refuses one without end nodes)
             fine = lk.element or interval_element(lk.degree)
@@ -1806,8 +1828,9 @@ class GlobalKernel:
         for i in range(nf):
             for a in range(nc):
                 s2.B[i * nc + a] = P[i, a]
-                d.B[a * nf + i] = R[a, i]
-        fm, cm = self.arguments[:2] if lk.form == "p_prolong" else self.arguments[1::-1]
+                if R is not None:
+                    d.B[a * nf + i] = R[a, i]
+        fm, cm = self.arguments[:2] if lk.form in ("p_prolong", "trace_prolong") else self.arguments[1::-1]
         keep = []
         if self.extruded:
             if fm.offset is None or cm.offset is None:

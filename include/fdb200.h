@@ -448,6 +448,31 @@ enum fdb_form {
                                      RECONSTRUCT  rank 1  [y_sigma INC, coords, lambda, f_sigma, w, y_u INC, f_u]
                                                           maps [NCF map, coord map, trace map, DQ map]
                                                           y_sigma += w o sigma_K, y_u += u_K               */
+    FDB_FORM_TRACE_PROLONG = 28,
+    FDB_FORM_TRACE_RESTRICT = 29,
+                                /* the transfers between CG1 (vertex values) and the HDiv-trace space of
+                                   FDB_FORM_MIXED_POISSON_HYBRID (k = 2, 3) on the SAME hex cells, the level transfers
+                                   of the two-level GTMG cycle for the trace system, cell-local and metric-free:
+                                     TRACE_PROLONG   lambda  = P c                 WRITE
+                                     TRACE_RESTRICT  c      += P^T (w o lambda)    INC
+                                   Trace dof t (face 2d + s, GL indices t0, t1 along the tangential axes in axis
+                                   order) takes the value at its face point of the trilinear interpolant of the cell's
+                                   8 vertex values (CG1 local vertex (a0 * 2 + a1) * 2 + a2).  w is one value per trace
+                                   dof, 1 / (number of cells holding it), so that the restriction is exactly P^T.
+                                   The descriptor describes the trace space: degree = k - 1 (1 or 2), nq = k, cdim 1,
+                                   offset0 = the trace map's 6k^2 layer offsets (B, D, wq, xq, offset1 unused);
+                                   fdb_space2_desc is CG1: degree 1, B = the CG1 basis at the k Gauss-Legendre points,
+                                   (k, 2), offset = the CG1 map's 8 layer offsets.  Created by fdb_kernel_create_mixed,
+                                   rank 1, cell integral; other degrees, other second spaces, rank 2 and the diagonal
+                                   are refused.  Prolong: every cell sharing a face writes its dofs, each summing its
+                                   four vertex terms in ascending order of the global vertex number, so both writers
+                                   store bitwise the same value (whatever the local vertex order of either cell).  The
+                                   maps are in first-use order of the arguments.  Device mode only, extruded and native
+                                   hexes:
+                                     TRACE_PROLONG   [lambda WRITE, c]        maps [trace map, CG1 map]
+                                     TRACE_RESTRICT  [c INC, lambda, w]       maps [CG1 map, trace map]
+                                                                              (atomic or coloured scatter, coloured
+                                                                              on the CG1 map: bit-reproducible)   */
 };
 
 enum fdb_cell {
@@ -526,7 +551,8 @@ typedef struct fdb_kernel_desc {
  * B: its basis at the descriptor's nq Gauss points, row-major (nq, degree+1), 1-D dof numbering;
  * offset: the extruded layer offsets of the second space's map, (degree+1)^3 entries, NULL for
  * native hexes, copied at creation.  The p-multigrid transfers (FDB_FORM_P_PROLONG, _RESTRICT, _INJECT)
- * describe their coarse space CG_q here: degree = q and B = P, (fine degree + 1, q + 1). */
+ * describe their coarse space CG_q here: degree = q and B = P, (fine degree + 1, q + 1); the trace transfers
+ * (FDB_FORM_TRACE_PROLONG, _RESTRICT) their CG1 space: degree = 1 and B = the CG1 basis at the k trace points. */
 typedef struct fdb_space2_desc {
     int32_t degree;
     double B[FDB_MAX_1D * FDB_MAX_1D];
